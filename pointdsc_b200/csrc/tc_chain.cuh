@@ -5,24 +5,29 @@
 //   MSG : msg --Wm0,relu--> --Wm1,relu--> --Wm2--> + feat1 --> feat (fp32 -> HBM)
 // (reference models/PointDSC.py:56-61 PointCN, :21-23/:36-38 projections, :12-20/:43-44 fc_message + residual)
 //
-// Persistent CTAs (one per SM), weights resident in shared memory, 128-row tiles, two warpgroups of 64 rows each.  Per tile
-// all 256 threads convert the tile's fp32 input rows into the swizzled 16-bit hi | lo A image, then each warpgroup runs its
-// chain with the accumulators in registers.  Chained steps never go back through shared memory: the epilogue of one GEMM
-// (bias, ReLU, hi/lo split) turns its accumulator fragment into the register A operand of the next.
+// Persistent CTAs (one per SM), weights resident in shared memory, 128-row tiles, two warpgroups of 64 rows each.  A tile's
+// fp32 input (64 KB of contiguous memory in every mode) arrives in shared memory by one bulk async copy; each thread reads its
+// own accumulator-layout fragment of it and splits it into the hi | lo register A operand of the first GEMM.  As soon as every
+// thread holds its fragments, the copy of the CTA's next tile is issued, so that tile's input streams in while this one
+// computes and stores.  Chained steps never go back through shared memory: the epilogue of one GEMM (bias, ReLU, hi/lo split)
+// turns its accumulator fragment into the register A operand of the next.  The Q / K / V images are written after a transpose
+// within each quad of lanes, one whole 16-byte swizzle chunk per lane and store (store_row).  The rows of a ragged last tile
+// beyond `rows` hold stale data; they feed only output rows that are never stored (a 1x1 convolution maps each row on its own).
 // feat1 (fp32, PCQ -> KV and MSG) lives in HBM in a BLOCKED layout keyed by the 128-row chain tile:
 //     [tile][32-column chunk cc][128 rows][128 B], 16-byte piece q of row r at piece q ^ (r & 7)
-// so that a loader warp reads 32 rows x 128 B of one chunk as 4 KB of contiguous memory (blocked_f32_offset).
+// so that the fragment reads of a staged feat1 tile are at most 2-way bank conflicted (blocked_f32_offset).
 #pragma once
 #include "tc_common.cuh"
 
 namespace pdsc {
 
 constexpr int kChainThreads = 256;
-constexpr int kChA = 0;                          // A image: [hi p0 16K][hi p1 16K][lo p0 16K][lo p1 16K]
+constexpr int kChIn = 0;                         // staged input tile (64 KB): row-major feat / msg, or blocked feat1
 constexpr int kChW = 65536;                      // weight images (128 KB for PCQ / KV, 80 KB for MSG)
-constexpr int kChBias = kChW + 131072;           // 256 floats: this mode's biases
-constexpr int kChBars = kChBias + 1024;
-constexpr int kChainSmem = kChBars + 64;         // 197,696 B
+constexpr int kChRes = kChW + 81920;             // MSG: staged blocked feat1 residual tile (64 KB) behind its weights
+constexpr int kChBias = kChRes + 65536;          // 256 floats: this mode's biases
+constexpr int kChBars = kChBias + 1024;          // mbarriers: weights, input, residual
+constexpr int kChainSmem = kChBars + 64;         // 214,080 B
 
 // (set, index within the set) of global row g
 __device__ __forceinline__ void locate_row(long long g, int N, int& bb, int& nn) {
@@ -35,30 +40,69 @@ __host__ __device__ __forceinline__ size_t blocked_f32_offset(long long g, uint3
   return (size_t)(g >> 7) * 65536 + (size_t)(piece >> 3) * 16384 + (size_t)(g & 127) * 128 + (size_t)(((piece & 7u) ^ ((uint32_t)g & 7u)) << 4);
 }
 
-// 16-bit pair (columns c, c + 1 of image row `row`) of a [rows][128] operand image whose 64-column panels are panel_bytes apart
-__device__ __forceinline__ void store_pair(uint8_t* img, uint32_t panel_bytes, uint32_t row, int c, uint32_t v) {
-  *reinterpret_cast<uint32_t*>(img + (uint32_t)(c >> 6) * panel_bytes + sw128_offset(row, (uint32_t)(c & 63))) = v;
+// 4 x 4 transpose of 32-bit words across the 4 lanes q of a quad (the lanes that share an accumulator row): on entry v[k] is
+// word q of chunk k, on return word k of chunk q.  Every lane of the warp takes part.
+__device__ __forceinline__ void quad_transpose(uint32_t (&v)[4], int q) {
+#pragma unroll
+  for (int s = 1; s <= 2; s <<= 1)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (k & s) continue;
+      const bool up = (q & s) != 0;
+      const uint32_t r = __shfl_xor_sync(0xffffffffu, up ? v[k] : v[k + s], s);
+      if (up) v[k] = r;
+      else v[k + s] = r;
+    }
+}
+
+// one row of a [rows][128] 16-bit operand image whose 64-column panels are panel_bytes apart, from the quad's fragments:
+// w[j] = columns 8 j + 2 q, + 1 (j = 0..15).  Each lane stores whole 16-byte chunks (8 columns), so every sector is written
+// in full by one instruction.  Only lanes with `store` write, but all must call.
+__device__ __forceinline__ void store_row(uint8_t* img, uint32_t panel_bytes, uint32_t row, const uint32_t (&w)[16], int q, bool store) {
+#pragma unroll
+  for (int m = 0; m < 4; ++m) {
+    uint32_t v[4] = {w[4 * m], w[4 * m + 1], w[4 * m + 2], w[4 * m + 3]};
+    quad_transpose(v, q);
+    const uint32_t j = 4u * m + q;
+    if (store) *reinterpret_cast<uint4*>(img + (j >> 3) * panel_bytes + sw128_offset(row, 8u * (j & 7u))) = make_uint4(v[0], v[1], v[2], v[3]);
+  }
 }
 
 template <int MODE, int FMT>
 __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* Abuf = smem + kChA;
+  const uint8_t* stage = smem + kChIn;
+  const uint8_t* resbuf = smem + kChRes;
   float* bias = reinterpret_cast<float*>(smem + kChBias);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kChBars);
   const uint32_t s0 = smem_u32(smem);
-  const uint32_t bar_w = smem_u32(bars);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int wg = warp >> 2, wt = tid & 127;
-  const uint32_t a_base = s0 + kChA + (uint32_t)wg * 8192u, w_base = s0 + kChW;   // this warpgroup's 64 rows of the A image
+  const uint32_t bar_w = smem_u32(bars), bar_in = smem_u32(bars + 1), bar_res = smem_u32(bars + 2);
+  const int tid = threadIdx.x;
+  const int wg = tid >> 7, wt = tid & 127;
+  const uint32_t w_base = s0 + kChW;
   // this mode's biases, packed: PCQ b1|bq, KV bk|bv, MSG bm0|bm1|bm2
   constexpr int kBiasSrc = (MODE == kPCQ) ? kB1 : (MODE == kKV) ? kBk : kBm0;
   const int N = a.N;
   const long long rows = a.rows;
+  const long long num_tiles = (rows + 127) / 128;
+
+  // a tile's input is the 64 KB at tile * 65536; feat and msg hold exactly `rows` rows, blocked feat1 is padded to whole tiles
+  auto issue_input = [&](long long t) {
+    const long long left = rows - t * 128;
+    const uint32_t bytes = (MODE == kKV || left >= 128) ? 65536u : (uint32_t)left * 512u;
+    mbar_expect_tx(bar_in, bytes);
+    bulk_g2s(s0 + kChIn, reinterpret_cast<const uint8_t*>(a.in) + (size_t)t * 65536, bytes, bar_in);
+  };
+  // byte offset of (row r, column c) in a staged input tile
+  auto in_offset = [](int r, int c) -> uint32_t {
+    return MODE == kKV ? (uint32_t)blocked_f32_offset(r, (uint32_t)c >> 2) + (c & 3) * 4 : (uint32_t)(r * kC + c) * 4u;
+  };
 
   if (tid == 0) {
-    if (s0 & 1023u) __trap();   // the swizzled operand images need 1024-byte aligned shared memory
+    if (s0 & 1023u) __trap();   // the swizzled weight images need 1024-byte aligned shared memory
     mbar_init(bar_w, 1);
+    mbar_init(bar_in, 1);
+    mbar_init(bar_res, 1);
     fence_barrier_init();
   }
   bias[tid] = a.bias[kBiasSrc + tid];
@@ -67,44 +111,37 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
     mbar_expect_tx(bar_w, (uint32_t)a.wbytes);
     for (int off = 0; off < a.wbytes; off += 32768)
       bulk_g2s(w_base + off, a.wimg + off, (uint32_t)min(32768, a.wbytes - off), bar_w);
+    if (blockIdx.x < num_tiles) issue_input(blockIdx.x);
   }
-  const long long num_tiles = (rows + 127) / 128;
+  mbar_wait(bar_w, 0);   // also keeps a CTA without tiles alive until its weight copy has landed
   const int fr = 64 * wg + frag_row(wt), fc = frag_col(wt);   // fragment rows fr, fr + 8 of the tile; columns 8 j + fc, + 1
-  bool weights = false;
+  const int quad = fc >> 1;                                   // this lane's place among the 4 lanes that share its rows
 
-  for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  uint32_t phase = 0;
+  for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, phase ^= 1u) {
     const long long row0 = tile * 128;
-    // ---- A image: warp w converts rows w + 8 i, lane = 16-byte column piece ----
+    // ---- this thread's fragment of the staged input tile -> hi / lo register A operand (K = 128) ----
+    uint32_t ahi[8][4], alo[8][4];
+    mbar_wait(bar_in, phase);
     {
-      float4 v[16];
-      const uint8_t* blk = reinterpret_cast<const uint8_t*>(a.in) + (size_t)tile * 65536 + (size_t)(lane >> 3) * 16384;
+      float x[64];
 #pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int rr = warp + 8 * i;
-        const bool ok = row0 + rr < rows;
-        if (MODE == kKV)   // feat1: blocked layout
-          v[i] = ok ? __ldg(reinterpret_cast<const float4*>(blk + (uint32_t)rr * 128u + ((((uint32_t)lane & 7u) ^ ((uint32_t)rr & 7u)) << 4)))
-                    : make_float4(0.f, 0.f, 0.f, 0.f);
-        else
-          v[i] = ok ? __ldg(reinterpret_cast<const float4*>(a.in + (row0 + rr) * kC) + lane) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      __syncthreads();   // both warpgroups have retired the MMAs that read the previous tile's image
+      for (int j = 0; j < 16; ++j)
 #pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int rr = warp + 8 * i;
-        uint32_t h0, l0, h1, l1;
-        split_pair<FMT>(v[i].x, v[i].y, h0, l0);
-        split_pair<FMT>(v[i].z, v[i].w, h1, l1);
-        const uint32_t off = (uint32_t)(lane >> 4) * 16384u + sw128_offset((uint32_t)rr, (uint32_t)(lane & 15) * 4u);
-        *reinterpret_cast<uint2*>(Abuf + off) = make_uint2(h0, h1);
-        if (a.split) *reinterpret_cast<uint2*>(Abuf + 32768 + off) = make_uint2(l0, l1);
-      }
-      fence_proxy_async_smem();
-      __syncthreads();
+        for (int h = 0; h < 2; ++h) {
+          const float2 v = *reinterpret_cast<const float2*>(stage + in_offset(fr + 8 * h, 8 * j + fc));
+          x[4 * j + 2 * h] = v.x;
+          x[4 * j + 2 * h + 1] = v.y;
+        }
+      frag_split<FMT, 8>(x, ahi, alo);
     }
-    if (!weights) {
-      mbar_wait(bar_w, 0);
-      weights = true;
+    __syncthreads();   // every thread holds its fragments and is past the previous tile's residual reads: refill both buffers
+    if (tid == 0) {
+      if (tile + gridDim.x < num_tiles) issue_input(tile + gridDim.x);
+      if (MODE == kMSG) {
+        mbar_expect_tx(bar_res, 65536u);
+        bulk_g2s(s0 + kChRes, reinterpret_cast<const uint8_t*>(a.res) + (size_t)tile * 65536, 65536u, bar_res);
+      }
     }
     // the two rows of this thread: global index, set and position within the set
     long long g[2];
@@ -119,7 +156,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
       // ---- PointCN: feat1 = relu(A W1^T + b1) -> HBM (fp32, blocked) and registers (A operand of the Q GEMM) ----
       float x[64];
       wgmma_fence();
-      gemm_ss<FMT, 2, 128>(x, a_base, a_base + 32768, 16384, w_base, w_base + 32768, 16384, a.split);
+      gemm_rs<FMT, 8, 128, 0>(x, ahi, alo, w_base, w_base + 32768, 16384, a.split, 0);
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(x);
@@ -134,7 +171,6 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
             *reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(a.out_f32) + blocked_f32_offset(g[h], (uint32_t)c >> 2) + (c & 3) * 4) =
                 make_float2(x[e], x[e + 1]);
         }
-      uint32_t ahi[8][4], alo[8][4];
       frag_split<FMT, 8>(x, ahi, alo);
       float q[64];
       wgmma_fence();
@@ -145,17 +181,16 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
       // ---- Q image (pre-scaled weights and bias) ----
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        if (g[h] >= rows) continue;
         uint8_t* img = a.qimg + ((size_t)bb[h] * a.QT + (nn[h] >> 7)) * 65536;
         const uint32_t r = (uint32_t)(nn[h] & 127);
+        uint32_t hi[16], lo[16];
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const int c = 8 * j + fc, e = 4 * j + 2 * h;
-          uint32_t hi, lo;
-          split_pair<FMT>(q[e] + bias[128 + c], q[e + 1] + bias[128 + c + 1], hi, lo);
-          store_pair(img, 16384u, r, c, hi);
-          if (a.split) store_pair(img + 32768, 16384u, r, c, lo);
+          split_pair<FMT>(q[e] + bias[128 + c], q[e + 1] + bias[128 + c + 1], hi[j], lo[j]);
         }
+        store_row(img, 16384u, r, hi, quad, g[h] < rows);
+        if (a.split) store_row(img + 32768, 16384u, r, lo, quad, g[h] < rows);
       }
     } else if (MODE == kKV) {
       // ---- K image, then V image (V behind K in the key tile's 64 KB) ----
@@ -164,31 +199,30 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
         float x[64];
         const uint32_t wb = w_base + (uint32_t)step * 65536u;
         wgmma_fence();
-        gemm_ss<FMT, 2, 128>(x, a_base, a_base + 32768, 16384, wb, wb + 32768, 16384, a.split);
+        gemm_rs<FMT, 8, 128, 0>(x, ahi, alo, wb, wb + 32768, 16384, a.split, 0);
         wgmma_commit();
         wgmma_wait<0>();
         fence_regs(x);
         const float* bvec = bias + 128 * step;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          if (g[h] >= rows) continue;
           uint8_t* img = a.kvimg + ((size_t)bb[h] * a.KT + (nn[h] >> 6)) * 65536 + 32768 * step;
           const uint32_t r = (uint32_t)(nn[h] & 63);
+          uint32_t hi[16], lo[16];
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
             const int c = 8 * j + fc, e = 4 * j + 2 * h;
-            uint32_t hi, lo;
-            split_pair<FMT>(x[e] + bvec[c], x[e + 1] + bvec[c + 1], hi, lo);
-            store_pair(img, 8192u, r, c, hi);
-            if (a.split) store_pair(img + 16384, 8192u, r, c, lo);
+            split_pair<FMT>(x[e] + bvec[c], x[e + 1] + bvec[c + 1], hi[j], lo[j]);
           }
+          store_row(img, 8192u, r, hi, quad, g[h] < rows);
+          if (a.split) store_row(img + 16384, 8192u, r, lo, quad, g[h] < rows);
         }
       }
     } else {
       // ---- fc_message: Wm0 64 x 128 (hi 16K | lo 16K, panel 8K), Wm1 64 x 64 (hi 8K | lo 8K), Wm2 128 x 64 (hi 16K | lo 16K) ----
       float h0[32];
       wgmma_fence();
-      gemm_ss<FMT, 2, 64>(h0, a_base, a_base + 32768, 16384, w_base, w_base + 16384, 8192, a.split);
+      gemm_rs<FMT, 8, 64, 0>(h0, ahi, alo, w_base, w_base + 16384, 8192, a.split, 0);
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(h0);
@@ -196,11 +230,11 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
       for (int j = 0; j < 8; ++j)
 #pragma unroll
         for (int e = 0; e < 4; ++e) h0[4 * j + e] = fmaxf(h0[4 * j + e] + bias[8 * j + fc + (e & 1)], 0.f);
-      uint32_t ahi[4][4], alo[4][4];
-      frag_split<FMT, 4>(h0, ahi, alo);
+      uint32_t bhi[4][4], blo[4][4];
+      frag_split<FMT, 4>(h0, bhi, blo);
       float h1[32];
       wgmma_fence();
-      gemm_rs<FMT, 4, 64, 0>(h1, ahi, alo, w_base + 32768, w_base + 32768 + 8192, 8192, a.split, 0);
+      gemm_rs<FMT, 4, 64, 0>(h1, bhi, blo, w_base + 32768, w_base + 32768 + 8192, 8192, a.split, 0);
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(h1);
@@ -208,29 +242,28 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
       for (int j = 0; j < 8; ++j)
 #pragma unroll
         for (int e = 0; e < 4; ++e) h1[4 * j + e] = fmaxf(h1[4 * j + e] + bias[64 + 8 * j + fc + (e & 1)], 0.f);
-      frag_split<FMT, 4>(h1, ahi, alo);
+      frag_split<FMT, 4>(h1, bhi, blo);
       float o[64];
       wgmma_fence();
-      gemm_rs<FMT, 4, 128, 0>(o, ahi, alo, w_base + 49152, w_base + 49152 + 16384, 16384, a.split, 0);
+      gemm_rs<FMT, 4, 128, 0>(o, bhi, blo, w_base + 49152, w_base + 49152 + 16384, 16384, a.split, 0);
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(o);
-      // feat = feat1 + (D2 + bm2)
+      // feat = feat1 + (D2 + bm2), feat1 from the staged residual tile
+      mbar_wait(bar_res, phase);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         if (g[h] >= rows) continue;
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const int c = 8 * j + fc, e = 4 * j + 2 * h;
-          const float2 rv = __ldg(reinterpret_cast<const float2*>(reinterpret_cast<const uint8_t*>(a.res) + blocked_f32_offset(g[h], (uint32_t)c >> 2) +
-                                                                  (c & 3) * 4));
+          const float2 rv = *reinterpret_cast<const float2*>(resbuf + blocked_f32_offset(fr + 8 * h, (uint32_t)c >> 2) + (c & 3) * 4);
           *reinterpret_cast<float2*>(a.out_f32 + g[h] * kC + c) =
               make_float2(rv.x + (o[e] + bias[128 + c]), rv.y + (o[e + 1] + bias[128 + c + 1]));
         }
       }
     }
   }
-  if (!weights && tid == 0) mbar_wait(bar_w, 0);   // no tile: the weight copy must still land before the CTA exits
 }
 
 }  // namespace pdsc
