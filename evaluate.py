@@ -134,13 +134,29 @@ def dataset_pairs(root, scenes, descriptor, device):
 
 
 @torch.no_grad()
-def evaluate(model, pairs, cfg, use_mutual=False, device="cuda"):
+def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1):
     """The loop of evaluation/test_3DMatch.py:21-103 over an iterable of (scene index, (src xyz, src desc), (tgt xyz, tgt desc),
     gt_trans): returns a [pairs, 13] float64 array, columns = COLUMNS.  Nothing is read from the device inside the loop except the
-    correspondence count of `match` (it fixes the tensor shapes)."""
+    correspondence count of `match` (it fixes the tensor shapes).
+    batch_size P > 1: pairs are still matched one by one, but every P of them (each with its own number of correspondences) go
+    through ONE mixed-size forward (`PointDSC.forward_many`), then through eval_stats pair by pair.  The model-time column of a
+    pair is then its group's device time divided by the group's size."""
     from pointdsc_b200.frontend import match
     from pointdsc_b200.metrics import eval_stats
     rows, scene_ids, data_s, events = [], [], [], []
+    group = []          # batch_size > 1: (data, gt_t, labels) of the pairs waiting for the group's forward
+
+    def run_group():
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        results = model.forward_many([g[0] for g in group])
+        e1.record()
+        for (data, gt_t, labels), res in zip(group, results):
+            rows.append(eval_stats(res["final_trans"], gt_t[None], data["src_keypts"], data["tgt_keypts"], res["final_labels"],
+                                   labels, re_thre=cfg["re_thre"], te_thre=cfg["te_thre"]))
+            events.append((e0, e1, len(group)))
+        group.clear()
+
     t_data = time.perf_counter()
     for si, (src_xyz, src_desc), (tgt_xyz, tgt_desc), gt in pairs:
         data = match(src_desc, tgt_desc, src_xyz, tgt_xyz, use_mutual=use_mutual)
@@ -148,21 +164,29 @@ def evaluate(model, pairs, cfg, use_mutual=False, device="cuda"):
         labels = gt_labels(data, gt_t, cfg["inlier_threshold"])
         data["testing"] = True
         data_s.append(time.perf_counter() - t_data)
+        scene_ids.append(si)
+        if batch_size > 1:
+            group.append((data, gt_t, labels))
+            if len(group) == batch_size:
+                run_group()
+            t_data = time.perf_counter()
+            continue
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         res = model(data)
         e1.record()
         rows.append(eval_stats(res["final_trans"], gt_t[None], data["src_keypts"], data["tgt_keypts"], res["final_labels"], labels,
                                re_thre=cfg["re_thre"], te_thre=cfg["te_thre"]))
-        events.append((e0, e1))
-        scene_ids.append(si)
+        events.append((e0, e1, 1))
         t_data = time.perf_counter()
+    if group:
+        run_group()
     if not rows:
         return np.zeros((0, len(COLUMNS)))
     dev_stats = torch.cat(rows, 0).double().cpu().numpy()          # the one read of the statistics
     out = np.zeros((len(rows), len(COLUMNS)))
     out[:, :9] = dev_stats[:, :9]
-    out[:, 9] = [a.elapsed_time(b) * 1e-3 for a, b in events]
+    out[:, 9] = [a.elapsed_time(b) * 1e-3 / n for a, b, n in events]
     out[:, 10] = data_s
     out[:, 11] = scene_ids
     out[:, 12] = dev_stats[:, 9]
@@ -210,6 +234,8 @@ def main(argv=None):
     ap.add_argument("--synthetic", type=int, default=0, help="evaluate on this many synthetic scene pairs instead of --root")
     ap.add_argument("--precision", default=None, help="fp16x3 (default) | fp32 | bf16x3 | bf16")
     ap.add_argument("--save_npy", default=None, help="write the [pairs, 13] statistics table here")
+    ap.add_argument("--batch_size", type=int, default=1,
+                    help="pairs per forward: > 1 runs every group of pairs (of different sizes) as one mixed-size call")
     args = ap.parse_args(argv)
     cfg = load_config(args.chosen_snapshot)
     descriptor = args.descriptor or cfg["descriptor"]
@@ -221,7 +247,9 @@ def main(argv=None):
         if not names:
             sys.exit(f"no 3DMatch test scene under {args.root}/fragments (this image has no data set: try --synthetic 8)")
         pairs = dataset_pairs(args.root, names, descriptor, "cuda")
-    stats = evaluate(model, pairs, cfg, use_mutual=args.use_mutual or cfg["use_mutual"])
+    if args.batch_size < 1:
+        sys.exit("--batch_size must be >= 1")
+    stats = evaluate(model, pairs, cfg, use_mutual=args.use_mutual or cfg["use_mutual"], batch_size=args.batch_size)
     summary = summarise(stats, names)
     if args.save_npy:
         np.save(args.save_npy, stats)

@@ -14,7 +14,8 @@
  *   - all device work is enqueued on the caller's stream; pdsc_forward() performs NO host
  *     synchronisation and no allocation, so it can be captured in a CUDA graph.
  *   - tensors are dense, row-major, fp32 unless stated; B = number of correspondence sets
- *     in the call, N = correspondences per set (the same N for the whole call).
+ *     in the call, N = correspondences per set (the same N for the whole call, except in
+ *     pdsc_forward_packed(), where set b has its own N_b and the sets' rows are packed back to back).
  *   - a batched call is, by definition, the loop of per-set testing forwards (the reference
  *     asserts bs == 1 in testing mode, PointDSC.py:210, :414); in particular the power
  *     iteration's early exit is decided per set (PointDSC.py:354).
@@ -133,6 +134,21 @@ size_t pdsc_workspace_bytes(const pdsc_engine* e, int32_t B, int32_t N);
 int pdsc_forward(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr_pos, const float* d_src_keypts,
                  const float* d_tgt_keypts, float* d_final_trans, float* d_final_labels,
                  const pdsc_stage_io* io, void* d_workspace, size_t workspace_bytes, void* cuda_stream);
+
+/* ---- the path over sets of different sizes (testing mode) -------------------------------------------
+ * B sets, set b owning rows [offsets[b], offsets[b+1]) of the packed inputs; offsets has B + 1 entries, offsets[0] = 0,
+ * R = offsets[B].  d_corr_pos [R,6], d_src_keypts [R,3], d_tgt_keypts [R,3]  ->  d_final_trans [B,4,4],
+ * d_final_labels [R].  h_offsets (host) sizes the launches and the workspace; d_offsets (device, caller-owned, the same
+ * values) is what the kernels read.  A set's outputs depend only on its own rows, its N_b and the call's attention regime:
+ * within one regime they are bit for bit those of a pdsc_forward() call holding that set (DESIGN.md §3).  No host
+ * synchronisation, no allocation, capturable in a CUDA graph.  PDSC_ERR_SHAPE for B < 1, offsets[0] != 0, a set with
+ * N_b < 2 (non-increasing offsets) or N_b above the supported maximum; pdsc_workspace_bytes_packed() returns 0 for such
+ * offsets. */
+size_t pdsc_workspace_bytes_packed(const pdsc_engine* e, int32_t B, const int32_t* h_offsets);
+int pdsc_forward_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                        const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts,
+                        float* d_final_trans, float* d_final_labels, void* d_workspace, size_t workspace_bytes,
+                        void* cuda_stream);
 
 /* pdsc_forward as ONE graph launch: the first call with a given (B, N, buffer addresses) runs eagerly and captures the
  * forward's kernels into a CUDA graph; later calls with the same arguments replay it (one cudaGraphLaunch instead of ~60

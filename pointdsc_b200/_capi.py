@@ -21,6 +21,9 @@ class PdscError(RuntimeError):
     pass
 
 
+PDSC_ERR_SHAPE = 3
+
+
 class Config(C.Structure):
     _fields_ = [
         ("in_dim", C.c_int32), ("num_layers", C.c_int32), ("num_channels", C.c_int32),
@@ -57,6 +60,9 @@ SYMBOLS = {
     "pdsc_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_int32]),
     "pdsc_forward": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                C.c_void_p, C.POINTER(StageIO), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "pdsc_workspace_bytes_packed": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_void_p]),
+    "pdsc_forward_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "pdsc_forward_graph": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "pdsc_forward_host": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

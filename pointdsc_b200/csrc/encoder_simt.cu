@@ -28,6 +28,14 @@ __global__ void __launch_bounds__(256) linear_simt_kernel(LinearArgs a) {
   const float* W = a.W + (size_t)bz * a.strideW;
   float* out = a.out + (size_t)bz * a.strideO;
   const int m0 = blockIdx.y * LBM, n0 = blockIdx.x * LBN;
+  if (a.sets) {          // seed-row distances of set bz of a packed call; the grid is sized by the largest set
+    const SetDesc d = a.sets[bz];
+    A = a.A + (size_t)d.seed0 * a.lda;
+    W = a.W + (size_t)d.row0 * a.ldw;
+    out = a.out + d.dist0;
+    a.M = d.S; a.Nout = d.N; a.ldo = d.N;
+    if (m0 >= a.M || n0 >= a.Nout) return;
+  }
   const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
   const int lr = tid / 4, lc = (tid % 4) * 4;  // loader: row within tile, k offset
   float acc[4][4];
@@ -145,15 +153,19 @@ constexpr int kAttnSmem = (kC * AQ + kC * AK + AK * kC + AQ * AK) * (int)sizeof(
 
 __global__ void __launch_bounds__(256) attention_simt_kernel(const float* __restrict__ Q, const float* __restrict__ K,
                                                              const float* __restrict__ V, const float* __restrict__ SC,
-                                                             float* __restrict__ MSG, int N, int NS) {
+                                                             float* __restrict__ MSG, SetTable sets) {
   extern __shared__ __align__(16) float smem[];
   float* Qs = smem;                 // [C][AQ]   Qs[c][q]
   float* Ks = Qs + kC * AQ;         // [C][AK]   Ks[c][key]
   float* Vs = Ks + kC * AK;         // [AK][C]   Vs[key][c]
   float* Ps = Vs + AK * kC;         // [AQ][AK]  Ps[q][key]
   const int b = blockIdx.y, q0 = blockIdx.x * AQ;
+  const SetDesc d = set_desc(sets, b);
+  const int N = d.N, NS = round_up(N, 64);
+  if (q0 >= N) return;                 // a packed call's grid is sized by its largest set
   const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
-  const size_t base = (size_t)b * N;
+  const size_t base = (size_t)d.row0;
+  SC += d.sc0;
   const float inv_sqrt_c = 1.0f / sqrtf((float)kC);
 
   // Q tile, transposed into smem: lane <-> query (conflict-free smem stores; L1 absorbs the strided reads)
@@ -214,7 +226,7 @@ __global__ void __launch_bounds__(256) attention_simt_kernel(const float* __rest
     for (int i = 0; i < 4; ++i) {
       const int qi = q0 + ty * 4 + i;
       float4 scv = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (qi < N) scv = *reinterpret_cast<const float4*>(SC + (base + qi) * NS + j0 + tx * 4);
+      if (qi < N) scv = *reinterpret_cast<const float4*>(SC + (size_t)qi * NS + j0 + tx * 4);
       const float scr[4] = {scv.x, scv.y, scv.z, scv.w};
       float tmax = -INFINITY;
 #pragma unroll
@@ -273,10 +285,10 @@ __global__ void __launch_bounds__(256) attention_simt_kernel(const float* __rest
 }
 
 void launch_attention_simt(const float* q, const float* k, const float* v, const float* sc, float* msg, int B, int N,
-                           int NS, cudaStream_t st) {
+                           cudaStream_t st, const SetDesc* sets) {
   ensure_dynamic_smem(reinterpret_cast<const void*>(attention_simt_kernel), kAttnSmem);
   dim3 grid((N + AQ - 1) / AQ, B);
-  attention_simt_kernel<<<grid, 256, kAttnSmem, st>>>(q, k, v, sc, msg, N, NS);
+  attention_simt_kernel<<<grid, 256, kAttnSmem, st>>>(q, k, v, sc, msg, SetTable{sets, N, 0, 0, 0, 1, 0});
 }
 
 }  // namespace pdsc

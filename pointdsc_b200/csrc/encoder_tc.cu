@@ -117,26 +117,43 @@ static inline int k_tiles(int N) { return (N + 63) / 64; }
 constexpr int kAttnSplitMaxItems = 320;
 constexpr size_t kAttnSplitBytes = (size_t)kAttnSplitMaxItems * (65536 + 1024);
 
-size_t tc_scratch_bytes(int B, int N) {
-  return ((size_t)B * q_tiles(N) + (size_t)B * k_tiles(N)) * 65536 + 1024 + kAttnSplitBytes;
+size_t tc_scratch_bytes(int B, int N) { return tc_scratch_bytes_tiles((long long)B * q_tiles(N), (long long)B * k_tiles(N)); }
+size_t tc_scratch_bytes_tiles(long long qtiles, long long ktiles) {
+  return ((size_t)qtiles + (size_t)ktiles) * 65536 + 1024 + kAttnSplitBytes;
 }
 
 // Key split policy.  When a call's (set, query tile) items cover less than half of the SMs (the evaluation loops' bs = 1:
-// 8 items at N = 1000, 40 at N = 5000), every item is split along the keys into chunks of TS tiles, TS a function of N ONLY:
-// calls of the small regime therefore agree bit for bit whatever their batch size, and so do calls of the large regime
-// (no split); across the two regimes the softmax sums are associated differently (fp32 rounding, far inside the parity bar).
+// 8 items at N = 1000, 40 at N = 5000), every item is split along the keys into chunks of TS tiles, TS a function of N ONLY
+// (attn_set_split, sets.cuh): calls of the small regime therefore agree bit for bit whatever their batch size, and so do calls
+// of the large regime (no split); across the two regimes the softmax sums are associated differently (fp32 rounding, far
+// inside the parity bar).  A call whose split would exceed kAttnSplitMaxItems work items is not split.
 static void attn_split_policy(int B, int N, int num_sms, int* splits, int* TS) {
-  const int QT = q_tiles(N), KT = k_tiles(N);
+  const int QT = q_tiles(N);
   *splits = 1;
-  *TS = KT;
-  if (2 * B * QT > num_sms || KT < 4) return;
-  const int want = (num_sms + QT - 1) / QT;          // splits that would fill the SMs with ONE set
-  int ts = (KT + want - 1) / want;
-  if (ts < 2) ts = 2;
-  const int sp = (KT + ts - 1) / ts;
+  *TS = k_tiles(N);
+  if (2 * B * QT > num_sms) return;
+  int sp, ts;
+  attn_set_split(N, num_sms, &sp, &ts);
   if (sp < 2 || B * QT * sp > kAttnSplitMaxItems) return;
   *splits = sp;
   *TS = ts;
+}
+
+// The same policy for a packed call: the call is in the split regime when its query tiles cover at most half of the SMs;
+// each set is then split as attn_set_split says for its N, unless the whole call would exceed kAttnSplitMaxItems items.
+// An equal-N call gets exactly attn_split_policy's decision.
+int tc_packed_split(const int* Ns, int B, int* items) {
+  const int num_sms = device_sm_count();
+  long long qtiles = 0, split_items = 0;
+  for (int b = 0; b < B; ++b) {
+    int sp, ts;
+    attn_set_split(Ns[b], num_sms, &sp, &ts);
+    qtiles += q_tiles(Ns[b]);
+    split_items += (long long)q_tiles(Ns[b]) * sp;
+  }
+  const bool split = 2 * qtiles <= num_sms && split_items > qtiles && split_items <= kAttnSplitMaxItems;
+  *items = (int)(split ? split_items : qtiles);
+  return split ? 1 : 0;
 }
 
 int tc_launches(int num_layers, int B, int N) {   // layer0 + pad clear + 4 per layer (+ the merge of a key-split attention)
@@ -146,11 +163,12 @@ int tc_launches(int num_layers, int B, int N) {   // layer0 + pad clear + 4 per 
 }
 
 // ---- zero the never-written pad rows/columns of the last key tile of every set ---------------------------
-__global__ void tc_clear_pads_kernel(uint8_t* kvimg, int N, int KT) {
+__global__ void tc_clear_pads_kernel(uint8_t* kvimg, SetTable sets) {
   const int b = blockIdx.x;
-  const int first_pad = N & 63;
+  const SetDesc d = set_desc(sets, b);
+  const int first_pad = d.N & 63;
   if (first_pad == 0) return;
-  uint8_t* base = kvimg + ((size_t)b * KT + (KT - 1)) * 65536;
+  uint8_t* base = kvimg + ((size_t)d.kt0 + (d.N + 63) / 64 - 1) * 65536;
   const int pads = 64 - first_pad;
   // K rows n in [first_pad, 64): both panels, hi and lo;  V rows likewise
   for (int t = threadIdx.x; t < pads * 128; t += blockDim.x) {
@@ -206,13 +224,16 @@ static cudaError_t tc_configure_fmt() {
 
 template <int FMT>
 static int tc_encoder_forward_fmt(const TcWeights& w, const TcForwardArgs& a, cudaStream_t st) {
-  const long long rows = (long long)a.B * a.N;
+  const bool packed = a.sets != nullptr;
+  const long long rows = packed ? a.rows : (long long)a.B * a.N;
   if (rows >= (1LL << 31)) return (int)cudaErrorInvalidValue;  // kernels index rows with 32-bit arithmetic
   const int QT = q_tiles(a.N), KT = k_tiles(a.N);
+  const long long qtiles = packed ? a.qtiles : (long long)a.B * QT;
+  const long long ktiles = packed ? a.ktiles : (long long)a.B * KT;
   uint8_t* qimg = static_cast<uint8_t*>(a.scratch);
   qimg = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(qimg) + 1023) & ~uintptr_t(1023));
-  uint8_t* kvimg = qimg + (size_t)a.B * QT * 65536;
-  float* part_o = reinterpret_cast<float*>(kvimg + (size_t)a.B * KT * 65536);
+  uint8_t* kvimg = qimg + (size_t)qtiles * 65536;
+  float* part_o = reinterpret_cast<float*>(kvimg + (size_t)ktiles * 65536);
   float* part_ml = part_o + (size_t)kAttnSplitMaxItems * 128 * kC;
   const long long tiles = (rows + 127) / 128;
   const int num_sms = device_sm_count();
@@ -221,11 +242,20 @@ static int tc_encoder_forward_fmt(const TcWeights& w, const TcForwardArgs& a, cu
   const uint8_t* arena = static_cast<const uint8_t*>(w.arena) + (size_t)FMT * w.num_layers * kLayerBytes;
 
   launch_layer0(a.corr_pos, a.l0w, a.l0b, a.feat, rows, a.in_dim, st);
-  tc_clear_pads_kernel<<<a.B, 256, 0, st>>>(kvimg, a.N, KT);
+  tc_clear_pads_kernel<<<a.B, 256, 0, st>>>(kvimg, SetTable{a.sets, a.N, 0, 0, 1, 1, 0});
+  int splits = 1, ts = KT, items = 0;
+  if (packed) {
+    items = a.attn_items;
+    splits = a.attn_split ? 2 : 1;     // > 1: some sets are split (their merge runs per query tile)
+  } else {
+    attn_split_policy(a.B, a.N, num_sms, &splits, &ts);
+    items = a.B * QT * splits;
+  }
   for (int l = 0; l < a.num_layers; ++l) {
     const uint8_t* base = arena + (size_t)l * kLayerBytes;
     ChainArgs c{};
     c.rows = rows; c.N = a.N; c.QT = QT; c.KT = KT; c.split = a.split;
+    c.sets = a.sets; c.nsets = a.B;
     c.qimg = qimg; c.kvimg = kvimg; c.bias = reinterpret_cast<const float*>(base + kBias);
     // PointCN + Q
     c.in = a.feat; c.res = nullptr; c.out_f32 = a.feat1; c.wimg = base + kW1; c.wbytes = 131072;
@@ -234,14 +264,13 @@ static int tc_encoder_forward_fmt(const TcWeights& w, const TcForwardArgs& a, cu
     c.in = a.feat1; c.out_f32 = nullptr; c.wimg = base + kWk; c.wbytes = 131072;
     tc_chain_kernel<kKV, FMT><<<grid, kChainThreads, kChainSmem, st>>>(c);
     // attention
-    int splits, ts;
-    attn_split_policy(a.B, a.N, num_sms, &splits, &ts);
-    AttnArgs at{a.N, a.NS, QT, KT, a.split, qimg, kvimg, a.sc, a.msg, a.B * QT * splits, splits, ts, part_o, part_ml};
+    AttnArgs at{a.N, a.NS, QT, KT, a.split, qimg, kvimg, a.sc, a.msg, items, splits, ts, part_o, part_ml, a.sets, a.B};
     if (a.attn_events) cudaEventRecord(a.attn_events[2 * l], st);
     {
       const int items = at.items;
       tc_attention_persistent_kernel<FMT><<<items < num_sms ? items : num_sms, kAttnThreads, kAttnPSmem, st>>>(at);
-      if (splits > 1) tc_attention_merge_kernel<<<a.B * QT * 4, 256, 0, st>>>(part_o, part_ml, a.msg, a.N, QT, splits);
+      if (splits > 1)
+        tc_attention_merge_kernel<<<(unsigned)(qtiles * 4), 256, 0, st>>>(part_o, part_ml, a.msg, a.N, QT, splits, a.sets, a.B);
     }
     if (a.attn_events) cudaEventRecord(a.attn_events[2 * l + 1], st);
     if (a.debug_out && a.debug_layer == l) {

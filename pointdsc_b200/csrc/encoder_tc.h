@@ -4,6 +4,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "sets.cuh"
+
 namespace pdsc {
 
 // Host pointers to one layer's folded fp32 weights (row-major [Cout][Cin]) and biases.
@@ -35,11 +37,20 @@ struct TcForwardArgs {
   float* debug_out;          // [5][B*N][128]: feat1, q (scaled by log2e/sqrt(C)), k, v, msg — or nullptr
   long long* timeline;       // not written by the wgmma kernels (kept for the C ABI)
   cudaEvent_t* attn_events;  // nullptr or 2 events per layer, recorded around the attention launch
+  // packed call (pdsc_forward_packed): the descriptor table; B is the number of sets and N the largest of them
+  const SetDesc* sets;       // nullptr: uniform call
+  long long rows;            // rows of the call
+  long long qtiles, ktiles;  // query / key tiles of all sets
+  int attn_items;            // attention work items (tc_packed_split)
+  int attn_split;            // 1: the call is in the key-split regime
 };
 
 int tc_build_weights(const TcLayerHost* layers, int num_layers, TcWeights* out);  // returns cudaError_t
 void tc_free_weights(TcWeights* w);
 size_t tc_scratch_bytes(int B, int N);
+size_t tc_scratch_bytes_tiles(long long qtiles, long long ktiles);
+// key-split decision of a packed call of sets of Ns[0..B) rows: returns 1 in the split regime; *items = attention work items
+int tc_packed_split(const int* Ns, int B, int* items);
 int tc_launches(int num_layers, int B, int N);
 int tc_encoder_forward(const TcWeights& w, const TcForwardArgs& a, cudaStream_t st);  // returns cudaError_t
 

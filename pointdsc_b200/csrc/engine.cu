@@ -139,21 +139,70 @@ struct Workspace {
   int32_t *seeds, *knn, *counts;
   uint32_t* conv_mask;
   unsigned long long* best_key;
+  pdsc::SetDesc* sets;   // packed call: the descriptor table
   void* tc_scratch;
   size_t bytes;
 };
 
-Workspace carve(const pdsc_engine* e, void* ptr, int B, int N) {
+// What a call needs to size its launches and its workspace.  A uniform call: B sets of N rows.  A packed call: B sets of
+// Ns[b] rows; N, S and k are then the largest of its sets (launch sizes) and the totals sum over the sets.
+struct CallShape {
+  int B = 0, N = 0, S = 0, k = 0, k_min = 0;
+  bool packed = false;
+  size_t R = 0;
+  size_t sc_rowmajor = 0, sc_tiled = 0;   // floats of the row-major (fp32) and tiled (tensor-core) SC layouts
+  size_t seeds = 0, dist = 0, knn = 0;    // seed slots, seed-row distance floats, neighbour slots
+  long long qtiles = 0, ktiles = 0;
+  int attn_items = 0, attn_split = 0;     // packed tensor-core calls (tc_packed_split)
+};
+
+CallShape uniform_shape(const pdsc_engine* e, int B, int N) {
+  CallShape s;
+  s.B = B; s.N = N;
+  s.S = pdsc_num_seeds(e, N); s.k = s.k_min = pdsc_num_neighbours(e, N);
+  s.R = (size_t)B * N;
+  s.sc_rowmajor = s.R * pdsc::round_up(N, 64);
+  s.sc_tiled = (size_t)B * ((N + 63) / 64) * ((N + 127) / 128) * 8192;
+  s.seeds = (size_t)B * s.S;
+  s.dist = (size_t)B * s.S * N;
+  s.knn = (size_t)B * s.S * s.k;
+  s.qtiles = (long long)B * ((N + 127) / 128);
+  s.ktiles = (long long)B * ((N + 63) / 64);
+  return s;
+}
+
+// h_offsets[0..B] already validated
+CallShape packed_shape(const pdsc_engine* e, int B, const int32_t* h_offsets) {
+  CallShape s;
+  s.B = B; s.packed = true;
+  s.k_min = e->cfg.k;
+  std::vector<int> Ns(B);
+  for (int b = 0; b < B; ++b) {
+    const int N = h_offsets[b + 1] - h_offsets[b];
+    const int S = pdsc_num_seeds(e, N), k = pdsc_num_neighbours(e, N);
+    Ns[b] = N;
+    s.N = std::max(s.N, N); s.S = std::max(s.S, S); s.k = std::max(s.k, k);
+    if (S > 0) s.k_min = std::min(s.k_min, k);
+    s.sc_rowmajor += (size_t)N * pdsc::round_up(N, 64);
+    s.sc_tiled += (size_t)((N + 63) / 64) * ((N + 127) / 128) * 8192;
+    s.seeds += S;
+    s.dist += ((size_t)S * N + 3) & ~size_t(3);       // every set's block starts 16-byte aligned (vector loads)
+    s.knn += (size_t)S * k;
+    s.qtiles += (N + 127) / 128;
+    s.ktiles += (N + 63) / 64;
+  }
+  s.R = (size_t)h_offsets[B];
+  if (e->cfg.precision != PDSC_FP32_SIMT) s.attn_split = pdsc::tc_packed_split(Ns.data(), B, &s.attn_items);
+  return s;
+}
+
+Workspace carve(const pdsc_engine* e, void* ptr, const CallShape& sh) {
   Workspace w{};
   Carver c(ptr);
-  const size_t R = (size_t)B * N;
-  const int NS = pdsc::round_up(N, 64);
-  const int S = pdsc_num_seeds(e, N), k = pdsc_num_neighbours(e, N);
+  const int B = sh.B;
+  const size_t R = sh.R;
   const int T = e->cfg.num_iterations;
-  {
-    const size_t tiled = (size_t)B * ((N + 63) / 64) * ((N + 127) / 128) * 8192;  // tensor-core layout (sc_matrix.cu)
-    w.sc = c.take<float>(R * NS > tiled ? R * NS : tiled);
-  }
+  w.sc = c.take<float>(sh.sc_rowmajor > sh.sc_tiled ? sh.sc_rowmajor : sh.sc_tiled);
   w.feat_a = c.take<float>(R * kC);
   w.feat_b = c.take<float>((R + 127) / 128 * 128 * kC);   // tensor-core modes keep feat1 blocked by 128-row tile (tc_chain.cuh)
   w.msg = c.take<float>(R * kC);
@@ -165,20 +214,21 @@ Workspace carve(const pdsc_engine* e, void* ptr, int B, int N) {
     w.h2 = c.take<float>(R * 64);
     w.tc_scratch = nullptr;
   } else {
-    w.tc_scratch = c.take<char>(pdsc::tc_scratch_bytes(B, N));
+    w.tc_scratch = c.take<char>(pdsc::tc_scratch_bytes_tiles(sh.qtiles, sh.ktiles));
   }
   w.normed = c.take<float>(R * kC);
   w.conf = c.take<float>(R);
   w.key = c.take<float>(R);
-  w.seeds = c.take<int32_t>((size_t)B * S + 1);
-  w.seedfeat = c.take<float>((size_t)B * S * kC + 1);
-  w.dist = c.take<float>((size_t)B * S * N + 1);
-  w.knn = c.take<int32_t>((size_t)B * S * k + 1);
-  w.iterates = c.take<float>((size_t)B * S * T * k + 1);
-  w.seed_trans = c.take<float>((size_t)B * S * 16 + 16);
-  w.counts = c.take<int32_t>((size_t)B * S + 1);
+  w.seeds = c.take<int32_t>(sh.seeds + 1);
+  w.seedfeat = c.take<float>(sh.seeds * kC + 1);
+  w.dist = c.take<float>(sh.dist + 1);
+  w.knn = c.take<int32_t>(sh.knn + 1);
+  w.iterates = c.take<float>(sh.knn * T + 1);
+  w.seed_trans = c.take<float>(sh.seeds * 16 + 16);
+  w.counts = c.take<int32_t>(sh.seeds + 1);
   w.conv_mask = c.take<uint32_t>(B);
   w.best_key = c.take<unsigned long long>(B);
+  w.sets = sh.packed ? c.take<pdsc::SetDesc>(B) : nullptr;
   w.bytes = (c.off + 255) & ~size_t(255);
   return w;
 }
@@ -234,11 +284,10 @@ float refinement_threshold(float ctor_threshold) {
   return (std::fabs((double)ctor_threshold - 0.10) < 1e-7) ? 0.10f : 1.2f;
 }
 
-int encoder_simt(const pdsc_engine* e, const Workspace& w, int B, int N, const float* corr_pos, const pdsc_stage_io* io,
+int encoder_simt(const pdsc_engine* e, const Workspace& w, const CallShape& sh, const float* corr_pos, const pdsc_stage_io* io,
                  cudaEvent_t* attn_events, cudaStream_t st) {
   using namespace pdsc;
-  const long long R = (long long)B * N;
-  const int NS = round_up(N, 64);
+  const long long R = (long long)sh.R;
   const float* W = e->d_weights;
   launch_layer0(corr_pos, W + e->off_l0w, W + e->off_l0b, w.feat_a, R, e->cfg.in_dim, st);
   auto lin = [&](const float* A, int K, size_t ow, size_t ob, const float* res, float* out, int Nout, int relu) {
@@ -257,7 +306,7 @@ int encoder_simt(const pdsc_engine* e, const Workspace& w, int B, int N, const f
     lin(w.feat_b, kC, L.wk, L.bk, nullptr, w.k, kC, 0);
     lin(w.feat_b, kC, L.wv, L.bv, nullptr, w.v, kC, 0);
     if (attn_events) cudaEventRecord(attn_events[2 * l], st);
-    launch_attention_simt(w.q, w.k, w.v, w.sc, w.msg, B, N, NS, st);
+    launch_attention_simt(w.q, w.k, w.v, w.sc, w.msg, sh.B, sh.N, st, w.sets);
     if (attn_events) cudaEventRecord(attn_events[2 * l + 1], st);
     if (io && io->out_layer_debug && io->layer_tap == l) {
       const size_t plane = (size_t)R * kC;
@@ -271,6 +320,52 @@ int encoder_simt(const pdsc_engine* e, const Workspace& w, int B, int N, const f
       copy_tap(io->out_layer_features, w.feat_a, (size_t)R * kC * sizeof(float), st);
   }
   return PDSC_OK;
+}
+
+// Descriptor table of a packed call, from the device copy of its offsets: one warp walks the sets 32 at a time and forms
+// every running offset (tiles, seeds, attention items, SC / distance / neighbour blocks) by warp-wide inclusive scans.
+__device__ __forceinline__ long long warp_scan_incl(long long v, int lane) {
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const long long u = __shfl_up_sync(0xffffffffu, v, o);
+    if (lane >= o) v += u;
+  }
+  return v;
+}
+
+__global__ void set_table_kernel(const int32_t* __restrict__ offsets, int B, double ratio, int k_cfg, int tiled, int split,
+                                 int num_sms, pdsc::SetDesc* __restrict__ table) {
+  const int lane = threadIdx.x;
+  long long base[7] = {0, 0, 0, 0, 0, 0, 0};   // qt0, kt0, seed0, item0, sc0, dist0, knn0
+  for (int b0 = 0; b0 < B; b0 += 32) {
+    const int b = b0 + lane;
+    const bool live = b < B;
+    const int row0 = live ? offsets[b] : 0;
+    const int N = live ? offsets[b + 1] - row0 : 0;
+    const int S = (int)((double)N * ratio);          // int(num_corr * self.ratio), as pdsc_num_seeds
+    const int k = live ? max(min(k_cfg, N - 1), 0) : 0;
+    const int QT = (N + 127) / 128, KT = (N + 63) / 64;
+    int sp = 1, TS = KT;
+    if (split) pdsc::attn_set_split(N, num_sms, &sp, &TS);
+    const long long size[7] = {QT, KT, S, (long long)QT * sp,
+                               tiled ? (long long)KT * QT * 8192 : (long long)N * pdsc::round_up(N, 64),
+                               ((long long)S * N + 3) & ~3ll, (long long)S * k};
+    long long first[7];
+#pragma unroll
+    for (int i = 0; i < 7; ++i) {
+      const long long incl = warp_scan_incl(size[i], lane);
+      first[i] = base[i] + incl - size[i];
+      base[i] += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    if (live) {
+      pdsc::SetDesc d;
+      d.row0 = row0; d.N = N; d.S = S; d.k = k;
+      d.qt0 = (int)first[0]; d.kt0 = (int)first[1]; d.seed0 = (int)first[2]; d.item0 = (int)first[3];
+      d.sp = sp; d.TS = TS; d.pad0 = d.pad1 = 0;
+      d.sc0 = first[4]; d.dist0 = first[5]; d.knn0 = first[6];
+      table[b] = d;
+    }
+  }
 }
 
 }  // namespace
@@ -426,7 +521,7 @@ int32_t pdsc_num_neighbours(const pdsc_engine* e, int32_t N) {
 
 size_t pdsc_workspace_bytes(const pdsc_engine* e, int32_t B, int32_t N) {
   if (!e || B <= 0 || N <= 0) return 0;
-  return carve(e, nullptr, B, N).bytes;
+  return carve(e, nullptr, uniform_shape(e, B, N)).bytes;
 }
 
 int32_t pdsc_launches_per_forward(const pdsc_engine* e, int32_t B, int32_t N) {
@@ -440,29 +535,39 @@ int32_t pdsc_launches_per_forward(const pdsc_engine* e, int32_t B, int32_t N) {
 // mode 0: testing (PointDSC.py: NMS seeds, per-set early exit, labels = inlier mask, post-refinement)
 // mode 1: non-testing / validation (PointDSC.py:158-165, :176, :190-191): seeds = top-S by confidence, batch-global early
 //         exit, no refinement, final_labels = confidence logits, optional feature-similarity matrix M [B,N,N]
-static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const float* d_corr_pos, const float* d_src,
+// h_offsets / d_offsets: a packed call (mode 0, no io), offsets validated by pdsc_forward_packed; N is then ignored
+static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const int32_t* h_offsets, const int32_t* d_offsets,
+                        const float* d_corr_pos, const float* d_src,
                         const float* d_tgt, float* d_final_trans, float* d_final_labels, float* d_M, const pdsc_stage_io* io,
                         void* d_workspace, size_t workspace_bytes, void* cuda_stream) {
   using namespace pdsc;
   const int mask_stride = mode == 0 ? 1 : 0;
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
   if (!e->committed) return fail(PDSC_ERR_NOT_COMMITTED, "pdsc_commit_params() has not been called since the last pdsc_set_param()");
-  if (B <= 0 || N <= 1) return fail(PDSC_ERR_SHAPE, "need B >= 1 and N >= 2 (got B=%d N=%d)", B, N);
-  if (N > pick_seeds_max_n()) return fail(PDSC_ERR_UNSUPPORTED, "N=%d exceeds the supported maximum %d", N, pick_seeds_max_n());
+  if (!h_offsets) {
+    if (B <= 0 || N <= 1) return fail(PDSC_ERR_SHAPE, "need B >= 1 and N >= 2 (got B=%d N=%d)", B, N);
+    if (N > pick_seeds_max_n()) return fail(PDSC_ERR_UNSUPPORTED, "N=%d exceeds the supported maximum %d", N, pick_seeds_max_n());
+  }
   if (!d_src || !d_tgt || !d_final_trans || !d_final_labels) return fail(PDSC_ERR_INVALID_ARGUMENT, "null tensor pointer");
   const bool inject_feat = io && io->in_features;
   if (!inject_feat && !d_corr_pos) return fail(PDSC_ERR_INVALID_ARGUMENT, "corr_pos is null");
   if (io && io->in_confidence && !inject_feat) return fail(PDSC_ERR_INVALID_ARGUMENT, "in_confidence requires in_features");
-  const size_t need = pdsc_workspace_bytes(e, B, N);
+  DeviceGuard g(e->cfg.device);   // tc_packed_split reads the SM count of the engine's device
+  const CallShape sh = h_offsets ? packed_shape(e, B, h_offsets) : uniform_shape(e, B, N);
+  const size_t need = carve(e, nullptr, sh).bytes;
   if (!d_workspace || workspace_bytes < need)
     return fail(PDSC_ERR_WORKSPACE, "workspace too small: %zu bytes given, %zu needed", workspace_bytes, need);
   if (reinterpret_cast<uintptr_t>(d_workspace) % 256) return fail(PDSC_ERR_WORKSPACE, "workspace must be 256-byte aligned");
-  DeviceGuard g(e->cfg.device);
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  const Workspace w = carve(e, d_workspace, B, N);
-  const size_t R = (size_t)B * N;
+  const Workspace w = carve(e, d_workspace, sh);
+  N = sh.N;                        // a packed call: the largest set, which sizes the launches
+  const size_t R = sh.R;
   const int NS = round_up(N, 64);
-  const int S = pdsc_num_seeds(e, N), k = pdsc_num_neighbours(e, N), T = e->cfg.num_iterations;
+  const int S = sh.S, k = sh.k, T = e->cfg.num_iterations;
+  const SetDesc* sets = w.sets;    // nullptr: uniform call
+  if (sets)
+    set_table_kernel<<<1, 32, 0, st>>>(d_offsets, B, (double)e->cfg.ratio, e->cfg.k, e->cfg.precision == PDSC_FP32_SIMT ? 0 : 1,
+                                       sh.attn_split, device_sm_count(), w.sets);
   const float* W = e->d_weights;
   const int L = e->cfg.num_layers;
   cudaEvent_t* attn_ev = nullptr;
@@ -478,8 +583,8 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const fl
   // ---- stages i + ii ------------------------------------------------------------------------------
   if (!inject_feat) {
     const bool simt = e->cfg.precision == PDSC_FP32_SIMT;
-    if (simt) launch_sc_matrix(d_src, d_tgt, w.sc, B, N, NS, e->sigma_spat, st);
-    else launch_sc_matrix_tiled(d_src, d_tgt, w.sc, B, N, e->sigma_spat, st);
+    if (simt) launch_sc_matrix(d_src, d_tgt, w.sc, B, N, e->sigma_spat, st, sets);
+    else launch_sc_matrix_tiled(d_src, d_tgt, w.sc, B, N, e->sigma_spat, st, sets);
     mark(1);
     if (e->corr_pending) {   // host path: corr_pos is still arriving on the side stream
       PDSC_CUDA(cudaStreamWaitEvent(st, e->corr_ready, 0));
@@ -493,7 +598,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const fl
         launch_sc_untile(w.sc, io->out_sc, B, N, st);
     }
     if (simt) {
-      const int rc = encoder_simt(e, w, B, N, d_corr_pos, io, attn_ev, st);
+      const int rc = encoder_simt(e, w, sh, d_corr_pos, io, attn_ev, st);
       if (rc) return rc;
     } else {
       TcForwardArgs a{};
@@ -507,6 +612,8 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const fl
       a.debug_layer = io ? io->layer_tap : -1;
       a.debug_out = io ? io->out_layer_debug : nullptr;
       a.attn_events = attn_ev;
+      a.sets = sets; a.rows = (long long)R; a.qtiles = sh.qtiles; a.ktiles = sh.ktiles;
+      a.attn_items = sh.attn_items; a.attn_split = sh.attn_split;
       a.timeline = io ? reinterpret_cast<long long*>(io->out_timeline) : nullptr;
       const int rc = tc_encoder_forward(e->tc, a, st);
       if (rc) return fail(PDSC_ERR_CUDA, "tensor-core encoder launch failed: %s", cudaGetErrorString((cudaError_t)rc));
@@ -534,7 +641,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const fl
     if (io && io->in_seeds)
       PDSC_CUDA(cudaMemcpyAsync(w.seeds, io->in_seeds, (size_t)B * S * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
     else if (mode == 0)
-      launch_pick_seeds(d_src, w.conf, w.seeds, w.key, B, N, S, e->cfg.nms_radius, st);
+      launch_pick_seeds(d_src, w.conf, w.seeds, w.key, B, N, S, e->cfg.nms_radius, st, sets);
     else
       launch_top_seeds(w.conf, w.seeds, B, N, S, st);
     if (io) copy_tap(io->out_seeds, w.seeds, (size_t)B * S * sizeof(int32_t), st);
@@ -545,18 +652,19 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const fl
       PDSC_CUDA(cudaMemcpyAsync(w.knn, io->in_knn_idx, (size_t)B * S * k * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
     } else {
       if (e->cfg.precision == PDSC_FP32_SIMT) {
-        launch_gather_rows(w.normed, w.seeds, w.seedfeat, B, N, S, st);
+        launch_gather_rows(w.normed, w.seeds, w.seedfeat, B, N, S, st, sets);
         LinearArgs a{};
         a.A = w.seedfeat; a.strideA = (long long)S * kC; a.lda = kC;
         a.W = w.normed; a.strideW = (long long)N * kC; a.ldw = kC;
         a.bias = nullptr; a.res = nullptr; a.ldres = 0;
         a.out = w.dist; a.strideO = (long long)S * N; a.ldo = N;
         a.M = S; a.K = kC; a.Nout = N; a.relu = 0; a.epi = 1; a.batch = B;
+        a.sets = sets;
         launch_linear_simt(a, st);
       } else {
-        launch_knn_dist_tc(w.normed, w.seeds, w.dist, B, N, S, st);
+        launch_knn_dist_tc(w.normed, w.seeds, w.dist, B, N, S, st, sets);
       }
-      launch_knn_select(w.dist, w.knn, B, N, S, k, st);
+      launch_knn_select(w.dist, w.knn, B, N, S, k, st, sets, (int)sh.seeds);
     }
     if (io) copy_tap(io->out_knn_idx, w.knn, (size_t)B * S * k * sizeof(int32_t), st);
     mark(5);
@@ -565,12 +673,12 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const fl
     launch_fill_u32(w.conv_mask, 0xFFFFFFFFu, B, st);
     launch_fill_u64(w.best_key, 0ull, B, st);
     launch_nsm_power(w.normed, d_src, d_tgt, w.knn, w.iterates, w.conv_mask, io ? io->out_compat : nullptr, B, N, S, k, T,
-                     e->sigma, e->sigma_spat, mask_stride, e->cfg.precision != PDSC_FP32_SIMT, st);
+                     e->sigma, e->sigma_spat, mask_stride, e->cfg.precision != PDSC_FP32_SIMT, st, sets, sh.k_min);
     mark(6);
     // ---- a10 + a11 --------------------------------------------------------------------------------
     launch_seed_hypotheses(d_src, d_tgt, w.knn, w.iterates, w.conv_mask, io ? io->in_seed_trans : nullptr, w.seed_trans,
                            w.counts, w.best_key, io ? io->out_eig : nullptr, io ? io->out_power_iters : nullptr, B, N, S,
-                           k, T, e->cfg.inlier_threshold, mask_stride, st);
+                           k, T, e->cfg.inlier_threshold, mask_stride, st, sets);
     if (io) {
       copy_tap(io->out_seed_trans, w.seed_trans, (size_t)B * S * 16 * sizeof(float), st);
       copy_tap(io->out_inlier_counts, w.counts, (size_t)B * S * sizeof(int32_t), st);
@@ -584,7 +692,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const fl
   launch_select_refine(d_src, d_tgt, w.seed_trans, w.best_key, d_final_trans, mode == 0 ? d_final_labels : nullptr,
                        io ? io->out_init_trans : nullptr, io ? io->out_best : nullptr,
                        io ? io->out_refine_solves : nullptr, B, N, S, e->cfg.inlier_threshold,
-                       refinement_threshold(e->cfg.inlier_threshold), mode == 0 ? 20 : 0, st);
+                       refinement_threshold(e->cfg.inlier_threshold), mode == 0 ? 20 : 0, st, sets);
   if (mode == 1) {
     PDSC_CUDA(cudaMemcpyAsync(d_final_labels, w.conf, R * sizeof(float), cudaMemcpyDeviceToDevice, st));
     if (d_M) {   // M = clamp(1 - (1 - F F^T) / sigma^2, 0, 1), zero diagonal  (PointDSC.py:160-165)
@@ -611,8 +719,39 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const fl
 int pdsc_forward(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr_pos, const float* d_src, const float* d_tgt,
                  float* d_final_trans, float* d_final_labels, const pdsc_stage_io* io, void* d_workspace,
                  size_t workspace_bytes, void* cuda_stream) {
-  return forward_impl(e, 0, B, N, d_corr_pos, d_src, d_tgt, d_final_trans, d_final_labels, nullptr, io, d_workspace,
+  return forward_impl(e, 0, B, N, nullptr, nullptr, d_corr_pos, d_src, d_tgt, d_final_trans, d_final_labels, nullptr, io, d_workspace,
                       workspace_bytes, cuda_stream);
+}
+
+static int check_offsets(const pdsc_engine* e, int32_t B, const int32_t* h_offsets) {
+  if (B < 1) return fail(PDSC_ERR_SHAPE, "need B >= 1 sets (got B=%d)", B);
+  if (!h_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "h_offsets is null");
+  if (h_offsets[0] != 0) return fail(PDSC_ERR_SHAPE, "offsets[0] must be 0 (got %d)", h_offsets[0]);
+  for (int b = 0; b < B; ++b) {
+    const long long n = (long long)h_offsets[b + 1] - h_offsets[b];
+    if (n < 2) return fail(PDSC_ERR_SHAPE, "set %d has N=%lld rows: offsets must increase by at least 2 per set", b, n);
+    if (n > pdsc::pick_seeds_max_n())
+      return fail(PDSC_ERR_SHAPE, "set %d has N=%lld rows, above the supported maximum %d", b, n, pdsc::pick_seeds_max_n());
+  }
+  (void)e;
+  return PDSC_OK;
+}
+
+size_t pdsc_workspace_bytes_packed(const pdsc_engine* e, int32_t B, const int32_t* h_offsets) {
+  if (!e || check_offsets(e, B, h_offsets) != PDSC_OK) return 0;
+  DeviceGuard g(e->cfg.device);
+  return carve(e, nullptr, packed_shape(e, B, h_offsets)).bytes;
+}
+
+int pdsc_forward_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_corr_pos,
+                        const float* d_src, const float* d_tgt, float* d_final_trans, float* d_final_labels, void* d_workspace,
+                        size_t workspace_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  const int rc = check_offsets(e, B, h_offsets);
+  if (rc) return rc;
+  if (!d_offsets || !d_corr_pos) return fail(PDSC_ERR_INVALID_ARGUMENT, "null tensor pointer");
+  return forward_impl(e, 0, B, 0, h_offsets, d_offsets, d_corr_pos, d_src, d_tgt, d_final_trans, d_final_labels, nullptr, nullptr,
+                      d_workspace, workspace_bytes, cuda_stream);
 }
 
 int pdsc_forward_graph(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr_pos, const float* d_src, const float* d_tgt,
@@ -624,7 +763,7 @@ int pdsc_forward_graph(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   PDSC_CUDA(cudaStreamIsCapturing(st, &cap));
   if (cap != cudaStreamCaptureStatusNone || e->profiling || !e->committed)   // already inside someone's capture (or nothing to cache): plain enqueue
-    return forward_impl(e, 0, B, N, d_corr_pos, d_src, d_tgt, d_final_trans, d_final_labels, nullptr, nullptr, d_workspace,
+    return forward_impl(e, 0, B, N, nullptr, nullptr, d_corr_pos, d_src, d_tgt, d_final_trans, d_final_labels, nullptr, nullptr, d_workspace,
                         workspace_bytes, cuda_stream);
   for (size_t i = 0; i < e->graphs.size(); ++i) {
     const auto& q = e->graphs[i];
@@ -636,12 +775,12 @@ int pdsc_forward_graph(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr
     }
   }
   // first call with these buffers: run once eagerly (per-device opt-ins, lazy module loading), then capture
-  int rc = forward_impl(e, 0, B, N, d_corr_pos, d_src, d_tgt, d_final_trans, d_final_labels, nullptr, nullptr, d_workspace,
+  int rc = forward_impl(e, 0, B, N, nullptr, nullptr, d_corr_pos, d_src, d_tgt, d_final_trans, d_final_labels, nullptr, nullptr, d_workspace,
                         workspace_bytes, cuda_stream);
   if (rc) return rc;
   if (!e->capture_stream) PDSC_CUDA(cudaStreamCreateWithFlags(&e->capture_stream, cudaStreamNonBlocking));
   PDSC_CUDA(cudaStreamBeginCapture(e->capture_stream, cudaStreamCaptureModeThreadLocal));
-  rc = forward_impl(e, 0, B, N, d_corr_pos, d_src, d_tgt, d_final_trans, d_final_labels, nullptr, nullptr, d_workspace,
+  rc = forward_impl(e, 0, B, N, nullptr, nullptr, d_corr_pos, d_src, d_tgt, d_final_trans, d_final_labels, nullptr, nullptr, d_workspace,
                     workspace_bytes, e->capture_stream);
   cudaGraph_t graph = nullptr;
   const cudaError_t end = cudaStreamEndCapture(e->capture_stream, &graph);
@@ -666,7 +805,7 @@ int pdsc_forward_graph(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr
 int pdsc_forward_eval(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr_pos, const float* d_src, const float* d_tgt,
                       float* d_final_trans, float* d_confidence, float* d_M, const pdsc_stage_io* io, void* d_workspace,
                       size_t workspace_bytes, void* cuda_stream) {
-  return forward_impl(e, 1, B, N, d_corr_pos, d_src, d_tgt, d_final_trans, d_confidence, d_M, io, d_workspace,
+  return forward_impl(e, 1, B, N, nullptr, nullptr, d_corr_pos, d_src, d_tgt, d_final_trans, d_confidence, d_M, io, d_workspace,
                       workspace_bytes, cuda_stream);
 }
 

@@ -14,6 +14,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "sets.cuh"
 #include "tc_common.cuh"
 
 namespace pdsc {
@@ -46,16 +47,19 @@ __device__ __forceinline__ void knn_stage_keys(uint8_t* Bs, const float* rows, i
 
 __global__ void __launch_bounds__(kKnnThreads, 1) knn_dist_tc_kernel(const float* __restrict__ normed,
                                                                      const int32_t* __restrict__ seeds,
-                                                                     float* __restrict__ dist, int N, int S, int tiles_per_cta) {
+                                                                     float* __restrict__ dist, SetTable sets, int tiles_per_cta) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t s0 = smem_u32(smem);
   const int tid = threadIdx.x, wg = tid >> 7, wt = tid & 127;
   const int b = blockIdx.y, s_base = blockIdx.x * 128;
+  const SetDesc sd = set_desc(sets, b);
+  const int N = sd.N, S = sd.S;
+  if (s_base >= S) return;                 // a packed call's grid is sized by its largest set
   // key tiles [t0, t0 + T) of this CTA: blockIdx.z splits the keys when seed-row tiles x sets alone would leave SMs idle
   const int t0 = blockIdx.z * tiles_per_cta;
   const int T = min(tiles_per_cta, (N + 63) / 64 - t0);
   constexpr int FMT = kFmtF16;
-  const float* rows = normed + (size_t)b * N * kC;
+  const float* rows = normed + (size_t)sd.row0 * kC;
   const int fr = frag_row(wt), fc = frag_col(wt);
 
   // A operand: this thread's fragment of its warpgroup's 64 seed rows (rows fr, fr + 8), all 128 channels
@@ -67,7 +71,7 @@ __global__ void __launch_bounds__(kKnnThreads, 1) knn_dist_tc_kernel(const float
     srow[h] = s;
     const float* frow = nullptr;
     if (s < S) {
-      int idx = seeds[(size_t)b * S + s];
+      int idx = seeds[(size_t)sd.seed0 + s];
       idx = min(max(idx, 0), N - 1);
       frow = rows + (size_t)idx * kC;
     }
@@ -97,7 +101,7 @@ __global__ void __launch_bounds__(kKnnThreads, 1) knn_dist_tc_kernel(const float
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (srow[h] >= S) continue;
-      float* drow = dist + ((size_t)b * S + srow[h]) * N;
+      float* drow = dist + sd.dist0 + (size_t)srow[h] * N;
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj) {
         const int j = j0 + 8 * jj + fc;
@@ -113,7 +117,8 @@ __global__ void __launch_bounds__(kKnnThreads, 1) knn_dist_tc_kernel(const float
   }
 }
 
-void launch_knn_dist_tc(const float* normed, const int32_t* seeds, float* dist, int B, int N, int S, cudaStream_t st) {
+void launch_knn_dist_tc(const float* normed, const int32_t* seeds, float* dist, int B, int N, int S, cudaStream_t st,
+                        const SetDesc* sets) {
   if (S <= 0) return;
   ensure_dynamic_smem(reinterpret_cast<const void*>(knn_dist_tc_kernel), kKnnSmem);
   const int T = (N + 63) / 64, ctas = ((S + 127) / 128) * B, sms = device_sm_count();
@@ -121,7 +126,8 @@ void launch_knn_dist_tc(const float* normed, const int32_t* seeds, float* dist, 
   if (chunks > T) chunks = T;
   const int per = (T + chunks - 1) / chunks;
   chunks = (T + per - 1) / per;
-  knn_dist_tc_kernel<<<dim3((S + 127) / 128, B, chunks), kKnnThreads, kKnnSmem, st>>>(normed, seeds, dist, N, S, per);
+  knn_dist_tc_kernel<<<dim3((S + 127) / 128, B, chunks), kKnnThreads, kKnnSmem, st>>>(normed, seeds, dist,
+                                                                                      SetTable{sets, N, S, 0, 1, 1, 0}, per);
 }
 
 }  // namespace pdsc

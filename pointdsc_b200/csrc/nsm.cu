@@ -20,22 +20,26 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "sets.cuh"
 #include "warp_select.cuh"
 
 namespace pdsc {
 
 // ---- seed feature rows -----------------------------------------------------------------------------
 __global__ void gather_rows_kernel(const float* __restrict__ normed, const int32_t* __restrict__ seeds,
-                                   float* __restrict__ out, int N, int S) {
+                                   float* __restrict__ out, SetTable sets) {
   const int b = blockIdx.y, s = blockIdx.x, lane = threadIdx.x;
-  int idx = seeds[(size_t)b * S + s];
-  idx = min(max(idx, 0), N - 1);
-  const float4 v = *reinterpret_cast<const float4*>(normed + ((size_t)b * N + idx) * kC + lane * 4);
-  *reinterpret_cast<float4*>(out + ((size_t)b * S + s) * kC + lane * 4) = v;
+  const SetDesc d = set_desc(sets, b);
+  if (s >= d.S) return;                    // a packed call's grid is sized by its largest set
+  int idx = seeds[(size_t)d.seed0 + s];
+  idx = min(max(idx, 0), d.N - 1);
+  const float4 v = *reinterpret_cast<const float4*>(normed + ((size_t)d.row0 + idx) * kC + lane * 4);
+  *reinterpret_cast<float4*>(out + ((size_t)d.seed0 + s) * kC + lane * 4) = v;
 }
-void launch_gather_rows(const float* normed, const int32_t* seeds, float* out, int B, int N, int S, cudaStream_t st) {
+void launch_gather_rows(const float* normed, const int32_t* seeds, float* out, int B, int N, int S, cudaStream_t st,
+                        const SetDesc* sets) {
   if (S <= 0) return;
-  gather_rows_kernel<<<dim3(S, B), 32, 0, st>>>(normed, seeds, out, N, S);
+  gather_rows_kernel<<<dim3(S, B), 32, 0, st>>>(normed, seeds, out, SetTable{sets, N, S, 0, 0, 1, 0});
 }
 
 // ---- top-(k+1) smallest per seed row ---------------------------------------------------------------
@@ -47,23 +51,37 @@ void launch_gather_rows(const float* normed, const int32_t* seeds, float* out, i
 // in ascending order.  Rank 0 (the seed itself, ignore_self) is dropped.  ~1.5 k instructions per row at N = 1000 instead
 // of the 6.5 k of k + 1 serial argmin rounds, and no register-resident copy of the row, so one kernel serves every N.
 
-__global__ void __launch_bounds__(256) knn_select_kernel(const float* __restrict__ dist, int32_t* __restrict__ knn_idx, int N,
-                                                         int rows, int k, int warps_per_cta, int P) {
+// Packed calls: a warp finds its row's set by a binary search over the sets' first seed slots; the shared-memory slices are
+// laid out for the largest N and k of the call (NPmax, Pmax), the selection runs at the set's own N, k and P.
+__global__ void __launch_bounds__(256) knn_select_kernel(const float* __restrict__ dist, int32_t* __restrict__ knn_idx,
+                                                         SetTable sets, int nsets, int rows, int warps_per_cta, int NPmax,
+                                                         int Pmax) {
   extern __shared__ __align__(16) unsigned char knn_smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int row = blockIdx.x * warps_per_cta + warp;
   if (row >= rows) return;                   // whole warps leave: no block-level barrier below
+  int N = sets.N, k = sets.k, P = Pmax;
+  const float* d = dist + (size_t)row * N;
+  int32_t* out = knn_idx + (size_t)row * k;
+  if (sets.d) {
+    const SetDesc sd = sets.d[find_set(nsets, row, [&](int b) { return sets.d[b].seed0; })];
+    const int s = row - sd.seed0;
+    N = sd.N;
+    k = sd.k;
+    for (P = 2; P < k + 1; P <<= 1) {}
+    d = dist + sd.dist0 + (size_t)s * N;
+    out = knn_idx + sd.knn0 + (size_t)s * k;
+  }
   const int NP = (N + 31) & ~31;
-  const size_t per_warp = (size_t)NP * 4 + 1024 + (size_t)P * 8;
+  const size_t per_warp = (size_t)NPmax * 4 + 1024 + (size_t)Pmax * 8;
   unsigned char* base = knn_smem + (size_t)warp * per_warp;
   unsigned long long* sel = reinterpret_cast<unsigned long long*>(base);            // [P]   (first: 8-byte aligned)
-  uint32_t* hist = reinterpret_cast<uint32_t*>(base + (size_t)P * 8);               // [256]
+  uint32_t* hist = reinterpret_cast<uint32_t*>(base + (size_t)Pmax * 8);            // [256]
   uint32_t* keys = hist + 256;                                                      // [NP]
-  const float* d = dist + (size_t)row * N;
   // the row arrives with ALL of its loads in flight at once: 16-byte cp.async when the row is 16-byte aligned (N % 4 == 0),
   // else scalar loads in batches of eight — a plain `keys[j] = f(d[j])` loop waits one memory latency per iteration, which at
   // N = 5000 (157 iterations, 8 warps per SM) was nearly all of this kernel's 1.6 ms in the KITTI configuration
-  if ((N & 3) == 0) {
+  if ((N & 3) == 0 && (reinterpret_cast<uintptr_t>(d) & 15) == 0) {
     const uint32_t kbase = (uint32_t)__cvta_generic_to_shared(keys);
     for (int j4 = lane; j4 < (N >> 2); j4 += 32)
       asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(kbase + (uint32_t)j4 * 16u), "l"(d + 4 * j4) : "memory");
@@ -84,13 +102,14 @@ __global__ void __launch_bounds__(256) knn_select_kernel(const float* __restrict
   warp_select_sorted(keys, hist, sel, N, NP, k + 1, P, lane);
   for (int r = 1 + lane; r <= k; r += 32) {
     const unsigned long long v = sel[r];
-    knn_idx[(size_t)row * k + (r - 1)] = (v == ~0ull || (uint32_t)(v >> 32) == 0xFFFFFFFFu) ? 0 : (int32_t)(v & 0xFFFFFFFFull);
+    out[r - 1] = (v == ~0ull || (uint32_t)(v >> 32) == 0xFFFFFFFFu) ? 0 : (int32_t)(v & 0xFFFFFFFFull);
   }
 }
 
-void launch_knn_select(const float* dist, int32_t* knn_idx, int B, int N, int S, int k, cudaStream_t st) {
+void launch_knn_select(const float* dist, int32_t* knn_idx, int B, int N, int S, int k, cudaStream_t st,
+                       const SetDesc* sets, int total_seeds) {
   if (S <= 0) return;
-  const int rows = B * S;
+  const int rows = sets ? total_seeds : B * S;
   int P = 2;
   while (P < k + 1) P <<= 1;
   const int NP = (N + 31) & ~31;
@@ -99,7 +118,8 @@ void launch_knn_select(const float* dist, int32_t* knn_idx, int B, int N, int S,
   warps = warps > 8 ? 8 : (warps < 1 ? 1 : warps);
   const int smem = (int)(per_warp * warps);
   ensure_dynamic_smem(reinterpret_cast<const void*>(knn_select_kernel), smem);
-  knn_select_kernel<<<(rows + warps - 1) / warps, warps * 32, smem, st>>>(dist, knn_idx, N, rows, k, warps, P);
+  knn_select_kernel<<<(rows + warps - 1) / warps, warps * 32, smem, st>>>(dist, knn_idx, SetTable{sets, N, S, k, 0, 1, 0}, B, rows,
+                                                                           warps, NP, P);
 }
 
 // ---- compatibility matrix + power iteration: one warp (k <= 40) or one 4-warp CTA (k > 40) per seed ----------------------
@@ -138,7 +158,7 @@ template <int WPS>
 __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
     const float* __restrict__ normed, const float* __restrict__ src, const float* __restrict__ tgt,
     const int32_t* __restrict__ knn_idx, float* __restrict__ iterates, uint32_t* __restrict__ conv_mask,
-    float* __restrict__ compat_out, int N, int S, int k, int iters, float sigma2, float sigmad2, int mask_stride,
+    float* __restrict__ compat_out, SetTable sets, int k_lo, int k_hi, int iters, float sigma2, float sigmad2, int mask_stride,
     int groups_per_cta, int per_group_floats) {
   const float rc_sigma2 = 1.0f / sigma2, rc_sigmad2 = 1.0f / sigmad2;   // IEEE divisions (correctly rounded reciprocals)
   extern __shared__ __align__(16) float sm[];
@@ -147,8 +167,11 @@ __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
   const int group = (WPS == 1) ? warp : 0;
   const int tg = (WPS == 1) ? lane : (int)threadIdx.x;      // thread index within the seed's group
   const int b = blockIdx.y;
+  const SetDesc d = set_desc(sets, b);
+  const int N = d.N, S = d.S, k = d.k;
+  if (k < k_lo || k > k_hi) return;        // a packed call runs each kernel variant on the sets of its k range
   const int s = blockIdx.x * groups_per_cta + group;
-  if (s >= S) return;                      // WPS == 1: whole warps leave (no block barrier below); WPS == 4: never true
+  if (s >= S) return;                      // WPS == 1: whole warps leave (no block barrier below); WPS == 4: the whole CTA
   const int ms = k | 1;                    // odd row stride of M: conflict-free column reads
   const int kp = (k + 3) & ~3;
   float* F = sm + (size_t)group * per_group_floats;   // [kp][32]  one channel quarter, chunk-swizzled
@@ -158,14 +181,14 @@ __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
   float* v = pb + k * 3;                               // [k]
   int* idx = reinterpret_cast<int*>(v + k);            // [k]
   float* red = reinterpret_cast<float*>(idx + k);      // [8]: WPS == 4 cross-warp reductions
-  const size_t seed_row = (size_t)b * S + s;
+  const size_t nb0 = (size_t)d.knn0 + (size_t)s * k;   // the seed's first neighbour slot
 
   for (int a = tg; a < k; a += TS) {
-    int j = knn_idx[seed_row * k + a];
+    int j = knn_idx[nb0 + a];
     j = min(max(j, 0), N - 1);
     idx[a] = j;
-    const float* ps = src + ((size_t)b * N + j) * 3;
-    const float* pt = tgt + ((size_t)b * N + j) * 3;
+    const float* ps = src + ((size_t)d.row0 + j) * 3;
+    const float* pt = tgt + ((size_t)d.row0 + j) * 3;
     pa[a * 3 + 0] = ps[0]; pa[a * 3 + 1] = ps[1]; pa[a * 3 + 2] = ps[2];
     pb[a * 3 + 0] = pt[0]; pb[a * 3 + 1] = pt[1]; pb[a * 3 + 2] = pt[2];
     v[a] = 1.0f;
@@ -198,7 +221,7 @@ __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
       const int q = tg & 7;
       for (int a = tg >> 3; a < kp; a += TS / 8) {
         const uint32_t dst = f_base + (uint32_t)((a * 32 + ((q ^ ((a >> 2) & 7)) << 2)) * 4);
-        if (a < k) cp_async_16(dst, normed + ((size_t)b * N + idx[a]) * kC + quarter * 32 + q * 4);
+        if (a < k) cp_async_16(dst, normed + ((size_t)d.row0 + idx[a]) * kC + quarter * 32 + q * 4);
         else *reinterpret_cast<float4*>(F + a * 32 + ((q ^ ((a >> 2) & 7)) << 2)) = make_float4(0.f, 0.f, 0.f, 0.f);
       }
       cp_async_wait_all();
@@ -254,14 +277,14 @@ __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
   }
   seed_group_sync<WPS>();
   if (compat_out) {
-    float* dst = compat_out + seed_row * k * k;
+    float* dst = compat_out + nb0 * k;
     for (int t = tg; t < k * k; t += TS) dst[t] = M[(t / k) * ms + (t % k)];
   }
 
   // power iteration from the all-ones vector; record every iterate and a convergence bit per iteration.
   // Thread = (row group rg = tg >> 2, column quarter cq = tg & 3): rows rg + (TS / 4) i, the columns of quarter cq.
   uint32_t mask = 0u;
-  float* it_out = iterates + seed_row * (size_t)iters * k;
+  float* it_out = iterates + nb0 * iters;
   constexpr int RG = TS / 4;                         // row groups: 8 (one warp) or 32 (four warps)
   const int rg = tg >> 2, cq = tg & 3;
   const int CQ = (k + 3) >> 2;                       // columns per quarter
@@ -410,12 +433,15 @@ constexpr int kMmaTiles = 9;       // (i, j): 16-row tile i, 8-column tile j >= 
 __global__ void __launch_bounds__(256, 2) nsm_power_mma_kernel(
     const float* __restrict__ normed, const float* __restrict__ src, const float* __restrict__ tgt,
     const int32_t* __restrict__ knn_idx, float* __restrict__ iterates, uint32_t* __restrict__ conv_mask,
-    float* __restrict__ compat_out, int N, int S, int k, int iters, float sigma2, float sigmad2, int mask_stride,
+    float* __restrict__ compat_out, SetTable sets, int k_lo, int k_hi, int iters, float sigma2, float sigmad2, int mask_stride,
     int groups_per_cta, int per_group_floats) {
   const float rc_sigma2 = 1.0f / sigma2, rc_sigmad2 = 1.0f / sigmad2;   // IEEE divisions (correctly rounded reciprocals)
   extern __shared__ __align__(16) float sm[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int b = blockIdx.y;
+  const SetDesc d = set_desc(sets, b);
+  const int N = d.N, S = d.S, k = d.k;
+  if (k < k_lo || k > k_hi) return;        // a packed call runs each kernel variant on the sets of its k range
   const int s = blockIdx.x * groups_per_cta + warp;
   if (s >= S) return;                      // whole warps leave: nothing below synchronises the block
   const int ms = k | 1;                    // odd row stride of M: conflict-free column reads
@@ -423,16 +449,16 @@ __global__ void __launch_bounds__(256, 2) nsm_power_mma_kernel(
   float* v = P + 6 * kMmaRows;                        // [48]
   int* idx = reinterpret_cast<int*>(v + kMmaRows);    // [48]
   float* M = reinterpret_cast<float*>(idx + kMmaRows);   // [k][ms]
-  const size_t seed_row = (size_t)b * S + s;
+  const size_t nb0 = (size_t)d.knn0 + (size_t)s * k;   // the seed's first neighbour slot
 
   for (int a = lane; a < kMmaRows; a += 32) {
     int j = -1;
     float sx = 0.f, sy = 0.f, sz = 0.f, tx = 0.f, ty = 0.f, tz = 0.f;
     if (a < k) {
-      j = knn_idx[seed_row * k + a];
+      j = knn_idx[nb0 + a];
       j = min(max(j, 0), N - 1);
-      const float* ps = src + ((size_t)b * N + j) * 3;
-      const float* pt = tgt + ((size_t)b * N + j) * 3;
+      const float* ps = src + ((size_t)d.row0 + j) * 3;
+      const float* pt = tgt + ((size_t)d.row0 + j) * 3;
       sx = ps[0]; sy = ps[1]; sz = ps[2];
       tx = pt[0]; ty = pt[1]; tz = pt[2];
       M[a * ms + a] = 0.0f;                // total_knn_M[:, i, i] = 0  (PointDSC.py:278)
@@ -450,7 +476,7 @@ __global__ void __launch_bounds__(256, 2) nsm_power_mma_kernel(
 #pragma unroll
   for (int m = 0; m < 5; ++m) {
     const int j = idx[g + 8 * m];
-    rowp[m] = (j >= 0) ? normed + ((size_t)b * N + j) * kC + 2 * t : nullptr;
+    rowp[m] = (j >= 0) ? normed + ((size_t)d.row0 + j) * kC + 2 * t : nullptr;
   }
   float acc[kMmaTiles][4];
 #pragma unroll
@@ -532,13 +558,13 @@ __global__ void __launch_bounds__(256, 2) nsm_power_mma_kernel(
   }
   __syncwarp();
   if (compat_out) {
-    float* dst = compat_out + seed_row * k * k;
+    float* dst = compat_out + nb0 * k;
     for (int e = lane; e < k * k; e += 32) dst[e] = M[(e / k) * ms + (e % k)];
   }
 
   // ---- power iteration from the all-ones vector (as in nsm_power_kernel<1>, k <= 40) ----
   uint32_t mask = 0u;
-  float* it_out = iterates + seed_row * (size_t)iters * k;
+  float* it_out = iterates + nb0 * iters;
   const int rg = lane >> 2, cq = lane & 3;
   const int CQ = (k + 3) >> 2;                       // columns per quarter
   const int c_lo = cq * CQ, c_hi = min(k, c_lo + CQ);
@@ -701,27 +727,31 @@ __device__ __forceinline__ void mma4_gram_and_compat(const float* __restrict__ n
 __global__ void __launch_bounds__(128, 4) nsm_power_mma4_kernel(
     const float* __restrict__ normed, const float* __restrict__ src, const float* __restrict__ tgt,
     const int32_t* __restrict__ knn_idx, float* __restrict__ iterates, uint32_t* __restrict__ conv_mask,
-    float* __restrict__ compat_out, int N, int S, int k, int iters, float sigma2, float sigmad2, int mask_stride) {
+    float* __restrict__ compat_out, SetTable sets, int k_lo, int k_hi, int iters, float sigma2, float sigmad2,
+    int mask_stride) {
   const float rc_sigma2 = 1.0f / sigma2, rc_sigmad2 = 1.0f / sigmad2;   // IEEE divisions (correctly rounded reciprocals)
   extern __shared__ __align__(16) float sm[];
   const int tg = threadIdx.x, lane = tg & 31, warp = tg >> 5;
   const int b = blockIdx.y, s = blockIdx.x;
+  const SetDesc d = set_desc(sets, b);
+  const int N = d.N, k = d.k;
+  if (k < k_lo || k > k_hi || s >= d.S) return;   // packed call: the sets of this variant's k range; the whole CTA leaves
   const int ms = k | 1;
   float* P = sm;                                       // six coordinate arrays [80]
   float* v = P + 6 * kMma4Rows;                        // [80]
   int* idx = reinterpret_cast<int*>(v + kMma4Rows);    // [80]
   float* red = reinterpret_cast<float*>(idx + kMma4Rows);   // [8]
   float* M = red + 8;                                  // [k][ms]
-  const size_t seed_row = (size_t)b * S + s;
+  const size_t nb0 = (size_t)d.knn0 + (size_t)s * k;   // the seed's first neighbour slot
 
   for (int a = tg; a < kMma4Rows; a += 128) {
     int j = -1;
     float sx = 0.f, sy = 0.f, sz = 0.f, tx = 0.f, ty = 0.f, tz = 0.f;
     if (a < k) {
-      j = knn_idx[seed_row * k + a];
+      j = knn_idx[nb0 + a];
       j = min(max(j, 0), N - 1);
-      const float* ps = src + ((size_t)b * N + j) * 3;
-      const float* pt = tgt + ((size_t)b * N + j) * 3;
+      const float* ps = src + ((size_t)d.row0 + j) * 3;
+      const float* pt = tgt + ((size_t)d.row0 + j) * 3;
       sx = ps[0]; sy = ps[1]; sz = ps[2];
       tx = pt[0]; ty = pt[1]; tz = pt[2];
       M[a * ms + a] = 0.0f;                // total_knn_M[:, i, i] = 0  (PointDSC.py:278)
@@ -732,14 +762,14 @@ __global__ void __launch_bounds__(128, 4) nsm_power_mma4_kernel(
     v[a] = 1.0f;
   }
   __syncthreads();
-  const size_t set_row0 = (size_t)b * N;
+  const size_t set_row0 = (size_t)d.row0;
   if (warp == 0) mma4_gram_and_compat<0>(normed, set_row0, idx, P, M, k, ms, lane, sigma2, rc_sigma2, sigmad2, rc_sigmad2);
   else if (warp == 1) mma4_gram_and_compat<1>(normed, set_row0, idx, P, M, k, ms, lane, sigma2, rc_sigma2, sigmad2, rc_sigmad2);
   else if (warp == 2) mma4_gram_and_compat<2>(normed, set_row0, idx, P, M, k, ms, lane, sigma2, rc_sigma2, sigmad2, rc_sigmad2);
   else mma4_gram_and_compat<3>(normed, set_row0, idx, P, M, k, ms, lane, sigma2, rc_sigma2, sigmad2, rc_sigmad2);
   __syncthreads();
   if (compat_out) {
-    float* dst = compat_out + seed_row * k * k;
+    float* dst = compat_out + nb0 * k;
     for (int e = tg; e < k * k; e += 128) dst[e] = M[(e / k) * ms + (e % k)];
   }
 
@@ -747,7 +777,7 @@ __global__ void __launch_bounds__(128, 4) nsm_power_mma4_kernel(
   // quarter cq), rows rg + 32 i; the thread's 3 x 20 slice of the matrix stays in registers for all iterations (columns beyond
   // the quarter are zeros: fma(0, 0, p) == p, so the sums are those of the shared-memory form bit for bit)
   uint32_t mask = 0u;
-  float* it_out = iterates + seed_row * (size_t)iters * k;
+  float* it_out = iterates + nb0 * iters;
   constexpr int RG = 32, RI = 3, CW = 20;            // rows rg + 32 i < 96 and 4 x 20 columns cover k <= 80
   const int rg = tg >> 2, cq = tg & 3;
   const int CQ = (k + 3) >> 2;
@@ -806,14 +836,12 @@ __global__ void __launch_bounds__(128, 4) nsm_power_mma4_kernel(
   if (tg == 0) atomicAnd(conv_mask + (size_t)b * mask_stride, mask);
 }
 
-void launch_nsm_power(const float* normed, const float* src, const float* tgt, const int32_t* knn_idx, float* iterates,
-                      uint32_t* conv_mask, float* compat_out, int B, int N, int S, int k, int iters, float sigma,
-                      float sigma_d, int mask_stride, int tensor_gram, cudaStream_t st) {
-  if (S <= 0) return;
+// One variant over the sets whose k lies in [k_lo, k_hi]; k is the largest of them (shared-memory layout and grid).
+static void launch_nsm_variant(const float* normed, const float* src, const float* tgt, const int32_t* knn_idx, float* iterates,
+                               uint32_t* conv_mask, float* compat_out, int B, const SetTable& t, int k, int k_lo, int k_hi,
+                               int iters, float sigma, float sigma_d, int mask_stride, int tensor_gram, cudaStream_t st) {
+  const int S = t.S;
   const int ms = k | 1;
-  // developer switch for same-box A/B of the two Gram paths (tools/exp_variant.sh style): PDSC_NSM_FFMA=1 forces the FFMA kernels
-  static const bool force_ffma = [] { const char* v = getenv("PDSC_NSM_FFMA"); return v && v[0] == '1'; }();
-  if (force_ffma) tensor_gram = 0;
   if (tensor_gram && k <= 40) {
     // one warp per seed, two CTAs of eight warps per SM; per warp: key points 6 x 48, iterate 48, indices 48, M k x ms
     int per_group_floats = 8 * kMmaRows + k * ms;
@@ -822,16 +850,16 @@ void launch_nsm_power(const float* normed, const float* src, const float* tgt, c
     const int smem = warps * per_group_floats * (int)sizeof(float);
     ensure_dynamic_smem(reinterpret_cast<const void*>(nsm_power_mma_kernel), smem);
     nsm_power_mma_kernel<<<dim3((S + warps - 1) / warps, B), warps * 32, smem, st>>>(
-        normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, N, S, k, iters, sigma * sigma, sigma_d * sigma_d, mask_stride,
-        warps, per_group_floats);
+        normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, t, k_lo, k_hi, iters, sigma * sigma, sigma_d * sigma_d,
+        mask_stride, warps, per_group_floats);
     return;
   }
   if (tensor_gram && k <= kMma4Rows) {
     // 40 < k <= 80: four warps per seed, one seed per CTA
     const int smem = (8 * kMma4Rows + 8 + k * ms) * (int)sizeof(float);
     ensure_dynamic_smem(reinterpret_cast<const void*>(nsm_power_mma4_kernel), smem);
-    nsm_power_mma4_kernel<<<dim3(S, B), 128, smem, st>>>(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, N, S, k, iters,
-                                                         sigma * sigma, sigma_d * sigma_d, mask_stride);
+    nsm_power_mma4_kernel<<<dim3(S, B), 128, smem, st>>>(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, t, k_lo, k_hi,
+                                                         iters, sigma * sigma, sigma_d * sigma_d, mask_stride);
     return;
   }
   const int kp = (k + 3) & ~3;
@@ -845,14 +873,37 @@ void launch_nsm_power(const float* normed, const float* src, const float* tgt, c
     const int smem = warps * (int)group_bytes;
     ensure_dynamic_smem(reinterpret_cast<const void*>(nsm_power_kernel<1>), smem);
     nsm_power_kernel<1><<<dim3((S + warps - 1) / warps, B), warps * 32, smem, st>>>(
-        normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, N, S, k, iters, sigma * sigma, sigma_d * sigma_d, mask_stride,
-        warps, per_group_floats);
+        normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, t, k_lo, k_hi, iters, sigma * sigma, sigma_d * sigma_d,
+        mask_stride, warps, per_group_floats);
   } else {
     // four warps per seed, one seed per CTA
     const int smem = (int)group_bytes;
     ensure_dynamic_smem(reinterpret_cast<const void*>(nsm_power_kernel<4>), smem);
-    nsm_power_kernel<4><<<dim3(S, B), 128, smem, st>>>(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, N, S, k, iters,
-                                                        sigma * sigma, sigma_d * sigma_d, mask_stride, 1, per_group_floats);
+    nsm_power_kernel<4><<<dim3(S, B), 128, smem, st>>>(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, t, k_lo, k_hi,
+                                                        iters, sigma * sigma, sigma_d * sigma_d, mask_stride, 1, per_group_floats);
+  }
+}
+
+void launch_nsm_power(const float* normed, const float* src, const float* tgt, const int32_t* knn_idx, float* iterates,
+                      uint32_t* conv_mask, float* compat_out, int B, int N, int S, int k, int iters, float sigma,
+                      float sigma_d, int mask_stride, int tensor_gram, cudaStream_t st, const SetDesc* sets, int k_min) {
+  if (S <= 0) return;
+  // developer switch for same-box A/B of the two Gram paths (tools/exp_variant.sh style): PDSC_NSM_FFMA=1 forces the FFMA kernels
+  static const bool force_ffma = [] { const char* v = getenv("PDSC_NSM_FFMA"); return v && v[0] == '1'; }();
+  if (force_ffma) tensor_gram = 0;
+  const SetTable t{sets, N, S, k, 0, 1, 0};
+  if (!sets) {
+    launch_nsm_variant(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, B, t, k, 0, k, iters, sigma, sigma_d, mask_stride,
+                       tensor_gram, st);
+    return;
+  }
+  // a packed call's sets may differ in k (N_b <= cfg.k): each set runs the variant a uniform call of its k would run
+  const int bounds[3][2] = {{1, 40}, {41, tensor_gram ? kMma4Rows : kMaxK}, {kMma4Rows + 1, kMaxK}};
+  for (int r = 0; r < (tensor_gram ? 3 : 2); ++r) {
+    const int lo = bounds[r][0] > k_min ? bounds[r][0] : k_min, hi = bounds[r][1] < k ? bounds[r][1] : k;
+    if (lo > hi) continue;
+    launch_nsm_variant(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, B, t, hi, lo, hi, iters, sigma, sigma_d,
+                       mask_stride, tensor_gram, st);
   }
 }
 

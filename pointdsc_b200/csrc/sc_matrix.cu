@@ -11,18 +11,22 @@
 // `src_dist` is NOT materialised: its only consumer, the seed NMS (a6), recomputes it from the points.
 #include "common.cuh"
 #include "kernels.h"
+#include "sets.cuh"
 
 namespace pdsc {
 
 constexpr int kScRows = 32;
 
 __global__ void __launch_bounds__(256) sc_matrix_kernel(const float* __restrict__ src, const float* __restrict__ tgt,
-                                                        float* __restrict__ sc, int N, int NS, float s2) {
+                                                        float* __restrict__ sc, SetTable sets, float s2) {
   __shared__ float rs[kScRows][3], rt[kScRows][3];
   const int b = blockIdx.y;
+  const SetDesc d = set_desc(sets, b);
+  const int N = d.N, NS = round_up(N, 64);
   const int i0 = blockIdx.x * kScRows;
-  const float* ps = src + (size_t)b * N * 3;
-  const float* pt = tgt + (size_t)b * N * 3;
+  if (i0 >= N) return;                     // a packed call's grid is sized by its largest set
+  const float* ps = src + (size_t)d.row0 * 3;
+  const float* pt = tgt + (size_t)d.row0 * 3;
   for (int t = threadIdx.x; t < kScRows * 3; t += blockDim.x) {
     const int r = t / 3, c = t % 3;
     const int i = min(i0 + r, N - 1);
@@ -31,7 +35,7 @@ __global__ void __launch_bounds__(256) sc_matrix_kernel(const float* __restrict_
   }
   __syncthreads();
   const int rows = min(kScRows, N - i0);
-  float* out = sc + ((size_t)b * N + i0) * NS;
+  float* out = sc + d.sc0 + (size_t)i0 * NS;
   for (int j = threadIdx.x; j < NS; j += blockDim.x) {
     if (j < N) {
       const float sx = ps[(size_t)j * 3], sy = ps[(size_t)j * 3 + 1], sz = ps[(size_t)j * 3 + 2];
@@ -48,11 +52,11 @@ __global__ void __launch_bounds__(256) sc_matrix_kernel(const float* __restrict_
   }
 }
 
-void launch_sc_matrix(const float* src, const float* tgt, float* sc, int B, int N, int NS, float sigma_d,
-                      cudaStream_t st) {
+void launch_sc_matrix(const float* src, const float* tgt, float* sc, int B, int N, float sigma_d, cudaStream_t st,
+                      const SetDesc* sets) {
   const float s2 = sigma_d * sigma_d;  // fp32 product, as `self.sigma_spat ** 2`
   dim3 grid((N + kScRows - 1) / kScRows, B);
-  sc_matrix_kernel<<<grid, 256, 0, st>>>(src, tgt, sc, N, NS, s2);
+  sc_matrix_kernel<<<grid, 256, 0, st>>>(src, tgt, sc, SetTable{sets, N, 0, 0, 0, 1, 0}, s2);
 }
 
 // ---- tiled layout for the tensor-core attention (tc_attention.cuh) ---------------------------------------
@@ -69,19 +73,21 @@ void launch_sc_matrix(const float* src, const float* tgt, float* sc, int B, int 
 constexpr int kScTStride = 129;   // smem transpose tile [32 i][128 j], odd stride: conflict-free both ways
 
 __global__ void __launch_bounds__(256) sc_matrix_tiled_kernel(const float* __restrict__ src, const float* __restrict__ tgt,
-                                                              float* __restrict__ sc, int N, int KT, int QT, float s2,
-                                                              float rc_s2) {
+                                                              float* __restrict__ sc, SetTable sets, float s2, float rc_s2) {
   // the A range's points as six arrays: an 8-byte broadcast load is the same coordinate of TWO consecutive rows, so the distance
   // chains of two matrix elements run as pairs (each lane rounded exactly like the scalar sequence)
   __shared__ __align__(8) float isx[128], isy[128], isz[128], itx[128], ity[128], itz[128];
   __shared__ float tr[32 * kScTStride];
   const int b = blockIdx.y;
+  const SetDesc d = set_desc(sets, b);
+  const int N = d.N, KT = (N + 63) / 64, QT = (N + 127) / 128;
+  if ((int)blockIdx.x >= QT * (QT + 1) / 2) return;   // a packed call's grid is sized by its largest set
   // blockIdx.x enumerates the pairs A <= Bq
   int A = 0, rem = blockIdx.x;
   while (rem >= QT - A) { rem -= QT - A; ++A; }
   const int Bq = A + rem;
-  const float* ps = src + (size_t)b * N * 3;
-  const float* pt = tgt + (size_t)b * N * 3;
+  const float* ps = src + (size_t)d.row0 * 3;
+  const float* pt = tgt + (size_t)d.row0 * 3;
   if (threadIdx.x < 128) {
     const int i = min(A * 128 + (int)threadIdx.x, N - 1);
     isx[threadIdx.x] = ps[(size_t)i * 3]; isy[threadIdx.x] = ps[(size_t)i * 3 + 1]; isz[threadIdx.x] = ps[(size_t)i * 3 + 2];
@@ -93,13 +99,13 @@ __global__ void __launch_bounds__(256) sc_matrix_tiled_kernel(const float* __res
   const int jc = min(j, N - 1);
   const float sx = ps[(size_t)jc * 3], sy = ps[(size_t)jc * 3 + 1], sz = ps[(size_t)jc * 3 + 2];
   const float tx = pt[(size_t)jc * 3], ty = pt[(size_t)jc * 3 + 1], tz = pt[(size_t)jc * 3 + 2];
-  const size_t set_base = (size_t)b * KT * QT;
+  float* const set_sc = sc + d.sc0;
   const int ti = threadIdx.x & 31, tg = threadIdx.x >> 5;   // transposed write-out: lane = i within the chunk, 16 j per warp
   for (int ic = 0; ic < 4; ++ic) {             // 32-row chunks of the A range
     // orientation 1: key = 128 A + i, query = j   ->  tile (kt = 2 A + (ic >> 1), qt = Bq), element [(i & 63)][jl]
     const int kt1 = 2 * A + (ic >> 1);
     const int il0 = ic * 32 + half * 16;
-    float* out1 = sc + ((set_base + (size_t)min(kt1, KT - 1) * QT + Bq) << 13) + (((il0 & 63) >> 2) * 128 + jl) * 4;
+    float* out1 = set_sc + (((size_t)min(kt1, KT - 1) * QT + Bq) << 13) + (((il0 & 63) >> 2) * 128 + jl) * 4;
     float* trw = tr + (half * 16) * kScTStride + jl;
     const bool col_ok = j < N;
     const int i_lim = N - A * 128 - il0;       // rows ii < i_lim are real correspondences
@@ -135,7 +141,7 @@ __global__ void __launch_bounds__(256) sc_matrix_tiled_kernel(const float* __res
       // orientation 2: key = 128 Bq + j, query = 128 A + i  ->  tile (kt = 2 Bq + (j >> 6), qt = A), element (j & 63, i)
       const int kt2 = 2 * Bq + (tg >> 2);      // the warp's 16 j share one key tile
       if (kt2 < KT) {
-        float* out2 = sc + ((set_base + (size_t)kt2 * QT + A) << 13) + (((tg & 3) * 4) * 128 + ic * 32 + ti) * 4;
+        float* out2 = set_sc + (((size_t)kt2 * QT + A) << 13) + (((tg & 3) * 4) * 128 + ic * 32 + ti) * 4;
         const float* trr = tr + ti * kScTStride + tg * 16;
 #pragma unroll
         for (int gq = 0; gq < 4; ++gq)
@@ -146,10 +152,11 @@ __global__ void __launch_bounds__(256) sc_matrix_tiled_kernel(const float* __res
   }
 }
 
-void launch_sc_matrix_tiled(const float* src, const float* tgt, float* sc, int B, int N, float sigma_d, cudaStream_t st) {
+void launch_sc_matrix_tiled(const float* src, const float* tgt, float* sc, int B, int N, float sigma_d, cudaStream_t st,
+                            const SetDesc* sets) {
   const float s2 = sigma_d * sigma_d;
-  const int KT = (N + 63) / 64, QT = (N + 127) / 128;
-  sc_matrix_tiled_kernel<<<dim3(QT * (QT + 1) / 2, B), 256, 0, st>>>(src, tgt, sc, N, KT, QT, s2, 1.0f / s2);
+  const int QT = (N + 127) / 128;
+  sc_matrix_tiled_kernel<<<dim3(QT * (QT + 1) / 2, B), 256, 0, st>>>(src, tgt, sc, SetTable{sets, N, 0, 0, 1, 1, 0}, s2, 1.0f / s2);
 }
 
 // tiled -> dense [B][N][N] (stage tap only)

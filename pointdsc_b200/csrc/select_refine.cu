@@ -13,6 +13,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "sets.cuh"
 #include "svd3.cuh"
 
 namespace pdsc {
@@ -33,18 +34,22 @@ __global__ void __launch_bounds__(256) seed_hypotheses_kernel(
     const float* __restrict__ src, const float* __restrict__ tgt, const int32_t* __restrict__ knn_idx,
     const float* __restrict__ iterates, const uint32_t* __restrict__ conv_mask, const float* __restrict__ seed_trans_in,
     float* __restrict__ seed_trans, int32_t* __restrict__ inlier_counts, unsigned long long* __restrict__ best_key,
-    float* __restrict__ eig_out, int32_t* __restrict__ power_iters, int N, int S, int k, int iters, float d2_lim,
+    float* __restrict__ eig_out, int32_t* __restrict__ power_iters, SetTable sets, int iters, float d2_lim,
     int mask_stride) {
   // the set's points, staged once per CTA for its eight seeds: six arrays so that an 8-byte load is the same coordinate of two points
   __shared__ __align__(8) float pts_s[6][kHypChunk];
   const int b = blockIdx.y;
+  const SetDesc d = set_desc(sets, b);
+  const int N = d.N, S = d.S, k = d.k;
+  if ((int)blockIdx.x * 8 >= S) return;     // a packed call's grid is sized by its largest set: the whole CTA leaves
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int s_raw = blockIdx.x * 8 + warp;
   const bool active = s_raw < S;            // inactive warps still take part in the staging barriers
   const int s = active ? s_raw : S - 1;
-  const size_t row = (size_t)b * S + s;
-  const float* ps = src + (size_t)b * N * 3;
-  const float* pt = tgt + (size_t)b * N * 3;
+  const size_t row = (size_t)d.seed0 + s;
+  const size_t nb0 = (size_t)d.knn0 + (size_t)s * k;   // the seed's first neighbour slot
+  const float* ps = src + (size_t)d.row0 * 3;
+  const float* pt = tgt + (size_t)d.row0 * 3;
 
   // exit iteration of this set: first iteration at which every seed passed allclose, else the cap
   const uint32_t m = conv_mask[(size_t)b * mask_stride] & ((iters >= 32) ? 0xFFFFFFFFu : ((1u << iters) - 1u));
@@ -64,10 +69,10 @@ __global__ void __launch_bounds__(256) seed_hypotheses_kernel(
       const int a = lane + q * 32;
       w[q] = 0.f; ax[q] = ay[q] = az[q] = bx[q] = by[q] = bz[q] = 0.f;
       if (a < k) {
-        float e = iterates[(row * iters + t_exit) * k + a];
-        if (eig_out && active) eig_out[row * k + a] = e;
+        float e = iterates[nb0 * iters + (size_t)t_exit * k + a];
+        if (eig_out && active) eig_out[nb0 + a] = e;
         w[q] = e;
-        int j = knn_idx[row * k + a];
+        int j = knn_idx[nb0 + a];
         j = min(max(j, 0), N - 1);
         ax[q] = ps[(size_t)j * 3]; ay[q] = ps[(size_t)j * 3 + 1]; az[q] = ps[(size_t)j * 3 + 2];
         bx[q] = pt[(size_t)j * 3]; by[q] = pt[(size_t)j * 3 + 1]; bz[q] = pt[(size_t)j * 3 + 2];
@@ -164,7 +169,7 @@ void launch_seed_hypotheses(const float* src, const float* tgt, const int32_t* k
                             const uint32_t* conv_mask, const float* seed_trans_in, float* seed_trans,
                             int32_t* inlier_counts, unsigned long long* best_key, float* eig_out, int32_t* power_iters,
                             int B, int N, int S, int k, int iters, float inlier_threshold, int mask_stride,
-                            cudaStream_t st) {
+                            cudaStream_t st, const SetDesc* sets) {
   if (S <= 0) return;
   // smallest float x with sqrtf(x) >= threshold (IEEE sqrt on the host == the device's sqrt.rn): residual < threshold <=> its square < x
   float d2_lim = inlier_threshold * inlier_threshold;
@@ -172,7 +177,7 @@ void launch_seed_hypotheses(const float* src, const float* tgt, const int32_t* k
   while (std::sqrt(d2_lim) < inlier_threshold) d2_lim = std::nextafter(d2_lim, INFINITY);
   seed_hypotheses_kernel<<<dim3((S + 7) / 8, B), 256, 0, st>>>(src, tgt, knn_idx, iterates, conv_mask, seed_trans_in,
                                                               seed_trans, inlier_counts, best_key, eig_out, power_iters,
-                                                              N, S, k, iters, d2_lim, mask_stride);
+                                                              SetTable{sets, N, S, k, 0, 1, 0}, iters, d2_lim, mask_stride);
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -201,21 +206,23 @@ __device__ __forceinline__ void block_sum(double (&vals)[NV], double* red /* [16
 __global__ void __launch_bounds__(kRefThreads) select_refine_kernel(
     const float* __restrict__ src, const float* __restrict__ tgt, const float* __restrict__ seed_trans,
     const unsigned long long* __restrict__ best_key, float* __restrict__ final_trans, float* __restrict__ final_labels,
-    float* __restrict__ init_trans_out, int32_t* __restrict__ best_out, int32_t* __restrict__ refine_solves, int N,
-    int S, float thr, float rthr, int max_refine) {
+    float* __restrict__ init_trans_out, int32_t* __restrict__ best_out, int32_t* __restrict__ refine_solves, SetTable sets,
+    float thr, float rthr, int max_refine) {
   __shared__ float T[12];
   __shared__ double red[(kRefThreads / 32) * 10];
   __shared__ double tot[10];
   const int b = blockIdx.x, tid = threadIdx.x;
-  const float* ps = src + (size_t)b * N * 3;
-  const float* pt = tgt + (size_t)b * N * 3;
+  const SetDesc d = set_desc(sets, b);
+  const int N = d.N, S = d.S;
+  const float* ps = src + (size_t)d.row0 * 3;
+  const float* pt = tgt + (size_t)d.row0 * 3;
 
   int best = 0;
   if (S > 0) {
     best = (int)(0xFFFFFFFFu - (unsigned)(best_key[b] & 0xFFFFFFFFull));
     best = min(max(best, 0), S - 1);
   }
-  if (tid < 12) T[tid] = (S > 0) ? seed_trans[((size_t)b * S + best) * 16 + tid] : ((tid % 5 == 0) ? 1.f : 0.f);
+  if (tid < 12) T[tid] = (S > 0) ? seed_trans[((size_t)d.seed0 + best) * 16 + tid] : ((tid % 5 == 0) ? 1.f : 0.f);
   __syncthreads();
   if (tid < 16 && init_trans_out) init_trans_out[(size_t)b * 16 + tid] = (tid < 12) ? T[tid] : (tid == 15 ? 1.f : 0.f);
   if (tid == 0 && best_out) best_out[b] = best;
@@ -223,9 +230,9 @@ __global__ void __launch_bounds__(kRefThreads) select_refine_kernel(
   // final_labels: inlier mask of the selected hypothesis BEFORE refinement (PointDSC.py:333-335)
   // (non-testing mode returns the confidence logits instead, PointDSC.py:190-191: final_labels is null there)
   for (int j = tid; final_labels && j < N; j += kRefThreads) {
-    const float d = residual(T, ps[(size_t)j * 3], ps[(size_t)j * 3 + 1], ps[(size_t)j * 3 + 2], pt[(size_t)j * 3],
+    const float r = residual(T, ps[(size_t)j * 3], ps[(size_t)j * 3 + 1], ps[(size_t)j * 3 + 2], pt[(size_t)j * 3],
                              pt[(size_t)j * 3 + 1], pt[(size_t)j * 3 + 2]);
-    final_labels[(size_t)b * N + j] = (d < thr) ? 1.0f : 0.0f;
+    final_labels[(size_t)d.row0 + j] = (r < thr) ? 1.0f : 0.0f;
   }
 
   long long prev = 0;
@@ -294,9 +301,11 @@ __global__ void __launch_bounds__(kRefThreads) select_refine_kernel(
 void launch_select_refine(const float* src, const float* tgt, const float* seed_trans,
                           const unsigned long long* best_key, float* final_trans, float* final_labels,
                           float* init_trans_out, int32_t* best_out, int32_t* refine_solves, int B, int N, int S,
-                          float inlier_threshold, float refine_threshold, int max_refine, cudaStream_t st) {
+                          float inlier_threshold, float refine_threshold, int max_refine, cudaStream_t st,
+                          const SetDesc* sets) {
   select_refine_kernel<<<B, kRefThreads, 0, st>>>(src, tgt, seed_trans, best_key, final_trans, final_labels,
-                                                  init_trans_out, best_out, refine_solves, N, S, inlier_threshold,
+                                                  init_trans_out, best_out, refine_solves, SetTable{sets, N, S, 0, 0, 1, 0},
+                                                  inlier_threshold,
                                                   refine_threshold, max_refine);
 }
 

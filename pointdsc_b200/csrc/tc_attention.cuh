@@ -23,7 +23,39 @@ struct AttnArgs {
   int splits, TS;
   float* part_o;      // [items][128][128] unnormalised O of every work item           (splits > 1)
   float* part_ml;     // [items][128][2]   its final reference maximum (log2 units) and row sum
+  // packed call: the descriptor table (nullptr for a uniform call).  Its work items are numbered set by set from each set's
+  // item0; set b has QT_b * sp_b of them, each covering TS_b key tiles; items, N, QT, KT, splits and TS above are unused
+  const SetDesc* sets;
+  int nsets;
 };
+
+// one work item: (set, query tile, split)
+struct AttnItem {
+  int N, QT, KT;      // the set's size and tiles
+  int qt, t0, T;      // query tile within the set, first key tile and key tiles of the item
+  int sp;             // the set's key splits (1: the item writes msg itself)
+  int qtile, kt0;     // the item's tile in the Q image, the set's first tile in the K / V image
+  int row0;           // the set's first row
+  long long sc0;      // the set's SC block
+};
+
+__device__ __forceinline__ AttnItem attn_item(const AttnArgs& a, int witem) {
+  AttnItem w;
+  if (a.sets) {
+    const int b = find_set(a.nsets, witem, [&](int i) { return a.sets[i].item0; });
+    const SetDesc d = a.sets[b];
+    const int local = witem - d.item0;
+    w.N = d.N; w.QT = (d.N + 127) / 128; w.KT = (d.N + 63) / 64;
+    w.qt = local / d.sp; w.t0 = (local % d.sp) * d.TS; w.T = d.TS; w.sp = d.sp;
+    w.qtile = d.qt0 + w.qt; w.kt0 = d.kt0; w.row0 = d.row0; w.sc0 = d.sc0;
+  } else {
+    const int item = witem / a.splits, b = item / a.QT;
+    w.N = a.N; w.QT = a.QT; w.KT = a.KT;
+    w.qt = item % a.QT; w.t0 = (witem % a.splits) * a.TS; w.T = a.TS; w.sp = a.splits;
+    w.qtile = item; w.kt0 = b * a.KT; w.row0 = b * a.N; w.sc0 = ((long long)b * a.KT * a.QT) << 13;
+  }
+  return w;
+}
 
 constexpr int kAttnThreads = 288;                       // two consumer warpgroups + one producer warp
 

@@ -31,7 +31,6 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
   const uint32_t q_full = smem_u32(bars + 0), q_empty = smem_u32(bars + 1);
   const uint32_t kv_full = smem_u32(bars + 2), kv_empty = smem_u32(bars + 4);   // [kAttnStages]
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int T = a.TS;                                          // key tiles per work item (== a.KT unless the keys are split)
   const int my_items = (a.items > (int)blockIdx.x) ? (a.items - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
 
   if (tid == 0) {
@@ -54,16 +53,16 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
       int gt = 0;                                              // running tile count of the CTA
       for (int it = 0; it < my_items; ++it) {
         const int witem = blockIdx.x + it * gridDim.x;
-        const int item = witem / a.splits, t0 = (witem % a.splits) * T;
+        const AttnItem w = attn_item(a, witem);
         if (it > 0) mbar_wait(q_empty, (uint32_t)((it - 1) & 1));   // the previous item's last QK has retired
         mbar_expect_tx(q_full, q_bytes);
         for (uint32_t off = 0; off < q_bytes; off += 32768u)
-          bulk_g2s(s0 + kAttnPQ + off, a.qimg + (size_t)item * 65536 + off, 32768u, q_full);
-        for (int j = 0; j < T; ++j, ++gt) {
+          bulk_g2s(s0 + kAttnPQ + off, a.qimg + (size_t)w.qtile * 65536 + off, 32768u, q_full);
+        for (int j = 0; j < w.T; ++j, ++gt) {
           const int st = gt % kAttnStages, use = gt / kAttnStages;
           if (use > 0) mbar_wait(kv_empty + 8 * st, (uint32_t)((use - 1) & 1));
-          const int kt = min(t0 + j, a.KT - 1);                // a virtual tile re-reads the last real one (it is masked)
-          const uint8_t* kv = a.kvimg + ((size_t)(item / a.QT) * a.KT + kt) * 65536;
+          const int kt = min(w.t0 + j, w.KT - 1);              // a virtual tile re-reads the last real one (it is masked)
+          const uint8_t* kv = a.kvimg + ((size_t)w.kt0 + kt) * 65536;
           const uint32_t dst = s0 + kAttnPKV + st * 65536;
           mbar_expect_tx(kv_full + 8 * st, 2 * tile_bytes);
           bulk_g2s(dst, kv, tile_bytes, kv_full + 8 * st);
@@ -79,13 +78,13 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
   const int wg = warp >> 2, wt = tid & 127;
   const int r0 = 64 * wg + frag_row(wt), fc = frag_col(wt);   // query rows r0, r0 + 8 of the tile; key columns 8 j + fc, + 1
   const uint32_t qa = s0 + kAttnPQ + (uint32_t)wg * 8192u;     // this warpgroup's 64 rows of the Q image
-  const size_t tile_stride = (size_t)a.QT << 13;
   int gt = 0;
   for (int it = 0; it < my_items; ++it) {
     const int witem = blockIdx.x + it * gridDim.x;
-    const int item = witem / a.splits, t0 = (witem % a.splits) * T;   // (set, query tile) and the split's first key tile
-    const int b = item / a.QT, qt = item % a.QT;
-    const float* sc_cta = a.sc + ((((size_t)b * a.KT) * a.QT + qt) << 13);
+    const AttnItem w = attn_item(a, witem);   // (set, query tile) and the split's key tiles
+    const int N = w.N, qt = w.qt, t0 = w.t0, T = w.T, KT = w.KT;
+    const size_t tile_stride = (size_t)w.QT << 13;
+    const float* sc_cta = a.sc + w.sc0 + ((size_t)qt << 13);
     float o[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) o[i] = 0.f;
@@ -102,7 +101,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
       // this thread's 32 SC values, loaded while the MMA runs: tile layout [16 key groups][128 queries][4 keys]
       float sc[32];
       {
-        const float* tile = sc_cta + (size_t)min(t0 + j, a.KT - 1) * tile_stride;
+        const float* tile = sc_cta + (size_t)min(t0 + j, KT - 1) * tile_stride;
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
@@ -118,10 +117,10 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
       if (j == T - 1) mbar_arrive(q_empty);   // the item's last QK has retired: the Q buffer may be refilled
 #pragma unroll
       for (int i = 0; i < 32; ++i) s[i] *= sc[i];
-      if ((t0 + j) * 64 + 63 >= a.N) {     // the set's last, ragged key tile - or a virtual tile behind it (all masked)
+      if ((t0 + j) * 64 + 63 >= N) {       // the set's last, ragged key tile - or a virtual tile behind it (all masked)
 #pragma unroll
         for (int i = 0; i < 32; ++i)
-          if ((t0 + j) * 64 + 8 * (i >> 2) + fc + (i & 1) >= a.N) s[i] = -INFINITY;
+          if ((t0 + j) * 64 + 8 * (i >> 2) + fc + (i & 1) >= N) s[i] = -INFINITY;
       }
       // online softmax: row maximum over the quad that shares the row, rescale O and the row sum when it moves
       float scale[2];
@@ -159,7 +158,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
     }
     // ---- epilogue: O / l -> msg.  Key split: the item's UNNORMALISED O, its maximum and its row sum go to the partial
     //      buffers; tc_attention_merge_kernel combines the splits of a query tile in ascending split order ----
-    const bool partial = a.splits > 1;
+    const bool partial = w.sp > 1;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float lt = l_sum[h];
@@ -168,8 +167,8 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
       const int r = r0 + 8 * h;
       const float inv_l = partial ? 1.0f : 1.0f / lt;
       if (partial && (lane & 3) == 0) *reinterpret_cast<float2*>(a.part_ml + ((size_t)witem * 128 + r) * 2) = make_float2(m[h], lt);
-      if (!partial && qt * 128 + r >= a.N) continue;
-      float* dst = partial ? a.part_o + ((size_t)witem * 128 + r) * kC : a.msg + ((size_t)b * a.N + qt * 128 + r) * kC;
+      if (!partial && qt * 128 + r >= N) continue;
+      float* dst = partial ? a.part_o + ((size_t)witem * 128 + r) * kC : a.msg + ((size_t)w.row0 + qt * 128 + r) * kC;
 #pragma unroll
       for (int jj = 0; jj < 16; ++jj)
         *reinterpret_cast<float2*>(dst + 8 * jj + fc) = make_float2(o[4 * jj + 2 * h] * inv_l, o[4 * jj + 2 * h + 1] * inv_l);
@@ -179,18 +178,28 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
 
 // ---- key split: combine the partial results of one query tile -------------------------------------------------------------
 // msg_i = sum_s O_s[i] 2^(m_s - m*) / sum_s l_s 2^(m_s - m*),  m* = max_s m_s, splits added in ascending order (deterministic).
-// One CTA per (query tile, 32-row quarter), thread = (row, 16-byte column piece stride).
+// One CTA per (query tile, 32-row quarter), thread = (row, 16-byte column piece stride).  A packed call numbers its query tiles
+// set by set (qt0); the tiles of its sets without a split wrote msg themselves.
 __global__ void __launch_bounds__(256) tc_attention_merge_kernel(const float* __restrict__ part_o, const float* __restrict__ part_ml,
-                                                                 float* __restrict__ msg, int N, int QT, int splits) {
-  const int item = blockIdx.x >> 2, quarter = blockIdx.x & 3;
-  const int b = item / QT, qt = item % QT;
+                                                                 float* __restrict__ msg, int N, int QT, int splits,
+                                                                 const SetDesc* __restrict__ sets, int nsets) {
+  const int qtile = blockIdx.x >> 2, quarter = blockIdx.x & 3;
+  int qt, item, row0;     // item: the tile's first work item
+  if (sets) {
+    const SetDesc d = sets[find_set(nsets, qtile, [&](int i) { return sets[i].qt0; })];
+    if (d.sp < 2) return;
+    N = d.N; qt = qtile - d.qt0; splits = d.sp; item = d.item0 + qt * d.sp; row0 = d.row0;
+  } else {
+    const int b = qtile / QT;
+    qt = qtile % QT; item = qtile * splits; row0 = b * N;
+  }
   const int row = quarter * 32 + (threadIdx.x >> 3);
   if (qt * 128 + row >= N) return;
   // the reference maxima first (independent loads), then the partial rows four splits at a time so that their loads overlap:
   // at bs = 1 this kernel is pure L2 latency (8 splits x 5 dependent round trips took 9.5 us per layer)
   float mstar = -INFINITY;
 #pragma unroll 4
-  for (int s = 0; s < splits; ++s) mstar = fmaxf(mstar, part_ml[(((size_t)item * splits + s) * 128 + row) * 2]);
+  for (int s = 0; s < splits; ++s) mstar = fmaxf(mstar, part_ml[(((size_t)item + s) * 128 + row) * 2]);
   float L = 0.f;
   float4 acc[4];
 #pragma unroll
@@ -201,7 +210,7 @@ __global__ void __launch_bounds__(256) tc_attention_merge_kernel(const float* __
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int s = s0 + u < splits ? s0 + u : splits - 1;      // a clamped re-read of the last split is given weight 0 below
-      const size_t w = (size_t)item * splits + s;
+      const size_t w = (size_t)item + s;
       ml[u] = *reinterpret_cast<const float2*>(part_ml + (w * 128 + row) * 2);
       const float* o = part_o + (w * 128 + row) * kC;
 #pragma unroll
@@ -221,7 +230,7 @@ __global__ void __launch_bounds__(256) tc_attention_merge_kernel(const float* __
     }
   }
   const float inv = 1.0f / L;
-  float* dst = msg + ((size_t)b * N + qt * 128 + row) * kC;
+  float* dst = msg + ((size_t)row0 + qt * 128 + row) * kC;
 #pragma unroll
   for (int i = 0; i < 4; ++i)
     *reinterpret_cast<float4*>(dst + ((threadIdx.x & 7) + 8 * i) * 4) = make_float4(acc[i].x * inv, acc[i].y * inv, acc[i].z * inv, acc[i].w * inv);

@@ -35,6 +35,25 @@ __device__ __forceinline__ void locate_row(long long g, int N, int& bb, int& nn)
   nn = (int)(g - (long long)bb * N);
 }
 
+// operand image tile of global row g (PCQ: its set's 128-query tile in the Q image, KV: its 64-key tile in the K / V image)
+// and the row's place within that tile.  A packed call's rows are not padded per set, so a chain tile may span several sets:
+// each row finds its own set by a binary search over the sets' first rows.
+template <int MODE>
+__device__ __forceinline__ void locate_tile(const ChainArgs& a, long long g, int& tile, int& r) {
+  int nn, t0;
+  if (a.sets) {
+    const int b = find_set(a.nsets, g, [&](int i) { return a.sets[i].row0; });
+    nn = (int)(g - a.sets[b].row0);
+    t0 = MODE == kPCQ ? a.sets[b].qt0 : a.sets[b].kt0;
+  } else {
+    int bb;
+    locate_row(g, a.N, bb, nn);
+    t0 = bb * (MODE == kPCQ ? a.QT : a.KT);
+  }
+  tile = t0 + (MODE == kPCQ ? (nn >> 7) : (nn >> 6));
+  r = MODE == kPCQ ? (nn & 127) : (nn & 63);
+}
+
 // byte offset of the 16-byte piece `piece` (0..31) of global row `g` in the blocked fp32 layout described in the header
 __host__ __device__ __forceinline__ size_t blocked_f32_offset(long long g, uint32_t piece) {
   return (size_t)(g >> 7) * 65536 + (size_t)(piece >> 3) * 16384 + (size_t)(g & 127) * 128 + (size_t)(((piece & 7u) ^ ((uint32_t)g & 7u)) << 4);
@@ -82,7 +101,6 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
   const uint32_t w_base = s0 + kChW;
   // this mode's biases, packed: PCQ b1|bq, KV bk|bv, MSG bm0|bm1|bm2
   constexpr int kBiasSrc = (MODE == kPCQ) ? kB1 : (MODE == kKV) ? kBk : kBm0;
-  const int N = a.N;
   const long long rows = a.rows;
   const long long num_tiles = (rows + 127) / 128;
 
@@ -143,13 +161,13 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
         bulk_g2s(s0 + kChRes, reinterpret_cast<const uint8_t*>(a.res) + (size_t)tile * 65536, 65536u, bar_res);
       }
     }
-    // the two rows of this thread: global index, set and position within the set
+    // the two rows of this thread: global index, operand image tile and row within it
     long long g[2];
-    int bb[2], nn[2];
+    int tl[2], tr[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       g[h] = row0 + fr + 8 * h;
-      locate_row(g[h] < rows ? g[h] : 0, N, bb[h], nn[h]);
+      if (MODE != kMSG) locate_tile<MODE>(a, g[h] < rows ? g[h] : 0, tl[h], tr[h]);
     }
 
     if (MODE == kPCQ) {
@@ -181,8 +199,8 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
       // ---- Q image (pre-scaled weights and bias) ----
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        uint8_t* img = a.qimg + ((size_t)bb[h] * a.QT + (nn[h] >> 7)) * 65536;
-        const uint32_t r = (uint32_t)(nn[h] & 127);
+        uint8_t* img = a.qimg + (size_t)tl[h] * 65536;
+        const uint32_t r = (uint32_t)tr[h];
         uint32_t hi[16], lo[16];
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
@@ -206,8 +224,8 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
         const float* bvec = bias + 128 * step;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          uint8_t* img = a.kvimg + ((size_t)bb[h] * a.KT + (nn[h] >> 6)) * 65536 + 32768 * step;
-          const uint32_t r = (uint32_t)(nn[h] & 63);
+          uint8_t* img = a.kvimg + (size_t)tl[h] * 65536 + 32768 * step;
+          const uint32_t r = (uint32_t)tr[h];
           uint32_t hi[16], lo[16];
 #pragma unroll
           for (int j = 0; j < 16; ++j) {

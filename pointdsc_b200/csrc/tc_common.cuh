@@ -1,6 +1,7 @@
 // Shared definitions of the tensor-core kernels (encoder_tc.cu, knn_tc.cu).
 #pragma once
 #include "common.cuh"
+#include "sets.cuh"
 #include "tc_ptx.cuh"
 
 namespace pdsc {
@@ -17,8 +18,10 @@ constexpr float kQScale = 1.4426950408889634f / 11.313708498984761f;  // log2(e)
 enum ChainMode { kPCQ = 0, kKV = 1, kMSG = 2 };
 
 struct ChainArgs {
-  long long rows;        // B * N
-  int N, QT, KT, split;
+  long long rows;        // B * N, or the rows of a packed call
+  int N, QT, KT, split;  // uniform call: every set's N and its tiles
+  const SetDesc* sets;   // packed call: the descriptor table (row0, qt0, kt0), nullptr for a uniform call
+  int nsets;
   const float* in;       // [rows][128] fp32 A operand
   const float* res;      // MSG: feat1 (residual)
   float* out_f32;        // PCQ: feat1, MSG: feat

@@ -21,7 +21,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Dict, Iterable, Optional
+from typing import Dict, Iterable, List, Optional
 
 import torch
 import torch.nn as nn
@@ -278,6 +278,58 @@ class PointDSC(nn.Module):
                     lib.pdsc_forward_host_wait(self._engine, pending[0])
                 except Exception:
                     pass
+
+    @torch.no_grad()
+    def forward_many(self, batches: List[Dict[str, torch.Tensor]]) -> List[Dict[str, Optional[torch.Tensor]]]:
+        """Testing-mode forwards of several batches of DIFFERENT sizes in one engine call (pdsc_forward_packed).  Each element
+        is what `forward` accepts in testing mode (device tensors [bs_i, N_i, ...] and the 'testing' key); the result is, per
+        element, what `forward` returns for it.  All their sets are packed back to back into one mixed-size call, so a loop
+        over data of varying N pays one call's latency instead of one per pair.  Within one attention regime (DESIGN.md §3)
+        every set's result is bit-identical to that of a `forward` call holding it."""
+        dev = self._device()
+        sizes = []
+        for i, data in enumerate(batches):
+            if "testing" not in data.keys():
+                raise ValueError(f"forward_many runs the testing-mode forward: batch {i} has no 'testing' key")
+            cp, s, t = data["corr_pos"], data["src_keypts"], data["tgt_keypts"]
+            if cp.dim() != 3 or s.shape[:2] != cp.shape[:2] or t.shape != s.shape or s.shape[-1] != 3 \
+                    or cp.shape[-1] != self.in_dim:
+                raise ValueError(f"batch {i}: expected corr_pos [bs,N,{self.in_dim}] and src/tgt_keypts [bs,N,3], got "
+                                 f"{tuple(cp.shape)}, {tuple(s.shape)}, {tuple(t.shape)}")
+            if any(x.device.type != "cuda" or x.device != dev for x in (cp, s, t)):
+                raise ValueError(f"batch {i}: inputs must be device tensors on {dev} (got {cp.device}, {s.device}, {t.device})")
+            sizes.append((int(cp.shape[0]), int(cp.shape[1])))
+        if not batches:
+            return []
+        lib = self._ensure_engine()
+        counts = [n for bs, n in sizes for _ in range(bs)]
+        offsets = [0]
+        for n in counts:
+            offsets.append(offsets[-1] + n)
+        B = len(counts)
+        h_off = (C.c_int32 * (B + 1))(*offsets)
+        d_off = torch.tensor(offsets, dtype=torch.int32, device=dev)
+        cp, s, t = (torch.cat([d[key].to(torch.float32).reshape(-1, d[key].shape[-1]) for d in batches]).contiguous()
+                    for key in ("corr_pos", "src_keypts", "tgt_keypts"))
+        need = int(lib.pdsc_workspace_bytes_packed(self._engine, B, h_off))
+        if need == 0:
+            _capi.check(_capi.PDSC_ERR_SHAPE)
+        stream_handle = torch.cuda.current_stream(dev).cuda_stream
+        workspace = self._workspace_for(dev, need, stream_handle)
+        trans = torch.empty(B, 4, 4, dtype=torch.float32, device=dev)
+        labels = torch.empty(offsets[-1], dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _capi.check(lib.pdsc_forward_packed(self._engine, B, h_off, C.c_void_p(d_off.data_ptr()), C.c_void_p(cp.data_ptr()),
+                                                C.c_void_p(s.data_ptr()), C.c_void_p(t.data_ptr()),
+                                                C.c_void_p(trans.data_ptr()), C.c_void_p(labels.data_ptr()),
+                                                C.c_void_p(workspace.data_ptr()), workspace.numel(),
+                                                C.c_void_p(stream_handle)))
+        out, set0, row0 = [], 0, 0
+        for bs, n in sizes:
+            out.append({"final_trans": trans[set0:set0 + bs], "final_labels": labels[row0:row0 + bs * n].view(bs, n), "M": None})
+            set0 += bs
+            row0 += bs * n
+        return out
 
     def _workspace_for(self, dev, need: int, stream_handle: int) -> torch.Tensor:
         ws = self._workspaces.get(stream_handle)

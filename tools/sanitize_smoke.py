@@ -25,6 +25,9 @@ for k, n, b in ((40, 300, 3), (80, 257, 2)):
           "testing": True}
     streamed = list(m.forward_stream(hd for _ in range(3)))      # pdsc_forward_host_submit / _wait, two calls in flight
     assert all(torch.equal(o["final_trans"], host["final_trans"]) for o in streamed)
+    mixed = [bench.make_inputs(nn, 1, "3dmatch", 0) for nn in (n, 41, 7, 130)]   # pdsc_forward_packed, sets of four sizes
+    many = m.forward_many([{**{x: q[x].cuda() for x in ("corr_pos", "src_keypts", "tgt_keypts")}, "testing": True} for q in mixed])
+    assert [tuple(o["final_labels"].shape) for o in many] == [(1, n), (1, 41), (1, 7), (1, 130)]
 g = torch.Generator().manual_seed(0)
 for dt in (torch.float32, torch.float64):
     sd = torch.nn.functional.normalize(torch.randn(301, 33, generator=g, dtype=dt), dim=1).cuda()
