@@ -51,19 +51,27 @@ __device__ __forceinline__ Vec3 any_perpendicular(Vec3 a) {
 
 // H row-major (H[i*3+j] = sum_n w_n Am[n][i] Bm[n][j]); writes R row-major with  b ~= R a.
 __device__ __forceinline__ void kabsch_rotation(const float* H, float* R) {
-  // scale to O(1) so the squared norms stay well inside fp32 range; R is scale invariant
+  // scale to O(1) so the squared norms stay well inside fp32 range; R is scale invariant.  First by 2^-ilogb(hmax), which is
+  // exact (subnormal H included) and leaves the largest entry in [1, 2), then by the reciprocal of that entry.  Dividing by
+  // hmax itself overflows to +Inf for hmax below 2^-128 (0 * Inf = NaN).  In this order every scaled entry equals
+  // H[i] * (1 / hmax) bit for bit wherever both are normal floats, and R is bit-identical for H and 2^e H.
   float hmax = 0.f;
+  bool nan = false;   // fmaxf returns the other operand of a NaN: hmax alone would not see one
 #pragma unroll
-  for (int i = 0; i < 9; ++i) hmax = fmaxf(hmax, fabsf(H[i]));
-  if (!(hmax > 0.f) || !isfinite(hmax)) {
+  for (int i = 0; i < 9; ++i) {
+    hmax = fmaxf(hmax, fabsf(H[i]));
+    nan = nan || isnan(H[i]);
+  }
+  if (nan || !(hmax > 0.f) || !isfinite(hmax)) {
     // H == 0 (or non-finite): LAPACK returns U = V = I for a zero matrix -> R = I
     R[0] = 1.f; R[1] = 0.f; R[2] = 0.f; R[3] = 0.f; R[4] = 1.f; R[5] = 0.f; R[6] = 0.f; R[7] = 0.f; R[8] = 1.f;
     return;
   }
-  const float inv = 1.0f / hmax;
-  Vec3 g0 = {H[0] * inv, H[3] * inv, H[6] * inv};   // columns of H
-  Vec3 g1 = {H[1] * inv, H[4] * inv, H[7] * inv};
-  Vec3 g2 = {H[2] * inv, H[5] * inv, H[8] * inv};
+  const int e = -ilogbf(hmax);
+  const float inv = 1.0f / scalbnf(hmax, e);
+  Vec3 g0 = {scalbnf(H[0], e) * inv, scalbnf(H[3], e) * inv, scalbnf(H[6], e) * inv};   // columns of H
+  Vec3 g1 = {scalbnf(H[1], e) * inv, scalbnf(H[4], e) * inv, scalbnf(H[7], e) * inv};
+  Vec3 g2 = {scalbnf(H[2], e) * inv, scalbnf(H[5], e) * inv, scalbnf(H[8], e) * inv};
   Vec3 v0 = {1.f, 0.f, 0.f}, v1 = {0.f, 1.f, 0.f}, v2 = {0.f, 0.f, 1.f};
 #pragma unroll 1
   for (int sweep = 0; sweep < 8; ++sweep) {
