@@ -136,6 +136,7 @@ int pdsc_forward(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr_pos, 
                  const pdsc_stage_io* io, void* d_workspace, size_t workspace_bytes, void* cuda_stream);
 
 /* ---- the path over sets of different sizes (testing mode) -------------------------------------------
+ * pdsc_forward(e, B, N, ...) is this call with offsets b * N (the engine builds the same per-set table for both).
  * B sets, set b owning rows [offsets[b], offsets[b+1]) of the packed inputs; offsets has B + 1 entries, offsets[0] = 0,
  * R = offsets[B].  d_corr_pos [R,6], d_src_keypts [R,3], d_tgt_keypts [R,3]  ->  d_final_trans [B,4,4],
  * d_final_labels [R].  h_offsets (host) sizes the launches and the workspace; d_offsets (device, caller-owned, the same

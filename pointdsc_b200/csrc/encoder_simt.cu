@@ -28,7 +28,7 @@ __global__ void __launch_bounds__(256) linear_simt_kernel(LinearArgs a) {
   const float* W = a.W + (size_t)bz * a.strideW;
   float* out = a.out + (size_t)bz * a.strideO;
   const int m0 = blockIdx.y * LBM, n0 = blockIdx.x * LBN;
-  if (a.sets) {          // seed-row distances of set bz of a packed call; the grid is sized by the largest set
+  if (a.epi == 1) {      // seed-row distances of set bz; the grid is sized by the largest set
     const SetDesc d = a.sets[bz];
     A = a.A + (size_t)d.seed0 * a.lda;
     W = a.W + (size_t)d.row0 * a.ldw;
@@ -153,16 +153,16 @@ constexpr int kAttnSmem = (kC * AQ + kC * AK + AK * kC + AQ * AK) * (int)sizeof(
 
 __global__ void __launch_bounds__(256) attention_simt_kernel(const float* __restrict__ Q, const float* __restrict__ K,
                                                              const float* __restrict__ V, const float* __restrict__ SC,
-                                                             float* __restrict__ MSG, SetTable sets) {
+                                                             float* __restrict__ MSG, const SetDesc* __restrict__ sets) {
   extern __shared__ __align__(16) float smem[];
   float* Qs = smem;                 // [C][AQ]   Qs[c][q]
   float* Ks = Qs + kC * AQ;         // [C][AK]   Ks[c][key]
   float* Vs = Ks + kC * AK;         // [AK][C]   Vs[key][c]
   float* Ps = Vs + AK * kC;         // [AQ][AK]  Ps[q][key]
   const int b = blockIdx.y, q0 = blockIdx.x * AQ;
-  const SetDesc d = set_desc(sets, b);
+  const SetDesc d = sets[b];
   const int N = d.N, NS = round_up(N, 64);
-  if (q0 >= N) return;                 // a packed call's grid is sized by its largest set
+  if (q0 >= N) return;                 // the grid is sized by the largest set
   const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
   const size_t base = (size_t)d.row0;
   SC += d.sc0;
@@ -288,7 +288,7 @@ void launch_attention_simt(const float* q, const float* k, const float* v, const
                            cudaStream_t st, const SetDesc* sets) {
   ensure_dynamic_smem(reinterpret_cast<const void*>(attention_simt_kernel), kAttnSmem);
   dim3 grid((N + AQ - 1) / AQ, B);
-  attention_simt_kernel<<<grid, 256, kAttnSmem, st>>>(q, k, v, sc, msg, SetTable{sets, N, 0, 0, 0, 1, 0});
+  attention_simt_kernel<<<grid, 256, kAttnSmem, st>>>(q, k, v, sc, msg, sets);
 }
 
 }  // namespace pdsc

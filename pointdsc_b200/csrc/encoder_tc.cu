@@ -111,37 +111,21 @@ void tc_free_weights(TcWeights* w) {
 }
 
 static inline int q_tiles(int N) { return (N + 127) / 128; }
-static inline int k_tiles(int N) { return (N + 63) / 64; }
 
 // key split of the attention (small calls): at most this many work items, each with a 64 KB partial O and 1 KB of (m, l)
 constexpr int kAttnSplitMaxItems = 320;
 constexpr size_t kAttnSplitBytes = (size_t)kAttnSplitMaxItems * (65536 + 1024);
 
-size_t tc_scratch_bytes(int B, int N) { return tc_scratch_bytes_tiles((long long)B * q_tiles(N), (long long)B * k_tiles(N)); }
 size_t tc_scratch_bytes_tiles(long long qtiles, long long ktiles) {
   return ((size_t)qtiles + (size_t)ktiles) * 65536 + 1024 + kAttnSplitBytes;
 }
 
-// Key split policy.  When a call's (set, query tile) items cover less than half of the SMs (the evaluation loops' bs = 1:
-// 8 items at N = 1000, 40 at N = 5000), every item is split along the keys into chunks of TS tiles, TS a function of N ONLY
-// (attn_set_split, sets.cuh): calls of the small regime therefore agree bit for bit whatever their batch size, and so do calls
-// of the large regime (no split); across the two regimes the softmax sums are associated differently (fp32 rounding, far
-// inside the parity bar).  A call whose split would exceed kAttnSplitMaxItems work items is not split.
-static void attn_split_policy(int B, int N, int num_sms, int* splits, int* TS) {
-  const int QT = q_tiles(N);
-  *splits = 1;
-  *TS = k_tiles(N);
-  if (2 * B * QT > num_sms) return;
-  int sp, ts;
-  attn_set_split(N, num_sms, &sp, &ts);
-  if (sp < 2 || B * QT * sp > kAttnSplitMaxItems) return;
-  *splits = sp;
-  *TS = ts;
-}
-
-// The same policy for a packed call: the call is in the split regime when its query tiles cover at most half of the SMs;
-// each set is then split as attn_set_split says for its N, unless the whole call would exceed kAttnSplitMaxItems items.
-// An equal-N call gets exactly attn_split_policy's decision.
+// Key split policy.  When a call's (set, query tile) items cover at most half of the SMs (the evaluation loops' bs = 1:
+// 8 items at N = 1000, 40 at N = 5000), the call is in the split regime: each set's items are split along the keys into sp
+// chunks of TS tiles, sp and TS a function of the set's N ONLY (attn_set_split, sets.cuh).  Calls of the small regime therefore
+// agree bit for bit whatever their batch size, and so do calls of the large regime (no split); across the two regimes the
+// softmax sums are associated differently (fp32 rounding, far inside the parity bar).  A call whose split would exceed
+// kAttnSplitMaxItems work items, or in which no set would split, is not split.
 int tc_packed_split(const int* Ns, int B, int* items) {
   const int num_sms = device_sm_count();
   long long qtiles = 0, split_items = 0;
@@ -156,16 +140,14 @@ int tc_packed_split(const int* Ns, int B, int* items) {
   return split ? 1 : 0;
 }
 
-int tc_launches(int num_layers, int B, int N) {   // layer0 + pad clear + 4 per layer (+ the merge of a key-split attention)
-  int splits, ts;
-  attn_split_policy(B, N, device_sm_count(), &splits, &ts);
-  return 2 + (splits > 1 ? 5 : 4) * num_layers;
+int tc_launches(int num_layers, int attn_split) {   // layer0 + pad clear + 4 per layer (+ the merge of a key-split attention)
+  return 2 + (attn_split ? 5 : 4) * num_layers;
 }
 
 // ---- zero the never-written pad rows/columns of the last key tile of every set ---------------------------
-__global__ void tc_clear_pads_kernel(uint8_t* kvimg, SetTable sets) {
+__global__ void tc_clear_pads_kernel(uint8_t* kvimg, const SetDesc* __restrict__ sets) {
   const int b = blockIdx.x;
-  const SetDesc d = set_desc(sets, b);
+  const SetDesc d = sets[b];
   const int first_pad = d.N & 63;
   if (first_pad == 0) return;
   uint8_t* base = kvimg + ((size_t)d.kt0 + (d.N + 63) / 64 - 1) * 65536;
@@ -181,20 +163,21 @@ __global__ void tc_clear_pads_kernel(uint8_t* kvimg, SetTable sets) {
   }
 }
 
-// ---- debug: decode operand images back to fp32 [B*N][128] -------------------------------------------------
+// ---- debug: decode operand images back to fp32 [rows][128] -------------------------------------------------
 template <int FMT>
 __global__ void tc_decode_kernel(const uint8_t* qimg, const uint8_t* kvimg, float* q, float* k, float* v, long long rows,
-                                 int N, int QT, int KT, int split) {
+                                 const SetDesc* __restrict__ sets, int nsets, int split) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long row = idx / kC;
   const uint32_t c = (uint32_t)(idx % kC);
   if (row >= rows) return;
-  const int b = (int)(row / N), n = (int)(row % N);
+  const SetDesc d = sets[find_set(nsets, row, [&](int i) { return sets[i].row0; })];
+  const int n = (int)(row - d.row0);
   auto rd = [](const uint8_t* p) { return from_16<FMT>(*reinterpret_cast<const uint16_t*>(p)); };
-  const uint8_t* qb = qimg + ((size_t)b * QT + (n >> 7)) * 65536;
+  const uint8_t* qb = qimg + ((size_t)d.qt0 + (n >> 7)) * 65536;
   const uint32_t qo = (c >> 6) * 16384u + sw128_offset((uint32_t)(n & 127), c & 63u);
   q[idx] = rd(qb + qo) + (split ? rd(qb + 32768 + qo) : 0.f);
-  const uint8_t* kb = kvimg + ((size_t)b * KT + (n >> 6)) * 65536;
+  const uint8_t* kb = kvimg + ((size_t)d.kt0 + (n >> 6)) * 65536;
   const uint32_t ko = (c >> 6) * 8192u + sw128_offset((uint32_t)(n & 63), c & 63u);
   k[idx] = rd(kb + ko) + (split ? rd(kb + 16384 + ko) : 0.f);
   v[idx] = rd(kb + 32768 + ko) + (split ? rd(kb + 49152 + ko) : 0.f);
@@ -224,16 +207,12 @@ static cudaError_t tc_configure_fmt() {
 
 template <int FMT>
 static int tc_encoder_forward_fmt(const TcWeights& w, const TcForwardArgs& a, cudaStream_t st) {
-  const bool packed = a.sets != nullptr;
-  const long long rows = packed ? a.rows : (long long)a.B * a.N;
+  const long long rows = a.rows;
   if (rows >= (1LL << 31)) return (int)cudaErrorInvalidValue;  // kernels index rows with 32-bit arithmetic
-  const int QT = q_tiles(a.N), KT = k_tiles(a.N);
-  const long long qtiles = packed ? a.qtiles : (long long)a.B * QT;
-  const long long ktiles = packed ? a.ktiles : (long long)a.B * KT;
   uint8_t* qimg = static_cast<uint8_t*>(a.scratch);
   qimg = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(qimg) + 1023) & ~uintptr_t(1023));
-  uint8_t* kvimg = qimg + (size_t)qtiles * 65536;
-  float* part_o = reinterpret_cast<float*>(kvimg + (size_t)ktiles * 65536);
+  uint8_t* kvimg = qimg + (size_t)a.qtiles * 65536;
+  float* part_o = reinterpret_cast<float*>(kvimg + (size_t)a.ktiles * 65536);
   float* part_ml = part_o + (size_t)kAttnSplitMaxItems * 128 * kC;
   const long long tiles = (rows + 127) / 128;
   const int num_sms = device_sm_count();
@@ -242,20 +221,12 @@ static int tc_encoder_forward_fmt(const TcWeights& w, const TcForwardArgs& a, cu
   const uint8_t* arena = static_cast<const uint8_t*>(w.arena) + (size_t)FMT * w.num_layers * kLayerBytes;
 
   launch_layer0(a.corr_pos, a.l0w, a.l0b, a.feat, rows, a.in_dim, st);
-  tc_clear_pads_kernel<<<a.B, 256, 0, st>>>(kvimg, SetTable{a.sets, a.N, 0, 0, 1, 1, 0});
-  int splits = 1, ts = KT, items = 0;
-  if (packed) {
-    items = a.attn_items;
-    splits = a.attn_split ? 2 : 1;     // > 1: some sets are split (their merge runs per query tile)
-  } else {
-    attn_split_policy(a.B, a.N, num_sms, &splits, &ts);
-    items = a.B * QT * splits;
-  }
+  tc_clear_pads_kernel<<<a.nsets, 256, 0, st>>>(kvimg, a.sets);
   for (int l = 0; l < a.num_layers; ++l) {
     const uint8_t* base = arena + (size_t)l * kLayerBytes;
     ChainArgs c{};
-    c.rows = rows; c.N = a.N; c.QT = QT; c.KT = KT; c.split = a.split;
-    c.sets = a.sets; c.nsets = a.B;
+    c.rows = rows; c.split = a.split;
+    c.sets = a.sets; c.tile_set = a.tile_set; c.nsets = a.nsets;
     c.qimg = qimg; c.kvimg = kvimg; c.bias = reinterpret_cast<const float*>(base + kBias);
     // PointCN + Q
     c.in = a.feat; c.res = nullptr; c.out_f32 = a.feat1; c.wimg = base + kW1; c.wbytes = 131072;
@@ -264,20 +235,17 @@ static int tc_encoder_forward_fmt(const TcWeights& w, const TcForwardArgs& a, cu
     c.in = a.feat1; c.out_f32 = nullptr; c.wimg = base + kWk; c.wbytes = 131072;
     tc_chain_kernel<kKV, FMT><<<grid, kChainThreads, kChainSmem, st>>>(c);
     // attention
-    AttnArgs at{a.N, a.NS, QT, KT, a.split, qimg, kvimg, a.sc, a.msg, items, splits, ts, part_o, part_ml, a.sets, a.B};
+    const AttnArgs at{a.split, qimg, kvimg, a.sc, a.msg, a.attn_items, part_o, part_ml, a.sets, a.nsets};
     if (a.attn_events) cudaEventRecord(a.attn_events[2 * l], st);
-    {
-      const int items = at.items;
-      tc_attention_persistent_kernel<FMT><<<items < num_sms ? items : num_sms, kAttnThreads, kAttnPSmem, st>>>(at);
-      if (splits > 1)
-        tc_attention_merge_kernel<<<(unsigned)(qtiles * 4), 256, 0, st>>>(part_o, part_ml, a.msg, a.N, QT, splits, a.sets, a.B);
-    }
+    tc_attention_persistent_kernel<FMT><<<at.items < num_sms ? at.items : num_sms, kAttnThreads, kAttnPSmem, st>>>(at);
+    if (a.attn_split)   // some sets are split: their merge runs per query tile
+      tc_attention_merge_kernel<<<(unsigned)(a.qtiles * 4), 256, 0, st>>>(part_o, part_ml, a.msg, a.sets, a.nsets);
     if (a.attn_events) cudaEventRecord(a.attn_events[2 * l + 1], st);
     if (a.debug_out && a.debug_layer == l) {
       const size_t plane = (size_t)rows * kC;
       tc_unblock_f32_kernel<<<(unsigned)((plane / 4 + 255) / 256), 256, 0, st>>>(a.feat1, a.debug_out, rows);
       tc_decode_kernel<FMT><<<(unsigned)((plane + 255) / 256), 256, 0, st>>>(qimg, kvimg, a.debug_out + plane, a.debug_out + 2 * plane,
-                                                                             a.debug_out + 3 * plane, rows, a.N, QT, KT, a.split);
+                                                                             a.debug_out + 3 * plane, rows, a.sets, a.nsets, a.split);
       cudaMemcpyAsync(a.debug_out + 4 * plane, a.msg, plane * sizeof(float), cudaMemcpyDeviceToDevice, st);
     }
     // fc_message + residual

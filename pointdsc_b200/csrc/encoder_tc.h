@@ -21,24 +21,23 @@ struct TcWeights {
 };
 
 struct TcForwardArgs {
-  int B, N, NS, in_dim, num_layers;
+  int nsets, in_dim, num_layers;
   int split;                 // 1: hi/lo operand split (3 products)   0: single 16-bit operands
   int fmt;                   // operand format of the kind::f16 MMAs: 0 = fp16, 1 = bf16
-  const float* corr_pos;     // [B*N][in_dim]
+  const float* corr_pos;     // [rows][in_dim]
   const float *l0w, *l0b;    // layer0 weights (fp32, device)
-  const float* sc;           // [B][N][NS]
-  float* feat;               // [B*N][128]  layer output / final features
-  float* feat1;              // [B*N][128]  PointCN output (residual source)
-  float* msg;                // [B*N][128]  attention output
-  void* scratch;             // tc_scratch_bytes(B, N)
+  const float* sc;           // tiled SC blocks of the sets (SetDesc::sc0)
+  float* feat;               // [rows][128]  layer output / final features
+  float* feat1;              // [rows][128]  PointCN output (residual source)
+  float* msg;                // [rows][128]  attention output
+  void* scratch;             // tc_scratch_bytes_tiles(qtiles, ktiles)
   int layer_tap;             // -1 or layer index to copy out
   float* layer_tap_out;
   int debug_layer;           // layer whose internals are decoded into debug_out
-  float* debug_out;          // [5][B*N][128]: feat1, q (scaled by log2e/sqrt(C)), k, v, msg — or nullptr
-  long long* timeline;       // not written by the wgmma kernels (kept for the C ABI)
+  float* debug_out;          // [5][rows][128]: feat1, q (scaled by log2e/sqrt(C)), k, v, msg — or nullptr
   cudaEvent_t* attn_events;  // nullptr or 2 events per layer, recorded around the attention launch
-  // packed call (pdsc_forward_packed): the descriptor table; B is the number of sets and N the largest of them
-  const SetDesc* sets;       // nullptr: uniform call
+  const SetDesc* sets;       // the call's descriptor table (sets.cuh), nsets entries
+  const int* tile_set;       // the set of the first row of every 128-row tile of the call's rows
   long long rows;            // rows of the call
   long long qtiles, ktiles;  // query / key tiles of all sets
   int attn_items;            // attention work items (tc_packed_split)
@@ -47,11 +46,10 @@ struct TcForwardArgs {
 
 int tc_build_weights(const TcLayerHost* layers, int num_layers, TcWeights* out);  // returns cudaError_t
 void tc_free_weights(TcWeights* w);
-size_t tc_scratch_bytes(int B, int N);
 size_t tc_scratch_bytes_tiles(long long qtiles, long long ktiles);
-// key-split decision of a packed call of sets of Ns[0..B) rows: returns 1 in the split regime; *items = attention work items
+// key-split decision of a call of sets of Ns[0..B) rows: returns 1 in the split regime; *items = attention work items
 int tc_packed_split(const int* Ns, int B, int* items);
-int tc_launches(int num_layers, int B, int N);
+int tc_launches(int num_layers, int attn_split);
 int tc_encoder_forward(const TcWeights& w, const TcForwardArgs& a, cudaStream_t st);  // returns cudaError_t
 
 }  // namespace pdsc

@@ -139,48 +139,34 @@ struct Workspace {
   int32_t *seeds, *knn, *counts;
   uint32_t* conv_mask;
   unsigned long long* best_key;
-  pdsc::SetDesc* sets;   // packed call: the descriptor table
+  pdsc::SetDesc* sets;   // the call's descriptor table
+  int32_t* tile_set;     // the set of the first row of every 128-row tile of the call's rows
   void* tc_scratch;
   size_t bytes;
 };
 
-// What a call needs to size its launches and its workspace.  A uniform call: B sets of N rows.  A packed call: B sets of
-// Ns[b] rows; N, S and k are then the largest of its sets (launch sizes) and the totals sum over the sets.
+// What a call needs to size its launches and its workspace: B sets of Ns[b] rows.  N, S and k are the largest of its sets
+// (launch sizes), k_min the smallest k of its sets with seeds, and the totals sum over the sets.
 struct CallShape {
   int B = 0, N = 0, S = 0, k = 0, k_min = 0;
-  bool packed = false;
   size_t R = 0;
   size_t sc_rowmajor = 0, sc_tiled = 0;   // floats of the row-major (fp32) and tiled (tensor-core) SC layouts
   size_t seeds = 0, dist = 0, knn = 0;    // seed slots, seed-row distance floats, neighbour slots
   long long qtiles = 0, ktiles = 0;
-  int attn_items = 0, attn_split = 0;     // packed tensor-core calls (tc_packed_split)
+  int attn_items = 0, attn_split = 0;     // tensor-core calls (tc_packed_split)
 };
 
-CallShape uniform_shape(const pdsc_engine* e, int B, int N) {
+// h_offsets: the validated offsets of a packed call, or nullptr for a uniform call of B sets of N rows
+CallShape call_shape(const pdsc_engine* e, int B, int N_uniform, const int32_t* h_offsets) {
   CallShape s;
-  s.B = B; s.N = N;
-  s.S = pdsc_num_seeds(e, N); s.k = s.k_min = pdsc_num_neighbours(e, N);
-  s.R = (size_t)B * N;
-  s.sc_rowmajor = s.R * pdsc::round_up(N, 64);
-  s.sc_tiled = (size_t)B * ((N + 63) / 64) * ((N + 127) / 128) * 8192;
-  s.seeds = (size_t)B * s.S;
-  s.dist = (size_t)B * s.S * N;
-  s.knn = (size_t)B * s.S * s.k;
-  s.qtiles = (long long)B * ((N + 127) / 128);
-  s.ktiles = (long long)B * ((N + 63) / 64);
-  return s;
-}
-
-// h_offsets[0..B] already validated
-CallShape packed_shape(const pdsc_engine* e, int B, const int32_t* h_offsets) {
-  CallShape s;
-  s.B = B; s.packed = true;
+  s.B = B;
   s.k_min = e->cfg.k;
   std::vector<int> Ns(B);
   for (int b = 0; b < B; ++b) {
-    const int N = h_offsets[b + 1] - h_offsets[b];
+    const int N = h_offsets ? h_offsets[b + 1] - h_offsets[b] : N_uniform;
     const int S = pdsc_num_seeds(e, N), k = pdsc_num_neighbours(e, N);
     Ns[b] = N;
+    s.R += (size_t)N;
     s.N = std::max(s.N, N); s.S = std::max(s.S, S); s.k = std::max(s.k, k);
     if (S > 0) s.k_min = std::min(s.k_min, k);
     s.sc_rowmajor += (size_t)N * pdsc::round_up(N, 64);
@@ -191,7 +177,6 @@ CallShape packed_shape(const pdsc_engine* e, int B, const int32_t* h_offsets) {
     s.qtiles += (N + 127) / 128;
     s.ktiles += (N + 63) / 64;
   }
-  s.R = (size_t)h_offsets[B];
   if (e->cfg.precision != PDSC_FP32_SIMT) s.attn_split = pdsc::tc_packed_split(Ns.data(), B, &s.attn_items);
   return s;
 }
@@ -228,7 +213,8 @@ Workspace carve(const pdsc_engine* e, void* ptr, const CallShape& sh) {
   w.counts = c.take<int32_t>(sh.seeds + 1);
   w.conv_mask = c.take<uint32_t>(B);
   w.best_key = c.take<unsigned long long>(B);
-  w.sets = sh.packed ? c.take<pdsc::SetDesc>(B) : nullptr;
+  w.sets = c.take<pdsc::SetDesc>(B);
+  w.tile_set = c.take<int32_t>((R + 127) / 128);
   w.bytes = (c.off + 255) & ~size_t(255);
   return w;
 }
@@ -322,8 +308,10 @@ int encoder_simt(const pdsc_engine* e, const Workspace& w, const CallShape& sh, 
   return PDSC_OK;
 }
 
-// Descriptor table of a packed call, from the device copy of its offsets: one warp walks the sets 32 at a time and forms
-// every running offset (tiles, seeds, attention items, SC / distance / neighbour blocks) by warp-wide inclusive scans.
+// Descriptor table of a call, from the device copy of a packed call's offsets, or (offsets == nullptr) for B sets of N_uniform
+// rows: one warp walks the sets 32 at a time and forms every running offset (tiles, seeds, attention items, SC / distance /
+// neighbour blocks) by warp-wide inclusive scans, and records the set of the first row of every 128-row tile (tc_chain.cuh).  A
+// uniform call therefore needs no host-to-device copy.
 __device__ __forceinline__ long long warp_scan_incl(long long v, int lane) {
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
@@ -333,15 +321,18 @@ __device__ __forceinline__ long long warp_scan_incl(long long v, int lane) {
   return v;
 }
 
-__global__ void set_table_kernel(const int32_t* __restrict__ offsets, int B, double ratio, int k_cfg, int tiled, int split,
-                                 int num_sms, pdsc::SetDesc* __restrict__ table) {
+__global__ void set_table_kernel(const int32_t* __restrict__ offsets, int N_uniform, int B, double ratio, int k_cfg, int tiled,
+                                 int split, int num_sms, pdsc::SetDesc* __restrict__ table, int32_t* __restrict__ tile_set) {
   const int lane = threadIdx.x;
   long long base[7] = {0, 0, 0, 0, 0, 0, 0};   // qt0, kt0, seed0, item0, sc0, dist0, knn0
   for (int b0 = 0; b0 < B; b0 += 32) {
     const int b = b0 + lane;
     const bool live = b < B;
-    const int row0 = live ? offsets[b] : 0;
-    const int N = live ? offsets[b + 1] - row0 : 0;
+    int row0 = 0, N = 0;
+    if (live) {
+      row0 = offsets ? offsets[b] : b * N_uniform;
+      N = offsets ? offsets[b + 1] - row0 : N_uniform;
+    }
     const int S = (int)((double)N * ratio);          // int(num_corr * self.ratio), as pdsc_num_seeds
     const int k = live ? max(min(k_cfg, N - 1), 0) : 0;
     const int QT = (N + 127) / 128, KT = (N + 63) / 64;
@@ -364,6 +355,7 @@ __global__ void set_table_kernel(const int32_t* __restrict__ offsets, int B, dou
       d.sp = sp; d.TS = TS; d.pad0 = d.pad1 = 0;
       d.sc0 = first[4]; d.dist0 = first[5]; d.knn0 = first[6];
       table[b] = d;
+      for (long long t = (row0 + 127) / 128; t * 128 < (long long)row0 + N; ++t) tile_set[t] = b;
     }
   }
 }
@@ -521,15 +513,17 @@ int32_t pdsc_num_neighbours(const pdsc_engine* e, int32_t N) {
 
 size_t pdsc_workspace_bytes(const pdsc_engine* e, int32_t B, int32_t N) {
   if (!e || B <= 0 || N <= 0) return 0;
-  return carve(e, nullptr, uniform_shape(e, B, N)).bytes;
+  DeviceGuard g(e->cfg.device);
+  return carve(e, nullptr, call_shape(e, B, N, nullptr)).bytes;
 }
 
 int32_t pdsc_launches_per_forward(const pdsc_engine* e, int32_t B, int32_t N) {
-  if (!e) return 0;
+  if (!e || B <= 0 || N <= 0) return 0;
+  DeviceGuard g(e->cfg.device);
   const int L = e->cfg.num_layers;
-  const int enc = (e->cfg.precision == PDSC_FP32_SIMT) ? (1 + 8 * L) : pdsc::tc_launches(L, B, N);
-  // sc, encoder, head, nms, sort, (gather +) dist gemm, knn select, 2 fills, nsm, hypotheses, refine
-  return 1 + enc + 1 + 2 + ((e->cfg.precision == PDSC_FP32_SIMT) ? 3 : 2) + 2 + 3;
+  const int enc = (e->cfg.precision == PDSC_FP32_SIMT) ? (1 + 8 * L) : pdsc::tc_launches(L, call_shape(e, B, N, nullptr).attn_split);
+  // set table, sc, encoder, head, nms, sort, (gather +) dist gemm, knn select, 2 fills, nsm, hypotheses, refine
+  return 2 + enc + 1 + 2 + ((e->cfg.precision == PDSC_FP32_SIMT) ? 3 : 2) + 2 + 3;
 }
 
 // mode 0: testing (PointDSC.py: NMS seeds, per-set early exit, labels = inlier mask, post-refinement)
@@ -553,7 +547,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
   if (!inject_feat && !d_corr_pos) return fail(PDSC_ERR_INVALID_ARGUMENT, "corr_pos is null");
   if (io && io->in_confidence && !inject_feat) return fail(PDSC_ERR_INVALID_ARGUMENT, "in_confidence requires in_features");
   DeviceGuard g(e->cfg.device);   // tc_packed_split reads the SM count of the engine's device
-  const CallShape sh = h_offsets ? packed_shape(e, B, h_offsets) : uniform_shape(e, B, N);
+  const CallShape sh = call_shape(e, B, N, h_offsets);
   const size_t need = carve(e, nullptr, sh).bytes;
   if (!d_workspace || workspace_bytes < need)
     return fail(PDSC_ERR_WORKSPACE, "workspace too small: %zu bytes given, %zu needed", workspace_bytes, need);
@@ -564,10 +558,9 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
   const size_t R = sh.R;
   const int NS = round_up(N, 64);
   const int S = sh.S, k = sh.k, T = e->cfg.num_iterations;
-  const SetDesc* sets = w.sets;    // nullptr: uniform call
-  if (sets)
-    set_table_kernel<<<1, 32, 0, st>>>(d_offsets, B, (double)e->cfg.ratio, e->cfg.k, e->cfg.precision == PDSC_FP32_SIMT ? 0 : 1,
-                                       sh.attn_split, device_sm_count(), w.sets);
+  const SetDesc* sets = w.sets;
+  set_table_kernel<<<1, 32, 0, st>>>(d_offsets, N, B, (double)e->cfg.ratio, e->cfg.k, e->cfg.precision == PDSC_FP32_SIMT ? 0 : 1,
+                                     sh.attn_split, device_sm_count(), w.sets, w.tile_set);
   const float* W = e->d_weights;
   const int L = e->cfg.num_layers;
   cudaEvent_t* attn_ev = nullptr;
@@ -602,7 +595,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
       if (rc) return rc;
     } else {
       TcForwardArgs a{};
-      a.B = B; a.N = N; a.NS = NS; a.in_dim = e->cfg.in_dim; a.num_layers = e->cfg.num_layers;
+      a.nsets = B; a.in_dim = e->cfg.in_dim; a.num_layers = e->cfg.num_layers;
       a.split = (e->cfg.precision == PDSC_BF16X3 || e->cfg.precision == PDSC_FP16X3) ? 1 : 0;
       a.fmt = (e->cfg.precision == PDSC_FP16X3) ? 0 : 1;
       a.corr_pos = d_corr_pos; a.l0w = W + e->off_l0w; a.l0b = W + e->off_l0b;
@@ -612,9 +605,8 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
       a.debug_layer = io ? io->layer_tap : -1;
       a.debug_out = io ? io->out_layer_debug : nullptr;
       a.attn_events = attn_ev;
-      a.sets = sets; a.rows = (long long)R; a.qtiles = sh.qtiles; a.ktiles = sh.ktiles;
+      a.sets = sets; a.tile_set = w.tile_set; a.rows = (long long)R; a.qtiles = sh.qtiles; a.ktiles = sh.ktiles;
       a.attn_items = sh.attn_items; a.attn_split = sh.attn_split;
-      a.timeline = io ? reinterpret_cast<long long*>(io->out_timeline) : nullptr;
       const int rc = tc_encoder_forward(e->tc, a, st);
       if (rc) return fail(PDSC_ERR_CUDA, "tensor-core encoder launch failed: %s", cudaGetErrorString((cudaError_t)rc));
     }
@@ -643,7 +635,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
     else if (mode == 0)
       launch_pick_seeds(d_src, w.conf, w.seeds, w.key, B, N, S, e->cfg.nms_radius, st, sets);
     else
-      launch_top_seeds(w.conf, w.seeds, B, N, S, st);
+      launch_top_seeds(w.conf, w.seeds, B, N, S, st, sets);
     if (io) copy_tap(io->out_seeds, w.seeds, (size_t)B * S * sizeof(int32_t), st);
     mark(4);
 
@@ -653,11 +645,10 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
     } else {
       if (e->cfg.precision == PDSC_FP32_SIMT) {
         launch_gather_rows(w.normed, w.seeds, w.seedfeat, B, N, S, st, sets);
-        LinearArgs a{};
-        a.A = w.seedfeat; a.strideA = (long long)S * kC; a.lda = kC;
-        a.W = w.normed; a.strideW = (long long)N * kC; a.ldw = kC;
-        a.bias = nullptr; a.res = nullptr; a.ldres = 0;
-        a.out = w.dist; a.strideO = (long long)S * N; a.ldo = N;
+        LinearArgs a{};   // epi 1: every set's operands and distance block come from the table
+        a.A = w.seedfeat; a.lda = kC;
+        a.W = w.normed; a.ldw = kC;
+        a.out = w.dist; a.ldo = N;
         a.M = S; a.K = kC; a.Nout = N; a.relu = 0; a.epi = 1; a.batch = B;
         a.sets = sets;
         launch_linear_simt(a, st);
@@ -740,7 +731,7 @@ static int check_offsets(const pdsc_engine* e, int32_t B, const int32_t* h_offse
 size_t pdsc_workspace_bytes_packed(const pdsc_engine* e, int32_t B, const int32_t* h_offsets) {
   if (!e || check_offsets(e, B, h_offsets) != PDSC_OK) return 0;
   DeviceGuard g(e->cfg.device);
-  return carve(e, nullptr, packed_shape(e, B, h_offsets)).bytes;
+  return carve(e, nullptr, call_shape(e, B, 0, h_offsets)).bytes;
 }
 
 int pdsc_forward_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_corr_pos,

@@ -47,14 +47,14 @@ __device__ __forceinline__ void knn_stage_keys(uint8_t* Bs, const float* rows, i
 
 __global__ void __launch_bounds__(kKnnThreads, 1) knn_dist_tc_kernel(const float* __restrict__ normed,
                                                                      const int32_t* __restrict__ seeds,
-                                                                     float* __restrict__ dist, SetTable sets, int tiles_per_cta) {
+                                                                     float* __restrict__ dist, const SetDesc* __restrict__ sets, int tiles_per_cta) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t s0 = smem_u32(smem);
   const int tid = threadIdx.x, wg = tid >> 7, wt = tid & 127;
   const int b = blockIdx.y, s_base = blockIdx.x * 128;
-  const SetDesc sd = set_desc(sets, b);
+  const SetDesc sd = sets[b];
   const int N = sd.N, S = sd.S;
-  if (s_base >= S) return;                 // a packed call's grid is sized by its largest set
+  if (s_base >= S) return;                 // the grid is sized by the largest set
   // key tiles [t0, t0 + T) of this CTA: blockIdx.z splits the keys when seed-row tiles x sets alone would leave SMs idle
   const int t0 = blockIdx.z * tiles_per_cta;
   const int T = min(tiles_per_cta, (N + 63) / 64 - t0);
@@ -126,8 +126,7 @@ void launch_knn_dist_tc(const float* normed, const int32_t* seeds, float* dist, 
   if (chunks > T) chunks = T;
   const int per = (T + chunks - 1) / chunks;
   chunks = (T + per - 1) / per;
-  knn_dist_tc_kernel<<<dim3((S + 127) / 128, B, chunks), kKnnThreads, kKnnSmem, st>>>(normed, seeds, dist,
-                                                                                      SetTable{sets, N, S, 0, 1, 1, 0}, per);
+  knn_dist_tc_kernel<<<dim3((S + 127) / 128, B, chunks), kKnnThreads, kKnnSmem, st>>>(normed, seeds, dist, sets, per);
 }
 
 }  // namespace pdsc

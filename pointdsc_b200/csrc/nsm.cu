@@ -27,10 +27,10 @@ namespace pdsc {
 
 // ---- seed feature rows -----------------------------------------------------------------------------
 __global__ void gather_rows_kernel(const float* __restrict__ normed, const int32_t* __restrict__ seeds,
-                                   float* __restrict__ out, SetTable sets) {
+                                   float* __restrict__ out, const SetDesc* __restrict__ sets) {
   const int b = blockIdx.y, s = blockIdx.x, lane = threadIdx.x;
-  const SetDesc d = set_desc(sets, b);
-  if (s >= d.S) return;                    // a packed call's grid is sized by its largest set
+  const SetDesc d = sets[b];
+  if (s >= d.S) return;                    // the grid is sized by the largest set
   int idx = seeds[(size_t)d.seed0 + s];
   idx = min(max(idx, 0), d.N - 1);
   const float4 v = *reinterpret_cast<const float4*>(normed + ((size_t)d.row0 + idx) * kC + lane * 4);
@@ -39,7 +39,7 @@ __global__ void gather_rows_kernel(const float* __restrict__ normed, const int32
 void launch_gather_rows(const float* normed, const int32_t* seeds, float* out, int B, int N, int S, cudaStream_t st,
                         const SetDesc* sets) {
   if (S <= 0) return;
-  gather_rows_kernel<<<dim3(S, B), 32, 0, st>>>(normed, seeds, out, SetTable{sets, N, S, 0, 0, 1, 0});
+  gather_rows_kernel<<<dim3(S, B), 32, 0, st>>>(normed, seeds, out, sets);
 }
 
 // ---- top-(k+1) smallest per seed row ---------------------------------------------------------------
@@ -51,27 +51,21 @@ void launch_gather_rows(const float* normed, const int32_t* seeds, float* out, i
 // in ascending order.  Rank 0 (the seed itself, ignore_self) is dropped.  ~1.5 k instructions per row at N = 1000 instead
 // of the 6.5 k of k + 1 serial argmin rounds, and no register-resident copy of the row, so one kernel serves every N.
 
-// Packed calls: a warp finds its row's set by a binary search over the sets' first seed slots; the shared-memory slices are
-// laid out for the largest N and k of the call (NPmax, Pmax), the selection runs at the set's own N, k and P.
+// A warp finds its row's set by a binary search over the sets' first seed slots; the shared-memory slices are laid out for
+// the largest N and k of the call (NPmax, Pmax), the selection runs at the set's own N, k and P.
 __global__ void __launch_bounds__(256) knn_select_kernel(const float* __restrict__ dist, int32_t* __restrict__ knn_idx,
-                                                         SetTable sets, int nsets, int rows, int warps_per_cta, int NPmax,
-                                                         int Pmax) {
+                                                         const SetDesc* __restrict__ sets, int nsets, int rows, int warps_per_cta,
+                                                         int NPmax, int Pmax) {
   extern __shared__ __align__(16) unsigned char knn_smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int row = blockIdx.x * warps_per_cta + warp;
   if (row >= rows) return;                   // whole warps leave: no block-level barrier below
-  int N = sets.N, k = sets.k, P = Pmax;
-  const float* d = dist + (size_t)row * N;
-  int32_t* out = knn_idx + (size_t)row * k;
-  if (sets.d) {
-    const SetDesc sd = sets.d[find_set(nsets, row, [&](int b) { return sets.d[b].seed0; })];
-    const int s = row - sd.seed0;
-    N = sd.N;
-    k = sd.k;
-    for (P = 2; P < k + 1; P <<= 1) {}
-    d = dist + sd.dist0 + (size_t)s * N;
-    out = knn_idx + sd.knn0 + (size_t)s * k;
-  }
+  const SetDesc sd = sets[find_set(nsets, row, [&](int b) { return sets[b].seed0; })];
+  const int s = row - sd.seed0, N = sd.N, k = sd.k;
+  int P = 2;
+  while (P < k + 1) P <<= 1;
+  const float* d = dist + sd.dist0 + (size_t)s * N;
+  int32_t* out = knn_idx + sd.knn0 + (size_t)s * k;
   const int NP = (N + 31) & ~31;
   const size_t per_warp = (size_t)NPmax * 4 + 1024 + (size_t)Pmax * 8;
   unsigned char* base = knn_smem + (size_t)warp * per_warp;
@@ -109,7 +103,7 @@ __global__ void __launch_bounds__(256) knn_select_kernel(const float* __restrict
 void launch_knn_select(const float* dist, int32_t* knn_idx, int B, int N, int S, int k, cudaStream_t st,
                        const SetDesc* sets, int total_seeds) {
   if (S <= 0) return;
-  const int rows = sets ? total_seeds : B * S;
+  const int rows = total_seeds;
   int P = 2;
   while (P < k + 1) P <<= 1;
   const int NP = (N + 31) & ~31;
@@ -118,8 +112,7 @@ void launch_knn_select(const float* dist, int32_t* knn_idx, int B, int N, int S,
   warps = warps > 8 ? 8 : (warps < 1 ? 1 : warps);
   const int smem = (int)(per_warp * warps);
   ensure_dynamic_smem(reinterpret_cast<const void*>(knn_select_kernel), smem);
-  knn_select_kernel<<<(rows + warps - 1) / warps, warps * 32, smem, st>>>(dist, knn_idx, SetTable{sets, N, S, k, 0, 1, 0}, B, rows,
-                                                                           warps, NP, P);
+  knn_select_kernel<<<(rows + warps - 1) / warps, warps * 32, smem, st>>>(dist, knn_idx, sets, B, rows, warps, NP, P);
 }
 
 // ---- compatibility matrix + power iteration: one warp (k <= 40) or one 4-warp CTA (k > 40) per seed ----------------------
@@ -158,8 +151,8 @@ template <int WPS>
 __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
     const float* __restrict__ normed, const float* __restrict__ src, const float* __restrict__ tgt,
     const int32_t* __restrict__ knn_idx, float* __restrict__ iterates, uint32_t* __restrict__ conv_mask,
-    float* __restrict__ compat_out, SetTable sets, int k_lo, int k_hi, int iters, float sigma2, float sigmad2, int mask_stride,
-    int groups_per_cta, int per_group_floats) {
+    float* __restrict__ compat_out, const SetDesc* sets, int k_lo, int k_hi, int iters, float sigma2, float sigmad2,
+    int mask_stride, int groups_per_cta, int per_group_floats) {
   const float rc_sigma2 = 1.0f / sigma2, rc_sigmad2 = 1.0f / sigmad2;   // IEEE divisions (correctly rounded reciprocals)
   extern __shared__ __align__(16) float sm[];
   constexpr int TS = 32 * WPS;             // threads per seed
@@ -167,9 +160,9 @@ __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
   const int group = (WPS == 1) ? warp : 0;
   const int tg = (WPS == 1) ? lane : (int)threadIdx.x;      // thread index within the seed's group
   const int b = blockIdx.y;
-  const SetDesc d = set_desc(sets, b);
+  const SetDesc d = sets[b];
   const int N = d.N, S = d.S, k = d.k;
-  if (k < k_lo || k > k_hi) return;        // a packed call runs each kernel variant on the sets of its k range
+  if (k < k_lo || k > k_hi) return;        // each kernel variant runs on the sets of its k range
   const int s = blockIdx.x * groups_per_cta + group;
   if (s >= S) return;                      // WPS == 1: whole warps leave (no block barrier below); WPS == 4: the whole CTA
   const int ms = k | 1;                    // odd row stride of M: conflict-free column reads
@@ -276,15 +269,18 @@ __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
     }
   }
   seed_group_sync<WPS>();
+  // the seed's first neighbour slot again: held across the Gram it costs a spill at 128 registers (`sets` is not __restrict__,
+  // so this load is not merged with the one above)
+  const size_t nb1 = (size_t)sets[b].knn0 + (size_t)(s * k);
   if (compat_out) {
-    float* dst = compat_out + nb0 * k;
+    float* dst = compat_out + nb1 * k;
     for (int t = tg; t < k * k; t += TS) dst[t] = M[(t / k) * ms + (t % k)];
   }
 
   // power iteration from the all-ones vector; record every iterate and a convergence bit per iteration.
   // Thread = (row group rg = tg >> 2, column quarter cq = tg & 3): rows rg + (TS / 4) i, the columns of quarter cq.
   uint32_t mask = 0u;
-  float* it_out = iterates + nb0 * iters;
+  float* it_out = iterates + nb1 * iters;
   constexpr int RG = TS / 4;                         // row groups: 8 (one warp) or 32 (four warps)
   const int rg = tg >> 2, cq = tg & 3;
   const int CQ = (k + 3) >> 2;                       // columns per quarter
@@ -433,15 +429,15 @@ constexpr int kMmaTiles = 9;       // (i, j): 16-row tile i, 8-column tile j >= 
 __global__ void __launch_bounds__(256, 2) nsm_power_mma_kernel(
     const float* __restrict__ normed, const float* __restrict__ src, const float* __restrict__ tgt,
     const int32_t* __restrict__ knn_idx, float* __restrict__ iterates, uint32_t* __restrict__ conv_mask,
-    float* __restrict__ compat_out, SetTable sets, int k_lo, int k_hi, int iters, float sigma2, float sigmad2, int mask_stride,
-    int groups_per_cta, int per_group_floats) {
+    float* __restrict__ compat_out, const SetDesc* __restrict__ sets, int k_lo, int k_hi, int iters, float sigma2, float sigmad2,
+    int mask_stride, int groups_per_cta, int per_group_floats) {
   const float rc_sigma2 = 1.0f / sigma2, rc_sigmad2 = 1.0f / sigmad2;   // IEEE divisions (correctly rounded reciprocals)
   extern __shared__ __align__(16) float sm[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int b = blockIdx.y;
-  const SetDesc d = set_desc(sets, b);
+  const SetDesc d = sets[b];
   const int N = d.N, S = d.S, k = d.k;
-  if (k < k_lo || k > k_hi) return;        // a packed call runs each kernel variant on the sets of its k range
+  if (k < k_lo || k > k_hi) return;        // each kernel variant runs on the sets of its k range
   const int s = blockIdx.x * groups_per_cta + warp;
   if (s >= S) return;                      // whole warps leave: nothing below synchronises the block
   const int ms = k | 1;                    // odd row stride of M: conflict-free column reads
@@ -727,15 +723,15 @@ __device__ __forceinline__ void mma4_gram_and_compat(const float* __restrict__ n
 __global__ void __launch_bounds__(128, 4) nsm_power_mma4_kernel(
     const float* __restrict__ normed, const float* __restrict__ src, const float* __restrict__ tgt,
     const int32_t* __restrict__ knn_idx, float* __restrict__ iterates, uint32_t* __restrict__ conv_mask,
-    float* __restrict__ compat_out, SetTable sets, int k_lo, int k_hi, int iters, float sigma2, float sigmad2,
+    float* __restrict__ compat_out, const SetDesc* __restrict__ sets, int k_lo, int k_hi, int iters, float sigma2, float sigmad2,
     int mask_stride) {
   const float rc_sigma2 = 1.0f / sigma2, rc_sigmad2 = 1.0f / sigmad2;   // IEEE divisions (correctly rounded reciprocals)
   extern __shared__ __align__(16) float sm[];
   const int tg = threadIdx.x, lane = tg & 31, warp = tg >> 5;
   const int b = blockIdx.y, s = blockIdx.x;
-  const SetDesc d = set_desc(sets, b);
+  const SetDesc d = sets[b];
   const int N = d.N, k = d.k;
-  if (k < k_lo || k > k_hi || s >= d.S) return;   // packed call: the sets of this variant's k range; the whole CTA leaves
+  if (k < k_lo || k > k_hi || s >= d.S) return;   // the sets of this variant's k range; the whole CTA leaves
   const int ms = k | 1;
   float* P = sm;                                       // six coordinate arrays [80]
   float* v = P + 6 * kMma4Rows;                        // [80]
@@ -838,9 +834,8 @@ __global__ void __launch_bounds__(128, 4) nsm_power_mma4_kernel(
 
 // One variant over the sets whose k lies in [k_lo, k_hi]; k is the largest of them (shared-memory layout and grid).
 static void launch_nsm_variant(const float* normed, const float* src, const float* tgt, const int32_t* knn_idx, float* iterates,
-                               uint32_t* conv_mask, float* compat_out, int B, const SetTable& t, int k, int k_lo, int k_hi,
-                               int iters, float sigma, float sigma_d, int mask_stride, int tensor_gram, cudaStream_t st) {
-  const int S = t.S;
+                               uint32_t* conv_mask, float* compat_out, int B, int S, const SetDesc* sets, int k, int k_lo,
+                               int k_hi, int iters, float sigma, float sigma_d, int mask_stride, int tensor_gram, cudaStream_t st) {
   const int ms = k | 1;
   if (tensor_gram && k <= 40) {
     // one warp per seed, two CTAs of eight warps per SM; per warp: key points 6 x 48, iterate 48, indices 48, M k x ms
@@ -850,7 +845,7 @@ static void launch_nsm_variant(const float* normed, const float* src, const floa
     const int smem = warps * per_group_floats * (int)sizeof(float);
     ensure_dynamic_smem(reinterpret_cast<const void*>(nsm_power_mma_kernel), smem);
     nsm_power_mma_kernel<<<dim3((S + warps - 1) / warps, B), warps * 32, smem, st>>>(
-        normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, t, k_lo, k_hi, iters, sigma * sigma, sigma_d * sigma_d,
+        normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, sets, k_lo, k_hi, iters, sigma * sigma, sigma_d * sigma_d,
         mask_stride, warps, per_group_floats);
     return;
   }
@@ -858,7 +853,7 @@ static void launch_nsm_variant(const float* normed, const float* src, const floa
     // 40 < k <= 80: four warps per seed, one seed per CTA
     const int smem = (8 * kMma4Rows + 8 + k * ms) * (int)sizeof(float);
     ensure_dynamic_smem(reinterpret_cast<const void*>(nsm_power_mma4_kernel), smem);
-    nsm_power_mma4_kernel<<<dim3(S, B), 128, smem, st>>>(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, t, k_lo, k_hi,
+    nsm_power_mma4_kernel<<<dim3(S, B), 128, smem, st>>>(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, sets, k_lo, k_hi,
                                                          iters, sigma * sigma, sigma_d * sigma_d, mask_stride);
     return;
   }
@@ -873,13 +868,13 @@ static void launch_nsm_variant(const float* normed, const float* src, const floa
     const int smem = warps * (int)group_bytes;
     ensure_dynamic_smem(reinterpret_cast<const void*>(nsm_power_kernel<1>), smem);
     nsm_power_kernel<1><<<dim3((S + warps - 1) / warps, B), warps * 32, smem, st>>>(
-        normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, t, k_lo, k_hi, iters, sigma * sigma, sigma_d * sigma_d,
+        normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, sets, k_lo, k_hi, iters, sigma * sigma, sigma_d * sigma_d,
         mask_stride, warps, per_group_floats);
   } else {
     // four warps per seed, one seed per CTA
     const int smem = (int)group_bytes;
     ensure_dynamic_smem(reinterpret_cast<const void*>(nsm_power_kernel<4>), smem);
-    nsm_power_kernel<4><<<dim3(S, B), 128, smem, st>>>(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, t, k_lo, k_hi,
+    nsm_power_kernel<4><<<dim3(S, B), 128, smem, st>>>(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, sets, k_lo, k_hi,
                                                         iters, sigma * sigma, sigma_d * sigma_d, mask_stride, 1, per_group_floats);
   }
 }
@@ -891,18 +886,12 @@ void launch_nsm_power(const float* normed, const float* src, const float* tgt, c
   // developer switch for same-box A/B of the two Gram paths (tools/exp_variant.sh style): PDSC_NSM_FFMA=1 forces the FFMA kernels
   static const bool force_ffma = [] { const char* v = getenv("PDSC_NSM_FFMA"); return v && v[0] == '1'; }();
   if (force_ffma) tensor_gram = 0;
-  const SetTable t{sets, N, S, k, 0, 1, 0};
-  if (!sets) {
-    launch_nsm_variant(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, B, t, k, 0, k, iters, sigma, sigma_d, mask_stride,
-                       tensor_gram, st);
-    return;
-  }
-  // a packed call's sets may differ in k (N_b <= cfg.k): each set runs the variant a uniform call of its k would run
+  // the sets may differ in k (N_b <= cfg.k): each set runs the variant of its own k
   const int bounds[3][2] = {{1, 40}, {41, tensor_gram ? kMma4Rows : kMaxK}, {kMma4Rows + 1, kMaxK}};
   for (int r = 0; r < (tensor_gram ? 3 : 2); ++r) {
     const int lo = bounds[r][0] > k_min ? bounds[r][0] : k_min, hi = bounds[r][1] < k ? bounds[r][1] : k;
     if (lo > hi) continue;
-    launch_nsm_variant(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, B, t, hi, lo, hi, iters, sigma, sigma_d,
+    launch_nsm_variant(normed, src, tgt, knn_idx, iterates, conv_mask, compat_out, B, S, sets, hi, lo, hi, iters, sigma, sigma_d,
                        mask_stride, tensor_gram, st);
   }
 }

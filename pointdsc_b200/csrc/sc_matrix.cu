@@ -18,13 +18,13 @@ namespace pdsc {
 constexpr int kScRows = 32;
 
 __global__ void __launch_bounds__(256) sc_matrix_kernel(const float* __restrict__ src, const float* __restrict__ tgt,
-                                                        float* __restrict__ sc, SetTable sets, float s2) {
+                                                        float* __restrict__ sc, const SetDesc* __restrict__ sets, float s2) {
   __shared__ float rs[kScRows][3], rt[kScRows][3];
   const int b = blockIdx.y;
-  const SetDesc d = set_desc(sets, b);
+  const SetDesc d = sets[b];
   const int N = d.N, NS = round_up(N, 64);
   const int i0 = blockIdx.x * kScRows;
-  if (i0 >= N) return;                     // a packed call's grid is sized by its largest set
+  if (i0 >= N) return;                     // the grid is sized by the largest set
   const float* ps = src + (size_t)d.row0 * 3;
   const float* pt = tgt + (size_t)d.row0 * 3;
   for (int t = threadIdx.x; t < kScRows * 3; t += blockDim.x) {
@@ -56,7 +56,7 @@ void launch_sc_matrix(const float* src, const float* tgt, float* sc, int B, int 
                       const SetDesc* sets) {
   const float s2 = sigma_d * sigma_d;  // fp32 product, as `self.sigma_spat ** 2`
   dim3 grid((N + kScRows - 1) / kScRows, B);
-  sc_matrix_kernel<<<grid, 256, 0, st>>>(src, tgt, sc, SetTable{sets, N, 0, 0, 0, 1, 0}, s2);
+  sc_matrix_kernel<<<grid, 256, 0, st>>>(src, tgt, sc, sets, s2);
 }
 
 // ---- tiled layout for the tensor-core attention (tc_attention.cuh) ---------------------------------------
@@ -73,15 +73,15 @@ void launch_sc_matrix(const float* src, const float* tgt, float* sc, int B, int 
 constexpr int kScTStride = 129;   // smem transpose tile [32 i][128 j], odd stride: conflict-free both ways
 
 __global__ void __launch_bounds__(256) sc_matrix_tiled_kernel(const float* __restrict__ src, const float* __restrict__ tgt,
-                                                              float* __restrict__ sc, SetTable sets, float s2, float rc_s2) {
+                                                              float* __restrict__ sc, const SetDesc* __restrict__ sets, float s2, float rc_s2) {
   // the A range's points as six arrays: an 8-byte broadcast load is the same coordinate of TWO consecutive rows, so the distance
   // chains of two matrix elements run as pairs (each lane rounded exactly like the scalar sequence)
   __shared__ __align__(8) float isx[128], isy[128], isz[128], itx[128], ity[128], itz[128];
   __shared__ float tr[32 * kScTStride];
   const int b = blockIdx.y;
-  const SetDesc d = set_desc(sets, b);
+  const SetDesc d = sets[b];
   const int N = d.N, KT = (N + 63) / 64, QT = (N + 127) / 128;
-  if ((int)blockIdx.x >= QT * (QT + 1) / 2) return;   // a packed call's grid is sized by its largest set
+  if ((int)blockIdx.x >= QT * (QT + 1) / 2) return;   // the grid is sized by the largest set
   // blockIdx.x enumerates the pairs A <= Bq
   int A = 0, rem = blockIdx.x;
   while (rem >= QT - A) { rem -= QT - A; ++A; }
@@ -156,7 +156,7 @@ void launch_sc_matrix_tiled(const float* src, const float* tgt, float* sc, int B
                             const SetDesc* sets) {
   const float s2 = sigma_d * sigma_d;
   const int QT = (N + 127) / 128;
-  sc_matrix_tiled_kernel<<<dim3(QT * (QT + 1) / 2, B), 256, 0, st>>>(src, tgt, sc, SetTable{sets, N, 0, 0, 1, 1, 0}, s2, 1.0f / s2);
+  sc_matrix_tiled_kernel<<<dim3(QT * (QT + 1) / 2, B), 256, 0, st>>>(src, tgt, sc, sets, s2, 1.0f / s2);
 }
 
 // tiled -> dense [B][N][N] (stage tap only)

@@ -26,14 +26,14 @@ constexpr int kSeedMaxN = 16384;
 // nms_key_warp_kernel below instead.
 template <int kNmsTile>
 __global__ void __launch_bounds__(kNmsTile) nms_key_kernel(const float* __restrict__ src, const float* __restrict__ conf,
-                                                           float* __restrict__ key, SetTable sets, float d2_min) {
+                                                           float* __restrict__ key, const SetDesc* __restrict__ sets, float d2_min) {
   // candidates staged as four arrays so that an 8-byte load yields the same coordinate of TWO neighbours: the distance chain
   // then runs on pairs (two candidates at a time, each lane rounded like the scalar operation)
   __shared__ __align__(8) float sx[kNmsTile], sy[kNmsTile], sz[kNmsTile], sw[kNmsTile];
   const int b = blockIdx.y;
-  const SetDesc d = set_desc(sets, b);
+  const SetDesc d = sets[b];
   const int N = d.N;
-  if ((int)blockIdx.x * kNmsTile >= N) return;   // a packed call's grid is sized by its largest set
+  if ((int)blockIdx.x * kNmsTile >= N) return;   // the grid is sized by the largest set
   const int i = blockIdx.x * kNmsTile + threadIdx.x;
   const float* p = src + (size_t)d.row0 * 3;
   const float* s = conf + d.row0;
@@ -68,9 +68,9 @@ __global__ void __launch_bounds__(kNmsTile) nms_key_kernel(const float* __restri
 // Small calls: one WARP per row i, the lanes stride over the candidates j, the verdict is a warp vote; a row is decided in
 // N / 32 iterations with 32 loads in flight, and N rows spread over N / 8 CTAs.  Same arithmetic, same result.
 __global__ void __launch_bounds__(256) nms_key_warp_kernel(const float* __restrict__ src, const float* __restrict__ conf,
-                                                           float* __restrict__ key, SetTable sets, float d2_min) {
+                                                           float* __restrict__ key, const SetDesc* __restrict__ sets, float d2_min) {
   const int b = blockIdx.y, lane = threadIdx.x & 31;
-  const SetDesc d = set_desc(sets, b);
+  const SetDesc d = sets[b];
   const int N = d.N;
   const int i = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (i >= N) return;
@@ -102,12 +102,12 @@ __device__ __forceinline__ uint32_t orderable(float f) {
 }
 
 // one CTA per set: bitonic sort of (descending key, ascending index), emit the first S indices.  P is a power of two >= N
-// (a packed call sorts every set at the P of its largest set: the pads sort last, the sorted prefix is the same)
+// (every set is sorted at the P of the call's largest set: the pads sort last, the sorted prefix is the same)
 __global__ void __launch_bounds__(1024) seed_sort_kernel(const float* __restrict__ key, int32_t* __restrict__ seeds,
-                                                         SetTable sets, int P) {
+                                                         const SetDesc* __restrict__ sets, int P) {
   extern __shared__ unsigned long long skeys[];
   const int b = blockIdx.x;
-  const SetDesc d = set_desc(sets, b);
+  const SetDesc d = sets[b];
   const int N = d.N, S = d.S;
   if (S <= 0) return;
   for (int i = threadIdx.x; i < P; i += blockDim.x) {
@@ -140,13 +140,13 @@ static void launch_seed_sort(const float* key, int32_t* seeds, int B, int N, int
   const int smem = P * (int)sizeof(unsigned long long);
   ensure_dynamic_smem(reinterpret_cast<const void*>(seed_sort_kernel), smem);
   const int threads = P / 2 < 1024 ? (P / 2 < 32 ? 32 : P / 2) : 1024;
-  seed_sort_kernel<<<B, threads, smem, st>>>(key, seeds, SetTable{sets, N, S, 0, 0, 1, 0}, P);
+  seed_sort_kernel<<<B, threads, smem, st>>>(key, seeds, sets, P);
 }
 
 // a6' — the non-testing seed rule (models/PointDSC.py:176): argsort(confidence, descending)[:S], no suppression.
 // Ties: lowest index first (the reference's argsort is unstable).
-void launch_top_seeds(const float* conf, int32_t* seeds, int B, int N, int S, cudaStream_t st) {
-  if (S > 0) launch_seed_sort(conf, seeds, B, N, S, st, nullptr);
+void launch_top_seeds(const float* conf, int32_t* seeds, int B, int N, int S, cudaStream_t st, const SetDesc* sets) {
+  if (S > 0) launch_seed_sort(conf, seeds, B, N, S, st, sets);
 }
 
 void launch_pick_seeds(const float* src, const float* conf, int32_t* seeds, float* key_scratch, int B, int N, int S,
@@ -155,11 +155,10 @@ void launch_pick_seeds(const float* src, const float* conf, int32_t* seeds, floa
   float d2_min = radius * radius;
   while (std::sqrt(d2_min) >= radius && d2_min > 0.f) d2_min = std::nextafter(d2_min, 0.0f);
   while (std::sqrt(d2_min) < radius) d2_min = std::nextafter(d2_min, INFINITY);
-  const SetTable t{sets, N, S, 0, 0, 1, 0};
   if ((long long)B * ((N + 255) / 256) >= 2LL * device_sm_count())
-    nms_key_kernel<256><<<dim3((N + 255) / 256, B), 256, 0, st>>>(src, conf, key_scratch, t, d2_min);
+    nms_key_kernel<256><<<dim3((N + 255) / 256, B), 256, 0, st>>>(src, conf, key_scratch, sets, d2_min);
   else
-    nms_key_warp_kernel<<<dim3((N + 7) / 8, B), 256, 0, st>>>(src, conf, key_scratch, t, d2_min);
+    nms_key_warp_kernel<<<dim3((N + 7) / 8, B), 256, 0, st>>>(src, conf, key_scratch, sets, d2_min);
   launch_seed_sort(key_scratch, seeds, B, N, S, st, sets);
 }
 

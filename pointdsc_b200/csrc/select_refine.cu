@@ -34,14 +34,14 @@ __global__ void __launch_bounds__(256) seed_hypotheses_kernel(
     const float* __restrict__ src, const float* __restrict__ tgt, const int32_t* __restrict__ knn_idx,
     const float* __restrict__ iterates, const uint32_t* __restrict__ conv_mask, const float* __restrict__ seed_trans_in,
     float* __restrict__ seed_trans, int32_t* __restrict__ inlier_counts, unsigned long long* __restrict__ best_key,
-    float* __restrict__ eig_out, int32_t* __restrict__ power_iters, SetTable sets, int iters, float d2_lim,
+    float* __restrict__ eig_out, int32_t* __restrict__ power_iters, const SetDesc* __restrict__ sets, int iters, float d2_lim,
     int mask_stride) {
   // the set's points, staged once per CTA for its eight seeds: six arrays so that an 8-byte load is the same coordinate of two points
   __shared__ __align__(8) float pts_s[6][kHypChunk];
   const int b = blockIdx.y;
-  const SetDesc d = set_desc(sets, b);
+  const SetDesc d = sets[b];
   const int N = d.N, S = d.S, k = d.k;
-  if ((int)blockIdx.x * 8 >= S) return;     // a packed call's grid is sized by its largest set: the whole CTA leaves
+  if ((int)blockIdx.x * 8 >= S) return;     // the grid is sized by the largest set: the whole CTA leaves
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int s_raw = blockIdx.x * 8 + warp;
   const bool active = s_raw < S;            // inactive warps still take part in the staging barriers
@@ -176,8 +176,8 @@ void launch_seed_hypotheses(const float* src, const float* tgt, const int32_t* k
   while (std::sqrt(d2_lim) >= inlier_threshold && d2_lim > 0.f) d2_lim = std::nextafter(d2_lim, 0.0f);
   while (std::sqrt(d2_lim) < inlier_threshold) d2_lim = std::nextafter(d2_lim, INFINITY);
   seed_hypotheses_kernel<<<dim3((S + 7) / 8, B), 256, 0, st>>>(src, tgt, knn_idx, iterates, conv_mask, seed_trans_in,
-                                                              seed_trans, inlier_counts, best_key, eig_out, power_iters,
-                                                              SetTable{sets, N, S, k, 0, 1, 0}, iters, d2_lim, mask_stride);
+                                                              seed_trans, inlier_counts, best_key, eig_out, power_iters, sets,
+                                                              iters, d2_lim, mask_stride);
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -206,13 +206,13 @@ __device__ __forceinline__ void block_sum(double (&vals)[NV], double* red /* [16
 __global__ void __launch_bounds__(kRefThreads) select_refine_kernel(
     const float* __restrict__ src, const float* __restrict__ tgt, const float* __restrict__ seed_trans,
     const unsigned long long* __restrict__ best_key, float* __restrict__ final_trans, float* __restrict__ final_labels,
-    float* __restrict__ init_trans_out, int32_t* __restrict__ best_out, int32_t* __restrict__ refine_solves, SetTable sets,
+    float* __restrict__ init_trans_out, int32_t* __restrict__ best_out, int32_t* __restrict__ refine_solves, const SetDesc* __restrict__ sets,
     float thr, float rthr, int max_refine) {
   __shared__ float T[12];
   __shared__ double red[(kRefThreads / 32) * 10];
   __shared__ double tot[10];
   const int b = blockIdx.x, tid = threadIdx.x;
-  const SetDesc d = set_desc(sets, b);
+  const SetDesc d = sets[b];
   const int N = d.N, S = d.S;
   const float* ps = src + (size_t)d.row0 * 3;
   const float* pt = tgt + (size_t)d.row0 * 3;
@@ -304,8 +304,7 @@ void launch_select_refine(const float* src, const float* tgt, const float* seed_
                           float inlier_threshold, float refine_threshold, int max_refine, cudaStream_t st,
                           const SetDesc* sets) {
   select_refine_kernel<<<B, kRefThreads, 0, st>>>(src, tgt, seed_trans, best_key, final_trans, final_labels,
-                                                  init_trans_out, best_out, refine_solves, SetTable{sets, N, S, 0, 0, 1, 0},
-                                                  inlier_threshold,
+                                                  init_trans_out, best_out, refine_solves, sets, inlier_threshold,
                                                   refine_threshold, max_refine);
 }
 

@@ -12,19 +12,17 @@
 namespace pdsc {
 
 struct AttnArgs {
-  int N, NS, QT, KT, split;
+  int split;
   const uint8_t* qimg;
   const uint8_t* kvimg;
-  const float* sc;    // tiled: [B][KT][QT][16 key groups][128 queries][4 keys]
+  const float* sc;    // tiled, per set from its sc0: [KT][QT][16 key groups][128 queries][4 keys]
   float* msg;
-  int items;          // work items of the launch: B * QT * splits
-  // key split (small calls only, see encoder_tc.cu): a work item is (set, query tile, split) and covers key tiles
-  // [split * TS, split * TS + TS); tiles beyond KT are "virtual" (fully masked).  splits == 1: TS == KT, one item per query tile.
-  int splits, TS;
-  float* part_o;      // [items][128][128] unnormalised O of every work item           (splits > 1)
+  int items;          // work items of the launch
+  float* part_o;      // [items][128][128] unnormalised O of every work item of a split set
   float* part_ml;     // [items][128][2]   its final reference maximum (log2 units) and row sum
-  // packed call: the descriptor table (nullptr for a uniform call).  Its work items are numbered set by set from each set's
-  // item0; set b has QT_b * sp_b of them, each covering TS_b key tiles; items, N, QT, KT, splits and TS above are unused
+  // the descriptor table.  Work items are numbered set by set from each set's item0: set b has QT_b * sp_b of them, a work
+  // item is (set, query tile, split) and covers key tiles [split * TS_b, split * TS_b + TS_b); tiles beyond KT_b are "virtual"
+  // (fully masked).  sp_b == 1 (key split: small calls only, see encoder_tc.cu): TS_b == KT_b, one item per query tile.
   const SetDesc* sets;
   int nsets;
 };
@@ -40,20 +38,12 @@ struct AttnItem {
 };
 
 __device__ __forceinline__ AttnItem attn_item(const AttnArgs& a, int witem) {
+  const SetDesc d = a.sets[find_set(a.nsets, witem, [&](int i) { return a.sets[i].item0; })];
+  const int local = witem - d.item0;
   AttnItem w;
-  if (a.sets) {
-    const int b = find_set(a.nsets, witem, [&](int i) { return a.sets[i].item0; });
-    const SetDesc d = a.sets[b];
-    const int local = witem - d.item0;
-    w.N = d.N; w.QT = (d.N + 127) / 128; w.KT = (d.N + 63) / 64;
-    w.qt = local / d.sp; w.t0 = (local % d.sp) * d.TS; w.T = d.TS; w.sp = d.sp;
-    w.qtile = d.qt0 + w.qt; w.kt0 = d.kt0; w.row0 = d.row0; w.sc0 = d.sc0;
-  } else {
-    const int item = witem / a.splits, b = item / a.QT;
-    w.N = a.N; w.QT = a.QT; w.KT = a.KT;
-    w.qt = item % a.QT; w.t0 = (witem % a.splits) * a.TS; w.T = a.TS; w.sp = a.splits;
-    w.qtile = item; w.kt0 = b * a.KT; w.row0 = b * a.N; w.sc0 = ((long long)b * a.KT * a.QT) << 13;
-  }
+  w.N = d.N; w.QT = (d.N + 127) / 128; w.KT = (d.N + 63) / 64;
+  w.qt = local / d.sp; w.t0 = (local % d.sp) * d.TS; w.T = d.TS; w.sp = d.sp;
+  w.qtile = d.qt0 + w.qt; w.kt0 = d.kt0; w.row0 = d.row0; w.sc0 = d.sc0;
   return w;
 }
 

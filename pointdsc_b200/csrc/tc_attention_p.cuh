@@ -178,21 +178,15 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
 
 // ---- key split: combine the partial results of one query tile -------------------------------------------------------------
 // msg_i = sum_s O_s[i] 2^(m_s - m*) / sum_s l_s 2^(m_s - m*),  m* = max_s m_s, splits added in ascending order (deterministic).
-// One CTA per (query tile, 32-row quarter), thread = (row, 16-byte column piece stride).  A packed call numbers its query tiles
-// set by set (qt0); the tiles of its sets without a split wrote msg themselves.
+// One CTA per (query tile, 32-row quarter), thread = (row, 16-byte column piece stride).  Query tiles are numbered set by set
+// (qt0); the tiles of sets without a split wrote msg themselves.
 __global__ void __launch_bounds__(256) tc_attention_merge_kernel(const float* __restrict__ part_o, const float* __restrict__ part_ml,
-                                                                 float* __restrict__ msg, int N, int QT, int splits,
-                                                                 const SetDesc* __restrict__ sets, int nsets) {
+                                                                 float* __restrict__ msg, const SetDesc* __restrict__ sets, int nsets) {
   const int qtile = blockIdx.x >> 2, quarter = blockIdx.x & 3;
-  int qt, item, row0;     // item: the tile's first work item
-  if (sets) {
-    const SetDesc d = sets[find_set(nsets, qtile, [&](int i) { return sets[i].qt0; })];
-    if (d.sp < 2) return;
-    N = d.N; qt = qtile - d.qt0; splits = d.sp; item = d.item0 + qt * d.sp; row0 = d.row0;
-  } else {
-    const int b = qtile / QT;
-    qt = qtile % QT; item = qtile * splits; row0 = b * N;
-  }
+  const SetDesc d = sets[find_set(nsets, qtile, [&](int i) { return sets[i].qt0; })];
+  if (d.sp < 2) return;
+  const int N = d.N, qt = qtile - d.qt0, splits = d.sp, row0 = d.row0;
+  const int item = d.item0 + qt * splits;   // the tile's first work item
   const int row = quarter * 32 + (threadIdx.x >> 3);
   if (qt * 128 + row >= N) return;
   // the reference maxima first (independent loads), then the partial rows four splits at a time so that their loads overlap:

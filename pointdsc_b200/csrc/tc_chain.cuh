@@ -17,6 +17,8 @@
 //     [tile][32-column chunk cc][128 rows][128 B], 16-byte piece q of row r at piece q ^ (r & 7)
 // so that the fragment reads of a staged feat1 tile are at most 2-way bank conflicted (blocked_f32_offset).
 #pragma once
+#include <climits>
+
 #include "tc_common.cuh"
 
 namespace pdsc {
@@ -29,27 +31,33 @@ constexpr int kChBias = kChRes + 65536;          // 256 floats: this mode's bias
 constexpr int kChBars = kChBias + 1024;          // mbarriers: weights, input, residual
 constexpr int kChainSmem = kChBars + 64;         // 214,080 B
 
-// (set, index within the set) of global row g
-__device__ __forceinline__ void locate_row(long long g, int N, int& bb, int& nn) {
-  bb = (int)(g / N);
-  nn = (int)(g - (long long)bb * N);
+// A chain tile may span several sets (rows are not padded per set).  Its rows find their sets in a window of the table: lane
+// l holds the first row and the first operand image tile (PCQ: 128-query tile of the Q image, KV: 64-key tile of the K / V
+// image) of set lo + l, lo the set of the tile's first row (ChainArgs::tile_set).
+struct SetWindow {
+  int lo, row0, t0;
+};
+template <int MODE>
+__device__ __forceinline__ SetWindow load_window(const ChainArgs& a, int lo) {
+  const int lane = threadIdx.x & 31, w = min(lo + lane, a.nsets - 1);
+  return {lo, lo + lane < a.nsets ? __ldg(&a.sets[w].row0) : INT_MAX, MODE == kPCQ ? __ldg(&a.sets[w].qt0) : __ldg(&a.sets[w].kt0)};
 }
 
-// operand image tile of global row g (PCQ: its set's 128-query tile in the Q image, KV: its 64-key tile in the K / V image)
-// and the row's place within that tile.  A packed call's rows are not padded per set, so a chain tile may span several sets:
-// each row finds its own set by a binary search over the sets' first rows.
+// operand image tile of row g of the window's chain tile and the row's place within that tile.  All lanes of the warp take part.
 template <int MODE>
-__device__ __forceinline__ void locate_tile(const ChainArgs& a, long long g, int& tile, int& r) {
-  int nn, t0;
-  if (a.sets) {
-    const int b = find_set(a.nsets, g, [&](int i) { return a.sets[i].row0; });
-    nn = (int)(g - a.sets[b].row0);
-    t0 = MODE == kPCQ ? a.sets[b].qt0 : a.sets[b].kt0;
-  } else {
-    int bb;
-    locate_row(g, a.N, bb, nn);
-    t0 = bb * (MODE == kPCQ ? a.QT : a.KT);
+__device__ __forceinline__ void locate_row(const ChainArgs& a, const SetWindow& win, long long g, int& tile, int& r) {
+  int k = 0;                                      // the last window set that starts at or below g
+#pragma unroll
+  for (int s = 16; s > 0; s >>= 1)
+    if (__shfl_sync(0xffffffffu, win.row0, k + s) <= g) k += s;
+  int row0 = __shfl_sync(0xffffffffu, win.row0, k), t0 = __shfl_sync(0xffffffffu, win.t0, k);
+  if (k == 31) {                                  // more than 31 sets start in the tile (N < 5): step on past the window
+    int b = win.lo + 31;
+    while (b + 1 < a.nsets && __ldg(&a.sets[b + 1].row0) <= g) ++b;
+    row0 = __ldg(&a.sets[b].row0);
+    t0 = MODE == kPCQ ? __ldg(&a.sets[b].qt0) : __ldg(&a.sets[b].kt0);
   }
+  const int nn = (int)(g - row0);
   tile = t0 + (MODE == kPCQ ? (nn >> 7) : (nn >> 6));
   r = MODE == kPCQ ? (nn & 127) : (nn & 63);
 }
@@ -135,9 +143,29 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
   const int fr = 64 * wg + frag_row(wt), fc = frag_col(wt);   // fragment rows fr, fr + 8 of the tile; columns 8 j + fc, + 1
   const int quad = fc >> 1;                                   // this lane's place among the 4 lanes that share its rows
 
+  // PCQ, KV: the set window of the CTA's next tile is loaded one tile ahead, from its first set loaded two tiles ahead, so that
+  // no lookup waits for memory
+  SetWindow win_next{};
+  int lo_after = 0;
+  if (MODE != kMSG && blockIdx.x < num_tiles) {
+    win_next = load_window<MODE>(a, __ldg(a.tile_set + blockIdx.x));
+    if (blockIdx.x + gridDim.x < num_tiles) lo_after = __ldg(a.tile_set + blockIdx.x + gridDim.x);
+  }
   uint32_t phase = 0;
   for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, phase ^= 1u) {
     const long long row0 = tile * 128;
+    // the two rows of this thread: global index, operand image tile and row within it
+    const long long g[2] = {row0 + fr, row0 + fr + 8};
+    int tl[2], tr[2];
+    if (MODE != kMSG) {
+      const SetWindow win = win_next;
+      if (tile + gridDim.x < num_tiles) {
+        win_next = load_window<MODE>(a, lo_after);
+        if (tile + 2 * gridDim.x < num_tiles) lo_after = __ldg(a.tile_set + tile + 2 * gridDim.x);
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) locate_row<MODE>(a, win, g[h] < rows ? g[h] : row0, tl[h], tr[h]);
+    }
     // ---- this thread's fragment of the staged input tile -> hi / lo register A operand (K = 128) ----
     uint32_t ahi[8][4], alo[8][4];
     mbar_wait(bar_in, phase);
@@ -160,14 +188,6 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
         mbar_expect_tx(bar_res, 65536u);
         bulk_g2s(s0 + kChRes, reinterpret_cast<const uint8_t*>(a.res) + (size_t)tile * 65536, 65536u, bar_res);
       }
-    }
-    // the two rows of this thread: global index, operand image tile and row within it
-    long long g[2];
-    int tl[2], tr[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      g[h] = row0 + fr + 8 * h;
-      if (MODE != kMSG) locate_tile<MODE>(a, g[h] < rows ? g[h] : 0, tl[h], tr[h]);
     }
 
     if (MODE == kPCQ) {

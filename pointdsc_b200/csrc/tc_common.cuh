@@ -18,9 +18,10 @@ constexpr float kQScale = 1.4426950408889634f / 11.313708498984761f;  // log2(e)
 enum ChainMode { kPCQ = 0, kKV = 1, kMSG = 2 };
 
 struct ChainArgs {
-  long long rows;        // B * N, or the rows of a packed call
-  int N, QT, KT, split;  // uniform call: every set's N and its tiles
-  const SetDesc* sets;   // packed call: the descriptor table (row0, qt0, kt0), nullptr for a uniform call
+  long long rows;        // rows of the call (all sets)
+  int split;
+  const SetDesc* sets;   // the call's descriptor table (row0, qt0, kt0)
+  const int* tile_set;   // [rows / 128]: the set of the first row of every 128-row chain tile
   int nsets;
   const float* in;       // [rows][128] fp32 A operand
   const float* res;      // MSG: feat1 (residual)

@@ -92,6 +92,23 @@ def test_split_regime_mixed_call_equals_single_calls(precision):
         assert torch.equal(o["final_labels"], one["final_labels"])
 
 
+@pytest.mark.parametrize("precision", PRECISIONS)
+def test_uniform_call_is_the_packed_call_with_equal_offsets(precision):
+    """pdsc_forward(B, N) runs the packed call whose offsets are b * N: the same workspace and the same bytes, in both
+    attention regimes (bs = 1 at N = 1000 is split, 64 sets are not)."""
+    m = get_model("3dmatch", precision)
+    lib = m._ensure_engine()
+    for B, N in ((1, 2), (3, 9), (1, 1000), (64, 1000), (1, 16384), (2, 16384)):
+        h = (C.c_int32 * (B + 1))(*range(0, (B + 1) * N, N))
+        assert lib.pdsc_workspace_bytes(m._engine, B, N) == lib.pdsc_workspace_bytes_packed(m._engine, B, h) > 0, (B, N)
+    for copies in (1, 64):
+        b = as_batch(synth_sets([1000] * copies, seed0=90))
+        ref = m.run(b["corr_pos"], b["src_keypts"], b["tgt_keypts"])
+        out = m.forward_many([b])[0]
+        assert torch.equal(out["final_trans"], ref["final_trans"]), copies
+        assert torch.equal(out["final_labels"], ref["final_labels"]), copies
+
+
 def test_batches_of_several_sets_keep_their_shapes():
     m = get_model("3dmatch", "fp16x3")
     a, b = synth_sets([300, 300], seed0=3), synth_sets([500], seed0=5)

@@ -1,0 +1,68 @@
+#!/usr/bin/env python
+"""Every output of bs = 1 uniform forwards, for comparing two builds of the engine byte for byte.
+
+    python tools/uniform_outputs.py --out DIR/uniform_outputs.npz
+    python tools/uniform_outputs.py --compare A.npz B.npz
+
+Seeded synthetic pairs (pointdsc_b200.synth, released 3DMatch weights) at N = 41, 257, 1003 and 5000 in every precision.
+N = 5000 at bs = 1 runs the attention's key split, the others are too small to split or split into few chunks.  Per (precision,
+N) the file holds the testing-mode forward with every stage tap (SC, features, the layer-0 internals, seeds, kNN, compatibility,
+eigenvectors, hypotheses, refinement) and the eval-mode forward (confidence, M) with its taps.  --compare exits non-zero unless
+both files hold the same arrays with the same bytes."""
+import argparse
+import os
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+SIZES = (41, 257, 1003, 5000)
+PRECISIONS = ("fp32", "fp16x3", "bf16x3", "bf16")
+TAPS = ("sc", "features", "normed", "confidence", "seeds", "knn_idx", "compat", "eig", "power_iters", "seed_trans",
+        "inlier_counts", "best", "init_trans", "refine_solves", "layer_features", "layer_debug")
+EVAL_TAPS = ("features", "confidence", "seeds", "knn_idx", "compat", "eig", "power_iters", "seed_trans", "inlier_counts",
+             "best", "init_trans")
+
+
+def collect():
+    import bench
+    from pointdsc_b200 import PointDSC
+    from pointdsc_b200.synth import make_pair
+    out = {}
+    for precision in PRECISIONS:
+        m = PointDSC(num_layers=12, k=40, precision=precision, **bench.CTOR["3dmatch"])
+        m.load_state_dict(bench.load_snapshot("3dmatch"), strict=False)
+        m = m.cuda().eval()
+        for n in SIZES:
+            p = make_pair(n, n, "3dmatch", 0.3)
+            cp, s, t = (p[key][None].cuda() for key in ("corr_pos", "src_keypts", "tgt_keypts"))
+            for mode, res in (("test", m.run(cp, s, t, taps=TAPS)), ("eval", m.run_eval(cp, s, t, taps=EVAL_TAPS))):
+                for name, v in res.items():
+                    if v is not None:
+                        out[f"{precision}/{n}/{mode}/{name}"] = v.cpu().numpy()
+        torch.cuda.synchronize()
+    return out
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--out")
+    ap.add_argument("--compare", nargs=2)
+    args = ap.parse_args(argv)
+    if args.compare:
+        a, b = (np.load(f) for f in args.compare)
+        bad = sorted(set(a.files) ^ set(b.files)) + [k for k in sorted(set(a.files) & set(b.files))
+                                                      if a[k].dtype != b[k].dtype or a[k].tobytes() != b[k].tobytes()]
+        print(f"{len(a.files)} arrays, {len(bad)} differ" + (": " + ", ".join(bad) if bad else ""))
+        return 1 if bad else 0
+    if not torch.cuda.is_available():
+        sys.exit("no CUDA device: this tool runs the engine")
+    np.savez(args.out, **collect())
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())
