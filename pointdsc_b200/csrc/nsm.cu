@@ -16,8 +16,6 @@
 // per-set word; the consumer (select_refine.cu) takes the iterate at the first all-converged bit.
 #include <cuda_fp16.h>
 
-#include <cstdlib>
-
 #include "common.cuh"
 #include "kernels.h"
 #include "sets.cuh"
@@ -115,27 +113,21 @@ void launch_knn_select(const float* dist, int32_t* knn_idx, int B, int N, int S,
   knn_select_kernel<<<(rows + warps - 1) / warps, warps * 32, smem, st>>>(dist, knn_idx, sets, B, rows, warps, NP, P);
 }
 
-// ---- compatibility matrix + power iteration: one warp (k <= 40) or one 4-warp CTA (k > 40) per seed ----------------------
-// (round 1 ran one 64-thread CTA per seed with block barriers between gather, Gram and each of the 10 iterations: every
-// phase waited for the slowest of two warps and a CTA held 28 KB of shared memory through its latency-bound phases — 0.71 ms
-// for B * S = 25 600 seeds.)  A seed is owned by a GROUP of WPS warps from the gather to the last iterate:
-//   WPS = 1 (k <= 40, the released configuration): nothing but __syncwarp() separates the phases, and 16 warps per SM sit in
-//           different phases and hide each other's latencies;
-//   WPS = 4 (k > 40, e.g. BASELINE config C with k = 80): the 210 register blocks of an 80 x 80 Gram are two rounds of 128
-//           threads (one warp would need seven rounds and four passes over the gathered features), five CTAs per SM.
-// Phases:
-//   gather   the k neighbour rows arrive with cp.async (16 bytes per lane, eight lanes per row), one 32-channel QUARTER at a
-//            time, so the feature tile costs k x 128 B of shared memory instead of k x 512 B;
-//   Gram     4 x 4 register blocks on or above the diagonal (55 blocks for k = 40), 8 LDS.128 per 64 FMAs, accumulated over the
-//            four quarters in ascending channel order, one fp32 FMA each;
-//   compat   feature-compat * spatial-compat with the reference's rounded operation sequence, M symmetric in shared memory;
-//   power    thread = (row group, column quarter): the k x k matrix-vector product is spread over all threads of the group; a
-//            row's four partial sums (ascending column order within a quarter) are combined by an xor butterfly,
-//            (q0 + q1) + (q2 + q3), the squared norm by a butterfly over the row groups (and, for WPS = 4, the four warps'
-//            sums in ascending order): fixed orders, identical on every thread.  Every iterate is stored and the "all rows
-//            passed allclose at iteration t" bits of the seed are ANDed into the set's word.
-// The 16-byte chunk index of a feature row is XOR-swizzled by (row >> 2) & 7 so that the rows of different 4-row blocks
-// fall into different banks (rows of one block are read by lanes that share them: broadcasts).
+// ---- compatibility matrix + power iteration ------------------------------------------------------------------------------
+// Each kernel below owns a seed with a group of WPS warps from the gather to the last iterate: it gathers the seed's k
+// neighbours, builds the k x k compatibility matrix M in shared memory and runs the power iteration.  launch_nsm_power picks
+// the kernel by precision and by the set's k:
+//
+//   kernel                  runs for                                            WPS  Gram
+//   nsm_power_kernel<1>     fp32, k <= 40                                       1    FFMA, shared-memory feature quarters
+//   nsm_power_kernel<4>     fp32, 41 <= k <= 128; tensor-core modes, k >= 81    4    FFMA, shared-memory feature quarters
+//   nsm_power_mma_kernel    fp16x3 / bf16x3 / bf16, k <= 40                     1    mma.sync fp16 hi/lo, register double buffer
+//   nsm_power_mma4_kernel   fp16x3 / bf16x3 / bf16, 41 <= k <= 80               4    mma.sync fp16 hi/lo, L1 prefetch
+//
+// Only the Gram loops differ, each tuned for its warps per seed and register budget: one warp over 48 rows keeps the next
+// 16-channel step in registers, four warps over 80 rows have no registers for that and prefetch into L1 instead, and the FFMA
+// Gram stages a quarter of the channels at a time in shared memory, which reaches k = 128.  With one warp per seed nothing but
+// __syncwarp() separates the phases, and the warps of an SM sit in different phases and hide each other's latencies.
 __device__ __forceinline__ void cp_async_16(uint32_t dst_smem, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst_smem), "l"(src) : "memory");
 }
@@ -147,6 +139,90 @@ __device__ __forceinline__ void seed_group_sync() {
   else __syncthreads();        // WPS == 4: the CTA is exactly one seed group
 }
 
+// The power iteration from the all-ones vector with the thread's slice of M (row stride ms) in registers; returns the bit mask
+// "every row passed torch.allclose at iteration t" and stores every iterate to it_out [iters][k].  Thread tg of the group is
+// (row group rg = tg >> 2, column quarter cq = tg & 3) and holds rows rg + 8 WPS i (i < RI), CW columns of quarter cq: (RI, CW)
+// = (5, 10) covers k <= 40 with one warp, (3, 20) k <= 80 with four.  Slots beyond k hold zeros: fma(0, 0, p) == p, so the sums
+// are those of the shared-memory loop in nsm_power_kernel<4> bit for bit.  A row's four partial sums (ascending columns within
+// a quarter) meet in an xor butterfly, (q0 + q1) + (q2 + q3), the squared norm in a butterfly over the row groups and, with four
+// warps, in the warps' sums in ascending order: fixed orders, identical on every thread.  v [k] and red [8] are shared scratch
+// (red only for WPS = 4).
+template <int WPS, int RI, int CW>
+__device__ __forceinline__ uint32_t power_iteration_regs(const float* M, int ms, int k, float* v, float* red, float* it_out,
+                                                         int iters, int tg) {
+  constexpr int RG = 8 * WPS;                        // row groups
+  const int lane = tg & 31, warp = tg >> 5;
+  const int rg = tg >> 2, cq = tg & 3;
+  const int CQ = (k + 3) >> 2;                       // columns per quarter
+  const int c_lo = cq * CQ, c_hi = min(k, c_lo + CQ);
+  float m[RI][CW], vq[CW], vrow[RI];
+#pragma unroll
+  for (int i = 0; i < RI; ++i) {
+    const int row = rg + RG * i;
+#pragma unroll
+    for (int c = 0; c < CW; ++c) m[i][c] = (row < k && c_lo + c < c_hi) ? M[row * ms + c_lo + c] : 0.f;
+    vrow[i] = 1.0f;
+  }
+#pragma unroll
+  for (int c = 0; c < CW; ++c) vq[c] = (c_lo + c < c_hi) ? 1.0f : 0.f;
+  uint32_t mask = 0u;
+  for (int t = 0; t < iters; ++t) {
+    float u[RI], ss = 0.f;
+#pragma unroll
+    for (int i = 0; i < RI; ++i) {
+      float p = 0.f;
+#pragma unroll
+      for (int c = 0; c < CW; ++c) p = fmaf(m[i][c], vq[c], p);
+      p += __shfl_xor_sync(0xffffffffu, p, 1);
+      p += __shfl_xor_sync(0xffffffffu, p, 2);
+      u[i] = p;
+      ss += (rg + RG * i < k) ? p * p : 0.f;
+    }
+    ss += __shfl_xor_sync(0xffffffffu, ss, 4);
+    ss += __shfl_xor_sync(0xffffffffu, ss, 8);
+    ss += __shfl_xor_sync(0xffffffffu, ss, 16);
+    if (WPS > 1) {
+      if (lane == 0) red[warp] = ss;
+      __syncthreads();
+      ss = ((red[0] + red[1]) + red[2]) + red[3];    // the four warps' sums in ascending warp order on every thread
+    }
+    const float nrm = sqrtf(ss) + 1e-6f;
+    bool ok = true;
+#pragma unroll
+    for (int i = 0; i < RI; ++i) {
+      const int row = rg + RG * i;
+      const float vn = u[i] / nrm;
+      // torch.allclose(new, last): |new - last| <= atol + rtol * |last|, atol 1e-8, rtol 1e-5
+      ok = ok && (row >= k || fabsf(vn - vrow[i]) <= 1e-8f + 1e-5f * fabsf(vrow[i]));
+      vrow[i] = vn;
+      if (row < k && cq == 0) {
+        v[row] = vn;                                 // nobody reads v before the barrier below (the iterate lives in vq)
+        it_out[(size_t)t * k + row] = vn;
+      }
+    }
+    bool all_ok = __all_sync(0xffffffffu, ok);
+    if (WPS > 1) {
+      if (lane == 0) red[4 + warp] = all_ok ? 1.f : 0.f;
+      __syncthreads();
+      all_ok = (red[4] + red[5] + red[6] + red[7]) == 4.f;
+    } else {
+      __syncwarp();
+    }
+    if (all_ok) mask |= (1u << t);
+#pragma unroll
+    for (int c = 0; c < CW; ++c) vq[c] = (c_lo + c < c_hi) ? v[c_lo + c] : 0.f;
+    // one warp: every lane has read v before the next iteration writes it.  Four warps need no third barrier: v and red[4..7]
+    // are next written behind the next iteration's first barrier, red[0..3] were read before this iteration's second one
+    if (WPS == 1) __syncwarp();
+  }
+  return mask;
+}
+
+// FFMA Gram: the k neighbour rows arrive with cp.async (16 bytes per lane, eight lanes per row) one 32-channel quarter at a
+// time, so the feature tile costs k x 128 B of shared memory instead of k x 512 B; 4 x 4 register blocks on or above the
+// diagonal accumulate over the four quarters in ascending channel order, one fp32 FMA each.  The 16-byte chunk index of a
+// feature row is XOR-swizzled by (row >> 2) & 7 so that the rows of different 4-row blocks fall into different banks (rows
+// of one block are read by lanes that share them: broadcasts).
 template <int WPS>
 __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
     const float* __restrict__ normed, const float* __restrict__ src, const float* __restrict__ tgt,
@@ -277,65 +353,17 @@ __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
     for (int t = tg; t < k * k; t += TS) dst[t] = M[(t / k) * ms + (t % k)];
   }
 
-  // power iteration from the all-ones vector; record every iterate and a convergence bit per iteration.
-  // Thread = (row group rg = tg >> 2, column quarter cq = tg & 3): rows rg + (TS / 4) i, the columns of quarter cq.
   uint32_t mask = 0u;
   float* it_out = iterates + nb1 * iters;
-  constexpr int RG = TS / 4;                         // row groups: 8 (one warp) or 32 (four warps)
-  const int rg = tg >> 2, cq = tg & 3;
-  const int CQ = (k + 3) >> 2;                       // columns per quarter
-  const int c_lo = cq * CQ, c_hi = min(k, c_lo + CQ);
-  if (WPS == 1 && k <= 40) {
-    // k = 40: 50 MACs per lane and iteration, the matrix slice held in registers for all iterations
-    constexpr int RI = 5, CW = 10;
-    float m[RI][CW], vq[CW], vrow[RI];
-#pragma unroll
-    for (int i = 0; i < RI; ++i) {
-      const int row = rg + 8 * i;
-#pragma unroll
-      for (int c = 0; c < CW; ++c) m[i][c] = (row < k && c_lo + c < c_hi) ? M[row * ms + c_lo + c] : 0.f;
-      vrow[i] = 1.0f;
-    }
-#pragma unroll
-    for (int c = 0; c < CW; ++c) vq[c] = (c_lo + c < c_hi) ? 1.0f : 0.f;
-    for (int t = 0; t < iters; ++t) {
-      float u[RI], ss = 0.f;
-#pragma unroll
-      for (int i = 0; i < RI; ++i) {
-        float p = 0.f;
-#pragma unroll
-        for (int c = 0; c < CW; ++c) p = fmaf(m[i][c], vq[c], p);
-        p += __shfl_xor_sync(0xffffffffu, p, 1);
-        p += __shfl_xor_sync(0xffffffffu, p, 2);
-        u[i] = p;
-        ss += (rg + 8 * i < k) ? p * p : 0.f;
-      }
-      ss += __shfl_xor_sync(0xffffffffu, ss, 4);
-      ss += __shfl_xor_sync(0xffffffffu, ss, 8);
-      ss += __shfl_xor_sync(0xffffffffu, ss, 16);
-      const float nrm = sqrtf(ss) + 1e-6f;
-      bool ok = true;
-#pragma unroll
-      for (int i = 0; i < RI; ++i) {
-        const int row = rg + 8 * i;
-        const float vn = u[i] / nrm;
-        // torch.allclose(new, last): |new - last| <= atol + rtol * |last|, atol 1e-8, rtol 1e-5
-        ok = ok && (row >= k || fabsf(vn - vrow[i]) <= 1e-8f + 1e-5f * fabsf(vrow[i]));
-        vrow[i] = vn;
-        if (row < k && cq == 0) {
-          v[row] = vn;
-          it_out[(size_t)t * k + row] = vn;
-        }
-      }
-      if (__all_sync(0xffffffffu, ok)) mask |= (1u << t);
-      __syncwarp();
-#pragma unroll
-      for (int c = 0; c < CW; ++c) vq[c] = (c_lo + c < c_hi) ? v[c_lo + c] : 0.f;
-      __syncwarp();
-    }
+  if constexpr (WPS == 1) {
+    mask = power_iteration_regs<1, 5, 10>(M, ms, k, v, red, it_out, iters, tg);
   } else {
-    // general k: the matrix stays in shared memory, rows rg + RG i (i < RI)
-    constexpr int RI = kMaxK / RG;                   // 16 (one warp) or 4 (four warps)
+    // up to k = 128 the matrix stays in shared memory: thread = (row group rg, column quarter cq), rows rg + 32 i (i < RI),
+    // in the same orders as power_iteration_regs
+    constexpr int RG = 32, RI = kMaxK / RG;
+    const int rg = tg >> 2, cq = tg & 3;
+    const int CQ = (k + 3) >> 2;                     // columns per quarter
+    const int c_lo = cq * CQ, c_hi = min(k, c_lo + CQ);
     float vrow[RI];
 #pragma unroll
     for (int i = 0; i < RI; ++i) vrow[i] = 1.0f;
@@ -357,14 +385,12 @@ __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
       ss += __shfl_xor_sync(0xffffffffu, ss, 4);
       ss += __shfl_xor_sync(0xffffffffu, ss, 8);
       ss += __shfl_xor_sync(0xffffffffu, ss, 16);
-      if (WPS > 1) {                                 // the four warps' sums, added in ascending warp order on every thread
-        if (lane == 0) red[warp] = ss;
-        __syncthreads();
-        ss = ((red[0] + red[1]) + red[2]) + red[3];
-      }
+      if (lane == 0) red[warp] = ss;
+      __syncthreads();
+      ss = ((red[0] + red[1]) + red[2]) + red[3];    // the four warps' sums in ascending warp order on every thread
       const float nrm = sqrtf(ss) + 1e-6f;
       bool ok = true;
-      seed_group_sync<WPS>();                        // every thread has read the old v (and red)
+      __syncthreads();                               // every thread has read the old v (and red)
 #pragma unroll
       for (int i = 0; i < RI; ++i) {
         const int row = rg + RG * i;
@@ -377,13 +403,9 @@ __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
         }
       }
       bool all_ok = __all_sync(0xffffffffu, ok);
-      if (WPS > 1) {
-        if (lane == 0) red[4 + warp] = all_ok ? 1.f : 0.f;
-        __syncthreads();
-        all_ok = (red[4] + red[5] + red[6] + red[7]) == 4.f;
-      } else {
-        __syncwarp();
-      }
+      if (lane == 0) red[4 + warp] = all_ok ? 1.f : 0.f;
+      __syncthreads();
+      all_ok = (red[4] + red[5] + red[6] + red[7]) == 4.f;
       if (all_ok) mask |= (1u << t);
     }
   }
@@ -392,22 +414,14 @@ __global__ void __launch_bounds__(WPS == 1 ? 256 : 128) nsm_power_kernel(
   if (tg == 0) atomicAnd(conv_mask + (size_t)b * mask_stride, mask);
 }
 
-// ---- k <= 40 in the tensor-core precisions: the Gram on the warp-level tensor-core path -------------------------------------
-// The FFMA kernel above spends 43 % of its ~12.7 k warp instructions per seed in the 40 x 40 x 128 Gram and 19 % in the
-// compatibility block.  Here one warp still owns one seed from the gather to the last iterate, but
-//   Gram     F F^T as fp16 hi/lo split products (hi*hi + hi*lo + lo*hi, fp32 accumulate: the arithmetic of the encoder's default
-//            mode and of the seed-row distances in knn_tc.cu) through mma.sync.m16n8k16.  The rows are padded to 48 = three
-//            16-row tiles; a lane loads its fragment elements STRAIGHT from the normalised rows in global memory (8 bytes per
-//            lane, the four lanes of a row cover one 32-byte sector; the next 16-channel step is in flight while the current one
-//            is multiplied) and splits each element exactly once: the A fragment of a 16-row tile is at the same time the B
-//            fragment of its two 8-column tiles.  Only the 9 tiles on or above the diagonal are computed (216 HMMA per seed).
-//            The features are L2-normalised (|x| <= 1): they are scaled by 2^6 before the split so that the low parts stay
-//            normal fp16 numbers, and the accumulator is scaled back by 2^-12 (both exact).
-//   compat   the accumulator fragment holds two neighbouring columns of a row: feature and spatial compatibility of the two
-//            matrix elements run as one paired chain (each lane rounded exactly like the scalar sequence of the
-//            FFMA kernel), key points staged as six arrays so that a column pair is one 8-byte load.
-//   power    unchanged (lane-parallel, matrix slice in registers).
-// No feature tile in shared memory: 8 KB per warp (M, key points, iterate).
+// ---- tensor-core Gram ------------------------------------------------------------------------------------------------------
+// F F^T as fp16 hi/lo split products (hi*hi + hi*lo + lo*hi, fp32 accumulate: the arithmetic of the encoder's default mode and
+// of the seed-row distances in knn_tc.cu) through mma.sync.m16n8k16, only the tiles on or above the diagonal.  The rows are
+// padded to whole 16-row tiles; a lane loads its fragment elements straight from the normalised rows in global memory (8 bytes
+// per lane, the four lanes of a row cover one 32-byte sector) and splits each element exactly once: the A fragment of a 16-row
+// tile is at the same time the B fragment of its two 8-column tiles.  The features are L2-normalised (|x| <= 1): they are
+// scaled by 2^6 before the split so that the low parts stay normal fp16 numbers, and the accumulator is scaled back by 2^-12
+// (both exact).  No feature tile in shared memory: per seed only M, the key points, the indices and the iterate.
 __device__ __forceinline__ void mma_f16_16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
                                               uint32_t b1) {
   asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
@@ -423,6 +437,67 @@ __device__ __forceinline__ void split_f16_pair(float a, float b, uint32_t& hi, u
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
+// The seed's neighbours, rows padded to ROWS, staged by threads tid, tid + nthreads, ...: the clamped indices (-1 on padding
+// rows), the key points as six arrays [ROWS] (src x y z, tgt x y z, zeros on padding rows), v = 1 and the zero diagonal of M.
+template <int ROWS>
+__device__ __forceinline__ void stage_neighbours(const int32_t* __restrict__ knn_idx, const float* __restrict__ src,
+                                                 const float* __restrict__ tgt, const SetDesc& d, size_t nb0, int ms, float* P,
+                                                 float* v, int* idx, float* M, int tid, int nthreads) {
+  for (int a = tid; a < ROWS; a += nthreads) {
+    int j = -1;
+    float sx = 0.f, sy = 0.f, sz = 0.f, tx = 0.f, ty = 0.f, tz = 0.f;
+    if (a < d.k) {
+      j = knn_idx[nb0 + a];
+      j = min(max(j, 0), d.N - 1);
+      const float* ps = src + ((size_t)d.row0 + j) * 3;
+      const float* pt = tgt + ((size_t)d.row0 + j) * 3;
+      sx = ps[0]; sy = ps[1]; sz = ps[2];
+      tx = pt[0]; ty = pt[1]; tz = pt[2];
+      M[a * ms + a] = 0.0f;                // total_knn_M[:, i, i] = 0  (PointDSC.py:278)
+    }
+    idx[a] = j;
+    P[a] = sx; P[ROWS + a] = sy; P[2 * ROWS + a] = sz;
+    P[3 * ROWS + a] = tx; P[4 * ROWS + a] = ty; P[5 * ROWS + a] = tz;
+    v[a] = 1.0f;
+  }
+}
+
+// Accumulator tile (i, j) of the Gram into M: element (half) holds row 16 i + g + 8 half, columns 8 j + 2 t, 8 j + 2 t + 1.
+// Feature and spatial compatibility of the two elements run as one paired chain, each lane rounded exactly like the scalar
+// sequence of nsm_power_kernel; the key points in P (six arrays [ROWS]) make a column pair one 8-byte load.
+template <int ROWS>
+__device__ __forceinline__ void compat_tile(const float (&acc)[4], int i, int j, int g, int t, const float* P, float* M, int k,
+                                            int ms, float sigma2, float rc_sigma2, float sigmad2, float rc_sigmad2) {
+  const int c = 8 * j + 2 * t;
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int a = 16 * i + g + 8 * half;
+    if (a < c + 1 && c < k) {              // at least the element (a, c + 1) or (a, c) is above the diagonal and real
+      const float2 dot = make_float2(acc[2 * half] * (1.0f / 4096.0f), acc[2 * half + 1] * (1.0f / 4096.0f));
+      const float2 one_minus = fsub2_scalar(1.0f, div_by_const2(fsub2_scalar(1.0f, dot), sigma2, rc_sigma2));
+      const float2 fm = make_float2(fmaxf(one_minus.x, 0.0f), fmaxf(one_minus.y, 0.0f));
+      const float2 la = length3_pow2(fsub2_scalar(P[a], *reinterpret_cast<const float2*>(P + c)),
+                                     fsub2_scalar(P[ROWS + a], *reinterpret_cast<const float2*>(P + ROWS + c)),
+                                     fsub2_scalar(P[2 * ROWS + a], *reinterpret_cast<const float2*>(P + 2 * ROWS + c)));
+      const float2 lb = length3_pow2(fsub2_scalar(P[3 * ROWS + a], *reinterpret_cast<const float2*>(P + 3 * ROWS + c)),
+                                     fsub2_scalar(P[4 * ROWS + a], *reinterpret_cast<const float2*>(P + 4 * ROWS + c)),
+                                     fsub2_scalar(P[5 * ROWS + a], *reinterpret_cast<const float2*>(P + 5 * ROWS + c)));
+      const float2 val = fmul2(fm, consistency_rc2(fsub2(la, lb), sigmad2, rc_sigmad2));
+      if (a < c) {
+        M[a * ms + c] = val.x;
+        M[c * ms + a] = val.x;
+      }
+      if (c + 1 < k) {                     // a < c + 1 holds
+        M[a * ms + c + 1] = val.y;
+        M[(c + 1) * ms + a] = val.y;
+      }
+    }
+  }
+}
+
+// ---- one warp per seed, k <= 40 -------------------------------------------------------------------------------------------
+// Rows padded to 48 = three 16-row tiles; the 9 tiles on or above the diagonal are 216 HMMA per seed.  The next 16-channel
+// step is in flight in registers while the current one is multiplied.
 constexpr int kMmaRows = 48;       // 40 neighbours padded to three 16-row tiles
 constexpr int kMmaTiles = 9;       // (i, j): 16-row tile i, 8-column tile j >= 2 i, j < 5
 
@@ -436,7 +511,7 @@ __global__ void __launch_bounds__(256, 2) nsm_power_mma_kernel(
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int b = blockIdx.y;
   const SetDesc d = sets[b];
-  const int N = d.N, S = d.S, k = d.k;
+  const int S = d.S, k = d.k;
   if (k < k_lo || k > k_hi) return;        // each kernel variant runs on the sets of its k range
   const int s = blockIdx.x * groups_per_cta + warp;
   if (s >= S) return;                      // whole warps leave: nothing below synchronises the block
@@ -447,23 +522,7 @@ __global__ void __launch_bounds__(256, 2) nsm_power_mma_kernel(
   float* M = reinterpret_cast<float*>(idx + kMmaRows);   // [k][ms]
   const size_t nb0 = (size_t)d.knn0 + (size_t)s * k;   // the seed's first neighbour slot
 
-  for (int a = lane; a < kMmaRows; a += 32) {
-    int j = -1;
-    float sx = 0.f, sy = 0.f, sz = 0.f, tx = 0.f, ty = 0.f, tz = 0.f;
-    if (a < k) {
-      j = knn_idx[nb0 + a];
-      j = min(max(j, 0), N - 1);
-      const float* ps = src + ((size_t)d.row0 + j) * 3;
-      const float* pt = tgt + ((size_t)d.row0 + j) * 3;
-      sx = ps[0]; sy = ps[1]; sz = ps[2];
-      tx = pt[0]; ty = pt[1]; tz = pt[2];
-      M[a * ms + a] = 0.0f;                // total_knn_M[:, i, i] = 0  (PointDSC.py:278)
-    }
-    idx[a] = j;
-    P[a] = sx; P[kMmaRows + a] = sy; P[2 * kMmaRows + a] = sz;
-    P[3 * kMmaRows + a] = tx; P[4 * kMmaRows + a] = ty; P[5 * kMmaRows + a] = tz;
-    v[a] = 1.0f;
-  }
+  stage_neighbours<kMmaRows>(knn_idx, src, tgt, d, nb0, ms, P, v, idx, M, lane, 32);
   __syncwarp();
 
   // ---- Gram ----
@@ -516,107 +575,27 @@ __global__ void __launch_bounds__(256, 2) nsm_power_mma_kernel(
     }
   }
 
-  // ---- compatibility: accumulator (q, half) = row 16 i + g + 8 half, columns 8 j + 2 t, 8 j + 2 t + 1 ----
   {
     int q = 0;
 #pragma unroll
-    for (int i = 0; i < 3; ++i) {
+    for (int i = 0; i < 3; ++i)
 #pragma unroll
-      for (int j = 2 * i; j < 5; ++j) {
-        const int c = 8 * j + 2 * t;
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          const int a = 16 * i + g + 8 * half;
-          if (a < c + 1 && c < k) {          // at least the element (a, c + 1) or (a, c) is above the diagonal and real
-            const float2 dot = make_float2(acc[q][2 * half] * (1.0f / 4096.0f), acc[q][2 * half + 1] * (1.0f / 4096.0f));
-            const float2 one_minus = fsub2_scalar(1.0f, div_by_const2(fsub2_scalar(1.0f, dot), sigma2, rc_sigma2));
-            const float2 fm = make_float2(fmaxf(one_minus.x, 0.0f), fmaxf(one_minus.y, 0.0f));
-            const float2 la = length3_pow2(fsub2_scalar(P[a], *reinterpret_cast<const float2*>(P + c)),
-                                           fsub2_scalar(P[kMmaRows + a], *reinterpret_cast<const float2*>(P + kMmaRows + c)),
-                                           fsub2_scalar(P[2 * kMmaRows + a], *reinterpret_cast<const float2*>(P + 2 * kMmaRows + c)));
-            const float2 lb = length3_pow2(fsub2_scalar(P[3 * kMmaRows + a], *reinterpret_cast<const float2*>(P + 3 * kMmaRows + c)),
-                                           fsub2_scalar(P[4 * kMmaRows + a], *reinterpret_cast<const float2*>(P + 4 * kMmaRows + c)),
-                                           fsub2_scalar(P[5 * kMmaRows + a], *reinterpret_cast<const float2*>(P + 5 * kMmaRows + c)));
-            const float2 val = fmul2(fm, consistency_rc2(fsub2(la, lb), sigmad2, rc_sigmad2));
-            if (a < c) {
-              M[a * ms + c] = val.x;
-              M[c * ms + a] = val.x;
-            }
-            if (c + 1 < k) {                 // a < c + 1 holds
-              M[a * ms + c + 1] = val.y;
-              M[(c + 1) * ms + a] = val.y;
-            }
-          }
-        }
-        ++q;
-      }
-    }
+      for (int j = 2 * i; j < 5; ++j)
+        compat_tile<kMmaRows>(acc[q++], i, j, g, t, P, M, k, ms, sigma2, rc_sigma2, sigmad2, rc_sigmad2);
   }
   __syncwarp();
   if (compat_out) {
     float* dst = compat_out + nb0 * k;
     for (int e = lane; e < k * k; e += 32) dst[e] = M[(e / k) * ms + (e % k)];
   }
-
-  // ---- power iteration from the all-ones vector (as in nsm_power_kernel<1>, k <= 40) ----
-  uint32_t mask = 0u;
-  float* it_out = iterates + nb0 * iters;
-  const int rg = lane >> 2, cq = lane & 3;
-  const int CQ = (k + 3) >> 2;                       // columns per quarter
-  const int c_lo = cq * CQ, c_hi = min(k, c_lo + CQ);
-  constexpr int RI = 5, CW = 10;
-  float m[RI][CW], vq[CW], vrow[RI];
-#pragma unroll
-  for (int i = 0; i < RI; ++i) {
-    const int row = rg + 8 * i;
-#pragma unroll
-    for (int c = 0; c < CW; ++c) m[i][c] = (row < k && c_lo + c < c_hi) ? M[row * ms + c_lo + c] : 0.f;
-    vrow[i] = 1.0f;
-  }
-#pragma unroll
-  for (int c = 0; c < CW; ++c) vq[c] = (c_lo + c < c_hi) ? 1.0f : 0.f;
-  for (int it = 0; it < iters; ++it) {
-    float u[RI], ss = 0.f;
-#pragma unroll
-    for (int i = 0; i < RI; ++i) {
-      float p = 0.f;
-#pragma unroll
-      for (int c = 0; c < CW; ++c) p = fmaf(m[i][c], vq[c], p);
-      p += __shfl_xor_sync(0xffffffffu, p, 1);
-      p += __shfl_xor_sync(0xffffffffu, p, 2);
-      u[i] = p;
-      ss += (rg + 8 * i < k) ? p * p : 0.f;
-    }
-    ss += __shfl_xor_sync(0xffffffffu, ss, 4);
-    ss += __shfl_xor_sync(0xffffffffu, ss, 8);
-    ss += __shfl_xor_sync(0xffffffffu, ss, 16);
-    const float nrm = sqrtf(ss) + 1e-6f;
-    bool ok = true;
-#pragma unroll
-    for (int i = 0; i < RI; ++i) {
-      const int row = rg + 8 * i;
-      const float vn = u[i] / nrm;
-      // torch.allclose(new, last): |new - last| <= atol + rtol * |last|, atol 1e-8, rtol 1e-5
-      ok = ok && (row >= k || fabsf(vn - vrow[i]) <= 1e-8f + 1e-5f * fabsf(vrow[i]));
-      vrow[i] = vn;
-      if (row < k && cq == 0) {
-        v[row] = vn;
-        it_out[(size_t)it * k + row] = vn;
-      }
-    }
-    if (__all_sync(0xffffffffu, ok)) mask |= (1u << it);
-    __syncwarp();
-#pragma unroll
-    for (int c = 0; c < CW; ++c) vq[c] = (c_lo + c < c_hi) ? v[c_lo + c] : 0.f;
-    __syncwarp();
-  }
+  const uint32_t mask = power_iteration_regs<1, 5, 10>(M, ms, k, v, nullptr, iterates + nb0 * iters, iters, lane);
   if (lane == 0) atomicAnd(conv_mask + (size_t)b * mask_stride, mask);
 }
 
-// ---- 40 < k <= 80 in the tensor-core precisions (BASELINE config C: k = 80): the same tensor-core Gram, four warps per seed ----
+// ---- four warps per seed, 40 < k <= 80 ------------------------------------------------------------------------------------
 // Rows padded to 80 = five 16-row tiles x ten 8-column tiles; the 30 tiles on or above the diagonal are dealt to the four warps
 // by 16-row tile so that a warp's A fragments are shared by its tiles (7 / 8 / 8 / 7 tiles; a warp loads and splits only the row
-// groups its tiles touch).  Compatibility as in nsm_power_mma_kernel; the power iteration is the four-warp one of nsm_power_kernel<4>.
+// groups its tiles touch).
 constexpr int kMma4Rows = 80;
 __host__ __device__ constexpr int mma4_count(int w) { return (w == 0 || w == 3) ? 7 : 8; }
 // tile q of warp w: 16-row tile i, 8-column tile j
@@ -688,36 +667,9 @@ __device__ __forceinline__ void mma4_gram_and_compat(const float* __restrict__ n
       mma_f16_16816(acc[q], lo[2 * i][0], lo[2 * i + 1][0], lo[2 * i][1], lo[2 * i + 1][1], hi[j][0], hi[j][1]);
     }
   }
-  // compatibility: accumulator (q, half) = row 16 i + g + 8 half, columns 8 j + 2 t, 8 j + 2 t + 1
 #pragma unroll
-  for (int q = 0; q < NT; ++q) {
-    const int i = mma4_i(W, q), j = mma4_j(W, q);
-    const int c = 8 * j + 2 * t;
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      const int a = 16 * i + g + 8 * half;
-      if (a < c + 1 && c < k) {
-        const float2 dot = make_float2(acc[q][2 * half] * (1.0f / 4096.0f), acc[q][2 * half + 1] * (1.0f / 4096.0f));
-        const float2 one_minus = fsub2_scalar(1.0f, div_by_const2(fsub2_scalar(1.0f, dot), sigma2, rc_sigma2));
-        const float2 fm = make_float2(fmaxf(one_minus.x, 0.0f), fmaxf(one_minus.y, 0.0f));
-        const float2 la = length3_pow2(fsub2_scalar(P[a], *reinterpret_cast<const float2*>(P + c)),
-                                       fsub2_scalar(P[kMma4Rows + a], *reinterpret_cast<const float2*>(P + kMma4Rows + c)),
-                                       fsub2_scalar(P[2 * kMma4Rows + a], *reinterpret_cast<const float2*>(P + 2 * kMma4Rows + c)));
-        const float2 lb = length3_pow2(fsub2_scalar(P[3 * kMma4Rows + a], *reinterpret_cast<const float2*>(P + 3 * kMma4Rows + c)),
-                                       fsub2_scalar(P[4 * kMma4Rows + a], *reinterpret_cast<const float2*>(P + 4 * kMma4Rows + c)),
-                                       fsub2_scalar(P[5 * kMma4Rows + a], *reinterpret_cast<const float2*>(P + 5 * kMma4Rows + c)));
-        const float2 val = fmul2(fm, consistency_rc2(fsub2(la, lb), sigmad2, rc_sigmad2));
-        if (a < c) {
-          M[a * ms + c] = val.x;
-          M[c * ms + a] = val.x;
-        }
-        if (c + 1 < k) {
-          M[a * ms + c + 1] = val.y;
-          M[(c + 1) * ms + a] = val.y;
-        }
-      }
-    }
-  }
+  for (int q = 0; q < NT; ++q)
+    compat_tile<kMma4Rows>(acc[q], mma4_i(W, q), mma4_j(W, q), g, t, P, M, k, ms, sigma2, rc_sigma2, sigmad2, rc_sigmad2);
 }
 
 __global__ void __launch_bounds__(128, 4) nsm_power_mma4_kernel(
@@ -730,7 +682,7 @@ __global__ void __launch_bounds__(128, 4) nsm_power_mma4_kernel(
   const int tg = threadIdx.x, lane = tg & 31, warp = tg >> 5;
   const int b = blockIdx.y, s = blockIdx.x;
   const SetDesc d = sets[b];
-  const int N = d.N, k = d.k;
+  const int k = d.k;
   if (k < k_lo || k > k_hi || s >= d.S) return;   // the sets of this variant's k range; the whole CTA leaves
   const int ms = k | 1;
   float* P = sm;                                       // six coordinate arrays [80]
@@ -740,23 +692,7 @@ __global__ void __launch_bounds__(128, 4) nsm_power_mma4_kernel(
   float* M = red + 8;                                  // [k][ms]
   const size_t nb0 = (size_t)d.knn0 + (size_t)s * k;   // the seed's first neighbour slot
 
-  for (int a = tg; a < kMma4Rows; a += 128) {
-    int j = -1;
-    float sx = 0.f, sy = 0.f, sz = 0.f, tx = 0.f, ty = 0.f, tz = 0.f;
-    if (a < k) {
-      j = knn_idx[nb0 + a];
-      j = min(max(j, 0), N - 1);
-      const float* ps = src + ((size_t)d.row0 + j) * 3;
-      const float* pt = tgt + ((size_t)d.row0 + j) * 3;
-      sx = ps[0]; sy = ps[1]; sz = ps[2];
-      tx = pt[0]; ty = pt[1]; tz = pt[2];
-      M[a * ms + a] = 0.0f;                // total_knn_M[:, i, i] = 0  (PointDSC.py:278)
-    }
-    idx[a] = j;
-    P[a] = sx; P[kMma4Rows + a] = sy; P[2 * kMma4Rows + a] = sz;
-    P[3 * kMma4Rows + a] = tx; P[4 * kMma4Rows + a] = ty; P[5 * kMma4Rows + a] = tz;
-    v[a] = 1.0f;
-  }
+  stage_neighbours<kMma4Rows>(knn_idx, src, tgt, d, nb0, ms, P, v, idx, M, tg, 128);
   __syncthreads();
   const size_t set_row0 = (size_t)d.row0;
   if (warp == 0) mma4_gram_and_compat<0>(normed, set_row0, idx, P, M, k, ms, lane, sigma2, rc_sigma2, sigmad2, rc_sigmad2);
@@ -768,67 +704,7 @@ __global__ void __launch_bounds__(128, 4) nsm_power_mma4_kernel(
     float* dst = compat_out + nb0 * k;
     for (int e = tg; e < k * k; e += 128) dst[e] = M[(e / k) * ms + (e % k)];
   }
-
-  // power iteration from the all-ones vector (the four-warp form of nsm_power_kernel<4>): thread = (row group rg, column
-  // quarter cq), rows rg + 32 i; the thread's 3 x 20 slice of the matrix stays in registers for all iterations (columns beyond
-  // the quarter are zeros: fma(0, 0, p) == p, so the sums are those of the shared-memory form bit for bit)
-  uint32_t mask = 0u;
-  float* it_out = iterates + nb0 * iters;
-  constexpr int RG = 32, RI = 3, CW = 20;            // rows rg + 32 i < 96 and 4 x 20 columns cover k <= 80
-  const int rg = tg >> 2, cq = tg & 3;
-  const int CQ = (k + 3) >> 2;
-  const int c_lo = cq * CQ, c_hi = min(k, c_lo + CQ);
-  float mreg[RI][CW], vq[CW], vrow[RI];
-#pragma unroll
-  for (int i = 0; i < RI; ++i) {
-    const int row = rg + RG * i;
-#pragma unroll
-    for (int c = 0; c < CW; ++c) mreg[i][c] = (row < k && c_lo + c < c_hi) ? M[row * ms + c_lo + c] : 0.f;
-    vrow[i] = 1.0f;
-  }
-#pragma unroll
-  for (int c = 0; c < CW; ++c) vq[c] = (c_lo + c < c_hi) ? 1.0f : 0.f;
-  for (int t = 0; t < iters; ++t) {
-    float u[RI], ss = 0.f;
-#pragma unroll
-    for (int i = 0; i < RI; ++i) {
-      float p = 0.f;
-#pragma unroll
-      for (int c = 0; c < CW; ++c) p = fmaf(mreg[i][c], vq[c], p);
-      p += __shfl_xor_sync(0xffffffffu, p, 1);
-      p += __shfl_xor_sync(0xffffffffu, p, 2);
-      u[i] = p;
-      ss += (rg + RG * i < k) ? p * p : 0.f;
-    }
-    ss += __shfl_xor_sync(0xffffffffu, ss, 4);
-    ss += __shfl_xor_sync(0xffffffffu, ss, 8);
-    ss += __shfl_xor_sync(0xffffffffu, ss, 16);
-    if (lane == 0) red[warp] = ss;
-    __syncthreads();
-    ss = ((red[0] + red[1]) + red[2]) + red[3];      // the four warps' sums in ascending warp order on every thread
-    const float nrm = sqrtf(ss) + 1e-6f;
-    bool ok = true;
-#pragma unroll
-    for (int i = 0; i < RI; ++i) {
-      const int row = rg + RG * i;
-      const float vn = u[i] / nrm;
-      ok = ok && (row >= k || fabsf(vn - vrow[i]) <= 1e-8f + 1e-5f * fabsf(vrow[i]));
-      vrow[i] = vn;
-      if (row < k && cq == 0) {
-        v[row] = vn;                                 // nobody reads v before the barrier below (the iterate lives in vq)
-        it_out[(size_t)t * k + row] = vn;
-      }
-    }
-    bool all_ok = __all_sync(0xffffffffu, ok);
-    if (lane == 0) red[4 + warp] = all_ok ? 1.f : 0.f;
-    __syncthreads();
-    all_ok = (red[4] + red[5] + red[6] + red[7]) == 4.f;
-    if (all_ok) mask |= (1u << t);
-#pragma unroll
-    for (int c = 0; c < CW; ++c) vq[c] = (c_lo + c < c_hi) ? v[c_lo + c] : 0.f;
-    // no third barrier: v and red[4..7] are next written behind the next iteration's first barrier, red[0..3] were read before
-    // this iteration's second one
-  }
+  const uint32_t mask = power_iteration_regs<4, 3, 20>(M, ms, k, v, red, iterates + nb0 * iters, iters, tg);
   if (tg == 0) atomicAnd(conv_mask + (size_t)b * mask_stride, mask);
 }
 
@@ -883,9 +759,6 @@ void launch_nsm_power(const float* normed, const float* src, const float* tgt, c
                       uint32_t* conv_mask, float* compat_out, int B, int N, int S, int k, int iters, float sigma,
                       float sigma_d, int mask_stride, int tensor_gram, cudaStream_t st, const SetDesc* sets, int k_min) {
   if (S <= 0) return;
-  // developer switch for same-box A/B of the two Gram paths (tools/exp_variant.sh style): PDSC_NSM_FFMA=1 forces the FFMA kernels
-  static const bool force_ffma = [] { const char* v = getenv("PDSC_NSM_FFMA"); return v && v[0] == '1'; }();
-  if (force_ffma) tensor_gram = 0;
   // the sets may differ in k (N_b <= cfg.k): each set runs the variant of its own k
   const int bounds[3][2] = {{1, 40}, {41, tensor_gram ? kMma4Rows : kMaxK}, {kMma4Rows + 1, kMaxK}};
   for (int r = 0; r < (tensor_gram ? 3 : 2); ++r) {

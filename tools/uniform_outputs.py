@@ -4,11 +4,13 @@
     python tools/uniform_outputs.py --out DIR/uniform_outputs.npz
     python tools/uniform_outputs.py --compare A.npz B.npz
 
-Seeded synthetic pairs (pointdsc_b200.synth, released 3DMatch weights) at N = 41, 257, 1003 and 5000 in every precision.
-N = 5000 at bs = 1 runs the attention's key split, the others are too small to split or split into few chunks.  Per (precision,
-N) the file holds the testing-mode forward with every stage tap (SC, features, the layer-0 internals, seeds, kNN, compatibility,
-eigenvectors, hypotheses, refinement) and the eval-mode forward (confidence, M) with its taps.  --compare exits non-zero unless
-both files hold the same arrays with the same bytes."""
+Seeded synthetic pairs (pointdsc_b200.synth, released 3DMatch weights) at N = 41, 257, 1003 and 5000 in every precision with
+k = 40, and at N = 41, 257 and 1003 in fp32 and fp16x3 with k = 80 and k = 128 (keys "<precision>/k<k>/..."), so that every
+NSM kernel runs: N = 41 falls back to k = 40 under the larger configurations.  N = 5000 at bs = 1 runs the attention's key
+split, the others are too small to split or split into few chunks.  Per (precision, k, N) the file holds the testing-mode
+forward with every stage tap (SC, features, the layer-0 internals, seeds, kNN, compatibility, eigenvectors, hypotheses,
+refinement) and the eval-mode forward (confidence, M) with its taps.  --compare exits non-zero unless both files hold the same
+arrays with the same bytes."""
 import argparse
 import os
 import sys
@@ -21,6 +23,8 @@ sys.path.insert(0, ROOT)
 
 SIZES = (41, 257, 1003, 5000)
 PRECISIONS = ("fp32", "fp16x3", "bf16x3", "bf16")
+# (k, precisions, sizes) beside k = 40: k = 80 and 128 reach the four-warp NSM kernels of both Gram forms
+LARGE_K = ((80, ("fp32", "fp16x3"), (41, 257, 1003)), (128, ("fp32", "fp16x3"), (41, 257, 1003)))
 TAPS = ("sc", "features", "normed", "confidence", "seeds", "knn_idx", "compat", "eig", "power_iters", "seed_trans",
         "inlier_counts", "best", "init_trans", "refine_solves", "layer_features", "layer_debug")
 EVAL_TAPS = ("features", "confidence", "seeds", "knn_idx", "compat", "eig", "power_iters", "seed_trans", "inlier_counts",
@@ -32,17 +36,19 @@ def collect():
     from pointdsc_b200 import PointDSC
     from pointdsc_b200.synth import make_pair
     out = {}
-    for precision in PRECISIONS:
-        m = PointDSC(num_layers=12, k=40, precision=precision, **bench.CTOR["3dmatch"])
+    configs = [(40, precision, SIZES, "") for precision in PRECISIONS]
+    configs += [(k, precision, sizes, f"k{k}/") for k, precisions, sizes in LARGE_K for precision in precisions]
+    for k, precision, sizes, prefix in configs:
+        m = PointDSC(num_layers=12, k=k, precision=precision, **bench.CTOR["3dmatch"])
         m.load_state_dict(bench.load_snapshot("3dmatch"), strict=False)
         m = m.cuda().eval()
-        for n in SIZES:
+        for n in sizes:
             p = make_pair(n, n, "3dmatch", 0.3)
             cp, s, t = (p[key][None].cuda() for key in ("corr_pos", "src_keypts", "tgt_keypts"))
             for mode, res in (("test", m.run(cp, s, t, taps=TAPS)), ("eval", m.run_eval(cp, s, t, taps=EVAL_TAPS))):
                 for name, v in res.items():
                     if v is not None:
-                        out[f"{precision}/{n}/{mode}/{name}"] = v.cpu().numpy()
+                        out[f"{precision}/{prefix}{n}/{mode}/{name}"] = v.cpu().numpy()
         torch.cuda.synchronize()
     return out
 
