@@ -92,9 +92,11 @@ def gt_labels(data, gt_trans, inlier_threshold):
     return ((warped - tgt).pow(2).sum(-1).sqrt() < inlier_threshold).float()[None]
 
 
-def build_model(snapshot, cfg, device, precision=None):
+def build_model(snapshot, cfg, device, precision=None, batch_invariant=False):
     from pointdsc_b200 import PointDSC
-    kw = {} if precision is None else {"precision": precision}
+    kw = {"batch_invariant": batch_invariant}
+    if precision is not None:
+        kw["precision"] = precision
     model = PointDSC(in_dim=cfg["in_dim"], num_layers=cfg["num_layers"], num_channels=cfg["num_channels"],
                      num_iterations=cfg["num_iterations"], ratio=cfg["ratio"], sigma_d=cfg["sigma_d"], k=cfg["k"],
                      nms_radius=cfg["inlier_threshold"], **kw)                           # evaluation/test_3DMatch.py:215-224
@@ -225,7 +227,7 @@ def summarise(stats, scene_names=None, log=print):
             "scene_recall": float(avg[0])}
 
 
-def main(argv=None):
+def parse_args(argv=None):
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--chosen_snapshot", default="PointDSC_3DMatch_release", choices=sorted(GOLDEN))
     ap.add_argument("--root", default="/data/3DMatch", help="data set root in the reference's layout (fragments/, gt_result/)")
@@ -236,10 +238,16 @@ def main(argv=None):
     ap.add_argument("--save_npy", default=None, help="write the [pairs, 13] statistics table here")
     ap.add_argument("--batch_size", type=int, default=1,
                     help="pairs per forward: > 1 runs every group of pairs (of different sizes) as one mixed-size call")
-    args = ap.parse_args(argv)
+    ap.add_argument("--batch_invariant", action="store_true",
+                    help="every pair's result independent of --batch_size and of the GPU's SM count (PointDSC batch_invariant)")
+    return ap.parse_args(argv)
+
+
+def main(argv=None):
+    args = parse_args(argv)
     cfg = load_config(args.chosen_snapshot)
     descriptor = args.descriptor or cfg["descriptor"]
-    model = build_model(args.chosen_snapshot, cfg, "cuda", args.precision)
+    model = build_model(args.chosen_snapshot, cfg, "cuda", args.precision, args.batch_invariant)
     if args.synthetic > 0:
         pairs, names = synthetic_pairs(args.synthetic, "cuda", 1.6 * cfg["downsample"]), ["synthetic-a", "synthetic-b"]
     else:

@@ -121,6 +121,16 @@ int pdsc_set_param(pdsc_engine* e, const char* name, const float* h_data, int64_
 int pdsc_commit_params(pdsc_engine* e);
 int pdsc_set_precision(pdsc_engine* e, int32_t precision);
 
+/* Batch-invariant mode (off by default).  On: the tensor-core attention splits every set along its keys by a rule of the
+ * set's N alone (chunks of PDSC_ATTN_INVARIANT_TILES = 8 key tiles, sets.cuh), in every call, so a set's outputs are bit for
+ * bit the same whatever else its call holds (batch size, other sets, their order), whichever entry point runs it and
+ * whatever the device's SM count.  Applies to pdsc_forward, _packed, _graph, _host, _host_submit / _wait and
+ * pdsc_forward_eval (the validation forward's transform still depends on its batch: the early exit spans the batch);
+ * pdsc_workspace_bytes* and pdsc_launches_per_forward report the mode's sizes and merge launches.  Graphs captured in one
+ * mode are never replayed in the other.  In PDSC_FP32_SIMT the flag is accepted and changes nothing: that attention never
+ * splits.  Off: the default key split, whose choice depends on the whole call and the SM count (DESIGN.md §3). */
+int pdsc_set_batch_invariant(pdsc_engine* e, int32_t enable);
+
 /* ---- sizes ------------------------------------------------------------------------------------- */
 int32_t pdsc_num_seeds(const pdsc_engine* e, int32_t N);       /* S = int(N * ratio)          */
 int32_t pdsc_num_neighbours(const pdsc_engine* e, int32_t N);  /* k = min(cfg.k, N - 1)       */
@@ -141,7 +151,8 @@ int pdsc_forward(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr_pos, 
  * R = offsets[B].  d_corr_pos [R,6], d_src_keypts [R,3], d_tgt_keypts [R,3]  ->  d_final_trans [B,4,4],
  * d_final_labels [R].  h_offsets (host) sizes the launches and the workspace; d_offsets (device, caller-owned, the same
  * values) is what the kernels read.  A set's outputs depend only on its own rows, its N_b and the call's attention regime:
- * within one regime they are bit for bit those of a pdsc_forward() call holding that set (DESIGN.md §3).  No host
+ * within one regime they are bit for bit those of a pdsc_forward() call holding that set (DESIGN.md §3); in the
+ * batch-invariant mode (pdsc_set_batch_invariant) there is one regime, so they are in every call.  No host
  * synchronisation, no allocation, capturable in a CUDA graph.  PDSC_ERR_SHAPE for B < 1, offsets[0] != 0, a set with
  * N_b < 2 (non-increasing offsets) or N_b above the supported maximum; pdsc_workspace_bytes_packed() returns 0 for such
  * offsets. */

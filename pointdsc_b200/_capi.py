@@ -55,6 +55,7 @@ SYMBOLS = {
     "pdsc_set_param": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64]),
     "pdsc_commit_params": (C.c_int, [C.c_void_p]),
     "pdsc_set_precision": (C.c_int, [C.c_void_p, C.c_int32]),
+    "pdsc_set_batch_invariant": (C.c_int, [C.c_void_p, C.c_int32]),
     "pdsc_num_seeds": (C.c_int32, [C.c_void_p, C.c_int32]),
     "pdsc_num_neighbours": (C.c_int32, [C.c_void_p, C.c_int32]),
     "pdsc_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_int32]),

@@ -4,6 +4,7 @@
 // driven from different host threads).
 #include <cuda_runtime.h>
 
+#include <cstdlib>
 #include <map>
 #include <mutex>
 
@@ -34,11 +35,27 @@ cudaError_t ensure_dynamic_smem(const void* kernel, int bytes) {
   return e;
 }
 
+// PDSC_SM_COUNT=<n> (developer override, read once): size every SM-count-dependent launch and split as if the device had
+// min(n, its real count) SMs, so that a test can check which results do not depend on the SM count.  Unset or not a
+// positive integer: the real count.
+static int sm_count_override() {
+  const char* s = std::getenv("PDSC_SM_COUNT");
+  if (!s || !*s) return 0;
+  char* end = nullptr;
+  const long v = std::strtol(s, &end, 10);
+  return (*end == '\0' && v > 0 && v < (1L << 20)) ? (int)v : 0;
+}
+
 int device_sm_count() {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return 0;
+  static const int forced = sm_count_override();
   std::lock_guard<std::mutex> lock(g_mu);
-  if (g_dev[dev].num_sms == 0) cudaDeviceGetAttribute(&g_dev[dev].num_sms, cudaDevAttrMultiProcessorCount, dev);
+  if (g_dev[dev].num_sms == 0) {
+    int n = 0;
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    g_dev[dev].num_sms = (forced > 0 && forced < n) ? forced : n;
+  }
   return g_dev[dev].num_sms;
 }
 

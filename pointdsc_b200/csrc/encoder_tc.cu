@@ -114,10 +114,16 @@ static inline int q_tiles(int N) { return (N + 127) / 128; }
 
 // key split of the attention (small calls): at most this many work items, each with a 64 KB partial O and 1 KB of (m, l)
 constexpr int kAttnSplitMaxItems = 320;
-constexpr size_t kAttnSplitBytes = (size_t)kAttnSplitMaxItems * (65536 + 1024);
+constexpr size_t kAttnPartialBytes = 65536 + 1024;
 
-size_t tc_scratch_bytes_tiles(long long qtiles, long long ktiles) {
-  return ((size_t)qtiles + (size_t)ktiles) * 65536 + 1024 + kAttnSplitBytes;
+// work items whose partial results the scratch holds: a fixed kAttnSplitMaxItems in the default mode (its split is capped
+// there), every work item of a split call in the batch-invariant mode
+static size_t partial_items(int invariant, int attn_split, int attn_items) {
+  return invariant ? (attn_split ? (size_t)attn_items : 0) : (size_t)kAttnSplitMaxItems;
+}
+
+size_t tc_scratch_bytes_tiles(long long qtiles, long long ktiles, int invariant, int attn_split, int attn_items) {
+  return ((size_t)qtiles + (size_t)ktiles) * 65536 + 1024 + partial_items(invariant, attn_split, attn_items) * kAttnPartialBytes;
 }
 
 // Key split policy.  When a call's (set, query tile) items cover at most half of the SMs (the evaluation loops' bs = 1:
@@ -126,16 +132,20 @@ size_t tc_scratch_bytes_tiles(long long qtiles, long long ktiles) {
 // agree bit for bit whatever their batch size, and so do calls of the large regime (no split); across the two regimes the
 // softmax sums are associated differently (fp32 rounding, far inside the parity bar).  A call whose split would exceed
 // kAttnSplitMaxItems work items, or in which no set would split, is not split.
-int tc_packed_split(const int* Ns, int B, int* items) {
-  const int num_sms = device_sm_count();
+// Batch-invariant mode: every set is split by attn_set_split_invariant (its N alone) in every call; the call runs the merge
+// whenever one of its sets has sp > 1.  No regime, no item cap: the partial buffers are sized by the call's items.
+int tc_packed_split(const int* Ns, int B, int invariant, int* items) {
+  const int num_sms = invariant ? 0 : device_sm_count();
   long long qtiles = 0, split_items = 0;
   for (int b = 0; b < B; ++b) {
     int sp, ts;
-    attn_set_split(Ns[b], num_sms, &sp, &ts);
+    if (invariant) attn_set_split_invariant(Ns[b], &sp, &ts);
+    else attn_set_split(Ns[b], num_sms, &sp, &ts);
     qtiles += q_tiles(Ns[b]);
     split_items += (long long)q_tiles(Ns[b]) * sp;
   }
-  const bool split = 2 * qtiles <= num_sms && split_items > qtiles && split_items <= kAttnSplitMaxItems;
+  const bool split = invariant ? split_items > qtiles
+                               : 2 * qtiles <= num_sms && split_items > qtiles && split_items <= kAttnSplitMaxItems;
   *items = (int)(split ? split_items : qtiles);
   return split ? 1 : 0;
 }
@@ -213,7 +223,7 @@ static int tc_encoder_forward_fmt(const TcWeights& w, const TcForwardArgs& a, cu
   qimg = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(qimg) + 1023) & ~uintptr_t(1023));
   uint8_t* kvimg = qimg + (size_t)a.qtiles * 65536;
   float* part_o = reinterpret_cast<float*>(kvimg + (size_t)a.ktiles * 65536);
-  float* part_ml = part_o + (size_t)kAttnSplitMaxItems * 128 * kC;
+  float* part_ml = part_o + partial_items(a.attn_invariant, a.attn_split, a.attn_items) * 128 * kC;
   const long long tiles = (rows + 127) / 128;
   const int num_sms = device_sm_count();
   if (num_sms <= 0) return (int)cudaErrorInvalidDevice;

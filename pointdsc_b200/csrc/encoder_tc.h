@@ -30,7 +30,7 @@ struct TcForwardArgs {
   float* feat;               // [rows][128]  layer output / final features
   float* feat1;              // [rows][128]  PointCN output (residual source)
   float* msg;                // [rows][128]  attention output
-  void* scratch;             // tc_scratch_bytes_tiles(qtiles, ktiles)
+  void* scratch;             // tc_scratch_bytes_tiles(qtiles, ktiles, attn_invariant, attn_split, attn_items)
   int layer_tap;             // -1 or layer index to copy out
   float* layer_tap_out;
   int debug_layer;           // layer whose internals are decoded into debug_out
@@ -42,13 +42,15 @@ struct TcForwardArgs {
   long long qtiles, ktiles;  // query / key tiles of all sets
   int attn_items;            // attention work items (tc_packed_split)
   int attn_split;            // 1: the call is in the key-split regime
+  int attn_invariant;        // 1: batch-invariant key split (attn_set_split_invariant)
 };
 
 int tc_build_weights(const TcLayerHost* layers, int num_layers, TcWeights* out);  // returns cudaError_t
 void tc_free_weights(TcWeights* w);
-size_t tc_scratch_bytes_tiles(long long qtiles, long long ktiles);
-// key-split decision of a call of sets of Ns[0..B) rows: returns 1 in the split regime; *items = attention work items
-int tc_packed_split(const int* Ns, int B, int* items);
+size_t tc_scratch_bytes_tiles(long long qtiles, long long ktiles, int invariant, int attn_split, int attn_items);
+// key-split decision of a call of sets of Ns[0..B) rows (invariant: the batch-invariant rule): returns 1 if the call runs
+// the merge; *items = attention work items
+int tc_packed_split(const int* Ns, int B, int invariant, int* items);
 int tc_launches(int num_layers, int attn_split);
 int tc_encoder_forward(const TcWeights& w, const TcForwardArgs& a, cudaStream_t st);  // returns cudaError_t
 

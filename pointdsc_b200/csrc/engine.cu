@@ -63,6 +63,7 @@ struct LayerOffsets {  // offsets (in floats) into the device weight arena
 
 struct pdsc_engine {
   pdsc_config cfg{};
+  bool batch_invariant = false;   // pdsc_set_batch_invariant: the attention's key split is a function of each set's N alone
   std::map<std::string, std::vector<float>> params;
   bool committed = false;
   float sigma = 1.0f;       // learned `sigma`      (PointDSC.py:97)
@@ -109,6 +110,7 @@ struct pdsc_engine {
     int B, N;
     const void *corr_pos, *src, *tgt, *trans, *labels, *workspace;
     int precision;
+    bool batch_invariant;
     cudaGraphExec_t exec;
   };
   std::vector<GraphEntry> graphs;
@@ -154,6 +156,7 @@ struct CallShape {
   size_t seeds = 0, dist = 0, knn = 0;    // seed slots, seed-row distance floats, neighbour slots
   long long qtiles = 0, ktiles = 0;
   int attn_items = 0, attn_split = 0;     // tensor-core calls (tc_packed_split)
+  int attn_invariant = 0;                 // the engine's key-split policy (pdsc_set_batch_invariant)
 };
 
 // h_offsets: the validated offsets of a packed call, or nullptr for a uniform call of B sets of N rows
@@ -177,7 +180,8 @@ CallShape call_shape(const pdsc_engine* e, int B, int N_uniform, const int32_t* 
     s.qtiles += (N + 127) / 128;
     s.ktiles += (N + 63) / 64;
   }
-  if (e->cfg.precision != PDSC_FP32_SIMT) s.attn_split = pdsc::tc_packed_split(Ns.data(), B, &s.attn_items);
+  s.attn_invariant = e->batch_invariant ? 1 : 0;
+  if (e->cfg.precision != PDSC_FP32_SIMT) s.attn_split = pdsc::tc_packed_split(Ns.data(), B, s.attn_invariant, &s.attn_items);
   return s;
 }
 
@@ -199,7 +203,7 @@ Workspace carve(const pdsc_engine* e, void* ptr, const CallShape& sh) {
     w.h2 = c.take<float>(R * 64);
     w.tc_scratch = nullptr;
   } else {
-    w.tc_scratch = c.take<char>(pdsc::tc_scratch_bytes_tiles(sh.qtiles, sh.ktiles));
+    w.tc_scratch = c.take<char>(pdsc::tc_scratch_bytes_tiles(sh.qtiles, sh.ktiles, sh.attn_invariant, sh.attn_split, sh.attn_items));
   }
   w.normed = c.take<float>(R * kC);
   w.conf = c.take<float>(R);
@@ -322,7 +326,8 @@ __device__ __forceinline__ long long warp_scan_incl(long long v, int lane) {
 }
 
 __global__ void set_table_kernel(const int32_t* __restrict__ offsets, int N_uniform, int B, double ratio, int k_cfg, int tiled,
-                                 int split, int num_sms, pdsc::SetDesc* __restrict__ table, int32_t* __restrict__ tile_set) {
+                                 int split, int invariant, int num_sms, pdsc::SetDesc* __restrict__ table,
+                                 int32_t* __restrict__ tile_set) {
   const int lane = threadIdx.x;
   long long base[7] = {0, 0, 0, 0, 0, 0, 0};   // qt0, kt0, seed0, item0, sc0, dist0, knn0
   for (int b0 = 0; b0 < B; b0 += 32) {
@@ -337,7 +342,8 @@ __global__ void set_table_kernel(const int32_t* __restrict__ offsets, int N_unif
     const int k = live ? max(min(k_cfg, N - 1), 0) : 0;
     const int QT = (N + 127) / 128, KT = (N + 63) / 64;
     int sp = 1, TS = KT;
-    if (split) pdsc::attn_set_split(N, num_sms, &sp, &TS);
+    if (split && invariant) pdsc::attn_set_split_invariant(N, &sp, &TS);
+    else if (split) pdsc::attn_set_split(N, num_sms, &sp, &TS);
     const long long size[7] = {QT, KT, S, (long long)QT * sp,
                                tiled ? (long long)KT * QT * 8192 : (long long)N * pdsc::round_up(N, 64),
                                ((long long)S * N + 3) & ~3ll, (long long)S * k};
@@ -432,6 +438,12 @@ int pdsc_set_precision(pdsc_engine* e, int32_t precision) {
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
   if (precision < PDSC_FP32_SIMT || precision > PDSC_FP16X3) return fail(PDSC_ERR_INVALID_ARGUMENT, "unknown precision %d", precision);
   e->cfg.precision = precision;
+  return PDSC_OK;
+}
+
+int pdsc_set_batch_invariant(pdsc_engine* e, int32_t enable) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  e->batch_invariant = enable != 0;
   return PDSC_OK;
 }
 
@@ -560,7 +572,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
   const int S = sh.S, k = sh.k, T = e->cfg.num_iterations;
   const SetDesc* sets = w.sets;
   set_table_kernel<<<1, 32, 0, st>>>(d_offsets, N, B, (double)e->cfg.ratio, e->cfg.k, e->cfg.precision == PDSC_FP32_SIMT ? 0 : 1,
-                                     sh.attn_split, device_sm_count(), w.sets, w.tile_set);
+                                     sh.attn_split, sh.attn_invariant, device_sm_count(), w.sets, w.tile_set);
   const float* W = e->d_weights;
   const int L = e->cfg.num_layers;
   cudaEvent_t* attn_ev = nullptr;
@@ -606,7 +618,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
       a.debug_out = io ? io->out_layer_debug : nullptr;
       a.attn_events = attn_ev;
       a.sets = sets; a.tile_set = w.tile_set; a.rows = (long long)R; a.qtiles = sh.qtiles; a.ktiles = sh.ktiles;
-      a.attn_items = sh.attn_items; a.attn_split = sh.attn_split;
+      a.attn_items = sh.attn_items; a.attn_split = sh.attn_split; a.attn_invariant = sh.attn_invariant;
       const int rc = tc_encoder_forward(e->tc, a, st);
       if (rc) return fail(PDSC_ERR_CUDA, "tensor-core encoder launch failed: %s", cudaGetErrorString((cudaError_t)rc));
     }
@@ -759,7 +771,8 @@ int pdsc_forward_graph(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr
   for (size_t i = 0; i < e->graphs.size(); ++i) {
     const auto& q = e->graphs[i];
     if (q.B == B && q.N == N && q.corr_pos == d_corr_pos && q.src == d_src && q.tgt == d_tgt && q.trans == d_final_trans &&
-        q.labels == d_final_labels && q.workspace == d_workspace && q.precision == e->cfg.precision) {
+        q.labels == d_final_labels && q.workspace == d_workspace && q.precision == e->cfg.precision &&
+        q.batch_invariant == e->batch_invariant) {
       if (i) std::swap(e->graphs[0], e->graphs[i]);
       PDSC_CUDA(cudaGraphLaunch(e->graphs[0].exec, st));
       return PDSC_OK;
@@ -789,7 +802,7 @@ int pdsc_forward_graph(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr
     e->graphs.pop_back();
   }
   e->graphs.insert(e->graphs.begin(), pdsc_engine::GraphEntry{B, N, d_corr_pos, d_src, d_tgt, d_final_trans, d_final_labels,
-                                                              d_workspace, e->cfg.precision, exec});
+                                                              d_workspace, e->cfg.precision, e->batch_invariant, exec});
   return PDSC_OK;   // the eager run above already produced this call's result
 }
 

@@ -38,6 +38,22 @@ __host__ __device__ __forceinline__ void attn_set_split(int N, int num_sms, int*
   *TS = ts;
 }
 
+// Key tiles per split of the batch-invariant mode (pdsc_set_batch_invariant).  Part of that mode's results: a different value
+// associates the softmax sums of every set with more than this many key tiles differently.  Chosen from the measurement in
+// DESIGN.md §4.
+#ifndef PDSC_ATTN_INVARIANT_TILES
+#define PDSC_ATTN_INVARIANT_TILES 8
+#endif
+constexpr int kAttnInvariantTiles = PDSC_ATTN_INVARIANT_TILES;
+
+// Key split of the tensor-core attention for one set of N rows in the batch-invariant mode: a function of N alone (no SM
+// count, no batch, no item cap), so a set gives the same bytes in every call and on every device.  sp == 1: not split.
+__host__ __device__ __forceinline__ void attn_set_split_invariant(int N, int* sp, int* TS) {
+  const int KT = (N + 63) / 64;
+  *sp = (KT + kAttnInvariantTiles - 1) / kAttnInvariantTiles;
+  *TS = (KT + *sp - 1) / *sp;
+}
+
 // the set b of a call with first(b) <= x < first(b + 1), `first` ascending in b
 template <typename F>
 __device__ __forceinline__ int find_set(int nsets, long long x, F first) {

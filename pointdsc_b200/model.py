@@ -86,7 +86,8 @@ class _EncoderParams(nn.Module):
 
 class PointDSC(nn.Module):
     def __init__(self, in_dim=6, num_layers=6, num_channels=128, num_iterations=10, ratio=0.1,
-                 inlier_threshold=0.10, sigma_d=0.10, k=40, nms_radius=0.10, *, precision: Optional[str] = None):
+                 inlier_threshold=0.10, sigma_d=0.10, k=40, nms_radius=0.10, *, precision: Optional[str] = None,
+                 batch_invariant: bool = False):
         super().__init__()
         self.in_dim = in_dim
         self.num_layers = num_layers
@@ -99,6 +100,9 @@ class PointDSC(nn.Module):
         self.precision = precision or DEFAULT_PRECISION
         if self.precision not in _capi.PRECISIONS:
             raise ValueError(f"precision must be one of {sorted(_capi.PRECISIONS)}, got {self.precision!r}")
+        # batch-invariant mode (pdsc_set_batch_invariant): every set's result is independent of its call and of the device's
+        # SM count, at the cost measured in DESIGN.md §4; a plain attribute, not part of the state dict
+        self.batch_invariant = bool(batch_invariant)
         self.sigma = nn.Parameter(torch.tensor([1.0], dtype=torch.float32), requires_grad=True)
         self.sigma_spat = nn.Parameter(torch.tensor([sigma_d], dtype=torch.float32), requires_grad=False)
         self.encoder = _EncoderParams(in_dim, num_layers, num_channels)
@@ -114,6 +118,7 @@ class PointDSC(nn.Module):
         self._engine_device = None
         self._engine_hyper = None
         self._pushed_signature = None
+        self._pushed_invariant = None
         self._workspaces = {}     # CUDA stream handle -> scratch tensor (two streams never share scratch)
         self._static = {}         # (B, N, stream) -> address-stable buffers of the graph-replay path
         self.graph_rows = 32768   # calls with B * N at most this replay a captured CUDA graph (launch-bound regime)
@@ -150,6 +155,10 @@ class PointDSC(nn.Module):
             handle = C.c_void_p()
             _capi.check(lib.pdsc_create(C.byref(cfg), C.byref(handle)))
             self._engine, self._engine_device, self._pushed_signature = handle, index, None
+            self._pushed_invariant = None
+        if self._pushed_invariant != self.batch_invariant:
+            _capi.check(lib.pdsc_set_batch_invariant(self._engine, 1 if self.batch_invariant else 0))
+            self._pushed_invariant = self.batch_invariant
         sig = self._signature()
         if sig != self._pushed_signature:
             _capi.check(lib.pdsc_set_precision(self._engine, _capi.PRECISIONS[self.precision]))
@@ -180,6 +189,11 @@ class PointDSC(nn.Module):
         if precision not in _capi.PRECISIONS:
             raise ValueError(precision)
         self.precision = precision
+        self._workspaces, self._static = {}, {}
+
+    def set_batch_invariant(self, enable: bool):
+        """Turn the batch-invariant mode on or off (see the constructor); the next call of any entry point runs in it."""
+        self.batch_invariant = bool(enable)
         self._workspaces, self._static = {}, {}
 
     def launches_per_forward(self, B: int, N: int) -> int:
@@ -285,7 +299,8 @@ class PointDSC(nn.Module):
         is what `forward` accepts in testing mode (device tensors [bs_i, N_i, ...] and the 'testing' key); the result is, per
         element, what `forward` returns for it.  All their sets are packed back to back into one mixed-size call, so a loop
         over data of varying N pays one call's latency instead of one per pair.  Within one attention regime (DESIGN.md §3)
-        every set's result is bit-identical to that of a `forward` call holding it."""
+        every set's result is bit-identical to that of a `forward` call holding it; with `batch_invariant` on, to that of every
+        call holding it."""
         dev = self._device()
         sizes = []
         for i, data in enumerate(batches):

@@ -9,8 +9,8 @@ from pointdsc_b200 import PointDSC
 from pointdsc_b200.frontend import match
 from pointdsc_b200.metrics import eval_stats
 from pointdsc_b200.spectral import leading_eigenvector
-for k, n, b in ((40, 300, 3), (80, 257, 2)):
-    m = PointDSC(num_layers=12, k=k, **bench.CTOR["3dmatch"]); m.load_state_dict(bench.load_snapshot("3dmatch"), strict=False); m = m.cuda().eval()
+for k, n, b, inv in ((40, 300, 3, False), (80, 257, 2, False), (40, 1000, 2, True)):   # the last: batch-invariant key split
+    m = PointDSC(num_layers=12, k=k, batch_invariant=inv, **bench.CTOR["3dmatch"]); m.load_state_dict(bench.load_snapshot("3dmatch"), strict=False); m = m.cuda().eval()
     h = bench.make_inputs(n, b, "3dmatch", 0)
     d = [h[x].cuda() for x in ("corr_pos", "src_keypts", "tgt_keypts")]
     out = m.run(*d, taps=["best"])                      # eager
