@@ -47,7 +47,10 @@ __device__ __forceinline__ AttnItem attn_item(const AttnArgs& a, int witem) {
   return w;
 }
 
-constexpr int kAttnThreads = 288;                       // two consumer warpgroups + one producer warp
+constexpr int kAttnThreads = 384;                       // two consumer warpgroups + one producer warpgroup
+// registers per thread after setmaxnreg.  An SM sub-partition (16,384 registers) holds one warp of each warpgroup, so
+// 2 x consumer + producer <= 512; the launch gives every thread 168 (65,536 / 384 rounded down to 8), 3 x 168 = 2 x 232 + 40.
+constexpr uint32_t kAttnConsumerRegs = 232, kAttnProducerRegs = 40;
 
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -59,6 +62,19 @@ __device__ __forceinline__ float2 ldg_stream2(const float* p) {
   float2 v;
   asm volatile("ld.global.nc.L1::no_allocate.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p));
   return v;
+}
+// this thread's 32 SC values of one tile (layout [16 key groups][128 queries][4 keys]) in the S fragment's order: query
+// rows r0 and r0 + 8, key columns 8 jj + fc and + 1
+__device__ __forceinline__ void attn_load_sc(float (&sc)[32], const float* tile, int r0, int fc) {
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int key = 8 * jj + fc;
+      const float2 v = ldg_stream2(tile + ((key >> 2) * 128 + r0 + 8 * h) * 4 + (key & 3));
+      sc[4 * jj + 2 * h] = v.x;
+      sc[4 * jj + 2 * h + 1] = v.y;
+    }
 }
 
 }  // namespace pdsc

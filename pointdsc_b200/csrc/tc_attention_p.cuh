@@ -5,13 +5,15 @@
 //     P = softmax_j( SC_ij * (q_i . k_j) / sqrt(C) ),   msg_i = sum_j P_ij v_j          (heads = 1, C = 128)
 // SC multiplies the logit (it is not a mask): SC_ij = 0 leaves logit 0, which still takes softmax mass.
 //
-// Roles (288 threads):
-//   warps 0-7  two consumer warpgroups, 64 query rows each.  Per 64-key tile: S = Q K^T (wgmma, Q and K from shared memory,
-//              S in registers), logits S * SC with the SC tile streamed from HBM while the MMA runs, online softmax in
-//              registers (log2 units: Q carries log2(e) / sqrt(C)), P split into 16-bit hi / lo register A operands, O += P V
-//              (wgmma, V read as an MN-major B operand, O in registers).
-//   warp  8    producer: one lane streams each item's Q image and its K / V tiles (bulk async copies, mbarrier complete_tx)
-//              through a two-stage ring, running ahead into the next item while the current one is computed.
+// Roles (384 threads):
+//   warps 0-7   two consumer warpgroups, 64 query rows each, 232 registers per thread (setmaxnreg.inc).  Per 64-key tile:
+//               S = Q K^T (wgmma, Q and K from shared memory, S in registers), logits S * SC with the SC tile streamed from
+//               HBM one tile-step ahead, online softmax in registers (log2 units: Q carries log2(e) / sqrt(C)), P split into
+//               16-bit hi / lo register A operands, O += P V (wgmma, V read as an MN-major B operand, O in registers).
+//   warps 8-11  producer warpgroup, 40 registers per thread (setmaxnreg.dec) so that the consumers can have more; warps 9-11
+//               leave at once, one lane of warp 8 streams each item's Q image and its K / V tiles (bulk async copies,
+//               mbarrier complete_tx) through a two-stage ring, running ahead into the next item while the current one is
+//               computed.
 #pragma once
 #include "tc_attention.cuh"
 
@@ -45,9 +47,10 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
   }
   __syncthreads();
 
-  if (warp == 8) {
+  if (warp >= 8) {
     // ===================================== producer =====================================
-    if (lane == 0) {
+    setmaxnreg_dec<kAttnProducerRegs>();   // the whole warpgroup gives its registers to the consumers
+    if (warp == 8 && lane == 0) {
       const uint32_t q_bytes = a.split ? 65536u : 32768u;
       const uint32_t tile_bytes = a.split ? 32768u : 16384u;   // hi (+ lo) image of one 64-key tile of K or V
       int gt = 0;                                              // running tile count of the CTA
@@ -75,6 +78,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
   }
 
   // ===================================== consumers =====================================
+  setmaxnreg_inc<kAttnConsumerRegs>();
   const int wg = warp >> 2, wt = tid & 127;
   const int r0 = 64 * wg + frag_row(wt), fc = frag_col(wt);   // query rows r0, r0 + 8 of the tile; key columns 8 j + fc, + 1
   const uint32_t qa = s0 + kAttnPQ + (uint32_t)wg * 8192u;     // this warpgroup's 64 rows of the Q image
@@ -89,6 +93,9 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
 #pragma unroll
     for (int i = 0; i < 64; ++i) o[i] = 0.f;
     float m[2] = {-INFINITY, -INFINITY}, l_sum[2] = {0.f, 0.f};
+    // this thread's 32 SC values of the next key tile, loaded a full tile-step before the softmax needs them
+    float sc[32];
+    attn_load_sc(sc, sc_cta + (size_t)min(t0, KT - 1) * tile_stride, r0, fc);
     mbar_wait(q_full, (uint32_t)(it & 1));
     for (int j = 0; j < T; ++j, ++gt) {
       const int st = gt % kAttnStages, use = gt / kAttnStages;
@@ -98,25 +105,13 @@ __global__ void __launch_bounds__(kAttnThreads, 1) tc_attention_persistent_kerne
       wgmma_fence();
       gemm_ss<FMT, 2, 64>(s, qa, qa + 32768, 16384, kb, kb + 16384, 8192, a.split);
       wgmma_commit();
-      // this thread's 32 SC values, loaded while the MMA runs: tile layout [16 key groups][128 queries][4 keys]
-      float sc[32];
-      {
-        const float* tile = sc_cta + (size_t)min(t0 + j, KT - 1) * tile_stride;
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int key = 8 * jj + fc;
-            const float2 v = ldg_stream2(tile + ((key >> 2) * 128 + r0 + 8 * h) * 4 + (key & 3));
-            sc[4 * jj + 2 * h] = v.x;
-            sc[4 * jj + 2 * h + 1] = v.y;
-          }
-      }
       wgmma_wait<0>();
       fence_regs(s);
       if (j == T - 1) mbar_arrive(q_empty);   // the item's last QK has retired: the Q buffer may be refilled
 #pragma unroll
       for (int i = 0; i < 32; ++i) s[i] *= sc[i];
+      // never past the item's last tile: the next item may belong to another set
+      if (j + 1 < T) attn_load_sc(sc, sc_cta + (size_t)min(t0 + j + 1, KT - 1) * tile_stride, r0, fc);
       if ((t0 + j) * 64 + 63 >= N) {       // the set's last, ragged key tile - or a virtual tile behind it (all masked)
 #pragma unroll
         for (int i = 0; i < 32; ++i)

@@ -88,6 +88,12 @@ __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.w
 template <int N>
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
+// ---- register reallocation between the warpgroups of a CTA (the counts are multiples of 8 in [24, 256]) ------------------
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // ---- proxy fence: generic-proxy shared-memory writes become visible to the async proxy (wgmma operand reads) ---------
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
