@@ -91,7 +91,7 @@ typedef struct pdsc_stage_io {
   int32_t* out_knn_idx;         /* [B,S,k]  (a7)                                                     */
   float* out_compat;            /* [B,S,k,k] (a8)                                                    */
   float* out_eig;               /* [B,S,k]  leading eigenvector at the set's exit iteration (a9)     */
-  int32_t* out_power_iters;     /* [B]      iterations run per set (a9)                              */
+  int32_t* out_power_iters;     /* [B]      iterations run per set (a9); 0 when S = 0                */
   float* out_seed_trans;        /* [B,S,4,4] (a10)                                                   */
   int32_t* out_inlier_counts;   /* [B,S]    inlier count of every hypothesis (a11)                   */
   int32_t* out_best;            /* [B]      selected hypothesis (a11)                                */

@@ -193,14 +193,16 @@ __global__ void tc_decode_kernel(const uint8_t* qimg, const uint8_t* kvimg, floa
   v[idx] = rd(kb + 32768 + ko) + (split ? rd(kb + 49152 + ko) : 0.f);
 }
 
-// debug tap: feat1 from its blocked layout (tc_chain.cuh) to plain [rows][128]
+// debug tap: feat1 from its blocked layout (tc_chain.cuh) to plain [rows][128].  The tap is a caller's fp32 tensor, only 4-byte
+// aligned by the ABI: scalar stores (the blocked source lives in the 256-byte aligned workspace)
 __global__ void tc_unblock_f32_kernel(const float* __restrict__ blocked, float* __restrict__ plain, long long rows) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // 16-byte piece index
   if (i >= rows * 32) return;
   const long long g = i >> 5;
   const uint32_t piece = (uint32_t)(i & 31);
-  reinterpret_cast<float4*>(plain)[i] =
-      *reinterpret_cast<const float4*>(reinterpret_cast<const uint8_t*>(blocked) + blocked_f32_offset(g, piece));
+  const float4 v = *reinterpret_cast<const float4*>(reinterpret_cast<const uint8_t*>(blocked) + blocked_f32_offset(g, piece));
+  float* o = plain + 4 * i;
+  o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
 }
 
 // =========================================================================================================

@@ -689,6 +689,8 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
     mark(7);
   } else {
     launch_fill_u64(w.best_key, 0ull, B, st);
+    // no seeds: no power iteration runs, and the tap says so (it would otherwise keep whatever the caller's buffer held)
+    if (io && io->out_power_iters) PDSC_CUDA(cudaMemsetAsync(io->out_power_iters, 0, (size_t)B * sizeof(int32_t), st));
     mark(4); mark(5); mark(6); mark(7);
   }
   // ---- a11 (labels) + a12 ---------------------------------------------------------------------------
