@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """The reference's evaluation driver (`evaluation/test_3DMatch.py`, `--solver SVD`) with every per-pair step on the H100 and no
 host synchronisation inside the loop: descriptor matching + network input (row f1, `pointdsc_b200.frontend.match`), ground-truth
-labels, `PointDSC.forward` (the path), registration + classification statistics (row f3, `pointdsc_b200.metrics.eval_stats`).
+labels, `PointDSC.forward` (the path), registration + classification statistics (row f3, `pointdsc_b200.metrics.eval_stats`);
+with --batch_size P every P pairs take one call of each (`match_many`, `forward_packed`, `eval_stats_packed`).
 
     python evaluate.py --chosen_snapshot PointDSC_3DMatch_release --root /data/3DMatch [--descriptor fcgf|fpfh] [--use_mutual]
     python evaluate.py --synthetic 8            # no dataset in this image: synthetic scene pairs, FPFH computed on the device
@@ -71,12 +72,19 @@ def list_pairs(root, scene):
     return [(int(k.split("_")[0]), int(k.split("_")[1]), np.linalg.inv(v)) for k, v in log.items()]
 
 
+def to_device(array, device):
+    """A host array on the device without waiting for the stream: staged in page-locked memory and copied asynchronously, so
+    that loading the next pair does not wait for the forward already enqueued (a copy from pageable memory would)."""
+    t = torch.from_numpy(array)
+    return t.pin_memory().to(device, non_blocking=True) if torch.device(device).type == "cuda" else t.to(device)
+
+
 def load_fragment(root, scene, idx, descriptor, device):
     """Key points [n,3] float32 and descriptors [n,D] of `cloud_bin_{idx}_{descriptor}.npz` (datasets/ThreeDMatch.py:240-258);
     FPFH rows are normalised as the reference does it, x / (||x|| + 1e-6) in float64."""
     z = np.load(os.path.join(root, "fragments", scene, f"cloud_bin_{idx}_{descriptor}.npz"))
-    xyz = torch.from_numpy(np.ascontiguousarray(z["xyz"], dtype=np.float32)).to(device)
-    feat = torch.from_numpy(np.ascontiguousarray(z["feature"])).to(device)
+    xyz = to_device(np.ascontiguousarray(z["xyz"], dtype=np.float32), device)
+    feat = to_device(np.ascontiguousarray(z["feature"]), device)
     if descriptor == "fpfh":
         feat = feat.double()
         feat = feat / (feat.norm(dim=1, keepdim=True) + 1e-6)
@@ -138,17 +146,23 @@ def dataset_pairs(root, scenes, descriptor, device):
 @torch.no_grad()
 def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1):
     """The loop of evaluation/test_3DMatch.py:21-103 over an iterable of (scene index, (src xyz, src desc), (tgt xyz, tgt desc),
-    gt_trans): returns a [pairs, 13] float64 array, columns = COLUMNS.  Nothing is read from the device inside the loop except the
-    correspondence count of `match` (it fixes the tensor shapes).
-    batch_size P > 1: pairs are still matched one by one, but every P of them (each with its own number of correspondences) go
-    through ONE mixed-size forward (`PointDSC.forward_many`), then through eval_stats pair by pair.  The model-time column of a
-    pair is then its group's device time divided by the group's size."""
-    from pointdsc_b200.frontend import match
-    from pointdsc_b200.metrics import eval_stats
+    gt_trans): returns a [pairs, 13] float64 array, columns = COLUMNS.
+    batch_size 1: per pair `match`, labels, `model(data)` and `eval_stats`; the only read from the device inside the loop is the
+    correspondence count of `match` with the mutual check (it fixes the tensor shapes).
+    batch_size P > 1: every P pairs (each with its own number of correspondences) are matched in ONE call (`match_many`),
+    labelled, run through ONE mixed-size forward (`PointDSC.forward_packed`) and scored by ONE `eval_stats_packed`, and nothing
+    is read from the device inside the loop (with the mutual check: the group's P + 1 offsets, once).  The model-time column
+    of a pair is then its group's device time divided by the group's size, and its data-time column its own loading time plus
+    its share of the group's matching.  A model without `forward_packed` that offers `forward_many` (a wrapper or stand-in
+    with the mixed-size interface only) is grouped pair by pair instead: `match`, labels, one `forward_many` per group and
+    `eval_stats` per pair."""
+    from pointdsc_b200.frontend import match, match_many
+    from pointdsc_b200.metrics import eval_stats, eval_stats_packed
     rows, scene_ids, data_s, events = [], [], [], []
-    group = []          # batch_size > 1: (data, gt_t, labels) of the pairs waiting for the group's forward
+    packed = batch_size > 1 and hasattr(model, "forward_packed")
+    group = []          # pairs waiting for the group: packed ((src xyz, src desc), (tgt xyz, tgt desc), gt), else (data, gt_t, labels)
 
-    def run_group():
+    def run_pair_group():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         results = model.forward_many([g[0] for g in group])
@@ -159,14 +173,42 @@ def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1):
             events.append((e0, e1, len(group)))
         group.clear()
 
+    def run_packed_group():
+        t0 = time.perf_counter()
+        m = match_many([(s[1], t[1], s[0], t[0]) for s, t, _ in group], use_mutual=use_mutual)
+        off = m["offsets"]
+        gts = to_device(np.stack([np.asarray(gt, dtype=np.float32) for _, _, gt in group]), device)
+        labels = torch.cat([gt_labels({"src_keypts": m["src_keypts"][None, a:b], "tgt_keypts": m["tgt_keypts"][None, a:b]},
+                                      gts[p], cfg["inlier_threshold"])[0] for p, (a, b) in enumerate(zip(off[:-1], off[1:]))])
+        share = (time.perf_counter() - t0) / len(group)
+        for p in range(len(group)):
+            data_s[len(data_s) - len(group) + p] += share
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        res = model.forward_packed(m["corr_pos"], m["src_keypts"], m["tgt_keypts"], off, d_offsets=m["d_offsets"])
+        e1.record()
+        rows.append(eval_stats_packed(res["final_trans"], gts, m["src_keypts"], m["tgt_keypts"], res["final_labels"], labels, off,
+                                      d_offsets=m["d_offsets"], re_thre=cfg["re_thre"], te_thre=cfg["te_thre"]))
+        events.extend([(e0, e1, len(group))] * len(group))
+        group.clear()
+
+    run_group = run_packed_group if packed else run_pair_group
     t_data = time.perf_counter()
-    for si, (src_xyz, src_desc), (tgt_xyz, tgt_desc), gt in pairs:
+    for si, src, tgt, gt in pairs:
+        scene_ids.append(si)
+        if packed:
+            data_s.append(time.perf_counter() - t_data)
+            group.append((src, tgt, gt))
+            if len(group) == batch_size:
+                run_group()
+            t_data = time.perf_counter()
+            continue
+        (src_xyz, src_desc), (tgt_xyz, tgt_desc) = src, tgt
         data = match(src_desc, tgt_desc, src_xyz, tgt_xyz, use_mutual=use_mutual)
         gt_t = torch.from_numpy(np.asarray(gt, dtype=np.float32)).to(device)
         labels = gt_labels(data, gt_t, cfg["inlier_threshold"])
         data["testing"] = True
         data_s.append(time.perf_counter() - t_data)
-        scene_ids.append(si)
         if batch_size > 1:
             group.append((data, gt_t, labels))
             if len(group) == batch_size:
@@ -186,7 +228,7 @@ def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1):
     if not rows:
         return np.zeros((0, len(COLUMNS)))
     dev_stats = torch.cat(rows, 0).double().cpu().numpy()          # the one read of the statistics
-    out = np.zeros((len(rows), len(COLUMNS)))
+    out = np.zeros((len(dev_stats), len(COLUMNS)))
     out[:, :9] = dev_stats[:, :9]
     out[:, 9] = [a.elapsed_time(b) * 1e-3 / n for a, b, n in events]
     out[:, 10] = data_s
@@ -237,7 +279,7 @@ def parse_args(argv=None):
     ap.add_argument("--precision", default=None, help="fp16x3 (default) | fp32 | bf16x3 | bf16")
     ap.add_argument("--save_npy", default=None, help="write the [pairs, 13] statistics table here")
     ap.add_argument("--batch_size", type=int, default=1,
-                    help="pairs per forward: > 1 runs every group of pairs (of different sizes) as one mixed-size call")
+                    help="pairs per group: > 1 matches, runs and scores every group of pairs (of different sizes) in one call each")
     ap.add_argument("--batch_invariant", action="store_true",
                     help="every pair's result independent of --batch_size and of the GPU's SM count (PointDSC batch_invariant)")
     return ap.parse_args(argv)

@@ -210,23 +210,50 @@ int pdsc_forward_eval(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr_
  * f3: per-pair evaluation statistics, replacing libs/loss.py:34-63 (TransformationLoss) + :94-100 (ClassificationLoss,
  * scikit-learn on the host) and the per-pair host synchronisation of evaluation/test_3DMatch.py:83-101.
  * d_stats [B,10] = [success, RE deg, TE cm, #gt inliers, gt inlier ratio, #gt inliers among the kept, precision, recall,
- * f1, rmse]; thresholds as the drivers pass them (3DMatch: 15 deg / 30 cm, KITTI: 5 deg / 60 cm). */
+ * f1, rmse]; thresholds as the drivers pass them (3DMatch: 15 deg / 30 cm, KITTI: 5 deg / 60 cm).
+ * pdsc_eval_stats: B sets of N rows, d_src_keypts / d_tgt_keypts [B,N,3], labels [B,N]; it is the packed call with offsets b * N. */
 int pdsc_eval_stats(pdsc_engine* e, int32_t B, int32_t N, const float* d_pred_trans, const float* d_gt_trans,
                     const float* d_src_keypts, const float* d_tgt_keypts, const float* d_pred_labels,
                     const float* d_gt_labels, float re_thre, float te_thre, float* d_stats, void* cuda_stream);
+/* The same statistics over sets of different sizes: set b owns rows [offsets[b], offsets[b+1]) of d_src_keypts / d_tgt_keypts
+ * [R,3] and the labels [R]; offsets has B + 1 entries, offsets[0] = 0, every set at least one row (else PDSC_ERR_SHAPE).
+ * h_offsets (host) is validated, d_offsets (device, the same values) is what the kernel reads; d_pred_trans / d_gt_trans
+ * [B,4,4].  A set's row is bit for bit the one pdsc_eval_stats gives for that set alone.  No host synchronisation. */
+int pdsc_eval_stats_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                           const float* d_pred_trans, const float* d_gt_trans, const float* d_src_keypts,
+                           const float* d_tgt_keypts, const float* d_pred_labels, const float* d_gt_labels, float re_thre,
+                           float te_thre, float* d_stats, void* cuda_stream);
 
 /* f1: the correspondence front end, replacing datasets/ThreeDMatch.py:283-291 + :299-308 (the same lines in
  * datasets/KITTI.py:80-114, demo_registration.py:101-108): nearest neighbour of every source descriptor among the target
  * descriptors under sqrt(2 - 2 <a,b> + 1e-6) evaluated in the descriptors' own dtype (desc_is_fp64: 0 = fp32 FCGF,
- * 1 = fp64 FPFH), first minimum wins, optional mutual check, then the in_dim = 6 network input.  One pair per call.
- * Outputs in the layout pdsc_forward consumes, sized for the worst case M = Ns: d_corr [Ns,2] int32 (source, target),
- * d_count [1] = M, d_corr_pos [Ns,6] (centred), d_out_src / d_out_tgt [Ns,3]; only the first M rows are written.
- * D <= 64; d_scratch holds pdsc_match_scratch_bytes(Ns, Nt) bytes, 8-byte aligned. */
+ * 1 = fp64 FPFH), first minimum wins, optional mutual check, then the in_dim = 6 network input.
+ * pdsc_match: one pair, the packed call below with P = 1.  Outputs in the layout pdsc_forward consumes, sized for the worst
+ * case M = Ns: d_corr [Ns,2] int32 (source, target), d_count [1] = M, d_corr_pos [Ns,6] (centred), d_out_src / d_out_tgt
+ * [Ns,3]; only the first M rows are written.  D <= 64; d_scratch holds pdsc_match_scratch_bytes(Ns, Nt) bytes, 8-byte
+ * aligned. */
 size_t pdsc_match_scratch_bytes(int32_t Ns, int32_t Nt);
 int pdsc_match(pdsc_engine* e, int32_t Ns, int32_t Nt, int32_t D, const void* d_src_desc, const void* d_tgt_desc,
                int32_t desc_is_fp64, const float* d_src_keypts, const float* d_tgt_keypts, int32_t use_mutual,
                int32_t* d_corr, int32_t* d_count, float* d_corr_pos, float* d_out_src, float* d_out_tgt, void* d_scratch,
                size_t scratch_bytes, void* cuda_stream);
+/* P pairs in one call.  Pair p owns source rows [src_offsets[p], src_offsets[p+1]) and target rows [tgt_offsets[p],
+ * tgt_offsets[p+1]) of d_src_desc [sum Ns, D] / d_src_keypts [sum Ns, 3] and d_tgt_desc [sum Nt, D] / d_tgt_keypts [sum Nt, 3];
+ * each offsets array has P + 1 entries, starts at 0, and every pair needs Ns_p >= 1 and Nt_p >= 1 (else PDSC_ERR_SHAPE, and
+ * pdsc_match_packed_scratch_bytes() returns 0).  h_* (host) size the launches, d_* (device, the same values) are what the
+ * kernels read.  A pair is matched exactly as pdsc_match matches it alone, against its own targets only (the mutual check
+ * too).  Pair p's kept correspondences fill rows [out_offsets[p], out_offsets[p+1]) of d_corr [sum Ns, 2] (pair-local
+ * (source, target) indices), d_corr_pos [sum Ns, 6] (centred by the pair's own mean), d_out_src / d_out_tgt [sum Ns, 3], in
+ * pair order and ascending source order: the layout pdsc_forward_packed consumes with d_out_offsets [P+1] as its offsets.
+ * Without the mutual check out_offsets equals src_offsets.  Rows at or beyond out_offsets[P] are not written.  d_scratch holds
+ * pdsc_match_packed_scratch_bytes() bytes, 8-byte aligned.  No host synchronisation, no allocation, capturable in a CUDA
+ * graph; results are bit-identical from run to run. */
+size_t pdsc_match_packed_scratch_bytes(int32_t P, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets);
+int pdsc_match_packed(pdsc_engine* e, int32_t P, int32_t D, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                      const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const void* d_src_desc, const void* d_tgt_desc,
+                      int32_t desc_is_fp64, const float* d_src_keypts, const float* d_tgt_keypts, int32_t use_mutual,
+                      int32_t* d_corr, int32_t* d_out_offsets, float* d_corr_pos, float* d_out_src, float* d_out_tgt,
+                      void* d_scratch, size_t scratch_bytes, void* cuda_stream);
 
 /* f2: the descriptor front end, replacing the open3d 0.9 calls of misc/cal_fpfh.py:21-26 (and demo_registration.py:37-44):
  *   pcd.voxel_down_sample(voxel)                                                -> pdsc_voxel_down_sample

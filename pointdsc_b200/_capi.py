@@ -75,6 +75,8 @@ SYMBOLS = {
                                     C.c_void_p, C.c_void_p, C.POINTER(StageIO), C.c_void_p, C.c_size_t, C.c_void_p]),
     "pdsc_eval_stats": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p]),
+    "pdsc_eval_stats_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p]),
     "pdsc_leading_eigenvector_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
     "pdsc_leading_eigenvector": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -82,6 +84,10 @@ SYMBOLS = {
     "pdsc_match": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                              C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                              C.c_size_t, C.c_void_p]),
+    "pdsc_match_packed_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_void_p, C.c_void_p]),
+    "pdsc_match_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "pdsc_voxel_down_sample_scratch_bytes": (C.c_size_t, [C.c_int64]),
     "pdsc_voxel_down_sample": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -120,7 +126,7 @@ _util_engines = {}
 
 
 def utility_engine(device_index: int):
-    """An engine handle for the stateless entry points (pdsc_match, pdsc_eval_stats): they only need the device."""
+    """An engine handle for the stateless entry points (pdsc_match*, pdsc_eval_stats*): they only need the device."""
     if device_index not in _util_engines:
         lib = load()
         cfg = Config(6, 12, 128, 10, 0.1, 0.1, 0.1, 40, 0.1, PRECISIONS["fp16x3"], device_index)

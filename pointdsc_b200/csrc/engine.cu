@@ -815,18 +815,51 @@ int pdsc_forward_eval(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr_
                       workspace_bytes, cuda_stream);
 }
 
+static int eval_stats_impl(pdsc_engine* e, int32_t B, const int32_t* d_offsets, int32_t N, const float* d_pred_trans,
+                           const float* d_gt_trans, const float* d_src, const float* d_tgt, const float* d_pred_labels,
+                           const float* d_gt_labels, float re_thre, float te_thre, float* d_stats, void* cuda_stream) {
+  if (!d_pred_trans || !d_gt_trans || !d_src || !d_tgt || !d_pred_labels || !d_gt_labels || !d_stats)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_eval_stats: null tensor pointer");
+  DeviceGuard g(e->cfg.device);
+  pdsc::launch_eval_stats(d_pred_trans, d_gt_trans, d_src, d_tgt, d_pred_labels, d_gt_labels, d_stats, B, d_offsets, N, re_thre,
+                          te_thre, static_cast<cudaStream_t>(cuda_stream));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
+
 int pdsc_eval_stats(pdsc_engine* e, int32_t B, int32_t N, const float* d_pred_trans, const float* d_gt_trans,
                     const float* d_src, const float* d_tgt, const float* d_pred_labels, const float* d_gt_labels,
                     float re_thre, float te_thre, float* d_stats, void* cuda_stream) {
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
   if (B <= 0 || N <= 0) return fail(PDSC_ERR_SHAPE, "need B >= 1 and N >= 1 (got B=%d N=%d)", B, N);
-  if (!d_pred_trans || !d_gt_trans || !d_src || !d_tgt || !d_pred_labels || !d_gt_labels || !d_stats)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_eval_stats: null tensor pointer");
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_eval_stats(d_pred_trans, d_gt_trans, d_src, d_tgt, d_pred_labels, d_gt_labels, d_stats, B, N, re_thre, te_thre,
-                          static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
+  return eval_stats_impl(e, B, nullptr, N, d_pred_trans, d_gt_trans, d_src, d_tgt, d_pred_labels, d_gt_labels, re_thre, te_thre,
+                         d_stats, cuda_stream);
+}
+
+// offsets [n + 1] of a packed call of the stateless entry points: offsets[0] = 0, every set at least `min_rows` rows
+static int check_pair_offsets(const char* who, const char* what, int32_t n, const int32_t* h_offsets, int min_rows) {
+  if (n < 1) return fail(PDSC_ERR_SHAPE, "%s: need at least one set (got %d)", who, n);
+  if (!h_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null host offsets", who);
+  if (h_offsets[0] != 0) return fail(PDSC_ERR_SHAPE, "%s: %soffsets[0] must be 0 (got %d)", who, what, h_offsets[0]);
+  for (int b = 0; b < n; ++b) {
+    const long long rows = (long long)h_offsets[b + 1] - h_offsets[b];
+    if (rows < min_rows)
+      return fail(PDSC_ERR_SHAPE, "%s: set %d has %lld %srows: offsets must increase by at least %d per set", who, b, rows, what,
+                  min_rows);
+  }
   return PDSC_OK;
+}
+
+int pdsc_eval_stats_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                           const float* d_pred_trans, const float* d_gt_trans, const float* d_src, const float* d_tgt,
+                           const float* d_pred_labels, const float* d_gt_labels, float re_thre, float te_thre, float* d_stats,
+                           void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  const int rc = check_pair_offsets("pdsc_eval_stats_packed", "", B, h_offsets, 1);
+  if (rc) return rc;
+  if (!d_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_eval_stats_packed: null device offsets");
+  return eval_stats_impl(e, B, d_offsets, 0, d_pred_trans, d_gt_trans, d_src, d_tgt, d_pred_labels, d_gt_labels, re_thre, te_thre,
+                         d_stats, cuda_stream);
 }
 
 size_t pdsc_leading_eigenvector_scratch_bytes(int32_t B, int32_t N) {
@@ -991,24 +1024,59 @@ size_t pdsc_match_scratch_bytes(int32_t Ns, int32_t Nt) {
   return (Ns > 0 && Nt > 0) ? pdsc::match_scratch_bytes(Ns, Nt) : 0;
 }
 
+size_t pdsc_match_packed_scratch_bytes(int32_t P, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets) {
+  if (P < 1 || !h_src_offsets || !h_tgt_offsets || h_src_offsets[0] != 0 || h_tgt_offsets[0] != 0) return 0;
+  for (int p = 0; p < P; ++p)
+    if (h_src_offsets[p + 1] <= h_src_offsets[p] || h_tgt_offsets[p + 1] <= h_tgt_offsets[p]) return 0;
+  return pdsc::match_scratch_bytes(h_src_offsets[P], h_tgt_offsets[P]);
+}
+
+static int match_impl(pdsc_engine* e, int32_t P, int32_t D, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                      const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const void* d_src_desc, const void* d_tgt_desc,
+                      int32_t desc_is_fp64, const float* d_src_keypts, const float* d_tgt_keypts, int32_t use_mutual,
+                      int32_t* d_corr, int32_t* d_out_first, int32_t* d_out_ends, float* d_corr_pos, float* d_out_src,
+                      float* d_out_tgt, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (D < 1 || D > pdsc::match_max_dim()) return fail(PDSC_ERR_UNSUPPORTED, "descriptor dimension %d outside [1, %d]", D, pdsc::match_max_dim());
+  if (e->cfg.in_dim != 6) return fail(PDSC_ERR_UNSUPPORTED, "pdsc_match builds the in_dim = 6 input (engine has in_dim = %d)", e->cfg.in_dim);
+  if (!d_src_desc || !d_tgt_desc || !d_src_keypts || !d_tgt_keypts || !d_corr || !d_out_ends || !d_corr_pos || !d_out_src || !d_out_tgt)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_match: null tensor pointer");
+  const size_t need = pdsc::match_scratch_bytes(h_src_offsets[P], h_tgt_offsets[P]);
+  if (!d_scratch || scratch_bytes < need)
+    return fail(PDSC_ERR_WORKSPACE, "pdsc_match: scratch too small (%zu bytes given, %zu needed)", scratch_bytes, need);
+  if (reinterpret_cast<uintptr_t>(d_scratch) % 8) return fail(PDSC_ERR_WORKSPACE, "pdsc_match: scratch must be 8-byte aligned");
+  DeviceGuard g(e->cfg.device);
+  pdsc::launch_match(P, h_src_offsets, h_tgt_offsets, d_src_offsets, d_tgt_offsets, d_src_desc, d_tgt_desc, desc_is_fp64,
+                     d_src_keypts, d_tgt_keypts, D, use_mutual, d_scratch, d_corr, d_out_first, d_out_ends, d_corr_pos, d_out_src,
+                     d_out_tgt, static_cast<cudaStream_t>(cuda_stream));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
+
 int pdsc_match(pdsc_engine* e, int32_t Ns, int32_t Nt, int32_t D, const void* d_src_desc, const void* d_tgt_desc,
                int32_t desc_is_fp64, const float* d_src_keypts, const float* d_tgt_keypts, int32_t use_mutual,
                int32_t* d_corr, int32_t* d_count, float* d_corr_pos, float* d_out_src, float* d_out_tgt, void* d_scratch,
                size_t scratch_bytes, void* cuda_stream) {
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
   if (Ns <= 0 || Nt <= 0) return fail(PDSC_ERR_SHAPE, "need Ns >= 1 and Nt >= 1 (got %d, %d)", Ns, Nt);
-  if (D < 1 || D > pdsc::match_max_dim()) return fail(PDSC_ERR_UNSUPPORTED, "descriptor dimension %d outside [1, %d]", D, pdsc::match_max_dim());
-  if (e->cfg.in_dim != 6) return fail(PDSC_ERR_UNSUPPORTED, "pdsc_match builds the in_dim = 6 input (engine has in_dim = %d)", e->cfg.in_dim);
-  if (!d_src_desc || !d_tgt_desc || !d_src_keypts || !d_tgt_keypts || !d_corr || !d_count || !d_corr_pos || !d_out_src || !d_out_tgt)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_match: null tensor pointer");
-  if (!d_scratch || scratch_bytes < pdsc::match_scratch_bytes(Ns, Nt))
-    return fail(PDSC_ERR_WORKSPACE, "pdsc_match: scratch too small (%zu bytes given, %zu needed)", scratch_bytes, pdsc::match_scratch_bytes(Ns, Nt));
-  if (reinterpret_cast<uintptr_t>(d_scratch) % 8) return fail(PDSC_ERR_WORKSPACE, "pdsc_match: scratch must be 8-byte aligned");
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_match(d_src_desc, d_tgt_desc, desc_is_fp64, d_src_keypts, d_tgt_keypts, Ns, Nt, D, use_mutual, d_scratch, d_corr,
-                     d_count, d_corr_pos, d_out_src, d_out_tgt, static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
+  // the packed call with one pair: its offsets need no device table, and its end row is the count
+  const int32_t src_off[2] = {0, Ns}, tgt_off[2] = {0, Nt};
+  return match_impl(e, 1, D, src_off, tgt_off, nullptr, nullptr, d_src_desc, d_tgt_desc, desc_is_fp64, d_src_keypts, d_tgt_keypts,
+                    use_mutual, d_corr, nullptr, d_count, d_corr_pos, d_out_src, d_out_tgt, d_scratch, scratch_bytes, cuda_stream);
+}
+
+int pdsc_match_packed(pdsc_engine* e, int32_t P, int32_t D, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                      const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const void* d_src_desc, const void* d_tgt_desc,
+                      int32_t desc_is_fp64, const float* d_src_keypts, const float* d_tgt_keypts, int32_t use_mutual,
+                      int32_t* d_corr, int32_t* d_out_offsets, float* d_corr_pos, float* d_out_src, float* d_out_tgt,
+                      void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  int rc = check_pair_offsets("pdsc_match_packed", "source ", P, h_src_offsets, 1);
+  if (!rc) rc = check_pair_offsets("pdsc_match_packed", "target ", P, h_tgt_offsets, 1);
+  if (rc) return rc;
+  if (!d_src_offsets || !d_tgt_offsets || !d_out_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_match_packed: null offsets");
+  return match_impl(e, P, D, h_src_offsets, h_tgt_offsets, d_src_offsets, d_tgt_offsets, d_src_desc, d_tgt_desc, desc_is_fp64,
+                    d_src_keypts, d_tgt_keypts, use_mutual, d_corr, d_out_offsets, d_out_offsets + 1, d_corr_pos, d_out_src,
+                    d_out_tgt, d_scratch, scratch_bytes, cuda_stream);
 }
 
 int pdsc_profile_enable(pdsc_engine* e, int32_t enable) {

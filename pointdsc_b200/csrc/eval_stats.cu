@@ -5,7 +5,8 @@
 // libs/loss.py:94-100 (ClassificationLoss: precision / recall / F1 of `pred > 0` against the ground-truth labels, computed
 // there with scikit-learn on the host after a device->host copy) and the columns evaluation/test_3DMatch.py:85-96 records
 // per pair.  The evaluation loop synchronises with the host once per pair for these numbers; here one CTA per set reduces
-// them on the device and a batch costs one launch.
+// them on the device and a batch costs one launch.  Set b owns rows [offsets[b], offsets[b+1]) of the packed key points and
+// labels (pdsc_eval_stats_packed), or rows [b N, (b + 1) N) (pdsc_eval_stats: the same kernel without a table).
 //
 // Output row (10 floats per set): [success, RE deg, TE cm, #gt inliers, gt inlier ratio, #gt inliers among the kept,
 //                                  precision, recall, f1, rmse]
@@ -14,6 +15,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "sets.cuh"
 
 namespace pdsc {
 
@@ -24,18 +26,20 @@ __global__ void __launch_bounds__(kStatsThreads) eval_stats_kernel(const float* 
                                                                    const float* __restrict__ src, const float* __restrict__ tgt,
                                                                    const float* __restrict__ pred_labels,
                                                                    const float* __restrict__ gt_labels, float* __restrict__ stats,
-                                                                   int N, float re_thre, float te_thre) {
+                                                                   Offsets off, float re_thre, float te_thre) {
   __shared__ double red_d[kStatsThreads / 32];
   __shared__ int red_i[4][kStatsThreads / 32];
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const size_t row0 = (size_t)off.at(b);
+  const int N = off.at(b + 1) - off.at(b);
   const float* T = pred_trans + (size_t)b * 16;
   const float* G = gt_trans + (size_t)b * 16;
   const float r00 = T[0], r01 = T[1], r02 = T[2], t0 = T[3], r10 = T[4], r11 = T[5], r12 = T[6], t1 = T[7], r20 = T[8],
               r21 = T[9], r22 = T[10], t2 = T[11];
-  const float* ps = src + (size_t)b * N * 3;
-  const float* pt = tgt + (size_t)b * N * 3;
-  const float* pl = pred_labels + (size_t)b * N;
-  const float* gl = gt_labels + (size_t)b * N;
+  const float* ps = src + row0 * 3;
+  const float* pt = tgt + row0 * 3;
+  const float* pl = pred_labels + row0;
+  const float* gl = gt_labels + row0;
   double dist_sum = 0.0;
   int tp = 0, fp = 0, fn = 0, gt_sum = 0;
   for (int i = tid; i < N; i += kStatsThreads) {
@@ -88,11 +92,11 @@ __global__ void __launch_bounds__(kStatsThreads) eval_stats_kernel(const float* 
 }
 
 void launch_eval_stats(const float* pred_trans, const float* gt_trans, const float* src, const float* tgt,
-                       const float* pred_labels, const float* gt_labels, float* stats, int B, int N, float re_thre,
-                       float te_thre, cudaStream_t st) {
+                       const float* pred_labels, const float* gt_labels, float* stats, int B, const int32_t* d_offsets, int N,
+                       float re_thre, float te_thre, cudaStream_t st) {
   if (B <= 0) return;
-  eval_stats_kernel<<<B, kStatsThreads, 0, st>>>(pred_trans, gt_trans, src, tgt, pred_labels, gt_labels, stats, N, re_thre,
-                                                 te_thre);
+  eval_stats_kernel<<<B, kStatsThreads, 0, st>>>(pred_trans, gt_trans, src, tgt, pred_labels, gt_labels, stats,
+                                                 Offsets{d_offsets, d_offsets ? 0 : N}, re_thre, te_thre);
 }
 
 }  // namespace pdsc

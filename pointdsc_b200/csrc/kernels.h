@@ -92,14 +92,17 @@ void launch_select_refine(const float* src, const float* tgt, const float* seed_
 
 // ---- f3: per-pair evaluation statistics (eval_stats.cu), 10 floats per set -----------------------------------
 void launch_eval_stats(const float* pred_trans, const float* gt_trans, const float* src, const float* tgt,
-                       const float* pred_labels, const float* gt_labels, float* stats, int B, int N, float re_thre,
-                       float te_thre, cudaStream_t st);
+                       const float* pred_labels, const float* gt_labels, float* stats, int B, const int32_t* d_offsets, int N,
+                       float re_thre, float te_thre, cudaStream_t st);   // set b: rows [offsets[b], offsets[b+1]), or b * N without a table
 
 // ---- f1: correspondence front end (frontend.cu): nearest neighbour in descriptor space, mutual check, centred input ----
-size_t match_scratch_bytes(int Ns, int Nt);
+// P pairs packed back to back (offsets [P + 1], host and device; null device tables: one pair).  Pair p's kept rows end at
+// out_ends[p], written by the call, as is out_first[0] = 0 unless out_first is null.
+size_t match_scratch_bytes(int Ns, int Nt);      // Ns, Nt: the call's total source / target rows
 int match_max_dim();
-void launch_match(const void* src_desc, const void* tgt_desc, int desc_is_fp64, const float* src_keypts, const float* tgt_keypts,
-                  int Ns, int Nt, int D, int mutual, void* scratch, int32_t* corr, int32_t* count, float* corr_pos,
+void launch_match(int P, const int32_t* h_src_off, const int32_t* h_tgt_off, const int32_t* d_src_off, const int32_t* d_tgt_off,
+                  const void* src_desc, const void* tgt_desc, int desc_is_fp64, const float* src_keypts, const float* tgt_keypts,
+                  int D, int mutual, void* scratch, int32_t* corr, int32_t* out_first, int32_t* out_ends, float* corr_pos,
                   float* out_src, float* out_tgt, cudaStream_t st);
 
 // ---- f4: N x N power iteration (eig_power.cu) -----------------------------------------------------------------

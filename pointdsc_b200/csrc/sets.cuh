@@ -54,6 +54,14 @@ __host__ __device__ __forceinline__ void attn_set_split_invariant(int N, int* sp
   *TS = (KT + *sp - 1) / *sp;
 }
 
+// Row offsets of a packed call of the stateless entry points (matching, statistics): set b owns rows [at(b), at(b + 1)), read
+// from a device table of B + 1 entries, or b * stride when the table is null (one set, or sets of equal size).
+struct Offsets {
+  const int32_t* table;
+  int stride;
+  __host__ __device__ __forceinline__ int at(int b) const { return table ? table[b] : b * stride; }
+};
+
 // the set b of a call with first(b) <= x < first(b + 1), `first` ascending in b
 template <typename F>
 __device__ __forceinline__ int find_set(int nsets, long long x, F first) {

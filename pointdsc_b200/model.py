@@ -21,12 +21,13 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Dict, Iterable, List, Optional
+from typing import Dict, Iterable, List, Optional, Sequence
 
 import torch
 import torch.nn as nn
 
 from . import _capi
+from .frontend import host_to_device
 
 DEFAULT_PRECISION = os.environ.get("POINTDSC_PRECISION", "fp16x3")
 
@@ -316,35 +317,63 @@ class PointDSC(nn.Module):
             sizes.append((int(cp.shape[0]), int(cp.shape[1])))
         if not batches:
             return []
-        lib = self._ensure_engine()
         counts = [n for bs, n in sizes for _ in range(bs)]
         offsets = [0]
         for n in counts:
             offsets.append(offsets[-1] + n)
-        B = len(counts)
-        h_off = (C.c_int32 * (B + 1))(*offsets)
-        d_off = torch.tensor(offsets, dtype=torch.int32, device=dev)
         cp, s, t = (torch.cat([d[key].to(torch.float32).reshape(-1, d[key].shape[-1]) for d in batches]).contiguous()
                     for key in ("corr_pos", "src_keypts", "tgt_keypts"))
-        need = int(lib.pdsc_workspace_bytes_packed(self._engine, B, h_off))
-        if need == 0:
-            _capi.check(_capi.PDSC_ERR_SHAPE)
-        stream_handle = torch.cuda.current_stream(dev).cuda_stream
-        workspace = self._workspace_for(dev, need, stream_handle)
-        trans = torch.empty(B, 4, 4, dtype=torch.float32, device=dev)
-        labels = torch.empty(offsets[-1], dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            _capi.check(lib.pdsc_forward_packed(self._engine, B, h_off, C.c_void_p(d_off.data_ptr()), C.c_void_p(cp.data_ptr()),
-                                                C.c_void_p(s.data_ptr()), C.c_void_p(t.data_ptr()),
-                                                C.c_void_p(trans.data_ptr()), C.c_void_p(labels.data_ptr()),
-                                                C.c_void_p(workspace.data_ptr()), workspace.numel(),
-                                                C.c_void_p(stream_handle)))
+        res = self.forward_packed(cp, s, t, offsets)
+        trans, labels = res["final_trans"], res["final_labels"]
         out, set0, row0 = [], 0, 0
         for bs, n in sizes:
             out.append({"final_trans": trans[set0:set0 + bs], "final_labels": labels[row0:row0 + bs * n].view(bs, n), "M": None})
             set0 += bs
             row0 += bs * n
         return out
+
+    @torch.no_grad()
+    def forward_packed(self, corr_pos: torch.Tensor, src_keypts: torch.Tensor, tgt_keypts: torch.Tensor, offsets: Sequence[int],
+                       d_offsets: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
+        """The testing-mode forward of B sets already packed back to back (pdsc_forward_packed): set b owns rows
+        offsets[b]:offsets[b+1] of corr_pos [R,in_dim], src_keypts [R,3] and tgt_keypts [R,3] (device tensors), as
+        `frontend.match_many` returns them.  `offsets`: B + 1 host ints; `d_offsets`: the same values as a device int32 tensor
+        (uploaded without a stream synchronisation when omitted).  -> {'final_trans' [B,4,4], 'final_labels' [R]}; set b's
+        results are what `forward_many` returns for it."""
+        dev = self._device()
+        offsets = [int(x) for x in offsets]
+        R = int(corr_pos.shape[0]) if corr_pos.dim() == 2 else -1
+        if corr_pos.dim() != 2 or corr_pos.shape[1] != self.in_dim or tuple(src_keypts.shape) != (R, 3) \
+                or tuple(tgt_keypts.shape) != (R, 3):
+            raise ValueError(f"expected corr_pos [R,{self.in_dim}] and src/tgt_keypts [R,3], got {tuple(corr_pos.shape)}, "
+                             f"{tuple(src_keypts.shape)}, {tuple(tgt_keypts.shape)}")
+        if any(x.device.type != "cuda" or x.device != dev for x in (corr_pos, src_keypts, tgt_keypts)):
+            raise ValueError(f"inputs must be device tensors on {dev} (got {corr_pos.device}, {src_keypts.device}, {tgt_keypts.device})")
+        if len(offsets) < 2 or offsets[-1] != R:
+            raise ValueError(f"expected B + 1 >= 2 offsets ending at R = {R}, got {len(offsets)} ending at {offsets[-1:]}")
+        lib = self._ensure_engine()
+        B = len(offsets) - 1
+        h_off = (C.c_int32 * (B + 1))(*offsets)
+        if d_offsets is None:
+            d_offsets = host_to_device(offsets, torch.int32, dev)
+        if d_offsets.dtype != torch.int32 or d_offsets.device != dev or d_offsets.numel() != B + 1:
+            raise ValueError("d_offsets must be a device int32 tensor of B + 1 entries")
+        d_off = d_offsets.contiguous()
+        cp, s, t = (x.to(torch.float32).contiguous() for x in (corr_pos, src_keypts, tgt_keypts))
+        need = int(lib.pdsc_workspace_bytes_packed(self._engine, B, h_off))
+        if need == 0:
+            _capi.check(_capi.PDSC_ERR_SHAPE)
+        stream_handle = torch.cuda.current_stream(dev).cuda_stream
+        workspace = self._workspace_for(dev, need, stream_handle)
+        trans = torch.empty(B, 4, 4, dtype=torch.float32, device=dev)
+        labels = torch.empty(R, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _capi.check(lib.pdsc_forward_packed(self._engine, B, h_off, C.c_void_p(d_off.data_ptr()), C.c_void_p(cp.data_ptr()),
+                                                C.c_void_p(s.data_ptr()), C.c_void_p(t.data_ptr()),
+                                                C.c_void_p(trans.data_ptr()), C.c_void_p(labels.data_ptr()),
+                                                C.c_void_p(workspace.data_ptr()), workspace.numel(),
+                                                C.c_void_p(stream_handle)))
+        return {"final_trans": trans, "final_labels": labels}
 
     def _workspace_for(self, dev, need: int, stream_handle: int) -> torch.Tensor:
         ws = self._workspaces.get(stream_handle)

@@ -6,8 +6,8 @@ import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench
 from pointdsc_b200 import PointDSC
-from pointdsc_b200.frontend import match
-from pointdsc_b200.metrics import eval_stats
+from pointdsc_b200.frontend import match, match_many
+from pointdsc_b200.metrics import eval_stats, eval_stats_packed
 from pointdsc_b200.spectral import leading_eigenvector
 for k, n, b, inv in ((40, 300, 3, False), (80, 257, 2, False), (40, 1000, 2, True)):   # the last: batch-invariant key split
     m = PointDSC(num_layers=12, k=k, batch_invariant=inv, **bench.CTOR["3dmatch"]); m.load_state_dict(bench.load_snapshot("3dmatch"), strict=False); m = m.cuda().eval()
@@ -34,6 +34,12 @@ for dt in (torch.float32, torch.float64):
     td = torch.nn.functional.normalize(torch.randn(277, 33, generator=g, dtype=dt), dim=1).cuda()
     for mutual in (False, True):
         r = match(sd, td, torch.rand(301, 3).cuda(), torch.rand(277, 3).cuda(), use_mutual=mutual)
+        pk = match_many([(sd, td, torch.rand(301, 3).cuda(), torch.rand(277, 3).cuda()), (sd[:1], td[:70], torch.rand(1, 3).cuda(),
+                         torch.rand(70, 3).cuda()), (sd[:130], td[:1], torch.rand(130, 3).cuda(), torch.rand(1, 3).cuda())],
+                        use_mutual=mutual)                       # pdsc_match_packed, pairs of three sizes
+        off = pk["offsets"]
+        sp = eval_stats_packed(torch.eye(4).expand(3, 4, 4).cuda(), torch.eye(4).expand(3, 4, 4).cuda(), pk["src_keypts"],
+                               pk["tgt_keypts"], pk["corr_pos"][:, 0], pk["corr_pos"][:, 1], off, d_offsets=pk["d_offsets"])
 from pointdsc_b200 import descriptors as D
 from pointdsc_b200.synth_scene import scene
 kp, feat = D.fpfh_descriptors(torch.from_numpy(scene(4000, seed=0)).cuda(), 0.15)
