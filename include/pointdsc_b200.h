@@ -276,6 +276,30 @@ int pdsc_estimate_normals(pdsc_engine* e, int32_t m, const float* d_points, doub
                           int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
 int pdsc_compute_fpfh(pdsc_engine* e, int32_t m, const float* d_points, const double* d_normals, double radius, int32_t max_nn,
                       int32_t normalise, double* d_fpfh, int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+/* The same three steps for P clouds in one call each (misc/cal_fpfh.py:21-26 run over a list of clouds); the calls above are
+ * these with P = 1.  Cloud p owns rows [offsets[p], offsets[p+1]) of the packed inputs; offsets has P + 1 entries, starts at 0,
+ * and every cloud needs at least one row (else PDSC_ERR_SHAPE, and the *_packed_scratch_bytes() functions return 0).  h_offsets
+ * (host) size the launches and the scratch, d_offsets (device, the same values) are what the kernels read.  d_status [P]: cloud
+ * p's bits (meanings as above) land in d_status[p] only.  Each cloud is computed exactly as the single-cloud call computes it
+ * alone, against its own rows only: its rows are bit for bit that call's.  No host synchronisation, no allocation.
+ * pdsc_voxel_down_sample_packed: d_points [n,3], n = offsets[P] <= 2^30; cloud p's voxel means fill rows [out_offsets[p],
+ * out_offsets[p+1]) of d_out_points (room for [n,3]), each cloud in ascending (ix, iy, iz) order of its own voxel grid (origin
+ * min - voxel / 2 of that cloud); d_out_offsets [P+1] is written on the stream (the key-point offsets of the next two calls).
+ * Rows at or beyond out_offsets[P] are not written.
+ * pdsc_estimate_normals_packed / pdsc_compute_fpfh_packed: d_points [m,3] key points, m = offsets[P], normals / FPFH as above
+ * for all m rows; a row's neighbours are searched among its own cloud's rows.  Scratch: 8-byte aligned,
+ * pdsc_voxel_down_sample_packed_scratch_bytes() / pdsc_fpfh_packed_scratch_bytes() bytes (the latter serves both calls). */
+size_t pdsc_voxel_down_sample_packed_scratch_bytes(int32_t P, const int32_t* h_offsets);
+int pdsc_voxel_down_sample_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
+                                  double voxel_size, float* d_out_points, int32_t* d_out_offsets, int32_t* d_status, void* d_scratch,
+                                  size_t scratch_bytes, void* cuda_stream);
+size_t pdsc_fpfh_packed_scratch_bytes(int32_t P, const int32_t* h_offsets, int32_t max_nn);
+int pdsc_estimate_normals_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
+                                 double radius, int32_t max_nn, double* d_normals, int32_t* d_status, void* d_scratch,
+                                 size_t scratch_bytes, void* cuda_stream);
+int pdsc_compute_fpfh_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
+                             const double* d_normals, double radius, int32_t max_nn, int32_t normalise, double* d_fpfh,
+                             int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
 /* Vertex positions of a PLY file (ascii or binary_little_endian; x, y, z float or double) into host memory as [n,3] float32.
  * Call with points = NULL to learn *n_vertices, then with a buffer of `capacity` >= n vertices. */
 int pdsc_read_ply(const char* path, float* points, int64_t capacity, int64_t* n_vertices);

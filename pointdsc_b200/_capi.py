@@ -96,6 +96,14 @@ SYMBOLS = {
                                         C.c_void_p, C.c_size_t, C.c_void_p]),
     "pdsc_compute_fpfh": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_double, C.c_int32, C.c_int32, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "pdsc_voxel_down_sample_packed_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_void_p]),
+    "pdsc_voxel_down_sample_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p,
+                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "pdsc_fpfh_packed_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_void_p, C.c_int32]),
+    "pdsc_estimate_normals_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int32,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "pdsc_compute_fpfh_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double,
+                                           C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "pdsc_read_ply": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
     "pdsc_launches_per_forward": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32]),
     "pdsc_profile_enable": (C.c_int, [C.c_void_p, C.c_int32]),

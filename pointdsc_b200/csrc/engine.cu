@@ -884,24 +884,67 @@ int pdsc_leading_eigenvector(pdsc_engine* e, int32_t B, int32_t N, const float* 
   return PDSC_OK;
 }
 
-size_t pdsc_voxel_down_sample_scratch_bytes(int64_t n) { return n > 0 ? pdsc::voxel_scratch_bytes(n) : 0; }
+// offsets of P clouds that the descriptor entry points accept: P >= 1, offsets[0] = 0, every cloud at least one row
+static bool cloud_offsets_ok(int32_t P, const int32_t* h_offsets) {
+  if (P < 1 || !h_offsets || h_offsets[0] != 0) return false;
+  for (int p = 0; p < P; ++p)
+    if (h_offsets[p + 1] <= h_offsets[p]) return false;
+  return true;
+}
+
+size_t pdsc_voxel_down_sample_scratch_bytes(int64_t n) {
+  if (n <= 0 || n > (1ll << 30)) return 0;
+  const int32_t off[2] = {0, (int32_t)n};
+  return pdsc::voxel_scratch_bytes(1, off);
+}
+
+size_t pdsc_voxel_down_sample_packed_scratch_bytes(int32_t P, const int32_t* h_offsets) {
+  return cloud_offsets_ok(P, h_offsets) && h_offsets[P] <= (1 << 30) ? pdsc::voxel_scratch_bytes(P, h_offsets) : 0;
+}
+
+static int voxel_impl(const char* who, pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets,
+                      const float* d_points, double voxel_size, float* d_out_points, int32_t* d_out_first, int32_t* d_out_ends,
+                      int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (h_offsets[P] > (1 << 30)) return fail(PDSC_ERR_SHAPE, "%s: need at most 2^30 points (got %d)", who, h_offsets[P]);
+  if (!(voxel_size > 0.0)) return fail(PDSC_ERR_INVALID_ARGUMENT, "voxel_size must be positive (got %g)", voxel_size);
+  if (!d_points || !d_out_points || !d_out_ends || !d_status) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", who);
+  const size_t need = pdsc::voxel_scratch_bytes(P, h_offsets);
+  if (!d_scratch || scratch_bytes < need || reinterpret_cast<uintptr_t>(d_scratch) % 8)
+    return fail(PDSC_ERR_WORKSPACE, "%s: scratch too small or not 8-byte aligned (%zu bytes given, %zu needed)", who, scratch_bytes,
+                need);
+  DeviceGuard g(e->cfg.device);
+  pdsc::launch_voxel_down_sample(P, h_offsets, d_offsets, d_points, voxel_size, d_out_points, d_out_first, d_out_ends, d_status,
+                                 d_scratch, static_cast<cudaStream_t>(cuda_stream));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
 
 int pdsc_voxel_down_sample(pdsc_engine* e, int64_t n, const float* d_points, double voxel_size, float* d_out_points,
                            int32_t* d_count, int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
   if (n <= 0 || n > (1ll << 30)) return fail(PDSC_ERR_SHAPE, "need 1 <= n <= 2^30 points (got %lld)", (long long)n);
-  if (!(voxel_size > 0.0)) return fail(PDSC_ERR_INVALID_ARGUMENT, "voxel_size must be positive (got %g)", voxel_size);
-  if (!d_points || !d_out_points || !d_count || !d_status) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_voxel_down_sample: null tensor pointer");
-  if (!d_scratch || scratch_bytes < pdsc::voxel_scratch_bytes(n) || reinterpret_cast<uintptr_t>(d_scratch) % 8)
-    return fail(PDSC_ERR_WORKSPACE, "pdsc_voxel_down_sample: scratch too small or not 8-byte aligned (%zu bytes given, %zu needed)",
-                scratch_bytes, pdsc::voxel_scratch_bytes(n));
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_voxel_down_sample(d_points, n, voxel_size, d_out_points, d_count, d_status, d_scratch, static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
+  // the packed call with one cloud: its offsets need no device table, and its end row is the count
+  const int32_t off[2] = {0, (int32_t)n};
+  return voxel_impl("pdsc_voxel_down_sample", e, 1, off, nullptr, d_points, voxel_size, d_out_points, nullptr, d_count, d_status,
+                    d_scratch, scratch_bytes, cuda_stream);
+}
+
+int pdsc_voxel_down_sample_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
+                                  double voxel_size, float* d_out_points, int32_t* d_out_offsets, int32_t* d_status, void* d_scratch,
+                                  size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  const int rc = check_pair_offsets("pdsc_voxel_down_sample_packed", "", P, h_offsets, 1);
+  if (rc) return rc;
+  if (!d_offsets || !d_out_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_voxel_down_sample_packed: null offsets");
+  return voxel_impl("pdsc_voxel_down_sample_packed", e, P, h_offsets, d_offsets, d_points, voxel_size, d_out_points, d_out_offsets,
+                    d_out_offsets + 1, d_status, d_scratch, scratch_bytes, cuda_stream);
 }
 
 size_t pdsc_fpfh_scratch_bytes(int32_t m, int32_t max_nn) { return (m > 0 && max_nn > 0) ? pdsc::fpfh_scratch_bytes(m, max_nn) : 0; }
+
+size_t pdsc_fpfh_packed_scratch_bytes(int32_t P, const int32_t* h_offsets, int32_t max_nn) {
+  return cloud_offsets_ok(P, h_offsets) && max_nn > 0 ? pdsc::fpfh_scratch_bytes(h_offsets[P], max_nn) : 0;
+}
 
 static int check_search_args(const char* who, pdsc_engine* e, int32_t m, double radius, int32_t max_nn, const void* a, const void* b,
                              const void* c, void* d_scratch, size_t scratch_bytes) {
@@ -916,29 +959,62 @@ static int check_search_args(const char* who, pdsc_engine* e, int32_t m, double 
   return PDSC_OK;
 }
 
-int pdsc_estimate_normals(pdsc_engine* e, int32_t m, const float* d_points, double radius, int32_t max_nn, double* d_normals,
-                          int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  const int bad = check_search_args("pdsc_estimate_normals", e, m, radius, max_nn, d_points, d_normals, d_status, d_scratch, scratch_bytes);
+static int search_impl(const char* who, pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets,
+                       const float* d_points, const double* d_normals, double radius, int32_t max_nn, int32_t normalise, double* d_out,
+                       int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  const int bad = check_search_args(who, e, h_offsets[P], radius, max_nn, d_points, d_out, d_status, d_scratch, scratch_bytes);
   if (bad) return bad;
   DeviceGuard g(e->cfg.device);
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  PDSC_CUDA(cudaMemsetAsync(d_status, 0, 4, st));
-  const int rc = pdsc::launch_estimate_normals(d_points, m, radius, max_nn, d_normals, d_status, d_scratch, st);
-  if (rc) return fail(PDSC_ERR_CUDA, "normal estimation launch failed: %s", cudaGetErrorString((cudaError_t)rc));
+  PDSC_CUDA(cudaMemsetAsync(d_status, 0, 4 * (size_t)P, st));
+  const int rc = d_normals ? pdsc::launch_compute_fpfh(P, h_offsets, d_offsets, d_points, d_normals, radius, max_nn, normalise, d_out,
+                                                       d_status, d_scratch, st)
+                           : pdsc::launch_estimate_normals(P, h_offsets, d_offsets, d_points, radius, max_nn, d_out, d_status, d_scratch,
+                                                           st);
+  if (rc) return fail(PDSC_ERR_CUDA, "%s: launch failed: %s", who, cudaGetErrorString((cudaError_t)rc));
   return PDSC_OK;
+}
+
+int pdsc_estimate_normals(pdsc_engine* e, int32_t m, const float* d_points, double radius, int32_t max_nn, double* d_normals,
+                          int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (m <= 0) return fail(PDSC_ERR_SHAPE, "pdsc_estimate_normals: need m >= 1 points (got %d)", m);
+  const int32_t off[2] = {0, m};                      // the packed call with one cloud and no device table
+  return search_impl("pdsc_estimate_normals", e, 1, off, nullptr, d_points, nullptr, radius, max_nn, 0, d_normals, d_status, d_scratch,
+                     scratch_bytes, cuda_stream);
+}
+
+int pdsc_estimate_normals_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
+                                 double radius, int32_t max_nn, double* d_normals, int32_t* d_status, void* d_scratch,
+                                 size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  const int rc = check_pair_offsets("pdsc_estimate_normals_packed", "", P, h_offsets, 1);
+  if (rc) return rc;
+  if (!d_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_estimate_normals_packed: null device offsets");
+  return search_impl("pdsc_estimate_normals_packed", e, P, h_offsets, d_offsets, d_points, nullptr, radius, max_nn, 0, d_normals,
+                     d_status, d_scratch, scratch_bytes, cuda_stream);
 }
 
 int pdsc_compute_fpfh(pdsc_engine* e, int32_t m, const float* d_points, const double* d_normals, double radius, int32_t max_nn,
                       int32_t normalise, double* d_fpfh, int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  const int bad = check_search_args("pdsc_compute_fpfh", e, m, radius, max_nn, d_points, d_fpfh, d_status, d_scratch, scratch_bytes);
-  if (bad) return bad;
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (m <= 0) return fail(PDSC_ERR_SHAPE, "pdsc_compute_fpfh: need m >= 1 points (got %d)", m);
   if (!d_normals) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_compute_fpfh: null normals");
-  DeviceGuard g(e->cfg.device);
-  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  PDSC_CUDA(cudaMemsetAsync(d_status, 0, 4, st));
-  const int rc = pdsc::launch_compute_fpfh(d_points, d_normals, m, radius, max_nn, normalise, d_fpfh, d_status, d_scratch, st);
-  if (rc) return fail(PDSC_ERR_CUDA, "FPFH launch failed: %s", cudaGetErrorString((cudaError_t)rc));
-  return PDSC_OK;
+  const int32_t off[2] = {0, m};
+  return search_impl("pdsc_compute_fpfh", e, 1, off, nullptr, d_points, d_normals, radius, max_nn, normalise, d_fpfh, d_status,
+                     d_scratch, scratch_bytes, cuda_stream);
+}
+
+int pdsc_compute_fpfh_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
+                             const double* d_normals, double radius, int32_t max_nn, int32_t normalise, double* d_fpfh,
+                             int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  const int rc = check_pair_offsets("pdsc_compute_fpfh_packed", "", P, h_offsets, 1);
+  if (rc) return rc;
+  if (!d_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_compute_fpfh_packed: null device offsets");
+  if (!d_normals) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_compute_fpfh_packed: null normals");
+  return search_impl("pdsc_compute_fpfh_packed", e, P, h_offsets, d_offsets, d_points, d_normals, radius, max_nn, normalise, d_fpfh,
+                     d_status, d_scratch, scratch_bytes, cuda_stream);
 }
 
 // Host-side PLY vertex reader (ascii / binary_little_endian; x, y, z as float or double; other vertex properties skipped).

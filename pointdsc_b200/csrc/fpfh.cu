@@ -9,15 +9,27 @@
 // Layout.  points [n,3] float32 in; key points [m,3] float32 out, in ascending voxel order (ix, iy, iz); normals [m,3] float64;
 // SPFH / FPFH [m,33] float64 (the dtype the reference's matcher consumes, pdsc_match desc_is_fp64 = 1).
 //
-// voxel        (1) min bound by atomicMin on order-preserving keys; (2) one thread per point: voxel index in fp64 exactly as
-//              floor((p - (min - voxel / 2)) / voxel), a 63-bit key, insertion into an open-addressing table (atomicCAS), and the
-//              point's offset inside its voxel added as 2^-40-voxel fixed point with INTEGER atomics — the sum does not depend on
-//              the order the threads arrive in, so the means are reproducible bit for bit; (3) compaction of the occupied slots;
-//              (4) rank of every key by counting the smaller ones (tiles of keys through shared memory), which is the output row.
-// search       one warp per point: squared distances in fp32 ((dx^2 + dy^2) + dz^2, each operation rounded), the in-radius
-//              candidates compacted in ascending index order into the warp's shared memory, then warp_select.cuh's radix
-//              select + bitonic sort for the max_nn nearest, ties by ascending index.  Brute force: m^2 distance evaluations, which
-//              for the m ~ 5 k key points of a 3DMatch fragment is 25 M — the k-d tree open3d builds buys nothing at this size.
+// Clouds.  Every launcher takes P clouds packed back to back, cloud p owning rows [off[p], off[p+1]) of its inputs, from host
+// offsets (launch sizes) and a device table (what the kernels read); the single-cloud entry points are the calls with P = 1 and
+// no table.  Nothing a cloud computes reads another cloud's rows, so a cloud's results are bit for bit those of a call holding
+// it alone, and the work is the sum over the clouds of what each would cost alone.  Status words are per cloud.
+//
+// voxel        (0) every cloud's own region of the hash table, table_slots(n_p) slots from slot0[p].  The 63-bit (ix, iy, iz)
+//              key has no spare bits for the cloud index; a region per cloud keeps the key, keeps a cloud's probe chains out of
+//              every other cloud's keys, and hands the compaction each cloud's slots as one contiguous range.
+//              (1) min bound of every cloud by atomicMin on order-preserving keys (open3d's origin is min - voxel / 2 of THAT
+//              cloud); (2) one thread per point: voxel index in fp64 exactly as floor((p - (min - voxel / 2)) / voxel), a 63-bit
+//              key, insertion into its cloud's open-addressing region (atomicCAS), and the point's offset inside its voxel added
+//              as 2^-40-voxel fixed point with INTEGER atomics — the sum does not depend on the order the threads arrive in, so
+//              the means are reproducible bit for bit; (3) compaction of the occupied slots into each cloud's rows; (4) the
+//              clouds' voxel counts scanned into the output offsets; (5) rank of every key among its cloud's keys by counting
+//              the smaller ones (tiles of keys through shared memory), O(m_p^2) per cloud, which is the row after the cloud's
+//              first output row.
+// search       one warp per point over its own cloud's rows: squared distances in fp32 ((dx^2 + dy^2) + dz^2, each operation
+//              rounded), the in-radius candidates compacted in ascending index order into the warp's shared memory, then
+//              warp_select.cuh's radix select + bitonic sort for the max_nn nearest, ties by ascending index.  Neighbour indices
+//              are rows of the packed array.  Brute force: m_p^2 distance evaluations per cloud, which for the m ~ 5 k key points
+//              of a 3DMatch fragment is 25 M — the k-d tree open3d builds buys nothing at this size.
 // normals      one thread per point: fp64 covariance of the neighbourhood, cyclic Jacobi on the 3 x 3 matrix, the eigenvector of
 //              the smallest eigenvalue, sign = largest-magnitude component positive; (0, 0, 1) below three neighbours.
 // spfh         one warp per point, lanes over neighbours: Darboux-frame pair features in fp64, three 11-bin histograms counted
@@ -26,8 +38,11 @@
 //              part scaled to 100, plus the point's own SPFH; optional row normalisation x / (||x|| + 1e-6) (demo_registration.py:43).
 #include <math.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 #include "kernels.h"
+#include "sets.cuh"
 #include "warp_select.cuh"
 
 namespace pdsc {
@@ -43,60 +58,98 @@ __host__ __device__ inline unsigned long long table_slots(long long n) {
   return c;
 }
 
+// first 256-row rank tile of cloud p: a function of the offsets alone (as frontend.cu's tile0); a cloud of n rows owns
+// ceil(n / 256) tiles or one more, which is idle
+__host__ __device__ inline long long rank_tile0(const Offsets& off, int p) { return ((long long)off.at(p) + 255ll * p) / 256; }
+
 struct VoxScratch {
-  uint32_t* minkey;            // [4]
-  int* counter;                // [1]  (+ padding)
-  unsigned long long* keys;    // [slots]
-  unsigned long long* sums;    // [slots][3]
-  int* counts;                 // [slots]
-  unsigned long long* ckeys;   // [n]
-  uint32_t* cslot;             // [n]
+  unsigned long long* slot0;   // [P+1] first hash slot of every cloud's region
+  unsigned long long* keys;    // [S]
+  unsigned long long* sums;    // [S][3]
+  unsigned long long* ckeys;   // [n]   cloud p's occupied keys at rows [off[p], off[p] + count[p])
+  uint32_t* minkey;            // [P][3]
+  int* counter;                // [P]   occupied voxels of every cloud
+  int* counts;                 // [S]
+  uint32_t* cslot;             // [n]   slot of ckeys[i] inside its cloud's region
 };
 
-VoxScratch vox_carve(void* scratch, long long n) {
-  const unsigned long long slots = table_slots(n);
+unsigned long long total_slots(int P, const int32_t* h_off) {
+  unsigned long long s = 0;
+  for (int p = 0; p < P; ++p) s += table_slots((long long)h_off[p + 1] - h_off[p]);
+  return s;
+}
+
+VoxScratch vox_carve(void* scratch, int P, long long n, unsigned long long slots) {
   unsigned char* p = static_cast<unsigned char*>(scratch);
   VoxScratch s;
-  s.minkey = reinterpret_cast<uint32_t*>(p);
-  s.counter = reinterpret_cast<int*>(p + 16);
-  p += 32;
-  s.keys = reinterpret_cast<unsigned long long*>(p);  p += slots * 8;
-  s.sums = reinterpret_cast<unsigned long long*>(p);  p += slots * 24;
-  s.ckeys = reinterpret_cast<unsigned long long*>(p); p += (size_t)n * 8;
-  s.counts = reinterpret_cast<int*>(p);               p += slots * 4;
+  s.slot0 = reinterpret_cast<unsigned long long*>(p);  p += (size_t)(P + 1) * 8;
+  s.keys = reinterpret_cast<unsigned long long*>(p);   p += slots * 8;
+  s.sums = reinterpret_cast<unsigned long long*>(p);   p += slots * 24;
+  s.ckeys = reinterpret_cast<unsigned long long*>(p);  p += (size_t)n * 8;
+  s.minkey = reinterpret_cast<uint32_t*>(p);           p += (size_t)P * 12;
+  s.counter = reinterpret_cast<int*>(p);               p += (size_t)P * 4;
+  s.counts = reinterpret_cast<int*>(p);                p += slots * 4;
   s.cslot = reinterpret_cast<uint32_t*>(p);
   return s;
 }
 }  // namespace
 
-size_t voxel_scratch_bytes(long long n) {
-  const unsigned long long slots = table_slots(n);
-  return 32 + slots * 36 + (size_t)n * 12;
+size_t voxel_scratch_bytes(int P, const int32_t* h_off) {
+  return (size_t)(P + 1) * 8 + total_slots(P, h_off) * 36 + (size_t)h_off[P] * 12 + (size_t)P * 16;
 }
 
 // ---- voxel down-sampling ---------------------------------------------------------------------------------------
-__global__ void vox_init_kernel(uint32_t* minkey, int* counter, unsigned long long* keys, unsigned long long* sums, int* counts,
-                                unsigned long long slots, int32_t* out_count, int32_t* status) {
+// exclusive prefix sums of v(0 .. n-1) by ONE CTA of 1024 threads: out_first[0] = 0 (unless null), out_ends[q] = v(0) + .. + v(q)
+template <typename T, typename F>
+__device__ void cta_offsets(int n, F v, T* out_first, T* out_ends) {
+  __shared__ T part[1024];
+  const int per = (n + 1023) / 1024;
+  const int q0 = min(n, (int)threadIdx.x * per), q1 = min(n, q0 + per);
+  T s = 0;
+  for (int q = q0; q < q1; ++q) s += v(q);
+  part[threadIdx.x] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    T run = 0;
+    for (int t = 0; t < 1024; ++t) { const T x = part[t]; part[t] = run; run += x; }
+    if (out_first) out_first[0] = 0;
+  }
+  __syncthreads();
+  T run = part[threadIdx.x];
+  for (int q = q0; q < q1; ++q) { run += v(q); out_ends[q] = run; }
+}
+
+// every cloud's hash-table region: table_slots(n_p) slots (a power of two, at least 1024) from slot0[p]
+__global__ void __launch_bounds__(1024) vox_plan_kernel(int P, Offsets off, unsigned long long* slot0) {
+  cta_offsets<unsigned long long>(P, [&](int q) { return table_slots((long long)off.at(q + 1) - off.at(q)); }, slot0, slot0 + 1);
+}
+
+__global__ void vox_init_kernel(int P, uint32_t* minkey, int* counter, unsigned long long* keys, unsigned long long* sums, int* counts,
+                                unsigned long long slots, int32_t* status) {
   const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < slots) {
     keys[i] = kEmpty;
     sums[3 * i] = 0ull; sums[3 * i + 1] = 0ull; sums[3 * i + 2] = 0ull;
     counts[i] = 0;
   }
-  if (i < 3) minkey[i] = 0xFFFFFFFFu;
-  if (i == 0) { *counter = 0; *out_count = 0; *status = 0; }
+  if (i < 3ull * P) minkey[i] = 0xFFFFFFFFu;
+  if (i < (unsigned long long)P) { counter[i] = 0; status[i] = 0; }
 }
 
-__global__ void vox_bounds_kernel(const float* __restrict__ pts, long long n, uint32_t* minkey) {
-  uint32_t m[3] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+// min bound of every cloud: blockIdx.y strides over the clouds, the CTAs of one cloud over its points
+__global__ void vox_bounds_kernel(const float* __restrict__ pts, int P, Offsets off, uint32_t* minkey) {
+  for (int p = blockIdx.y; p < P; p += gridDim.y) {
+    uint32_t m[3] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
+    const long long end = off.at(p + 1);
+    for (long long i = off.at(p) + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < end; i += (long long)gridDim.x * blockDim.x) {
 #pragma unroll
-    for (int c = 0; c < 3; ++c) m[c] = min(m[c], dist_key32(pts[3 * i + c]));
-  }
+      for (int c = 0; c < 3; ++c) m[c] = min(m[c], dist_key32(pts[3 * i + c]));
+    }
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    const uint32_t w = __reduce_min_sync(0xffffffffu, m[c]);
-    if ((threadIdx.x & 31) == 0) atomicMin(&minkey[c], w);
+    for (int c = 0; c < 3; ++c) {
+      const uint32_t w = __reduce_min_sync(0xffffffffu, m[c]);
+      if ((threadIdx.x & 31) == 0) atomicMin(&minkey[3 * p + c], w);
+    }
   }
 }
 
@@ -110,17 +163,18 @@ __device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
   return x;
 }
 
-__global__ void vox_insert_kernel(const float* __restrict__ pts, long long n, double voxel, const uint32_t* __restrict__ minkey,
-                                  unsigned long long* keys, unsigned long long* sums, int* counts, unsigned long long slots,
-                                  int32_t* status) {
+__global__ void vox_insert_kernel(const float* __restrict__ pts, long long n, int P, Offsets off, double voxel,
+                                  const uint32_t* __restrict__ minkey, const unsigned long long* __restrict__ slot0,
+                                  unsigned long long* keys, unsigned long long* sums, int* counts, int32_t* status) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  const int p = find_set(P, i, [&](int q) { return (long long)off.at(q); });
   long long ix[3];
   unsigned long long q[3];
   bool bad = false;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const double origin = (double)key32_to_float(minkey[c]) - voxel * 0.5;
+    const double origin = (double)key32_to_float(minkey[3 * p + c]) - voxel * 0.5;
     const double rel = (double)pts[3 * i + c] - origin;
     const double fi = floor(rel / voxel);
     bad |= !(fi >= 0.0 && fi < 2097152.0);             // also catches NaN / inf
@@ -130,85 +184,111 @@ __global__ void vox_insert_kernel(const float* __restrict__ pts, long long n, do
     q[c] = bad ? 0ull : (unsigned long long)__double2ll_rn(frac * kFix);
   }
   if (bad) {
-    atomicOr(status, 1);                               // more than 2^21 voxels along an axis, or a non-finite coordinate
+    atomicOr(&status[p], 1);                           // more than 2^21 voxels along an axis, or a non-finite coordinate
     return;
   }
   const unsigned long long key = ((unsigned long long)ix[0] << 42) | ((unsigned long long)ix[1] << 21) | (unsigned long long)ix[2];
-  unsigned long long s = mix64(key) & (slots - 1);
+  const unsigned long long base = slot0[p], mask = slot0[p + 1] - base - 1;
+  unsigned long long s = mix64(key) & mask;
   while (true) {
-    const unsigned long long prev = atomicCAS(&keys[s], kEmpty, key);
+    const unsigned long long prev = atomicCAS(&keys[base + s], kEmpty, key);
     if (prev == kEmpty || prev == key) break;
-    s = (s + 1) & (slots - 1);
+    s = (s + 1) & mask;
   }
+  s += base;
   atomicAdd(&sums[3 * s], q[0]); atomicAdd(&sums[3 * s + 1], q[1]); atomicAdd(&sums[3 * s + 2], q[2]);
   atomicAdd(&counts[s], 1);
 }
 
-__global__ void vox_compact_kernel(const unsigned long long* __restrict__ keys, unsigned long long slots, unsigned long long* ckeys,
-                                   uint32_t* cslot, int* counter) {
+// occupied slots of cloud p -> ckeys / cslot rows [off[p], off[p] + counter[p]).  Regions are multiples of 1024 slots, so a warp
+// never straddles two clouds.
+__global__ void vox_compact_kernel(const unsigned long long* __restrict__ keys, unsigned long long slots, int P, Offsets off,
+                                   const unsigned long long* __restrict__ slot0, unsigned long long* ckeys, uint32_t* cslot,
+                                   int* counter) {
   const unsigned long long s = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
   const bool occ = s < slots && keys[s] != kEmpty;
   const uint32_t b = __ballot_sync(0xffffffffu, occ);
+  if (!b) return;                                      // warp-uniform
+  const int p = find_set(P, (long long)s, [&](int q) { return (long long)slot0[q]; });
   const int lane = threadIdx.x & 31;
   int base = 0;
-  if (lane == 0 && b) base = atomicAdd(counter, __popc(b));
+  if (lane == 0) base = atomicAdd(&counter[p], __popc(b));
   base = __shfl_sync(0xffffffffu, base, 0);
   if (occ) {
-    const int j = base + __popc(b & ((1u << lane) - 1u));
+    const size_t j = (size_t)off.at(p) + base + __popc(b & ((1u << lane) - 1u));
     ckeys[j] = keys[s];
-    cslot[j] = (uint32_t)s;
+    cslot[j] = (uint32_t)(s - slot0[p]);
   }
 }
 
-// rank of every occupied voxel among all of them (keys are distinct) = its output row
-__global__ void __launch_bounds__(256) vox_rank_kernel(const unsigned long long* __restrict__ ckeys, const uint32_t* __restrict__ cslot,
-                                                       const int* __restrict__ counter, const unsigned long long* __restrict__ sums,
-                                                       const int* __restrict__ counts, const uint32_t* __restrict__ minkey, double voxel,
-                                                       float* __restrict__ out_pts, int32_t* out_count) {
+__global__ void __launch_bounds__(1024) vox_offsets_kernel(int P, const int* __restrict__ counter, int32_t* out_first,
+                                                           int32_t* out_ends) {
+  cta_offsets<int32_t>(P, [&](int q) { return counter[q]; }, out_first, out_ends);
+}
+
+// rank of every occupied voxel among its cloud's (keys are distinct within a cloud) = its row after the cloud's first output row
+__global__ void __launch_bounds__(256) vox_rank_kernel(int P, Offsets off, const unsigned long long* __restrict__ ckeys,
+                                                       const uint32_t* __restrict__ cslot, const int* __restrict__ counter,
+                                                       const unsigned long long* __restrict__ slot0,
+                                                       const unsigned long long* __restrict__ sums, const int* __restrict__ counts,
+                                                       const uint32_t* __restrict__ minkey, double voxel,
+                                                       const int32_t* __restrict__ out_ends, float* __restrict__ out_pts) {
   __shared__ unsigned long long tile[1024];
-  const int m = *counter;
-  if ((long long)blockIdx.x * 256 >= m) return;
-  const int i = blockIdx.x * 256 + threadIdx.x;
-  const unsigned long long mine = i < m ? ckeys[i] : 0ull;
+  const int p = find_set(P, (long long)blockIdx.x, [&](int q) { return rank_tile0(off, q); });
+  const int m = counter[p];
+  const long long local0 = ((long long)blockIdx.x - rank_tile0(off, p)) * 256;
+  if (local0 >= m) return;
+  const unsigned long long* ck = ckeys + off.at(p);
+  const int i = (int)local0 + threadIdx.x;
+  const unsigned long long mine = i < m ? ck[i] : 0ull;
   int rank = 0;
   for (int t0 = 0; t0 < m; t0 += 1024) {
     __syncthreads();
-    for (int j = threadIdx.x; j < 1024; j += 256) tile[j] = (t0 + j < m) ? ckeys[t0 + j] : kEmpty;
+    for (int j = threadIdx.x; j < 1024; j += 256) tile[j] = (t0 + j < m) ? ck[t0 + j] : kEmpty;
     __syncthreads();
 #pragma unroll 8
     for (int j = 0; j < 1024; ++j) rank += tile[j] < mine;
   }
-  if (i == 0) *out_count = m;
   if (i >= m) return;
-  const uint32_t s = cslot[i];
+  const unsigned long long s = slot0[p] + cslot[(size_t)off.at(p) + i];
   const double cnt = (double)counts[s];
   const long long idx[3] = {(long long)(mine >> 42), (long long)((mine >> 21) & 0x1FFFFF), (long long)(mine & 0x1FFFFF)};
+  const size_t row = (size_t)(p ? out_ends[p - 1] : 0) + rank;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const double origin = (double)key32_to_float(minkey[c]) - voxel * 0.5;
-    const double mean_frac = ((double)sums[3 * (size_t)s + c] / kFix) / cnt;
-    out_pts[3 * (size_t)rank + c] = (float)(origin + ((double)idx[c] + mean_frac) * voxel);
+    const double origin = (double)key32_to_float(minkey[3 * p + c]) - voxel * 0.5;
+    const double mean_frac = ((double)sums[3 * s + c] / kFix) / cnt;
+    out_pts[3 * row + c] = (float)(origin + ((double)idx[c] + mean_frac) * voxel);
   }
 }
 
-void launch_voxel_down_sample(const float* pts, long long n, double voxel, float* out_pts, int32_t* out_count, int32_t* status,
-                              void* scratch, cudaStream_t st) {
-  const VoxScratch s = vox_carve(scratch, n);
-  const unsigned long long slots = table_slots(n);
-  vox_init_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, st>>>(s.minkey, s.counter, s.keys, s.sums, s.counts, slots, out_count, status);
+void launch_voxel_down_sample(int P, const int32_t* h_off, const int32_t* d_off, const float* pts, double voxel, float* out_pts,
+                              int32_t* out_first, int32_t* out_ends, int32_t* status, void* scratch, cudaStream_t st) {
+  // without a device table (one cloud) the kernels read the offsets {0, n} as 0 * n, 1 * n
+  const Offsets off{d_off, d_off ? 0 : h_off[1]};
+  const long long n = h_off[P];
+  const unsigned long long slots = total_slots(P, h_off);
+  const VoxScratch s = vox_carve(scratch, P, n, slots);
+  long long most = 0;
+  for (int p = 0; p < P; ++p) most = std::max<long long>(most, (long long)h_off[p + 1] - h_off[p]);
+  vox_plan_kernel<<<1, 1024, 0, st>>>(P, off, s.slot0);
+  const unsigned long long init = std::max<unsigned long long>(slots, 3ull * P);
+  vox_init_kernel<<<(unsigned)((init + 255) / 256), 256, 0, st>>>(P, s.minkey, s.counter, s.keys, s.sums, s.counts, slots, status);
   const int sms = device_sm_count();
-  long long bg = (n + 255) / 256;
-  if (bg > 8LL * sms) bg = 8LL * sms;
-  vox_bounds_kernel<<<(unsigned)bg, 256, 0, st>>>(pts, n, s.minkey);
-  vox_insert_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pts, n, voxel, s.minkey, s.keys, s.sums, s.counts, slots, status);
-  vox_compact_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, st>>>(s.keys, slots, s.ckeys, s.cslot, s.counter);
-  vox_rank_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(s.ckeys, s.cslot, s.counter, s.sums, s.counts, s.minkey, voxel, out_pts,
-                                                              out_count);
+  long long bx = (most + 255) / 256, by = std::min(P, 65535);
+  bx = std::min<long long>(bx, std::max<long long>(1, 8LL * sms / by));
+  vox_bounds_kernel<<<dim3((unsigned)bx, (unsigned)by), 256, 0, st>>>(pts, P, off, s.minkey);
+  vox_insert_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pts, n, P, off, voxel, s.minkey, s.slot0, s.keys, s.sums, s.counts,
+                                                                  status);
+  vox_compact_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, st>>>(s.keys, slots, P, off, s.slot0, s.ckeys, s.cslot, s.counter);
+  vox_offsets_kernel<<<1, 1024, 0, st>>>(P, s.counter, out_first, out_ends);
+  vox_rank_kernel<<<(unsigned)rank_tile0(Offsets{h_off, 0}, P), 256, 0, st>>>(P, off, s.ckeys, s.cslot, s.counter, s.slot0, s.sums,
+                                                                              s.counts, s.minkey, voxel, out_ends, out_pts);
 }
 
 // ---- hybrid (radius + max_nn) neighbour search --------------------------------------------------------------------
-__global__ void __launch_bounds__(256) hybrid_search_kernel(const float* __restrict__ pts, int m, float r2, int max_nn, int P,
-                                                            int warps_per_cta, int32_t* __restrict__ nb_idx,
+__global__ void __launch_bounds__(256) hybrid_search_kernel(const float* __restrict__ pts, int m, int nclouds, Offsets off, float r2,
+                                                            int max_nn, int P, int warps_per_cta, int32_t* __restrict__ nb_idx,
                                                             int32_t* __restrict__ nb_cnt, int32_t* status) {
   extern __shared__ __align__(16) unsigned char hs_smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -220,15 +300,17 @@ __global__ void __launch_bounds__(256) hybrid_search_kernel(const float* __restr
   uint32_t* hist = reinterpret_cast<uint32_t*>(base + (size_t)P * 8);         // [256]
   uint32_t* keys = hist + 256;                                                // [kCandCap]
   int32_t* cidx = reinterpret_cast<int32_t*>(keys + kCandCap);                // [kCandCap]
+  const int cloud = find_set(nclouds, i, [&](int q) { return (long long)off.at(q); });
+  const int r0 = off.at(cloud), r1 = off.at(cloud + 1);
   const float px = pts[3 * (size_t)i], py = pts[3 * (size_t)i + 1], pz = pts[3 * (size_t)i + 2];
   const uint32_t lt_mask = (1u << lane) - 1u;
   int cnt = 0;
   bool overflow = false;
-  for (int j0 = 0; j0 < m; j0 += 32) {
+  for (int j0 = r0; j0 < r1; j0 += 32) {
     const int j = j0 + lane;
     float d2 = 0.f;
     bool in = false;
-    if (j < m) {
+    if (j < r1) {
       const float dx = __fsub_rn(pts[3 * (size_t)j], px), dy = __fsub_rn(pts[3 * (size_t)j + 1], py),
                   dz = __fsub_rn(pts[3 * (size_t)j + 2], pz);
       d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
@@ -244,7 +326,7 @@ __global__ void __launch_bounds__(256) hybrid_search_kernel(const float* __restr
     cnt += __popc(b);
   }
   if (overflow) {
-    if (lane == 0) { atomicOr(status, 2); nb_cnt[i] = 0; }
+    if (lane == 0) { atomicOr(&status[cloud], 2); nb_cnt[i] = 0; }
     for (int r = lane; r < max_nn; r += 32) nb_idx[(size_t)i * max_nn + r] = -1;
     return;
   }
@@ -259,8 +341,10 @@ __global__ void __launch_bounds__(256) hybrid_search_kernel(const float* __restr
   if (lane == 0) nb_cnt[i] = want;
 }
 
-static int launch_hybrid_search(const float* pts, int m, double radius, int max_nn, int32_t* nb_idx, int32_t* nb_cnt, int32_t* status,
-                                cudaStream_t st) {
+static int launch_hybrid_search(int nclouds, const int32_t* h_off, const int32_t* d_off, const float* pts, double radius, int max_nn,
+                                int32_t* nb_idx, int32_t* nb_cnt, int32_t* status, cudaStream_t st) {
+  const int m = h_off[nclouds];
+  const Offsets off{d_off, d_off ? 0 : h_off[1]};     // no device table: one cloud, offsets {0, m}
   int P = 2;
   while (P < max_nn) P <<= 1;
   const size_t per_warp = (size_t)P * 8 + 1024 + (size_t)kCandCap * 8;
@@ -269,8 +353,8 @@ static int launch_hybrid_search(const float* pts, int m, double radius, int max_
   const int smem = (int)(per_warp * warps);
   const cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(hybrid_search_kernel), smem);
   if (e != cudaSuccess) return (int)e;
-  hybrid_search_kernel<<<(m + warps - 1) / warps, warps * 32, smem, st>>>(pts, m, (float)(radius * radius), max_nn, P, warps, nb_idx,
-                                                                         nb_cnt, status);
+  hybrid_search_kernel<<<(m + warps - 1) / warps, warps * 32, smem, st>>>(pts, m, nclouds, off, (float)(radius * radius), max_nn, P,
+                                                                         warps, nb_idx, nb_cnt, status);
   return 0;
 }
 
@@ -459,24 +543,26 @@ size_t fpfh_scratch_bytes(int m, int max_nn) {
   return (size_t)m * max_nn * 4 + (size_t)m * 4 + 16 + (size_t)m * 33 * 8;
 }
 
-int launch_estimate_normals(const float* pts, int m, double radius, int max_nn, double* normals, int32_t* status, void* scratch,
-                            cudaStream_t st) {
+int launch_estimate_normals(int P, const int32_t* h_off, const int32_t* d_off, const float* pts, double radius, int max_nn,
+                            double* normals, int32_t* status, void* scratch, cudaStream_t st) {
+  const int m = h_off[P];
   unsigned char* p = static_cast<unsigned char*>(scratch);
   int32_t* nb_idx = reinterpret_cast<int32_t*>(p + (size_t)m * 33 * 8);
   int32_t* nb_cnt = nb_idx + (size_t)m * max_nn;
-  const int rc = launch_hybrid_search(pts, m, radius, max_nn, nb_idx, nb_cnt, status, st);
+  const int rc = launch_hybrid_search(P, h_off, d_off, pts, radius, max_nn, nb_idx, nb_cnt, status, st);
   if (rc) return rc;
   normals_kernel<<<(m + 127) / 128, 128, 0, st>>>(pts, m, max_nn, nb_idx, nb_cnt, normals);
   return (int)cudaGetLastError();
 }
 
-int launch_compute_fpfh(const float* pts, const double* normals, int m, double radius, int max_nn, int normalise, double* out,
-                        int32_t* status, void* scratch, cudaStream_t st) {
+int launch_compute_fpfh(int P, const int32_t* h_off, const int32_t* d_off, const float* pts, const double* normals, double radius,
+                        int max_nn, int normalise, double* out, int32_t* status, void* scratch, cudaStream_t st) {
+  const int m = h_off[P];
   unsigned char* p = static_cast<unsigned char*>(scratch);
   double* spfh = reinterpret_cast<double*>(p);
   int32_t* nb_idx = reinterpret_cast<int32_t*>(p + (size_t)m * 33 * 8);
   int32_t* nb_cnt = nb_idx + (size_t)m * max_nn;
-  const int rc = launch_hybrid_search(pts, m, radius, max_nn, nb_idx, nb_cnt, status, st);
+  const int rc = launch_hybrid_search(P, h_off, d_off, pts, radius, max_nn, nb_idx, nb_cnt, status, st);
   if (rc) return rc;
   spfh_kernel<<<(m + 7) / 8, 256, 0, st>>>(pts, normals, m, max_nn, nb_idx, nb_cnt, spfh);
   fpfh_kernel<<<(m + 7) / 8, 256, 0, st>>>(pts, m, max_nn, nb_idx, nb_cnt, spfh, normalise, out);

@@ -111,14 +111,17 @@ int launch_leading_eigenvector(const float* M, float* v, int* iters_run, int B, 
                                cudaStream_t st);   // returns cudaError_t
 
 // ---- f2: descriptor front end (fpfh.cu): voxel down-sampling, normals, FPFH -------------------------------------
-size_t voxel_scratch_bytes(long long n);
-void launch_voxel_down_sample(const float* pts, long long n, double voxel, float* out_pts, int32_t* out_count, int32_t* status,
-                              void* scratch, cudaStream_t st);
-size_t fpfh_scratch_bytes(int m, int max_nn);
-int launch_estimate_normals(const float* pts, int m, double radius, int max_nn, double* normals, int32_t* status, void* scratch,
-                            cudaStream_t st);      // returns cudaError_t
-int launch_compute_fpfh(const float* pts, const double* normals, int m, double radius, int max_nn, int normalise, double* out,
-                        int32_t* status, void* scratch, cudaStream_t st);      // returns cudaError_t
+// P clouds packed back to back (offsets [P + 1], host and device; null device tables: one cloud), status [P].  Cloud p's voxel
+// means end at row out_ends[p], written by the call, as is out_first[0] = 0 unless out_first is null.
+size_t voxel_scratch_bytes(int P, const int32_t* h_off);
+void launch_voxel_down_sample(int P, const int32_t* h_off, const int32_t* d_off, const float* pts, double voxel, float* out_pts,
+                              int32_t* out_first, int32_t* out_ends, int32_t* status, void* scratch, cudaStream_t st);
+size_t fpfh_scratch_bytes(int m, int max_nn);      // m: the call's total key points
+int launch_estimate_normals(int P, const int32_t* h_off, const int32_t* d_off, const float* pts, double radius, int max_nn,
+                            double* normals, int32_t* status, void* scratch, cudaStream_t st);      // returns cudaError_t
+int launch_compute_fpfh(int P, const int32_t* h_off, const int32_t* d_off, const float* pts, const double* normals, double radius,
+                        int max_nn, int normalise, double* out, int32_t* status, void* scratch,
+                        cudaStream_t st);      // returns cudaError_t
 
 // ---- per-device launch configuration (device_state.cu) ----------------------------------------------------
 // opt `kernel` in to `bytes` of dynamic shared memory on the CURRENT device (no-op if already granted there)

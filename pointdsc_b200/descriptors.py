@@ -6,18 +6,22 @@ Mirrors the open3d 0.9 calls the reference makes before matching (misc/cal_fpfh.
     pcd.estimate_normals(KDTreeSearchParamHybrid(radius=2 * voxel, max_nn=30))     -> estimate_normals(keypts, 2 * voxel, 30)
     compute_fpfh_feature(pcd, KDTreeSearchParamHybrid(radius=5 * voxel, max_nn=100)) -> compute_fpfh(keypts, normals, 5 * voxel, 100)
 
+`fpfh_descriptors_many` runs the same chain over a group of clouds of different sizes, one call per stage (what misc/cal_fpfh.py
+does cloud by cloud over a data set; `cal_fpfh.py` at the repository root is that script).
+
 open3d itself is not part of the reference tree or of this image: the kernels follow its published algorithms and are checked
 against the CPU restatement under oracle/ (parity unpinned, see its header).  Everything runs on the GPU; there is no CPU fallback.
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Tuple
+from typing import List, Sequence, Tuple
 
 import numpy as np
 import torch
 
 from . import _capi
+from .frontend import host_to_device
 
 _STATUS = {1: "more than 2^21 voxels along an axis, or a non-finite coordinate",
            2: "a neighbourhood holds more than 4096 points inside the search radius (the search is sized for down-sampled clouds)"}
@@ -116,3 +120,64 @@ def fpfh_descriptors(points: torch.Tensor, voxel_size: float) -> Tuple[torch.Ten
     normals = estimate_normals(keypts, 2.0 * voxel_size, 30)
     feat = compute_fpfh(keypts, normals, 5.0 * voxel_size, 100, normalise=True)
     return keypts, feat
+
+
+@torch.no_grad()
+def fpfh_descriptors_many(clouds: Sequence[torch.Tensor], voxel_size: float,
+                          normalise: bool = True) -> Tuple[torch.Tensor, torch.Tensor, List[int], torch.Tensor]:
+    """`fpfh_descriptors` of P clouds of different sizes, one call per stage (pdsc_*_packed).  `clouds`: device [n_p,3] tensors.
+    Returns (key points [M,3] float32, FPFH [M,33] float64, offsets (host list of P + 1 ints), d_offsets (the same offsets as a
+    device int32 tensor)); cloud p's rows are offsets[p]:offsets[p+1] and bit for bit what `fpfh_descriptors` gives for that
+    cloud alone (normalise=False: the raw FPFH, as misc/cal_fpfh.py stores it).  The group makes two host reads: the key-point
+    offsets after the down-sampling, which fix the shapes, and the status words at the end."""
+    if not clouds:
+        raise ValueError("fpfh_descriptors_many needs at least one cloud")
+    dev, lib, engine, stream = _ctx(clouds[0])
+    for i, c in enumerate(clouds):
+        if c.device != dev or c.dim() != 2 or c.shape[1] != 3 or c.shape[0] < 1:
+            raise ValueError(f"cloud {i}: expected a [n,3] tensor on {dev} with n >= 1, got {tuple(c.shape)} on {c.device}")
+    P = len(clouds)
+    in_off = [0]
+    for c in clouds:
+        in_off.append(in_off[-1] + int(c.shape[0]))
+    pts = (torch.cat([c.to(torch.float32) for c in clouds]) if P > 1 else clouds[0].to(torch.float32)).contiguous()
+    d_in = host_to_device(in_off, torch.int32, dev)
+    h_in = (C.c_int32 * (P + 1))(*in_off)
+    out = torch.empty(in_off[-1], 3, dtype=torch.float32, device=dev)
+    meta = torch.empty(2 * P + 1, dtype=torch.int32, device=dev)       # [key-point offsets (P + 1), voxel status (P)]
+    scratch = torch.empty(int(lib.pdsc_voxel_down_sample_packed_scratch_bytes(P, h_in)) + 8, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _capi.check(lib.pdsc_voxel_down_sample_packed(engine, P, h_in, C.c_void_p(d_in.data_ptr()), C.c_void_p(pts.data_ptr()),
+                                                      float(voxel_size), C.c_void_p(out.data_ptr()), C.c_void_p(meta.data_ptr()),
+                                                      C.c_void_p(meta.data_ptr() + 4 * (P + 1)),
+                                                      C.c_void_p((scratch.data_ptr() + 7) // 8 * 8), scratch.numel() - 8, stream))
+    h_meta = meta.tolist()                                         # read 1: the key-point offsets fix the shapes
+    offsets = h_meta[:P + 1]
+    _raise_cloud_status(h_meta[P + 1:])
+    d_offsets = meta[:P + 1]
+    keypts = out[:offsets[-1]].clone()
+    del out, scratch
+    h_kp = (C.c_int32 * (P + 1))(*offsets)
+    m = offsets[-1]
+    normals = torch.empty(m, 3, dtype=torch.float64, device=dev)
+    feat = torch.empty(m, 33, dtype=torch.float64, device=dev)
+    status = torch.empty(2, P, dtype=torch.int32, device=dev)
+    scratch = torch.empty(int(lib.pdsc_fpfh_packed_scratch_bytes(P, h_kp, 100)) + 8, dtype=torch.uint8, device=dev)
+    sc = C.c_void_p((scratch.data_ptr() + 7) // 8 * 8)
+    with torch.cuda.device(dev):                                   # the normals' search (max_nn 30) fits the FPFH's scratch
+        _capi.check(lib.pdsc_estimate_normals_packed(engine, P, h_kp, C.c_void_p(d_offsets.data_ptr()), C.c_void_p(keypts.data_ptr()),
+                                                     2.0 * voxel_size, 30, C.c_void_p(normals.data_ptr()),
+                                                     C.c_void_p(status.data_ptr()), sc, scratch.numel() - 8, stream))
+        _capi.check(lib.pdsc_compute_fpfh_packed(engine, P, h_kp, C.c_void_p(d_offsets.data_ptr()), C.c_void_p(keypts.data_ptr()),
+                                                 C.c_void_p(normals.data_ptr()), 5.0 * voxel_size, 100, 1 if normalise else 0,
+                                                 C.c_void_p(feat.data_ptr()), C.c_void_p(status[1].data_ptr()), sc,
+                                                 scratch.numel() - 8, stream))
+    st = status.cpu()                                              # read 2: the status words
+    _raise_cloud_status((st[0] | st[1]).tolist())
+    return keypts, feat, offsets, d_offsets
+
+
+def _raise_cloud_status(status: Sequence[int]) -> None:
+    for p, s in enumerate(status):
+        if s:
+            raise _capi.PdscError(f"cloud {p}: " + "; ".join(msg for bit, msg in _STATUS.items() if s & bit))

@@ -43,5 +43,6 @@ for dt in (torch.float32, torch.float64):
 from pointdsc_b200 import descriptors as D
 from pointdsc_b200.synth_scene import scene
 kp, feat = D.fpfh_descriptors(torch.from_numpy(scene(4000, seed=0)).cuda(), 0.15)
+kp_many, feat_many, _, _ = D.fpfh_descriptors_many([torch.from_numpy(scene(nn, seed=nn)).cuda() for nn in (4000, 1, 700)], 0.15)  # the packed calls
 torch.cuda.synchronize()
 print("sanitize_smoke ok", float(st.sum()), int(it.sum()), r["corr"].shape, tuple(feat.shape))
