@@ -15,8 +15,12 @@ What it replaces, line by line (reference file:line):
   evaluation/test_3DMatch.py:38-54            .cuda() + model(data)                                 -> model(data) on device tensors
   evaluation/test_3DMatch.py:83-101           TransformationLoss / ClassificationLoss per pair      -> eval_stats (one launch, no sync)
   evaluation/test_3DMatch.py:139-172          scene-level and pair-level summary                    -> summarise
-The statistics of ALL pairs stay on the device and are read once at the end.  RANSAC / ICP post-processing (open3d) and the FCGF
-network are out of scope (DESIGN.md section 8); the FCGF descriptors of the reference's data set are plain *.npz files and work."""
+  evaluation/test_3DMatch.py:79-80            --use_icp: icp_refine (open3d registration_icp, r 0.10) -> pointdsc_b200.icp (row f5)
+The statistics of ALL pairs stay on the device and are read once at the end.  With --use_icp the network's transform is refined by
+point-to-point ICP over the pair's correspondence key points (max correspondence distance 0.10 for every snapshot, as the reference
+passes it) after the forward and before the statistics, inside the model time; the labels stay the network's.  RANSAC
+post-processing (open3d) and the FCGF network are out of scope (DESIGN.md section 8); the FCGF descriptors of the reference's data
+set are plain *.npz files and work."""
 import argparse
 import json
 import os
@@ -144,7 +148,7 @@ def dataset_pairs(root, scenes, descriptor, device):
 
 
 @torch.no_grad()
-def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1):
+def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1, use_icp=False):
     """The loop of evaluation/test_3DMatch.py:21-103 over an iterable of (scene index, (src xyz, src desc), (tgt xyz, tgt desc),
     gt_trans): returns a [pairs, 13] float64 array, columns = COLUMNS.
     batch_size 1: per pair `match`, labels, `model(data)` and `eval_stats`; the only read from the device inside the loop is the
@@ -155,20 +159,28 @@ def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1):
     of a pair is then its group's device time divided by the group's size, and its data-time column its own loading time plus
     its share of the group's matching.  A model without `forward_packed` that offers `forward_many` (a wrapper or stand-in
     with the mixed-size interface only) is grouped pair by pair instead: `match`, labels, one `forward_many` per group and
-    `eval_stats` per pair."""
+    `eval_stats` per pair.
+    use_icp: the forward's transform is refined on the device before the statistics and inside the model-time events
+    (evaluation/test_3DMatch.py:79-80): `icp_refine` per pair, one `icp_refine_packed` per packed group."""
     from pointdsc_b200.frontend import match, match_many
     from pointdsc_b200.metrics import eval_stats, eval_stats_packed
     rows, scene_ids, data_s, events = [], [], [], []
     packed = batch_size > 1 and hasattr(model, "forward_packed")
     group = []          # pairs waiting for the group: packed ((src xyz, src desc), (tgt xyz, tgt desc), gt), else (data, gt_t, labels)
+    if use_icp:
+        from pointdsc_b200 import icp
+
+    def refine(data, trans):
+        return icp.icp_refine(data["src_keypts"], data["tgt_keypts"], trans) if use_icp else trans
 
     def run_pair_group():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         results = model.forward_many([g[0] for g in group])
+        trans = [refine(data, res["final_trans"]) for (data, _, _), res in zip(group, results)]
         e1.record()
-        for (data, gt_t, labels), res in zip(group, results):
-            rows.append(eval_stats(res["final_trans"], gt_t[None], data["src_keypts"], data["tgt_keypts"], res["final_labels"],
+        for (data, gt_t, labels), res, tr in zip(group, results, trans):
+            rows.append(eval_stats(tr, gt_t[None], data["src_keypts"], data["tgt_keypts"], res["final_labels"],
                                    labels, re_thre=cfg["re_thre"], te_thre=cfg["te_thre"]))
             events.append((e0, e1, len(group)))
         group.clear()
@@ -186,8 +198,11 @@ def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         res = model.forward_packed(m["corr_pos"], m["src_keypts"], m["tgt_keypts"], off, d_offsets=m["d_offsets"])
+        trans = res["final_trans"]
+        if use_icp:
+            trans = icp.icp_refine_packed(m["src_keypts"], m["tgt_keypts"], trans, off, d_offsets=m["d_offsets"])
         e1.record()
-        rows.append(eval_stats_packed(res["final_trans"], gts, m["src_keypts"], m["tgt_keypts"], res["final_labels"], labels, off,
+        rows.append(eval_stats_packed(trans, gts, m["src_keypts"], m["tgt_keypts"], res["final_labels"], labels, off,
                                       d_offsets=m["d_offsets"], re_thre=cfg["re_thre"], te_thre=cfg["te_thre"]))
         events.extend([(e0, e1, len(group))] * len(group))
         group.clear()
@@ -218,8 +233,9 @@ def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         res = model(data)
+        trans = refine(data, res["final_trans"])
         e1.record()
-        rows.append(eval_stats(res["final_trans"], gt_t[None], data["src_keypts"], data["tgt_keypts"], res["final_labels"], labels,
+        rows.append(eval_stats(trans, gt_t[None], data["src_keypts"], data["tgt_keypts"], res["final_labels"], labels,
                                re_thre=cfg["re_thre"], te_thre=cfg["te_thre"]))
         events.append((e0, e1, 1))
         t_data = time.perf_counter()
@@ -282,6 +298,8 @@ def parse_args(argv=None):
                     help="pairs per group: > 1 matches, runs and scores every group of pairs (of different sizes) in one call each")
     ap.add_argument("--batch_invariant", action="store_true",
                     help="every pair's result independent of --batch_size and of the GPU's SM count (PointDSC batch_invariant)")
+    ap.add_argument("--use_icp", action="store_true",
+                    help="refine every transform by point-to-point ICP on the device (max correspondence distance 0.10)")
     return ap.parse_args(argv)
 
 
@@ -299,7 +317,8 @@ def main(argv=None):
         pairs = dataset_pairs(args.root, names, descriptor, "cuda")
     if args.batch_size < 1:
         sys.exit("--batch_size must be >= 1")
-    stats = evaluate(model, pairs, cfg, use_mutual=args.use_mutual or cfg["use_mutual"], batch_size=args.batch_size)
+    stats = evaluate(model, pairs, cfg, use_mutual=args.use_mutual or cfg["use_mutual"], batch_size=args.batch_size,
+                     use_icp=args.use_icp)
     summary = summarise(stats, names)
     if args.save_npy:
         np.save(args.save_npy, stats)

@@ -300,6 +300,27 @@ int pdsc_estimate_normals_packed(pdsc_engine* e, int32_t P, const int32_t* h_off
 int pdsc_compute_fpfh_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
                              const double* d_normals, double radius, int32_t max_nn, int32_t normalise, double* d_fpfh,
                              int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+/* f5: point-to-point ICP over the correspondence key points, replacing icp_refine (evaluation/benchmark_utils.py:40-55): open3d 0.9's
+ * registration_icp(src, tgt, max_corr_dist, init, TransformationEstimationPointToPoint(False), ICPConvergenceCriteria()) with the
+ * criteria fixed at their defaults (relative fitness 1e-6, relative rmse 1e-6).  open3d is not part of the reference tree: this
+ * follows its published algorithm (oracle/icp_oracle.py; PARITY UNPINNED).  B sets; set b owns rows [offsets[b], offsets[b+1]) of
+ * d_src / d_tgt [R,3] (the pair's src_keypts / tgt_keypts); offsets has B + 1 entries, starts at 0, every set at least one row
+ * (else PDSC_ERR_SHAPE, and pdsc_icp_packed_scratch_bytes() returns 0); h_offsets (host) is validated and sizes the scratch,
+ * d_offsets (device, the same values) is what the kernel reads.  T starts at d_init [B,4,4] and is kept in fp64; every source row is
+ * matched to its nearest target row of the same set, kept iff d^2 < float32(max_corr_dist^2), ties to the lowest row; each
+ * iteration applies the unscaled Umeyama update over the kept pairs, for at most max_iteration (>= 1) updates.  Outputs:
+ * d_trans [B,4,4] float32; optional (may be NULL) d_fitness [B] (kept / N_b), d_rmse [B] (inlier RMSE), d_iterations [B] (updates
+ * applied), d_status [B] (1: a non-finite coordinate, or the target spans 2^21 or more cells of side max_corr_dist along an axis;
+ * such a set returns d_init after 0 iterations with fitness = rmse = 0).  PDSC_ERR_INVALID_ARGUMENT for max_corr_dist <= 0 or not
+ * finite and for max_iteration < 1.  A set's outputs depend on its own rows only: bit for bit the same in any call, in any order, on
+ * any SM count.  Scratch: pdsc_icp_packed_scratch_bytes() bytes, 8-byte aligned.  No host synchronisation, no allocation,
+ * capturable in a CUDA graph. */
+size_t pdsc_icp_packed_scratch_bytes(int32_t B, const int32_t* h_offsets);
+int pdsc_icp_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
+                    const float* d_tgt, const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans,
+                    double* d_fitness, double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
+                    void* cuda_stream);
+
 /* Vertex positions of a PLY file (ascii or binary_little_endian; x, y, z float or double) into host memory as [n,3] float32.
  * Call with points = NULL to learn *n_vertices, then with a buffer of `capacity` >= n vertices. */
 int pdsc_read_ply(const char* path, float* points, int64_t capacity, int64_t* n_vertices);

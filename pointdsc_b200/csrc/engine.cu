@@ -1017,6 +1017,32 @@ int pdsc_compute_fpfh_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets
                      d_status, d_scratch, scratch_bytes, cuda_stream);
 }
 
+size_t pdsc_icp_packed_scratch_bytes(int32_t B, const int32_t* h_offsets) {
+  return cloud_offsets_ok(B, h_offsets) ? pdsc::icp_scratch_bytes(h_offsets[B]) : 0;
+}
+
+int pdsc_icp_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
+                    const float* d_tgt, const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans,
+                    double* d_fitness, double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
+                    void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  const int rc = check_pair_offsets("pdsc_icp_packed", "", B, h_offsets, 1);
+  if (rc) return rc;
+  if (!d_offsets || !d_src || !d_tgt || !d_init || !d_trans) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_icp_packed: null tensor pointer");
+  if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_icp_packed: max_corr_dist must be positive and finite (got %g)", max_corr_dist);
+  if (max_iteration < 1) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_icp_packed: max_iteration must be >= 1 (got %d)", max_iteration);
+  const size_t need = pdsc::icp_scratch_bytes(h_offsets[B]);
+  if (!d_scratch || scratch_bytes < need || reinterpret_cast<uintptr_t>(d_scratch) % 8)
+    return fail(PDSC_ERR_WORKSPACE, "pdsc_icp_packed: scratch too small or not 8-byte aligned (%zu bytes given, %zu needed)",
+                scratch_bytes, need);
+  DeviceGuard g(e->cfg.device);
+  pdsc::launch_icp(B, d_offsets, h_offsets[B], d_src, d_tgt, d_init, max_corr_dist, max_iteration, d_trans, d_fitness, d_rmse,
+                   d_iterations, d_status, d_scratch, static_cast<cudaStream_t>(cuda_stream));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
+
 // Host-side PLY vertex reader (ascii / binary_little_endian; x, y, z as float or double; other vertex properties skipped).
 int pdsc_read_ply(const char* path, float* points, int64_t capacity, int64_t* n_vertices) {
   if (!path || !n_vertices) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_read_ply: null argument");

@@ -123,6 +123,14 @@ int launch_compute_fpfh(int P, const int32_t* h_off, const int32_t* d_off, const
                         int max_nn, int normalise, double* out, int32_t* status, void* scratch,
                         cudaStream_t st);      // returns cudaError_t
 
+// ---- point-to-point ICP over the correspondence key points (icp.cu) ---------------------------------------------
+// B sets packed back to back (device offsets [B + 1], R = offsets[B] rows), init / trans [B,4,4]; fitness, rmse, iterations and
+// status may be null.  Scratch: icp_scratch_bytes(R) bytes, 8-byte aligned.
+size_t icp_scratch_bytes(long long R);
+void launch_icp(int B, const int32_t* d_off, long long R, const float* src, const float* tgt, const float* init, double r,
+                int max_iteration, float* trans, double* fitness, double* rmse, int32_t* iterations, int32_t* status, void* scratch,
+                cudaStream_t st);
+
 // ---- per-device launch configuration (device_state.cu) ----------------------------------------------------
 // opt `kernel` in to `bytes` of dynamic shared memory on the CURRENT device (no-op if already granted there)
 cudaError_t ensure_dynamic_smem(const void* kernel, int bytes);

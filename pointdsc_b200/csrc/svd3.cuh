@@ -14,65 +14,103 @@
 
 namespace pdsc {
 
-struct Vec3 {
-  float x, y, z;
+// The solver is templated on its scalar: `float` for the forward's per-seed and refinement solves, `double` for the ICP
+// updates (icp.cu).  Each scalar has its own thresholds; the float ones are the literals the float solver has always used.
+template <typename T> struct KabschTol;
+template <> struct KabschTol<float> {
+  static constexpr float skip = 1e-9f;     // columns this close to orthogonal (cosine) are left alone
+  static constexpr float big = 1e8f;       // |zeta| above which t = 1 / (2 zeta)
+  static constexpr float tiny = 1e-30f;    // floor of the squared norms that are inverted
+  static constexpr float rank = 1e-12f;    // second squared singular value, relative to the first, below which H is rank 1
+  static constexpr float perp = 0.6f;
 };
-__device__ __forceinline__ float dot3(Vec3 a, Vec3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
-__device__ __forceinline__ Vec3 cross3(Vec3 a, Vec3 b) {
+template <> struct KabschTol<double> {
+  static constexpr double skip = 1e-18;
+  static constexpr double big = 1e8;
+  static constexpr double tiny = 1e-30;
+  static constexpr double rank = 1e-24;
+  static constexpr double perp = 0.6;
+};
+
+__device__ __forceinline__ float k_abs(float x) { return fabsf(x); }
+__device__ __forceinline__ double k_abs(double x) { return fabs(x); }
+__device__ __forceinline__ float k_sqrt(float x) { return sqrtf(x); }
+__device__ __forceinline__ double k_sqrt(double x) { return sqrt(x); }
+__device__ __forceinline__ float k_rsqrt(float x) { return rsqrtf(x); }
+__device__ __forceinline__ double k_rsqrt(double x) { return 1.0 / sqrt(x); }
+__device__ __forceinline__ float k_copysign(float a, float b) { return copysignf(a, b); }
+__device__ __forceinline__ double k_copysign(double a, double b) { return copysign(a, b); }
+__device__ __forceinline__ float k_max(float a, float b) { return fmaxf(a, b); }
+__device__ __forceinline__ double k_max(double a, double b) { return fmax(a, b); }
+__device__ __forceinline__ int k_ilogb(float x) { return ilogbf(x); }
+__device__ __forceinline__ int k_ilogb(double x) { return ilogb(x); }
+__device__ __forceinline__ float k_scalbn(float x, int e) { return scalbnf(x, e); }
+__device__ __forceinline__ double k_scalbn(double x, int e) { return scalbn(x, e); }
+
+template <typename T>
+struct Vec3T {
+  T x, y, z;
+};
+using Vec3 = Vec3T<float>;
+template <typename T> __device__ __forceinline__ T dot3(Vec3T<T> a, Vec3T<T> b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+template <typename T> __device__ __forceinline__ Vec3T<T> cross3(Vec3T<T> a, Vec3T<T> b) {
   return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x};
 }
-__device__ __forceinline__ Vec3 scale3(Vec3 a, float s) { return {a.x * s, a.y * s, a.z * s}; }
-__device__ __forceinline__ Vec3 sub3(Vec3 a, Vec3 b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
+template <typename T> __device__ __forceinline__ Vec3T<T> scale3(Vec3T<T> a, T s) { return {a.x * s, a.y * s, a.z * s}; }
+template <typename T> __device__ __forceinline__ Vec3T<T> sub3(Vec3T<T> a, Vec3T<T> b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
 
-__device__ __forceinline__ void jacobi_pair(Vec3& gp, Vec3& gq, Vec3& vp, Vec3& vq) {
-  const float alpha = dot3(gp, gp), beta = dot3(gq, gq), gamma = dot3(gp, gq);
-  if (fabsf(gamma) <= 1e-9f * sqrtf(alpha * beta) || gamma == 0.0f) return;
-  const float zeta = (beta - alpha) / (2.0f * gamma);
-  float t;
-  if (fabsf(zeta) > 1e8f) {
-    t = 0.5f / zeta;
+template <typename T>
+__device__ __forceinline__ void jacobi_pair(Vec3T<T>& gp, Vec3T<T>& gq, Vec3T<T>& vp, Vec3T<T>& vq) {
+  const T alpha = dot3(gp, gp), beta = dot3(gq, gq), gamma = dot3(gp, gq);
+  if (k_abs(gamma) <= KabschTol<T>::skip * k_sqrt(alpha * beta) || gamma == T(0)) return;
+  const T zeta = (beta - alpha) / (T(2) * gamma);
+  T t;
+  if (k_abs(zeta) > KabschTol<T>::big) {
+    t = T(0.5) / zeta;
   } else {
-    t = copysignf(1.0f, zeta) / (fabsf(zeta) + sqrtf(1.0f + zeta * zeta));
+    t = k_copysign(T(1), zeta) / (k_abs(zeta) + k_sqrt(T(1) + zeta * zeta));
   }
-  const float c = rsqrtf(1.0f + t * t), s = c * t;
-  const Vec3 gp2 = {c * gp.x - s * gq.x, c * gp.y - s * gq.y, c * gp.z - s * gq.z};
-  const Vec3 gq2 = {s * gp.x + c * gq.x, s * gp.y + c * gq.y, s * gp.z + c * gq.z};
-  const Vec3 vp2 = {c * vp.x - s * vq.x, c * vp.y - s * vq.y, c * vp.z - s * vq.z};
-  const Vec3 vq2 = {s * vp.x + c * vq.x, s * vp.y + c * vq.y, s * vp.z + c * vq.z};
+  const T c = k_rsqrt(T(1) + t * t), s = c * t;
+  const Vec3T<T> gp2 = {c * gp.x - s * gq.x, c * gp.y - s * gq.y, c * gp.z - s * gq.z};
+  const Vec3T<T> gq2 = {s * gp.x + c * gq.x, s * gp.y + c * gq.y, s * gp.z + c * gq.z};
+  const Vec3T<T> vp2 = {c * vp.x - s * vq.x, c * vp.y - s * vq.y, c * vp.z - s * vq.z};
+  const Vec3T<T> vq2 = {s * vp.x + c * vq.x, s * vp.y + c * vq.y, s * vp.z + c * vq.z};
   gp = gp2; gq = gq2; vp = vp2; vq = vq2;
 }
 
-__device__ __forceinline__ Vec3 any_perpendicular(Vec3 a) {
+template <typename T>
+__device__ __forceinline__ Vec3T<T> any_perpendicular(Vec3T<T> a) {
   // unit vector orthogonal to unit vector a
-  Vec3 e = (fabsf(a.x) < 0.6f) ? Vec3{1.f, 0.f, 0.f} : Vec3{0.f, 1.f, 0.f};
-  Vec3 p = sub3(e, scale3(a, dot3(e, a)));
-  return scale3(p, rsqrtf(fmaxf(dot3(p, p), 1e-30f)));
+  Vec3T<T> e = (k_abs(a.x) < KabschTol<T>::perp) ? Vec3T<T>{T(1), T(0), T(0)} : Vec3T<T>{T(0), T(1), T(0)};
+  Vec3T<T> p = sub3(e, scale3(a, dot3(e, a)));
+  return scale3(p, k_rsqrt(k_max(dot3(p, p), KabschTol<T>::tiny)));
 }
 
 // H row-major (H[i*3+j] = sum_n w_n Am[n][i] Bm[n][j]); writes R row-major with  b ~= R a.
-__device__ __forceinline__ void kabsch_rotation(const float* H, float* R) {
-  // scale to O(1) so the squared norms stay well inside fp32 range; R is scale invariant.  First by 2^-ilogb(hmax), which is
-  // exact (subnormal H included) and leaves the largest entry in [1, 2), then by the reciprocal of that entry.  Dividing by
-  // hmax itself overflows to +Inf for hmax below 2^-128 (0 * Inf = NaN).  In this order every scaled entry equals
-  // H[i] * (1 / hmax) bit for bit wherever both are normal floats, and R is bit-identical for H and 2^e H.
-  float hmax = 0.f;
-  bool nan = false;   // fmaxf returns the other operand of a NaN: hmax alone would not see one
+template <typename T>
+__device__ __forceinline__ void kabsch_rotation(const T* H, T* R) {
+  // scale to O(1) so the squared norms stay well inside the scalar's range; R is scale invariant.  First by 2^-ilogb(hmax), which
+  // is exact (subnormal H included) and leaves the largest entry in [1, 2), then by the reciprocal of that entry.  Dividing by
+  // hmax itself overflows to +Inf for hmax below 2^-128 (0 * Inf = NaN) in float.  In this order every scaled entry equals
+  // H[i] * (1 / hmax) bit for bit wherever both are normal numbers, and R is bit-identical for H and 2^e H.
+  T hmax = T(0);
+  bool nan = false;   // fmax returns the other operand of a NaN: hmax alone would not see one
 #pragma unroll
   for (int i = 0; i < 9; ++i) {
-    hmax = fmaxf(hmax, fabsf(H[i]));
+    hmax = k_max(hmax, k_abs(H[i]));
     nan = nan || isnan(H[i]);
   }
-  if (nan || !(hmax > 0.f) || !isfinite(hmax)) {
+  if (nan || !(hmax > T(0)) || !isfinite(hmax)) {
     // H == 0 (or non-finite): LAPACK returns U = V = I for a zero matrix -> R = I
-    R[0] = 1.f; R[1] = 0.f; R[2] = 0.f; R[3] = 0.f; R[4] = 1.f; R[5] = 0.f; R[6] = 0.f; R[7] = 0.f; R[8] = 1.f;
+    R[0] = T(1); R[1] = T(0); R[2] = T(0); R[3] = T(0); R[4] = T(1); R[5] = T(0); R[6] = T(0); R[7] = T(0); R[8] = T(1);
     return;
   }
-  const int e = -ilogbf(hmax);
-  const float inv = 1.0f / scalbnf(hmax, e);
-  Vec3 g0 = {scalbnf(H[0], e) * inv, scalbnf(H[3], e) * inv, scalbnf(H[6], e) * inv};   // columns of H
-  Vec3 g1 = {scalbnf(H[1], e) * inv, scalbnf(H[4], e) * inv, scalbnf(H[7], e) * inv};
-  Vec3 g2 = {scalbnf(H[2], e) * inv, scalbnf(H[5], e) * inv, scalbnf(H[8], e) * inv};
-  Vec3 v0 = {1.f, 0.f, 0.f}, v1 = {0.f, 1.f, 0.f}, v2 = {0.f, 0.f, 1.f};
+  const int e = -k_ilogb(hmax);
+  const T inv = T(1) / k_scalbn(hmax, e);
+  Vec3T<T> g0 = {k_scalbn(H[0], e) * inv, k_scalbn(H[3], e) * inv, k_scalbn(H[6], e) * inv};   // columns of H
+  Vec3T<T> g1 = {k_scalbn(H[1], e) * inv, k_scalbn(H[4], e) * inv, k_scalbn(H[7], e) * inv};
+  Vec3T<T> g2 = {k_scalbn(H[2], e) * inv, k_scalbn(H[5], e) * inv, k_scalbn(H[8], e) * inv};
+  Vec3T<T> v0 = {T(1), T(0), T(0)}, v1 = {T(0), T(1), T(0)}, v2 = {T(0), T(0), T(1)};
 #pragma unroll 1
   for (int sweep = 0; sweep < 8; ++sweep) {
     jacobi_pair(g0, g1, v0, v1);
@@ -80,19 +118,20 @@ __device__ __forceinline__ void kabsch_rotation(const float* H, float* R) {
     jacobi_pair(g1, g2, v1, v2);
   }
   // order by decreasing singular value (column swaps; the cross-product form is blind to det(V))
-  float n0 = dot3(g0, g0), n1 = dot3(g1, g1), n2 = dot3(g2, g2);
-  if (n0 < n1) { Vec3 t = g0; g0 = g1; g1 = t; t = v0; v0 = v1; v1 = t; float s = n0; n0 = n1; n1 = s; }
-  if (n0 < n2) { Vec3 t = g0; g0 = g2; g2 = t; t = v0; v0 = v2; v2 = t; float s = n0; n0 = n2; n2 = s; }
-  if (n1 < n2) { Vec3 t = g1; g1 = g2; g2 = t; t = v1; v1 = v2; v2 = t; float s = n1; n1 = n2; n2 = s; }
+  T n0 = dot3(g0, g0), n1 = dot3(g1, g1), n2 = dot3(g2, g2);
+  if (n0 < n1) { Vec3T<T> t = g0; g0 = g1; g1 = t; t = v0; v0 = v1; v1 = t; T s = n0; n0 = n1; n1 = s; }
+  if (n0 < n2) { Vec3T<T> t = g0; g0 = g2; g2 = t; t = v0; v0 = v2; v2 = t; T s = n0; n0 = n2; n2 = s; }
+  if (n1 < n2) { Vec3T<T> t = g1; g1 = g2; g2 = t; t = v1; v1 = v2; v2 = t; T s = n1; n1 = n2; n2 = s; }
   // u1, u2 (Gram-Schmidt clean-up); v1, v2 likewise
-  Vec3 u1 = scale3(g0, rsqrtf(fmaxf(n0, 1e-30f)));
-  Vec3 u2 = sub3(g1, scale3(u1, dot3(g1, u1)));
-  const float n1c = dot3(u2, u2);
-  if (n1c > 1e-12f * fmaxf(n0, 1e-30f)) u2 = scale3(u2, rsqrtf(n1c)); else u2 = any_perpendicular(u1);
-  Vec3 w1 = scale3(v0, rsqrtf(fmaxf(dot3(v0, v0), 1e-30f)));
-  Vec3 w2 = sub3(v1, scale3(w1, dot3(v1, w1)));
-  w2 = scale3(w2, rsqrtf(fmaxf(dot3(w2, w2), 1e-30f)));
-  const Vec3 u3 = cross3(u1, u2), w3 = cross3(w1, w2);
+  const T tiny = KabschTol<T>::tiny;
+  Vec3T<T> u1 = scale3(g0, k_rsqrt(k_max(n0, tiny)));
+  Vec3T<T> u2 = sub3(g1, scale3(u1, dot3(g1, u1)));
+  const T n1c = dot3(u2, u2);
+  if (n1c > KabschTol<T>::rank * k_max(n0, tiny)) u2 = scale3(u2, k_rsqrt(n1c)); else u2 = any_perpendicular(u1);
+  Vec3T<T> w1 = scale3(v0, k_rsqrt(k_max(dot3(v0, v0), tiny)));
+  Vec3T<T> w2 = sub3(v1, scale3(w1, dot3(v1, w1)));
+  w2 = scale3(w2, k_rsqrt(k_max(dot3(w2, w2), tiny)));
+  const Vec3T<T> u3 = cross3(u1, u2), w3 = cross3(w1, w2);
   R[0] = w1.x * u1.x + w2.x * u2.x + w3.x * u3.x;
   R[1] = w1.x * u1.y + w2.x * u2.y + w3.x * u3.y;
   R[2] = w1.x * u1.z + w2.x * u2.z + w3.x * u3.z;

@@ -44,5 +44,9 @@ from pointdsc_b200 import descriptors as D
 from pointdsc_b200.synth_scene import scene
 kp, feat = D.fpfh_descriptors(torch.from_numpy(scene(4000, seed=0)).cuda(), 0.15)
 kp_many, feat_many, _, _ = D.fpfh_descriptors_many([torch.from_numpy(scene(nn, seed=nn)).cuda() for nn in (4000, 1, 700)], 0.15)  # the packed calls
+from pointdsc_b200.icp import icp_refine, icp_refine_packed
+ic = icp_refine(h["src_keypts"].cuda(), h["tgt_keypts"].cuda(), out["final_trans"])
+ip, ii = icp_refine_packed(pk["src_keypts"], pk["tgt_keypts"], torch.eye(4).expand(3, 4, 4).cuda(), off, d_offsets=pk["d_offsets"],
+                           info=True)                    # pdsc_icp_packed, sets of three sizes
 torch.cuda.synchronize()
 print("sanitize_smoke ok", float(st.sum()), int(it.sum()), r["corr"].shape, tuple(feat.shape))
