@@ -18,11 +18,14 @@
 //     KVimg[b][kt]  kt = 64-key tile    : [Khi 16K][Klo 16K][Vhi 16K][Vlo 16K]   (V in the K format, read as an MN-major B operand)
 //
 // Kernels per layer (persistent: one CTA per SM):
-//   tc_chain<PCQ>   feat  -> PointCN -> feat1 (fp32, HBM; and as a register hi|lo A operand) -> Q image    tc_chain.cuh
+//   tc_chain<PCQ>   (layer 0) feat -> PointCN -> feat1 (fp32, HBM; and as a register hi|lo A operand) -> Q image  tc_chain.cuh
+//   tc_chain<Q>     (layers 1..) feat1 -> Q image
 //   tc_chain<KV>    feat1 -> K image, V image (K format)
 //   tc_attention_persistent   flash-style over (set, 128-query tile) items, S and O in registers, SC-weighted online softmax,
 //                   P as a register A operand of O += P V; msg (fp32, HBM)                                 tc_attention_p.cuh
-//   tc_chain<MSG>   msg -> fc_message chain (hidden activations stay in registers) -> + feat1 -> feat (fp32, HBM)
+//   tc_chain<MSGPC> msg -> fc_message chain (hidden activations stay in registers) -> + feat1 -> feat (registers) -> the
+//                   next layer's PointCN -> its feat1 (fp32, HBM, in place)
+//   tc_chain<MSG>   (last layer) msg -> fc_message chain -> + feat1 -> feat (fp32, HBM: the head's input)
 // Synchronisation rules of these kernels: tc_common.cuh.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -208,12 +211,32 @@ __global__ void tc_unblock_f32_kernel(const float* __restrict__ blocked, float* 
 // =========================================================================================================
 // host orchestration
 // =========================================================================================================
+// a chain kernel, launched with programmatic stream serialisation: its CTAs may be scheduled while the previous kernel in the
+// stream still runs, stage their weights and wait (griddep_wait, tc_chain.cuh) for that kernel's results, so neither the launch
+// nor the weight copy sits between two kernels of the encoder
+template <int MODE, int FMT>
+static void launch_chain(int grid, const ChainArgs& c, cudaStream_t st) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3((unsigned)grid);
+  cfg.blockDim = dim3(kChainThreads);
+  cfg.dynamicSmemBytes = kChainSmem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  cudaLaunchKernelEx(&cfg, tc_chain_kernel<MODE, FMT>, c);   // a failed launch is reported by the cudaGetLastError at the end
+}
+
 template <int FMT>
 static cudaError_t tc_configure_fmt() {
   cudaError_t e;
   if ((e = ensure_dynamic_smem(reinterpret_cast<const void*>(tc_chain_kernel<kPCQ, FMT>), kChainSmem))) return e;
   if ((e = ensure_dynamic_smem(reinterpret_cast<const void*>(tc_chain_kernel<kKV, FMT>), kChainSmem))) return e;
   if ((e = ensure_dynamic_smem(reinterpret_cast<const void*>(tc_chain_kernel<kMSG, FMT>), kChainSmem))) return e;
+  if ((e = ensure_dynamic_smem(reinterpret_cast<const void*>(tc_chain_kernel<kMSGPC, FMT>), kChainSmem))) return e;
+  if ((e = ensure_dynamic_smem(reinterpret_cast<const void*>(tc_chain_kernel<kQ, FMT>), kChainSmem))) return e;
   return ensure_dynamic_smem(reinterpret_cast<const void*>(tc_attention_persistent_kernel<FMT>), kAttnPSmem);
 }
 
@@ -236,16 +259,21 @@ static int tc_encoder_forward_fmt(const TcWeights& w, const TcForwardArgs& a, cu
   tc_clear_pads_kernel<<<a.nsets, 256, 0, st>>>(kvimg, a.sets);
   for (int l = 0; l < a.num_layers; ++l) {
     const uint8_t* base = arena + (size_t)l * kLayerBytes;
+    const bool last = l + 1 == a.num_layers;
     ChainArgs c{};
     c.rows = rows; c.split = a.split;
     c.sets = a.sets; c.tile_set = a.tile_set; c.nsets = a.nsets;
     c.qimg = qimg; c.kvimg = kvimg; c.bias = reinterpret_cast<const float*>(base + kBias);
-    // PointCN + Q
-    c.in = a.feat; c.res = nullptr; c.out_f32 = a.feat1; c.wimg = base + kW1; c.wbytes = 131072;
-    tc_chain_kernel<kPCQ, FMT><<<grid, kChainThreads, kChainSmem, st>>>(c);
+    if (l == 0) {   // PointCN + Q
+      c.in = a.feat; c.out_f32 = a.feat1; c.wimg = base + kW1; c.wbytes = 131072;
+      launch_chain<kPCQ, FMT>(grid, c, st);
+    } else {        // Q (the previous layer's MSGPC ran this layer's PointCN)
+      c.in = a.feat1; c.out_f32 = nullptr; c.wimg = base + kWq; c.wbytes = 65536;
+      launch_chain<kQ, FMT>(grid, c, st);
+    }
     // K + V
     c.in = a.feat1; c.out_f32 = nullptr; c.wimg = base + kWk; c.wbytes = 131072;
-    tc_chain_kernel<kKV, FMT><<<grid, kChainThreads, kChainSmem, st>>>(c);
+    launch_chain<kKV, FMT>(grid, c, st);
     // attention
     const AttnArgs at{a.split, qimg, kvimg, a.sc, a.msg, a.attn_items, part_o, part_ml, a.sets, a.nsets};
     if (a.attn_events) cudaEventRecord(a.attn_events[2 * l], st);
@@ -260,10 +288,20 @@ static int tc_encoder_forward_fmt(const TcWeights& w, const TcForwardArgs& a, cu
                                                                              a.debug_out + 3 * plane, rows, a.sets, a.nsets, a.split);
       cudaMemcpyAsync(a.debug_out + 4 * plane, a.msg, plane * sizeof(float), cudaMemcpyDeviceToDevice, st);
     }
-    // fc_message + residual
-    c.in = a.msg; c.res = a.feat1; c.out_f32 = a.feat; c.wimg = base + kWm0; c.wbytes = 81920;
-    tc_chain_kernel<kMSG, FMT><<<grid, kChainThreads, kChainSmem, st>>>(c);
-    if (a.layer_tap_out && a.layer_tap == l)
+    // fc_message + residual; then, but for the last layer (the head reads its feat), the next layer's PointCN, which
+    // overwrites feat1 in place and leaves feat in HBM only for the layer_features tap
+    const bool tap = a.layer_tap_out && a.layer_tap == l;
+    c.in = a.msg; c.res = a.feat1; c.wimg = base + kWm0; c.wbytes = 81920;
+    if (last) {
+      c.out_f32 = a.feat;
+      launch_chain<kMSG, FMT>(grid, c, st);
+    } else {
+      const uint8_t* next = base + kLayerBytes;
+      c.out_f32 = a.feat1; c.feat_out = tap ? a.feat : nullptr;
+      c.wimg1 = next + kW1; c.bias1 = reinterpret_cast<const float*>(next + kBias);
+      launch_chain<kMSGPC, FMT>(grid, c, st);
+    }
+    if (tap)
       cudaMemcpyAsync(a.layer_tap_out, a.feat, (size_t)rows * kC * sizeof(float), cudaMemcpyDeviceToDevice, st);
   }
   return (int)cudaGetLastError();

@@ -1,9 +1,13 @@
 // tc_chain: fused row-tile GEMM chains of the encoder's 1x1 convolutions on wgmma (included by encoder_tc.cu).
 //
-//   PCQ : feat  --W1,relu--> feat1 (fp32 -> HBM) --Wq--> Q image (HBM)
-//   KV  : feat1 --Wk--> K image (HBM) ;  feat1 --Wv--> V image (HBM, same row-major format as K)
-//   MSG : msg --Wm0,relu--> --Wm1,relu--> --Wm2--> + feat1 --> feat (fp32 -> HBM)
+//   PCQ   : feat  --W1,relu--> feat1 (fp32 -> HBM) --Wq--> Q image (HBM)
+//   Q     : feat1 --Wq--> Q image (HBM)
+//   KV    : feat1 --Wk--> K image (HBM) ;  feat1 --Wv--> V image (HBM, same row-major format as K)
+//   MSG   : msg --Wm0,relu--> --Wm1,relu--> --Wm2--> + feat1 --> feat (fp32 -> HBM)
+//   MSGPC : MSG, then feat --W1 of the next layer,relu--> the next layer's feat1 (fp32 -> HBM, in place over feat1)
 // (reference models/PointDSC.py:56-61 PointCN, :21-23/:36-38 projections, :12-20/:43-44 fc_message + residual)
+// A layer is PCQ (layer 0) or Q, then KV, attention, and MSGPC (MSG for the last layer, whose feat the head reads): feat
+// between two layers never goes through HBM.  MSGPC and Q compute exactly what MSG and PCQ did, instruction for instruction.
 //
 // Persistent CTAs (one per SM), weights resident in shared memory, 128-row tiles, two warpgroups of 64 rows each.  A tile's
 // fp32 input (64 KB of contiguous memory in every mode) arrives in shared memory by one bulk async copy; each thread reads its
@@ -13,7 +17,7 @@
 // turns its accumulator fragment into the register A operand of the next.  The Q / K / V images are written after a transpose
 // within each quad of lanes, one whole 16-byte swizzle chunk per lane and store (store_row).  The rows of a ragged last tile
 // beyond `rows` hold stale data; they feed only output rows that are never stored (a 1x1 convolution maps each row on its own).
-// feat1 (fp32, PCQ -> KV and MSG) lives in HBM in a BLOCKED layout keyed by the 128-row chain tile:
+// feat1 (fp32, PCQ / MSGPC -> Q, KV and MSG / MSGPC) lives in HBM in a BLOCKED layout keyed by the 128-row chain tile:
 //     [tile][32-column chunk cc][128 rows][128 B], 16-byte piece q of row r at piece q ^ (r & 7)
 // so that the fragment reads of a staged feat1 tile are at most 2-way bank conflicted (blocked_f32_offset).
 #pragma once
@@ -24,15 +28,21 @@
 namespace pdsc {
 
 constexpr int kChainThreads = 256;
-constexpr int kChIn = 0;                         // staged input tile (64 KB): row-major feat / msg, or blocked feat1
-constexpr int kChW = 65536;                      // weight images (128 KB for PCQ / KV, 80 KB for MSG)
-constexpr int kChRes = kChW + 81920;             // MSG: staged blocked feat1 residual tile (64 KB) behind its weights
-constexpr int kChBias = kChRes + 65536;          // 256 floats: this mode's biases
-constexpr int kChBars = kChBias + 1024;          // mbarriers: weights, input, residual
-constexpr int kChainSmem = kChBars + 64;         // 214,080 B
+constexpr int kChIn = 0;                         // staged input tile (64 KB): row-major feat / msg, or blocked feat1;
+                                                 // MSGPC: also its blocked feat1 residual tile, once the msg fragments are read
+constexpr int kChW = 65536;                      // weight images (128 KB for PCQ / KV, 80 KB for MSG / MSGPC, 64 KB for Q)
+constexpr int kChRes = kChW + 81920;             // 64 KB behind the fc_message weights.  MSG: staged blocked feat1 residual
+                                                 // tile;  MSGPC: the next layer's W1 images
+constexpr int kChBias = kChRes + 65536;          // 384 floats: this mode's biases
+constexpr int kChBars = kChBias + 1536;          // mbarriers: weights, input, residual
+constexpr int kChainSmem = kChBars + 64;         // 214,592 B
+
+// modes that write the Q image (the others that write an operand image write K / V)
+template <int MODE>
+constexpr bool kWritesQ = MODE == kPCQ || MODE == kQ;
 
 // A chain tile may span several sets (rows are not padded per set).  Its rows find their sets in a window of the table: lane
-// l holds the first row and the first operand image tile (PCQ: 128-query tile of the Q image, KV: 64-key tile of the K / V
+// l holds the first row and the first operand image tile (PCQ, Q: 128-query tile of the Q image, KV: 64-key tile of the K / V
 // image) of set lo + l, lo the set of the tile's first row (ChainArgs::tile_set).
 struct SetWindow {
   int lo, row0, t0;
@@ -40,7 +50,7 @@ struct SetWindow {
 template <int MODE>
 __device__ __forceinline__ SetWindow load_window(const ChainArgs& a, int lo) {
   const int lane = threadIdx.x & 31, w = min(lo + lane, a.nsets - 1);
-  return {lo, lo + lane < a.nsets ? __ldg(&a.sets[w].row0) : INT_MAX, MODE == kPCQ ? __ldg(&a.sets[w].qt0) : __ldg(&a.sets[w].kt0)};
+  return {lo, lo + lane < a.nsets ? __ldg(&a.sets[w].row0) : INT_MAX, kWritesQ<MODE> ? __ldg(&a.sets[w].qt0) : __ldg(&a.sets[w].kt0)};
 }
 
 // operand image tile of row g of the window's chain tile and the row's place within that tile.  All lanes of the warp take part.
@@ -55,11 +65,11 @@ __device__ __forceinline__ void locate_row(const ChainArgs& a, const SetWindow& 
     int b = win.lo + 31;
     while (b + 1 < a.nsets && __ldg(&a.sets[b + 1].row0) <= g) ++b;
     row0 = __ldg(&a.sets[b].row0);
-    t0 = MODE == kPCQ ? __ldg(&a.sets[b].qt0) : __ldg(&a.sets[b].kt0);
+    t0 = kWritesQ<MODE> ? __ldg(&a.sets[b].qt0) : __ldg(&a.sets[b].kt0);
   }
   const int nn = (int)(g - row0);
-  tile = t0 + (MODE == kPCQ ? (nn >> 7) : (nn >> 6));
-  r = MODE == kPCQ ? (nn & 127) : (nn & 63);
+  tile = t0 + (kWritesQ<MODE> ? (nn >> 7) : (nn >> 6));
+  r = kWritesQ<MODE> ? (nn & 127) : (nn & 63);
 }
 
 // byte offset of the 16-byte piece `piece` (0..31) of global row `g` in the blocked fp32 layout described in the header
@@ -107,23 +117,29 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
   const int tid = threadIdx.x;
   const int wg = tid >> 7, wt = tid & 127;
   const uint32_t w_base = s0 + kChW;
-  // this mode's biases, packed: PCQ b1|bq, KV bk|bv, MSG bm0|bm1|bm2
-  constexpr int kBiasSrc = (MODE == kPCQ) ? kB1 : (MODE == kKV) ? kBk : kBm0;
+  constexpr bool kFcMsg = MODE == kMSG || MODE == kMSGPC;   // the fc_message modes: row-major msg in, no operand image out
+  constexpr bool kBlockedIn = MODE == kKV || MODE == kQ;    // the modes whose input is blocked feat1
+  // this mode's biases, packed: PCQ b1|bq, Q bq, KV bk|bv, MSG bm0|bm1|bm2, MSGPC bm0|bm1|bm2|b1 (b1 of the next layer)
+  constexpr int kBiasSrc = (MODE == kPCQ) ? kB1 : (MODE == kQ) ? kBq : (MODE == kKV) ? kBk : kBm0;
   const long long rows = a.rows;
   const long long num_tiles = (rows + 127) / 128;
 
   // a tile's input is the 64 KB at tile * 65536; feat and msg hold exactly `rows` rows, blocked feat1 is padded to whole tiles
   auto issue_input = [&](long long t) {
     const long long left = rows - t * 128;
-    const uint32_t bytes = (MODE == kKV || left >= 128) ? 65536u : (uint32_t)left * 512u;
+    const uint32_t bytes = (kBlockedIn || left >= 128) ? 65536u : (uint32_t)left * 512u;
     mbar_expect_tx(bar_in, bytes);
     bulk_g2s(s0 + kChIn, reinterpret_cast<const uint8_t*>(a.in) + (size_t)t * 65536, bytes, bar_in);
   };
   // byte offset of (row r, column c) in a staged input tile
   auto in_offset = [](int r, int c) -> uint32_t {
-    return MODE == kKV ? (uint32_t)blocked_f32_offset(r, (uint32_t)c >> 2) + (c & 3) * 4 : (uint32_t)(r * kC + c) * 4u;
+    return kBlockedIn ? (uint32_t)blocked_f32_offset(r, (uint32_t)c >> 2) + (c & 3) * 4 : (uint32_t)(r * kC + c) * 4u;
   };
 
+  // The chain kernels are launched with programmatic stream serialisation: the next grid may be scheduled at once and its
+  // CTAs take the SMs this grid's CTAs leave, and this grid's CTAs may start while the previous kernel is still running.  Up
+  // to griddep_wait a CTA touches only what no kernel of the call writes (the weight arena); everything else comes after.
+  griddep_launch_dependents();
   if (tid == 0) {
     if (s0 & 1023u) __trap();   // the swizzled weight images need 1024-byte aligned shared memory
     mbar_init(bar_w, 1);
@@ -132,22 +148,26 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
     fence_barrier_init();
   }
   bias[tid] = a.bias[kBiasSrc + tid];
+  if (MODE == kMSGPC && tid < 128) bias[256 + tid] = a.bias1[kB1 + tid];
   __syncthreads();
   if (tid == 0) {
-    mbar_expect_tx(bar_w, (uint32_t)a.wbytes);
+    mbar_expect_tx(bar_w, (uint32_t)a.wbytes + (MODE == kMSGPC ? 65536u : 0u));
     for (int off = 0; off < a.wbytes; off += 32768)
       bulk_g2s(w_base + off, a.wimg + off, (uint32_t)min(32768, a.wbytes - off), bar_w);
-    if (blockIdx.x < num_tiles) issue_input(blockIdx.x);
+    if (MODE == kMSGPC)   // the arena keeps W1 apart from the fc_message weights: a second copy, behind them
+      for (int off = 0; off < 65536; off += 32768) bulk_g2s(s0 + kChRes + off, a.wimg1 + off, 32768u, bar_w);
   }
+  griddep_wait();   // every thread: the previous kernels' results are complete and visible from here on
+  if (tid == 0 && blockIdx.x < num_tiles) issue_input(blockIdx.x);
   mbar_wait(bar_w, 0);   // also keeps a CTA without tiles alive until its weight copy has landed
   const int fr = 64 * wg + frag_row(wt), fc = frag_col(wt);   // fragment rows fr, fr + 8 of the tile; columns 8 j + fc, + 1
   const int quad = fc >> 1;                                   // this lane's place among the 4 lanes that share its rows
 
-  // PCQ, KV: the set window of the CTA's next tile is loaded one tile ahead, from its first set loaded two tiles ahead, so that
-  // no lookup waits for memory
+  // PCQ, Q, KV: the set window of the CTA's next tile is loaded one tile ahead, from its first set loaded two tiles ahead, so
+  // that no lookup waits for memory
   SetWindow win_next{};
   int lo_after = 0;
-  if (MODE != kMSG && blockIdx.x < num_tiles) {
+  if (!kFcMsg && blockIdx.x < num_tiles) {
     win_next = load_window<MODE>(a, __ldg(a.tile_set + blockIdx.x));
     if (blockIdx.x + gridDim.x < num_tiles) lo_after = __ldg(a.tile_set + blockIdx.x + gridDim.x);
   }
@@ -157,7 +177,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
     // the two rows of this thread: global index, operand image tile and row within it
     const long long g[2] = {row0 + fr, row0 + fr + 8};
     int tl[2], tr[2];
-    if (MODE != kMSG) {
+    if (!kFcMsg) {
       const SetWindow win = win_next;
       if (tile + gridDim.x < num_tiles) {
         win_next = load_window<MODE>(a, lo_after);
@@ -183,36 +203,43 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
     }
     __syncthreads();   // every thread holds its fragments and is past the previous tile's residual reads: refill both buffers
     if (tid == 0) {
-      if (tile + gridDim.x < num_tiles) issue_input(tile + gridDim.x);
-      if (MODE == kMSG) {
+      // MSGPC has no room for a residual buffer behind the next layer's W1: its residual tile goes into the input stage, and
+      // the next tile's input follows once the residual has been read
+      if (MODE != kMSGPC && tile + gridDim.x < num_tiles) issue_input(tile + gridDim.x);
+      if (kFcMsg) {
         mbar_expect_tx(bar_res, 65536u);
-        bulk_g2s(s0 + kChRes, reinterpret_cast<const uint8_t*>(a.res) + (size_t)tile * 65536, 65536u, bar_res);
+        bulk_g2s(s0 + (MODE == kMSG ? kChRes : kChIn), reinterpret_cast<const uint8_t*>(a.res) + (size_t)tile * 65536, 65536u, bar_res);
       }
     }
 
-    if (MODE == kPCQ) {
-      // ---- PointCN: feat1 = relu(A W1^T + b1) -> HBM (fp32, blocked) and registers (A operand of the Q GEMM) ----
-      float x[64];
-      wgmma_fence();
-      gemm_rs<FMT, 8, 128, 0>(x, ahi, alo, w_base, w_base + 32768, 16384, a.split, 0);
-      wgmma_commit();
-      wgmma_wait<0>();
-      fence_regs(x);
+    if (kWritesQ<MODE>) {
+      if (MODE == kPCQ) {
+        // ---- PointCN: feat1 = relu(A W1^T + b1) -> HBM (fp32, blocked) and registers (A operand of the Q GEMM) ----
+        float x[64];
+        wgmma_fence();
+        gemm_rs<FMT, 8, 128, 0>(x, ahi, alo, w_base, w_base + 32768, 16384, a.split, 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(x);
 #pragma unroll
-      for (int j = 0; j < 16; ++j)
+        for (int j = 0; j < 16; ++j)
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int c = 8 * j + fc, e = 4 * j + 2 * h;
-          x[e] = fmaxf(x[e] + bias[c], 0.f);
-          x[e + 1] = fmaxf(x[e + 1] + bias[c + 1], 0.f);
-          if (g[h] < rows)
-            *reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(a.out_f32) + blocked_f32_offset(g[h], (uint32_t)c >> 2) + (c & 3) * 4) =
-                make_float2(x[e], x[e + 1]);
-        }
-      frag_split<FMT, 8>(x, ahi, alo);
+          for (int h = 0; h < 2; ++h) {
+            const int c = 8 * j + fc, e = 4 * j + 2 * h;
+            x[e] = fmaxf(x[e] + bias[c], 0.f);
+            x[e + 1] = fmaxf(x[e + 1] + bias[c + 1], 0.f);
+            if (g[h] < rows)
+              *reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(a.out_f32) + blocked_f32_offset(g[h], (uint32_t)c >> 2) + (c & 3) * 4) =
+                  make_float2(x[e], x[e + 1]);
+          }
+        frag_split<FMT, 8>(x, ahi, alo);
+      }
+      // PCQ: Wq behind W1, bq behind b1;  Q: Wq and bq alone
+      const uint32_t wq = w_base + (MODE == kPCQ ? 65536u : 0u);
+      const float* bq = bias + (MODE == kPCQ ? 128 : 0);
       float q[64];
       wgmma_fence();
-      gemm_rs<FMT, 8, 128, 0>(q, ahi, alo, w_base + 65536, w_base + 65536 + 32768, 16384, a.split, 0);
+      gemm_rs<FMT, 8, 128, 0>(q, ahi, alo, wq, wq + 32768, 16384, a.split, 0);
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(q);
@@ -225,7 +252,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const int c = 8 * j + fc, e = 4 * j + 2 * h;
-          split_pair<FMT>(q[e] + bias[128 + c], q[e + 1] + bias[128 + c + 1], hi[j], lo[j]);
+          split_pair<FMT>(q[e] + bq[c], q[e + 1] + bq[c + 1], hi[j], lo[j]);
         }
         store_row(img, 16384u, r, hi, quad, g[h] < rows);
         if (a.split) store_row(img + 32768, 16384u, r, lo, quad, g[h] < rows);
@@ -287,18 +314,56 @@ __global__ void __launch_bounds__(kChainThreads, 1) tc_chain_kernel(ChainArgs a)
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(o);
-      // feat = feat1 + (D2 + bm2), feat1 from the staged residual tile
-      mbar_wait(bar_res, phase);
+      if (MODE == kMSG) {
+        // feat = feat1 + (D2 + bm2), feat1 from the staged residual tile
+        mbar_wait(bar_res, phase);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (g[h] >= rows) continue;
+        for (int h = 0; h < 2; ++h) {
+          if (g[h] >= rows) continue;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int c = 8 * j + fc, e = 4 * j + 2 * h;
-          const float2 rv = *reinterpret_cast<const float2*>(resbuf + blocked_f32_offset(fr + 8 * h, (uint32_t)c >> 2) + (c & 3) * 4);
-          *reinterpret_cast<float2*>(a.out_f32 + g[h] * kC + c) =
-              make_float2(rv.x + (o[e] + bias[128 + c]), rv.y + (o[e + 1] + bias[128 + c + 1]));
+          for (int j = 0; j < 16; ++j) {
+            const int c = 8 * j + fc, e = 4 * j + 2 * h;
+            const float2 rv = *reinterpret_cast<const float2*>(resbuf + blocked_f32_offset(fr + 8 * h, (uint32_t)c >> 2) + (c & 3) * 4);
+            *reinterpret_cast<float2*>(a.out_f32 + g[h] * kC + c) =
+                make_float2(rv.x + (o[e] + bias[128 + c]), rv.y + (o[e + 1] + bias[128 + c + 1]));
+          }
         }
+      } else {
+        // feat = feat1 + (D2 + bm2), as MSG computes it, feat1 from the residual tile staged in the input buffer.  feat is then
+        // in the fragment layout the PCQ mode reads its staged input in (row fr + 8 h, column 8 j + fc at x[4 j + 2 h]), so
+        // its hi / lo split is the A operand PCQ would build.
+        mbar_wait(bar_res, phase);
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int c = 8 * j + fc, e = 4 * j + 2 * h;
+            const float2 rv = *reinterpret_cast<const float2*>(stage + blocked_f32_offset(fr + 8 * h, (uint32_t)c >> 2) + (c & 3) * 4);
+            o[e] = rv.x + (o[e] + bias[128 + c]);
+            o[e + 1] = rv.y + (o[e + 1] + bias[128 + c + 1]);
+            if (a.feat_out && g[h] < rows) *reinterpret_cast<float2*>(a.feat_out + g[h] * kC + c) = make_float2(o[e], o[e + 1]);
+          }
+        __syncthreads();   // every thread is past its residual reads: the stage takes the next tile's input
+        if (tid == 0 && tile + gridDim.x < num_tiles) issue_input(tile + gridDim.x);
+        frag_split<FMT, 8>(o, ahi, alo);
+        // ---- the next layer's PointCN: feat1 = relu(feat W1^T + b1) -> HBM (fp32, blocked), in place over this layer's feat1.
+        // The tile's residual copy has landed before any of these stores (mbar_wait above), no other CTA reads or writes the
+        // tile's rows, and no later kernel reads this layer's feat1.
+        float x[64];
+        wgmma_fence();
+        gemm_rs<FMT, 8, 128, 0>(x, ahi, alo, s0 + kChRes, s0 + kChRes + 32768, 16384, a.split, 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(x);
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int c = 8 * j + fc, e = 4 * j + 2 * h;
+            if (g[h] < rows)
+              *reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(a.out_f32) + blocked_f32_offset(g[h], (uint32_t)c >> 2) + (c & 3) * 4) =
+                  make_float2(fmaxf(x[e] + bias[256 + c], 0.f), fmaxf(x[e + 1] + bias[256 + c + 1], 0.f));
+          }
       }
     }
   }

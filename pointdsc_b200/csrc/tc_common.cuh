@@ -15,7 +15,7 @@ constexpr int kB1 = 0, kBq = 128, kBk = 256, kBv = 384, kBm0 = 512, kBm1 = 576, 
 
 constexpr float kQScale = 1.4426950408889634f / 11.313708498984761f;  // log2(e) / sqrt(128)
 
-enum ChainMode { kPCQ = 0, kKV = 1, kMSG = 2 };
+enum ChainMode { kPCQ = 0, kKV = 1, kMSG = 2, kMSGPC = 3, kQ = 4 };
 
 struct ChainArgs {
   long long rows;        // rows of the call (all sets)
@@ -24,13 +24,16 @@ struct ChainArgs {
   const int* tile_set;   // [rows / 128]: the set of the first row of every 128-row chain tile
   int nsets;
   const float* in;       // [rows][128] fp32 A operand
-  const float* res;      // MSG: feat1 (residual)
-  float* out_f32;        // PCQ: feat1, MSG: feat
+  const float* res;      // MSG, MSGPC: feat1 (residual)
+  float* out_f32;        // PCQ: feat1, MSG: feat, MSGPC: the next layer's feat1 (in place over res)
+  float* feat_out;       // MSGPC: where feat goes too (the layer_features tap), or nullptr
   uint8_t* qimg;
   uint8_t* kvimg;
   const uint8_t* wimg;   // this kernel's weight images (contiguous)
   const float* bias;     // the layer's bias block
   int wbytes;            // bytes of weight images to stage
+  const uint8_t* wimg1;  // MSGPC: the next layer's W1 images (64 KB)
+  const float* bias1;    // MSGPC: the next layer's bias block (b1)
 };
 
 // Synchronisation rules of the tensor-core kernels.

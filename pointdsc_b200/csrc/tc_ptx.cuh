@@ -97,6 +97,13 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 // ---- proxy fence: generic-proxy shared-memory writes become visible to the async proxy (wgmma operand reads) ---------
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// ---- programmatic dependent launch ------------------------------------------------------------------------
+// launch_dependents: this CTA no longer holds back the launch of the next grid in the stream (if that grid was launched with
+// programmatic stream serialisation).  wait: the executing thread waits until every grid it depends on has completed and
+// its memory operations are visible; without a programmatic dependency it returns at once.
+__device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
 // ---- 16-bit hi/lo operand split ---------------------------------------------------------------------------
 // x ~= hi + lo with hi = round16(x), lo = round16(x - hi); three products hi*hi + hi*lo + lo*hi.
 //   FMT 1 (bf16, 8-bit significand): 16 significant bits, per-product error ~2^-18

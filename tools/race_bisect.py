@@ -2,11 +2,12 @@
 """Developer tool: localise the run-to-run differences of the tensor-core encoder (DESIGN.md, "Run-to-run reproducibility").
 
 Every repetition runs the same B x N batch with the per-layer debug taps of ONE layer L (cycled over the layers):
-    layer_debug[0..4] = feat1 (PointCN output of chain<PCQ>), Q, K, V (decoded operand images), msg (attention output)
-    layer_features    = the layer's output (chain<MSG>)
+    layer_debug[0..4] = feat1 (PointCN output: chain<PCQ> at layer 0, the previous layer's chain<MSGPC> after it), Q, K, V
+                        (decoded operand images), msg (attention output)
+    layer_features    = the layer's output (chain<MSGPC>, chain<MSG> at the last layer)
 and compares them with the first run that tapped the same layer.  For a repetition that differs, the FIRST differing
 tensor in data-flow order names the kernel (feat1 differs: the layer's input already differed or PointCN; only Q differs:
-the Q GEMM of chain<PCQ>; K / V: chain<KV>; msg: attention; layer_features: chain<MSG>), and the row range tells which
+chain<Q>, or the Q GEMM of chain<PCQ>; K / V: chain<KV>; msg: attention; layer_features: chain<MSGPC / MSG>), and the row range tells which
 128-row tile (flat row tiles for the chain kernels, per-set query tiles for attention) and which CTA / iteration made it."""
 import os, sys
 import numpy as np, torch

@@ -28,6 +28,9 @@ for k, n, b, inv in ((40, 300, 3, False), (80, 257, 2, False), (40, 1000, 2, Tru
     mixed = [bench.make_inputs(nn, 1, "3dmatch", 0) for nn in (n, 41, 7, 130)]   # pdsc_forward_packed, sets of four sizes
     many = m.forward_many([{**{x: q[x].cuda() for x in ("corr_pos", "src_keypts", "tgt_keypts")}, "testing": True} for q in mixed])
     assert [tuple(o["final_labels"].shape) for o in many] == [(1, n), (1, 41), (1, 7), (1, 130)]
+for prec in ("bf16x3", "bf16"):   # the bf16 instantiations of every chain mode (PCQ, Q, KV, MSGPC, MSG), split on and off
+    m = PointDSC(num_layers=12, k=40, precision=prec, **bench.CTOR["3dmatch"]); m.load_state_dict(bench.load_snapshot("3dmatch"), strict=False); m = m.cuda().eval()
+    m.run(*d, taps=["layer_features", "layer_debug"], layer_tap=5)   # layer 5's MSGPC also writes feat for the tap
 g = torch.Generator().manual_seed(0)
 for dt in (torch.float32, torch.float64):
     sd = torch.nn.functional.normalize(torch.randn(301, 33, generator=g, dtype=dt), dim=1).cuda()
