@@ -1,7 +1,8 @@
 """ctypes binding of the C ABI in include/pointdsc_b200.h.
 
 This is the whole "FFI" a maintainer of the reference would add (the reference is pure Python and
-has none of its own): load the shared library, mirror the two structs, declare the entry points.
+has none of its own): load the shared library, mirror the two structs, declare the entry points,
+and pass the arguments every wrapper passes alike (engine and stream, aligned scratch, offsets).
 There is deliberately NO fallback: if the library is missing or no H100 is present the import /
 engine creation raises.
 """
@@ -9,6 +10,9 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from typing import Optional, Sequence
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("POINTDSC_B200_LIB") or os.path.join(_HERE, "libpointdsc_b200.so")   # env: developer A/B builds
@@ -151,3 +155,34 @@ def utility_engine(device_index: int):
 def check(rc: int):
     if rc != 0:
         raise PdscError(f"pointdsc_b200 error {rc}: {load().pdsc_last_error().decode()}")
+
+
+def device_context(device: torch.device):
+    """(library, utility engine, current stream handle) for a call of the stateless entry points on `device`."""
+    index = device.index if device.index is not None else torch.cuda.current_device()
+    return load(), utility_engine(index), C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
+def scratch(nbytes: int, device: torch.device, align: int = 8) -> torch.Tensor:
+    """A uint8 device buffer of `nbytes` bytes that starts on an `align`-byte boundary: its data_ptr() and numel() are the
+    scratch pointer and size an entry point takes.  The allocation is `align` bytes larger, so any start can be aligned."""
+    buf = torch.empty(int(nbytes) + align, dtype=torch.uint8, device=device)
+    skip = (buf.data_ptr() + align - 1) // align * align - buf.data_ptr()
+    return buf[skip:skip + int(nbytes)]
+
+
+def host_to_device(values, dtype, device) -> torch.Tensor:
+    """A small host list as a device tensor without waiting for the stream: staged in page-locked memory, copied
+    asynchronously (a copy from pageable memory would synchronise the stream first)."""
+    return torch.tensor(values, dtype=dtype).pin_memory().to(device, non_blocking=True)
+
+
+def offsets(values: Sequence[int], d_offsets: Optional[torch.Tensor], device: torch.device):
+    """The B + 1 offsets of a packed call as the packed entry points take them: (host int32 array, device int32 tensor).
+    `d_offsets` is the caller's device copy of the same values; when None, `values` is uploaded."""
+    h = (C.c_int32 * len(values))(*values)
+    if d_offsets is None:
+        return h, host_to_device(values, torch.int32, device)
+    if d_offsets.dtype != torch.int32 or d_offsets.device != device or d_offsets.numel() != len(values):
+        raise ValueError("d_offsets must be a device int32 tensor of B + 1 entries")
+    return h, d_offsets.contiguous()

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -23,7 +24,7 @@ namespace {
 
 thread_local std::string g_last_error;
 
-int fail(int code, const char* fmt, ...) {
+pdsc_status fail(pdsc_status code, const char* fmt, ...) {
   char buf[512];
   va_list ap;
   va_start(ap, fmt);
@@ -263,6 +264,32 @@ bool fold_conv(const pdsc_engine* e, const std::string& conv, const std::string&
   }
   while (arena->size() % 4) arena->push_back(0.f);
   return true;
+}
+
+// Host offsets [n + 1] of a call of n sets packed back to back: n >= 1, offsets[0] = 0, and every set between min_rows and
+// max_rows rows.  `what` prefixes "offsets" and "rows" in the message ("source " / "target " for a group of pairs, else "").
+pdsc_status check_offsets(const char* who, const char* what, int32_t n, const int32_t* h_offsets, int min_rows,
+                          int max_rows = INT_MAX) {
+  if (n < 1) return fail(PDSC_ERR_SHAPE, "%s: need at least one set (got %d)", who, n);
+  if (!h_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null host offsets", who);
+  if (h_offsets[0] != 0) return fail(PDSC_ERR_SHAPE, "%s: %soffsets[0] must be 0 (got %d)", who, what, h_offsets[0]);
+  for (int b = 0; b < n; ++b) {
+    const long long rows = (long long)h_offsets[b + 1] - h_offsets[b];
+    if (rows < min_rows)
+      return fail(PDSC_ERR_SHAPE, "%s: set %d has %lld %srows: offsets must increase by at least %d per set", who, b, rows, what,
+                  min_rows);
+    if (rows > max_rows)
+      return fail(PDSC_ERR_SHAPE, "%s: set %d has %lld %srows, above the supported maximum %d", who, b, rows, what, max_rows);
+  }
+  return PDSC_OK;
+}
+
+// A caller's workspace or scratch buffer: at least `need` bytes at an `align`-byte boundary.
+pdsc_status check_scratch(const char* who, const char* noun, const void* ptr, size_t bytes, size_t need, size_t align) {
+  if (!ptr || bytes < need || reinterpret_cast<uintptr_t>(ptr) % align)
+    return fail(PDSC_ERR_WORKSPACE, "%s: %s too small or not %zu-byte aligned (%zu bytes given, %zu needed)", who, noun, align,
+                bytes, need);
+  return PDSC_OK;
 }
 
 void copy_tap(void* dst, const void* src, size_t bytes, cudaStream_t st) {
@@ -560,10 +587,8 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
   if (io && io->in_confidence && !inject_feat) return fail(PDSC_ERR_INVALID_ARGUMENT, "in_confidence requires in_features");
   DeviceGuard g(e->cfg.device);   // tc_packed_split reads the SM count of the engine's device
   const CallShape sh = call_shape(e, B, N, h_offsets);
-  const size_t need = carve(e, nullptr, sh).bytes;
-  if (!d_workspace || workspace_bytes < need)
-    return fail(PDSC_ERR_WORKSPACE, "workspace too small: %zu bytes given, %zu needed", workspace_bytes, need);
-  if (reinterpret_cast<uintptr_t>(d_workspace) % 256) return fail(PDSC_ERR_WORKSPACE, "workspace must be 256-byte aligned");
+  if (int rc = check_scratch("pdsc_forward", "workspace", d_workspace, workspace_bytes, carve(e, nullptr, sh).bytes, 256))
+    return rc;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   const Workspace w = carve(e, d_workspace, sh);
   N = sh.N;                        // a packed call: the largest set, which sizes the launches
@@ -728,22 +753,8 @@ int pdsc_forward(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr_pos, 
                       workspace_bytes, cuda_stream);
 }
 
-static int check_offsets(const pdsc_engine* e, int32_t B, const int32_t* h_offsets) {
-  if (B < 1) return fail(PDSC_ERR_SHAPE, "need B >= 1 sets (got B=%d)", B);
-  if (!h_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "h_offsets is null");
-  if (h_offsets[0] != 0) return fail(PDSC_ERR_SHAPE, "offsets[0] must be 0 (got %d)", h_offsets[0]);
-  for (int b = 0; b < B; ++b) {
-    const long long n = (long long)h_offsets[b + 1] - h_offsets[b];
-    if (n < 2) return fail(PDSC_ERR_SHAPE, "set %d has N=%lld rows: offsets must increase by at least 2 per set", b, n);
-    if (n > pdsc::pick_seeds_max_n())
-      return fail(PDSC_ERR_SHAPE, "set %d has N=%lld rows, above the supported maximum %d", b, n, pdsc::pick_seeds_max_n());
-  }
-  (void)e;
-  return PDSC_OK;
-}
-
 size_t pdsc_workspace_bytes_packed(const pdsc_engine* e, int32_t B, const int32_t* h_offsets) {
-  if (!e || check_offsets(e, B, h_offsets) != PDSC_OK) return 0;
+  if (!e || check_offsets("pdsc_workspace_bytes_packed", "", B, h_offsets, 2, pdsc::pick_seeds_max_n())) return 0;
   DeviceGuard g(e->cfg.device);
   return carve(e, nullptr, call_shape(e, B, 0, h_offsets)).bytes;
 }
@@ -752,8 +763,7 @@ int pdsc_forward_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, con
                         const float* d_src, const float* d_tgt, float* d_final_trans, float* d_final_labels, void* d_workspace,
                         size_t workspace_bytes, void* cuda_stream) {
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  const int rc = check_offsets(e, B, h_offsets);
-  if (rc) return rc;
+  if (int rc = check_offsets("pdsc_forward_packed", "", B, h_offsets, 2, pdsc::pick_seeds_max_n())) return rc;
   if (!d_offsets || !d_corr_pos) return fail(PDSC_ERR_INVALID_ARGUMENT, "null tensor pointer");
   return forward_impl(e, 0, B, 0, h_offsets, d_offsets, d_corr_pos, d_src, d_tgt, d_final_trans, d_final_labels, nullptr, nullptr,
                       d_workspace, workspace_bytes, cuda_stream);
@@ -836,27 +846,12 @@ int pdsc_eval_stats(pdsc_engine* e, int32_t B, int32_t N, const float* d_pred_tr
                          d_stats, cuda_stream);
 }
 
-// offsets [n + 1] of a packed call of the stateless entry points: offsets[0] = 0, every set at least `min_rows` rows
-static int check_pair_offsets(const char* who, const char* what, int32_t n, const int32_t* h_offsets, int min_rows) {
-  if (n < 1) return fail(PDSC_ERR_SHAPE, "%s: need at least one set (got %d)", who, n);
-  if (!h_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null host offsets", who);
-  if (h_offsets[0] != 0) return fail(PDSC_ERR_SHAPE, "%s: %soffsets[0] must be 0 (got %d)", who, what, h_offsets[0]);
-  for (int b = 0; b < n; ++b) {
-    const long long rows = (long long)h_offsets[b + 1] - h_offsets[b];
-    if (rows < min_rows)
-      return fail(PDSC_ERR_SHAPE, "%s: set %d has %lld %srows: offsets must increase by at least %d per set", who, b, rows, what,
-                  min_rows);
-  }
-  return PDSC_OK;
-}
-
 int pdsc_eval_stats_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
                            const float* d_pred_trans, const float* d_gt_trans, const float* d_src, const float* d_tgt,
                            const float* d_pred_labels, const float* d_gt_labels, float re_thre, float te_thre, float* d_stats,
                            void* cuda_stream) {
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  const int rc = check_pair_offsets("pdsc_eval_stats_packed", "", B, h_offsets, 1);
-  if (rc) return rc;
+  if (int rc = check_offsets("pdsc_eval_stats_packed", "", B, h_offsets, 1)) return rc;
   if (!d_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_eval_stats_packed: null device offsets");
   return eval_stats_impl(e, B, d_offsets, 0, d_pred_trans, d_gt_trans, d_src, d_tgt, d_pred_labels, d_gt_labels, re_thre, te_thre,
                          d_stats, cuda_stream);
@@ -874,22 +869,13 @@ int pdsc_leading_eigenvector(pdsc_engine* e, int32_t B, int32_t N, const float* 
   if (num_iterations < 1 || num_iterations > 1000) return fail(PDSC_ERR_INVALID_ARGUMENT, "num_iterations %d out of range", num_iterations);
   if (N > 24576) return fail(PDSC_ERR_UNSUPPORTED, "N=%d exceeds the supported maximum 24576", N);
   if (!d_M || !d_eigenvector || !d_iterations_run) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_leading_eigenvector: null tensor pointer");
-  if (!d_scratch || scratch_bytes < pdsc::eig_scratch_bytes(B, N) || reinterpret_cast<uintptr_t>(d_scratch) % 16)
-    return fail(PDSC_ERR_WORKSPACE, "pdsc_leading_eigenvector: scratch too small or not 16-byte aligned (%zu bytes given, %zu needed)",
-                scratch_bytes, pdsc::eig_scratch_bytes(B, N));
+  if (int rc = check_scratch("pdsc_leading_eigenvector", "scratch", d_scratch, scratch_bytes, pdsc::eig_scratch_bytes(B, N), 16))
+    return rc;
   DeviceGuard g(e->cfg.device);
   const int rc = pdsc::launch_leading_eigenvector(d_M, d_eigenvector, d_iterations_run, B, N, num_iterations, early_exit, d_scratch,
                                                   static_cast<cudaStream_t>(cuda_stream));
   if (rc) return fail(PDSC_ERR_CUDA, "power iteration launch failed: %s", cudaGetErrorString((cudaError_t)rc));
   return PDSC_OK;
-}
-
-// offsets of P clouds that the descriptor entry points accept: P >= 1, offsets[0] = 0, every cloud at least one row
-static bool cloud_offsets_ok(int32_t P, const int32_t* h_offsets) {
-  if (P < 1 || !h_offsets || h_offsets[0] != 0) return false;
-  for (int p = 0; p < P; ++p)
-    if (h_offsets[p + 1] <= h_offsets[p]) return false;
-  return true;
 }
 
 size_t pdsc_voxel_down_sample_scratch_bytes(int64_t n) {
@@ -899,7 +885,8 @@ size_t pdsc_voxel_down_sample_scratch_bytes(int64_t n) {
 }
 
 size_t pdsc_voxel_down_sample_packed_scratch_bytes(int32_t P, const int32_t* h_offsets) {
-  return cloud_offsets_ok(P, h_offsets) && h_offsets[P] <= (1 << 30) ? pdsc::voxel_scratch_bytes(P, h_offsets) : 0;
+  if (check_offsets("pdsc_voxel_down_sample_packed_scratch_bytes", "", P, h_offsets, 1) || h_offsets[P] > (1 << 30)) return 0;
+  return pdsc::voxel_scratch_bytes(P, h_offsets);
 }
 
 static int voxel_impl(const char* who, pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets,
@@ -908,10 +895,7 @@ static int voxel_impl(const char* who, pdsc_engine* e, int32_t P, const int32_t*
   if (h_offsets[P] > (1 << 30)) return fail(PDSC_ERR_SHAPE, "%s: need at most 2^30 points (got %d)", who, h_offsets[P]);
   if (!(voxel_size > 0.0)) return fail(PDSC_ERR_INVALID_ARGUMENT, "voxel_size must be positive (got %g)", voxel_size);
   if (!d_points || !d_out_points || !d_out_ends || !d_status) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", who);
-  const size_t need = pdsc::voxel_scratch_bytes(P, h_offsets);
-  if (!d_scratch || scratch_bytes < need || reinterpret_cast<uintptr_t>(d_scratch) % 8)
-    return fail(PDSC_ERR_WORKSPACE, "%s: scratch too small or not 8-byte aligned (%zu bytes given, %zu needed)", who, scratch_bytes,
-                need);
+  if (int rc = check_scratch(who, "scratch", d_scratch, scratch_bytes, pdsc::voxel_scratch_bytes(P, h_offsets), 8)) return rc;
   DeviceGuard g(e->cfg.device);
   pdsc::launch_voxel_down_sample(P, h_offsets, d_offsets, d_points, voxel_size, d_out_points, d_out_first, d_out_ends, d_status,
                                  d_scratch, static_cast<cudaStream_t>(cuda_stream));
@@ -933,8 +917,7 @@ int pdsc_voxel_down_sample_packed(pdsc_engine* e, int32_t P, const int32_t* h_of
                                   double voxel_size, float* d_out_points, int32_t* d_out_offsets, int32_t* d_status, void* d_scratch,
                                   size_t scratch_bytes, void* cuda_stream) {
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  const int rc = check_pair_offsets("pdsc_voxel_down_sample_packed", "", P, h_offsets, 1);
-  if (rc) return rc;
+  if (int rc = check_offsets("pdsc_voxel_down_sample_packed", "", P, h_offsets, 1)) return rc;
   if (!d_offsets || !d_out_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_voxel_down_sample_packed: null offsets");
   return voxel_impl("pdsc_voxel_down_sample_packed", e, P, h_offsets, d_offsets, d_points, voxel_size, d_out_points, d_out_offsets,
                     d_out_offsets + 1, d_status, d_scratch, scratch_bytes, cuda_stream);
@@ -943,7 +926,8 @@ int pdsc_voxel_down_sample_packed(pdsc_engine* e, int32_t P, const int32_t* h_of
 size_t pdsc_fpfh_scratch_bytes(int32_t m, int32_t max_nn) { return (m > 0 && max_nn > 0) ? pdsc::fpfh_scratch_bytes(m, max_nn) : 0; }
 
 size_t pdsc_fpfh_packed_scratch_bytes(int32_t P, const int32_t* h_offsets, int32_t max_nn) {
-  return cloud_offsets_ok(P, h_offsets) && max_nn > 0 ? pdsc::fpfh_scratch_bytes(h_offsets[P], max_nn) : 0;
+  if (check_offsets("pdsc_fpfh_packed_scratch_bytes", "", P, h_offsets, 1) || max_nn <= 0) return 0;
+  return pdsc::fpfh_scratch_bytes(h_offsets[P], max_nn);
 }
 
 static int check_search_args(const char* who, pdsc_engine* e, int32_t m, double radius, int32_t max_nn, const void* a, const void* b,
@@ -953,10 +937,7 @@ static int check_search_args(const char* who, pdsc_engine* e, int32_t m, double 
   if (!(radius > 0.0)) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: radius must be positive (got %g)", who, radius);
   if (max_nn < 1 || max_nn > 256) return fail(PDSC_ERR_UNSUPPORTED, "%s: max_nn %d outside [1, 256]", who, max_nn);
   if (!a || !b || !c) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", who);
-  if (!d_scratch || scratch_bytes < pdsc::fpfh_scratch_bytes(m, max_nn) || reinterpret_cast<uintptr_t>(d_scratch) % 8)
-    return fail(PDSC_ERR_WORKSPACE, "%s: scratch too small or not 8-byte aligned (%zu bytes given, %zu needed)", who, scratch_bytes,
-                pdsc::fpfh_scratch_bytes(m, max_nn));
-  return PDSC_OK;
+  return check_scratch(who, "scratch", d_scratch, scratch_bytes, pdsc::fpfh_scratch_bytes(m, max_nn), 8);
 }
 
 static int search_impl(const char* who, pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets,
@@ -988,8 +969,7 @@ int pdsc_estimate_normals_packed(pdsc_engine* e, int32_t P, const int32_t* h_off
                                  double radius, int32_t max_nn, double* d_normals, int32_t* d_status, void* d_scratch,
                                  size_t scratch_bytes, void* cuda_stream) {
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  const int rc = check_pair_offsets("pdsc_estimate_normals_packed", "", P, h_offsets, 1);
-  if (rc) return rc;
+  if (int rc = check_offsets("pdsc_estimate_normals_packed", "", P, h_offsets, 1)) return rc;
   if (!d_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_estimate_normals_packed: null device offsets");
   return search_impl("pdsc_estimate_normals_packed", e, P, h_offsets, d_offsets, d_points, nullptr, radius, max_nn, 0, d_normals,
                      d_status, d_scratch, scratch_bytes, cuda_stream);
@@ -1009,8 +989,7 @@ int pdsc_compute_fpfh_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets
                              const double* d_normals, double radius, int32_t max_nn, int32_t normalise, double* d_fpfh,
                              int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  const int rc = check_pair_offsets("pdsc_compute_fpfh_packed", "", P, h_offsets, 1);
-  if (rc) return rc;
+  if (int rc = check_offsets("pdsc_compute_fpfh_packed", "", P, h_offsets, 1)) return rc;
   if (!d_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_compute_fpfh_packed: null device offsets");
   if (!d_normals) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_compute_fpfh_packed: null normals");
   return search_impl("pdsc_compute_fpfh_packed", e, P, h_offsets, d_offsets, d_points, d_normals, radius, max_nn, normalise, d_fpfh,
@@ -1018,7 +997,7 @@ int pdsc_compute_fpfh_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets
 }
 
 size_t pdsc_icp_packed_scratch_bytes(int32_t B, const int32_t* h_offsets) {
-  return cloud_offsets_ok(B, h_offsets) ? pdsc::icp_scratch_bytes(h_offsets[B]) : 0;
+  return check_offsets("pdsc_icp_packed_scratch_bytes", "", B, h_offsets, 1) ? 0 : pdsc::icp_scratch_bytes(h_offsets[B]);
 }
 
 int pdsc_icp_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
@@ -1026,16 +1005,13 @@ int pdsc_icp_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const i
                     double* d_fitness, double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
                     void* cuda_stream) {
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  const int rc = check_pair_offsets("pdsc_icp_packed", "", B, h_offsets, 1);
-  if (rc) return rc;
+  if (int rc = check_offsets("pdsc_icp_packed", "", B, h_offsets, 1)) return rc;
   if (!d_offsets || !d_src || !d_tgt || !d_init || !d_trans) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_icp_packed: null tensor pointer");
   if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
     return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_icp_packed: max_corr_dist must be positive and finite (got %g)", max_corr_dist);
   if (max_iteration < 1) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_icp_packed: max_iteration must be >= 1 (got %d)", max_iteration);
-  const size_t need = pdsc::icp_scratch_bytes(h_offsets[B]);
-  if (!d_scratch || scratch_bytes < need || reinterpret_cast<uintptr_t>(d_scratch) % 8)
-    return fail(PDSC_ERR_WORKSPACE, "pdsc_icp_packed: scratch too small or not 8-byte aligned (%zu bytes given, %zu needed)",
-                scratch_bytes, need);
+  if (int rc = check_scratch("pdsc_icp_packed", "scratch", d_scratch, scratch_bytes, pdsc::icp_scratch_bytes(h_offsets[B]), 8))
+    return rc;
   DeviceGuard g(e->cfg.device);
   pdsc::launch_icp(B, d_offsets, h_offsets[B], d_src, d_tgt, d_init, max_corr_dist, max_iteration, d_trans, d_fitness, d_rmse,
                    d_iterations, d_status, d_scratch, static_cast<cudaStream_t>(cuda_stream));
@@ -1127,9 +1103,8 @@ size_t pdsc_match_scratch_bytes(int32_t Ns, int32_t Nt) {
 }
 
 size_t pdsc_match_packed_scratch_bytes(int32_t P, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets) {
-  if (P < 1 || !h_src_offsets || !h_tgt_offsets || h_src_offsets[0] != 0 || h_tgt_offsets[0] != 0) return 0;
-  for (int p = 0; p < P; ++p)
-    if (h_src_offsets[p + 1] <= h_src_offsets[p] || h_tgt_offsets[p + 1] <= h_tgt_offsets[p]) return 0;
+  const char* who = "pdsc_match_packed_scratch_bytes";
+  if (check_offsets(who, "source ", P, h_src_offsets, 1) || check_offsets(who, "target ", P, h_tgt_offsets, 1)) return 0;
   return pdsc::match_scratch_bytes(h_src_offsets[P], h_tgt_offsets[P]);
 }
 
@@ -1142,10 +1117,9 @@ static int match_impl(pdsc_engine* e, int32_t P, int32_t D, const int32_t* h_src
   if (e->cfg.in_dim != 6) return fail(PDSC_ERR_UNSUPPORTED, "pdsc_match builds the in_dim = 6 input (engine has in_dim = %d)", e->cfg.in_dim);
   if (!d_src_desc || !d_tgt_desc || !d_src_keypts || !d_tgt_keypts || !d_corr || !d_out_ends || !d_corr_pos || !d_out_src || !d_out_tgt)
     return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_match: null tensor pointer");
-  const size_t need = pdsc::match_scratch_bytes(h_src_offsets[P], h_tgt_offsets[P]);
-  if (!d_scratch || scratch_bytes < need)
-    return fail(PDSC_ERR_WORKSPACE, "pdsc_match: scratch too small (%zu bytes given, %zu needed)", scratch_bytes, need);
-  if (reinterpret_cast<uintptr_t>(d_scratch) % 8) return fail(PDSC_ERR_WORKSPACE, "pdsc_match: scratch must be 8-byte aligned");
+  if (int rc = check_scratch("pdsc_match", "scratch", d_scratch, scratch_bytes,
+                             pdsc::match_scratch_bytes(h_src_offsets[P], h_tgt_offsets[P]), 8))
+    return rc;
   DeviceGuard g(e->cfg.device);
   pdsc::launch_match(P, h_src_offsets, h_tgt_offsets, d_src_offsets, d_tgt_offsets, d_src_desc, d_tgt_desc, desc_is_fp64,
                      d_src_keypts, d_tgt_keypts, D, use_mutual, d_scratch, d_corr, d_out_first, d_out_ends, d_corr_pos, d_out_src,
@@ -1172,9 +1146,8 @@ int pdsc_match_packed(pdsc_engine* e, int32_t P, int32_t D, const int32_t* h_src
                       int32_t* d_corr, int32_t* d_out_offsets, float* d_corr_pos, float* d_out_src, float* d_out_tgt,
                       void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  int rc = check_pair_offsets("pdsc_match_packed", "source ", P, h_src_offsets, 1);
-  if (!rc) rc = check_pair_offsets("pdsc_match_packed", "target ", P, h_tgt_offsets, 1);
-  if (rc) return rc;
+  if (int rc = check_offsets("pdsc_match_packed", "source ", P, h_src_offsets, 1)) return rc;
+  if (int rc = check_offsets("pdsc_match_packed", "target ", P, h_tgt_offsets, 1)) return rc;
   if (!d_src_offsets || !d_tgt_offsets || !d_out_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_match_packed: null offsets");
   return match_impl(e, P, D, h_src_offsets, h_tgt_offsets, d_src_offsets, d_tgt_offsets, d_src_desc, d_tgt_desc, desc_is_fp64,
                     d_src_keypts, d_tgt_keypts, use_mutual, d_corr, d_out_offsets, d_out_offsets + 1, d_corr_pos, d_out_src,

@@ -21,21 +21,18 @@ import numpy as np
 import torch
 
 from . import _capi
-from .frontend import host_to_device
 
 _STATUS = {1: "more than 2^21 voxels along an axis, or a non-finite coordinate",
            2: "a neighbourhood holds more than 4096 points inside the search radius (the search is sized for down-sampled clouds)"}
 
 
-def _ctx(points: torch.Tensor):
+def _points_device(points: torch.Tensor) -> torch.device:
+    """The device of `points`, once it is known to be a CUDA tensor [n,3] with n >= 1."""
     if points.device.type != "cuda":
         raise _capi.PdscError("pointdsc_b200.descriptors runs on an H100 only: pass CUDA tensors (there is no CPU fallback)")
     if points.dim() != 2 or points.shape[1] != 3 or points.shape[0] < 1:
         raise ValueError(f"expected points [n,3] with n >= 1, got {tuple(points.shape)}")
-    dev = points.device
-    lib = _capi.load()
-    engine = _capi.utility_engine(dev.index if dev.index is not None else torch.cuda.current_device())
-    return dev, lib, engine, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    return points.device
 
 
 def _raise_status(status: int) -> None:
@@ -56,39 +53,36 @@ def read_ply(path: str) -> np.ndarray:
 @torch.no_grad()
 def voxel_down_sample(points: torch.Tensor, voxel_size: float) -> torch.Tensor:
     """[n,3] -> [m,3] float32: the mean of the points of every occupied voxel, rows in ascending (ix, iy, iz) order."""
-    dev, lib, engine, stream = _ctx(points)
+    dev = _points_device(points)
+    lib, engine, stream = _capi.device_context(dev)
     pts = points.to(torch.float32).contiguous()
     n = int(pts.shape[0])
     out = torch.empty(n, 3, dtype=torch.float32, device=dev)
     meta = torch.zeros(2, dtype=torch.int32, device=dev)          # [count, status]
-    scratch = torch.empty(int(lib.pdsc_voxel_down_sample_scratch_bytes(n)) + 8, dtype=torch.uint8, device=dev)
+    scratch = _capi.scratch(lib.pdsc_voxel_down_sample_scratch_bytes(n), dev)
     with torch.cuda.device(dev):
         _capi.check(lib.pdsc_voxel_down_sample(engine, n, C.c_void_p(pts.data_ptr()), float(voxel_size), C.c_void_p(out.data_ptr()),
                                                C.c_void_p(meta.data_ptr()), C.c_void_p(meta.data_ptr() + 4),
-                                               C.c_void_p((scratch.data_ptr() + 7) // 8 * 8), scratch.numel() - 8, stream))
+                                               C.c_void_p(scratch.data_ptr()), scratch.numel(), stream))
     m, status = (int(v) for v in meta.tolist())                   # the one host read: it fixes the output shape
     _raise_status(status)
     return out[:m].clone()
 
 
-def _search_buffers(lib, dev, m: int, max_nn: int):
-    scratch = torch.empty(int(lib.pdsc_fpfh_scratch_bytes(m, max_nn)) + 8, dtype=torch.uint8, device=dev)
-    status = torch.zeros(1, dtype=torch.int32, device=dev)
-    return scratch, status
-
-
 @torch.no_grad()
 def estimate_normals(points: torch.Tensor, radius: float, max_nn: int = 30) -> torch.Tensor:
     """[m,3] -> unit normals [m,3] float64 (largest-magnitude component positive; (0,0,1) below three neighbours)."""
-    dev, lib, engine, stream = _ctx(points)
+    dev = _points_device(points)
+    lib, engine, stream = _capi.device_context(dev)
     pts = points.to(torch.float32).contiguous()
     m = int(pts.shape[0])
     normals = torch.empty(m, 3, dtype=torch.float64, device=dev)
-    scratch, status = _search_buffers(lib, dev, m, max_nn)
+    scratch = _capi.scratch(lib.pdsc_fpfh_scratch_bytes(m, max_nn), dev)
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
     with torch.cuda.device(dev):
         _capi.check(lib.pdsc_estimate_normals(engine, m, C.c_void_p(pts.data_ptr()), float(radius), int(max_nn),
                                               C.c_void_p(normals.data_ptr()), C.c_void_p(status.data_ptr()),
-                                              C.c_void_p((scratch.data_ptr() + 7) // 8 * 8), scratch.numel() - 8, stream))
+                                              C.c_void_p(scratch.data_ptr()), scratch.numel(), stream))
     _raise_status(int(status.item()))
     return normals
 
@@ -96,18 +90,20 @@ def estimate_normals(points: torch.Tensor, radius: float, max_nn: int = 30) -> t
 @torch.no_grad()
 def compute_fpfh(points: torch.Tensor, normals: torch.Tensor, radius: float, max_nn: int = 100, normalise: bool = False) -> torch.Tensor:
     """[m,3], [m,3] -> FPFH [m,33] float64 (`np.array(fpfh.data).T`); normalise=True applies x / (||x|| + 1e-6) per row."""
-    dev, lib, engine, stream = _ctx(points)
+    dev = _points_device(points)
+    lib, engine, stream = _capi.device_context(dev)
     pts = points.to(torch.float32).contiguous()
     m = int(pts.shape[0])
     if tuple(normals.shape) != (m, 3):
         raise ValueError(f"normals must be [{m},3], got {tuple(normals.shape)}")
     nrm = normals.to(device=dev, dtype=torch.float64).contiguous()
     out = torch.empty(m, 33, dtype=torch.float64, device=dev)
-    scratch, status = _search_buffers(lib, dev, m, max_nn)
+    scratch = _capi.scratch(lib.pdsc_fpfh_scratch_bytes(m, max_nn), dev)
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
     with torch.cuda.device(dev):
         _capi.check(lib.pdsc_compute_fpfh(engine, m, C.c_void_p(pts.data_ptr()), C.c_void_p(nrm.data_ptr()), float(radius), int(max_nn),
                                           1 if normalise else 0, C.c_void_p(out.data_ptr()), C.c_void_p(status.data_ptr()),
-                                          C.c_void_p((scratch.data_ptr() + 7) // 8 * 8), scratch.numel() - 8, stream))
+                                          C.c_void_p(scratch.data_ptr()), scratch.numel(), stream))
     _raise_status(int(status.item()))
     return out
 
@@ -132,7 +128,8 @@ def fpfh_descriptors_many(clouds: Sequence[torch.Tensor], voxel_size: float,
     offsets after the down-sampling, which fix the shapes, and the status words at the end."""
     if not clouds:
         raise ValueError("fpfh_descriptors_many needs at least one cloud")
-    dev, lib, engine, stream = _ctx(clouds[0])
+    dev = _points_device(clouds[0])
+    lib, engine, stream = _capi.device_context(dev)
     for i, c in enumerate(clouds):
         if c.device != dev or c.dim() != 2 or c.shape[1] != 3 or c.shape[0] < 1:
             raise ValueError(f"cloud {i}: expected a [n,3] tensor on {dev} with n >= 1, got {tuple(c.shape)} on {c.device}")
@@ -141,37 +138,35 @@ def fpfh_descriptors_many(clouds: Sequence[torch.Tensor], voxel_size: float,
     for c in clouds:
         in_off.append(in_off[-1] + int(c.shape[0]))
     pts = (torch.cat([c.to(torch.float32) for c in clouds]) if P > 1 else clouds[0].to(torch.float32)).contiguous()
-    d_in = host_to_device(in_off, torch.int32, dev)
-    h_in = (C.c_int32 * (P + 1))(*in_off)
+    h_in, d_in = _capi.offsets(in_off, None, dev)
     out = torch.empty(in_off[-1], 3, dtype=torch.float32, device=dev)
     meta = torch.empty(2 * P + 1, dtype=torch.int32, device=dev)       # [key-point offsets (P + 1), voxel status (P)]
-    scratch = torch.empty(int(lib.pdsc_voxel_down_sample_packed_scratch_bytes(P, h_in)) + 8, dtype=torch.uint8, device=dev)
+    scratch = _capi.scratch(lib.pdsc_voxel_down_sample_packed_scratch_bytes(P, h_in), dev)
     with torch.cuda.device(dev):
         _capi.check(lib.pdsc_voxel_down_sample_packed(engine, P, h_in, C.c_void_p(d_in.data_ptr()), C.c_void_p(pts.data_ptr()),
                                                       float(voxel_size), C.c_void_p(out.data_ptr()), C.c_void_p(meta.data_ptr()),
                                                       C.c_void_p(meta.data_ptr() + 4 * (P + 1)),
-                                                      C.c_void_p((scratch.data_ptr() + 7) // 8 * 8), scratch.numel() - 8, stream))
+                                                      C.c_void_p(scratch.data_ptr()), scratch.numel(), stream))
     h_meta = meta.tolist()                                         # read 1: the key-point offsets fix the shapes
     offsets = h_meta[:P + 1]
     _raise_cloud_status(h_meta[P + 1:])
-    d_offsets = meta[:P + 1]
+    h_kp, d_offsets = _capi.offsets(offsets, meta[:P + 1], dev)
     keypts = out[:offsets[-1]].clone()
     del out, scratch
-    h_kp = (C.c_int32 * (P + 1))(*offsets)
     m = offsets[-1]
     normals = torch.empty(m, 3, dtype=torch.float64, device=dev)
     feat = torch.empty(m, 33, dtype=torch.float64, device=dev)
     status = torch.empty(2, P, dtype=torch.int32, device=dev)
-    scratch = torch.empty(int(lib.pdsc_fpfh_packed_scratch_bytes(P, h_kp, 100)) + 8, dtype=torch.uint8, device=dev)
-    sc = C.c_void_p((scratch.data_ptr() + 7) // 8 * 8)
+    scratch = _capi.scratch(lib.pdsc_fpfh_packed_scratch_bytes(P, h_kp, 100), dev)
+    sc = C.c_void_p(scratch.data_ptr())
     with torch.cuda.device(dev):                                   # the normals' search (max_nn 30) fits the FPFH's scratch
         _capi.check(lib.pdsc_estimate_normals_packed(engine, P, h_kp, C.c_void_p(d_offsets.data_ptr()), C.c_void_p(keypts.data_ptr()),
                                                      2.0 * voxel_size, 30, C.c_void_p(normals.data_ptr()),
-                                                     C.c_void_p(status.data_ptr()), sc, scratch.numel() - 8, stream))
+                                                     C.c_void_p(status.data_ptr()), sc, scratch.numel(), stream))
         _capi.check(lib.pdsc_compute_fpfh_packed(engine, P, h_kp, C.c_void_p(d_offsets.data_ptr()), C.c_void_p(keypts.data_ptr()),
                                                  C.c_void_p(normals.data_ptr()), 5.0 * voxel_size, 100, 1 if normalise else 0,
                                                  C.c_void_p(feat.data_ptr()), C.c_void_p(status[1].data_ptr()), sc,
-                                                 scratch.numel() - 8, stream))
+                                                 scratch.numel(), stream))
     st = status.cpu()                                              # read 2: the status words
     _raise_cloud_status((st[0] | st[1]).tolist())
     return keypts, feat, offsets, d_offsets

@@ -16,12 +16,6 @@ import torch
 from . import _capi
 
 
-def host_to_device(values, dtype, device) -> torch.Tensor:
-    """A small host list as a device tensor without waiting for the stream: staged in page-locked memory, copied
-    asynchronously (a copy from pageable memory would synchronise the stream first)."""
-    return torch.tensor(values, dtype=dtype).pin_memory().to(device, non_blocking=True)
-
-
 @torch.no_grad()
 def match_many(pairs: Sequence[Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]],
                use_mutual: bool = False) -> Dict[str, object]:
@@ -47,8 +41,7 @@ def match_many(pairs: Sequence[Tuple[torch.Tensor, torch.Tensor, torch.Tensor, t
             raise ValueError(f"pair {i}: expected descriptors [Ns,D] and [Nt,D] of one D, got {tuple(sd.shape)}, {tuple(td.shape)}")
         if tuple(sk.shape) != (sd.shape[0], 3) or tuple(tk.shape) != (td.shape[0], 3):
             raise ValueError("key points must be [Ns,3] and [Nt,3]")
-    lib = _capi.load()
-    engine = _capi.utility_engine(dev.index if dev.index is not None else torch.cuda.current_device())
+    lib, engine, stream = _capi.device_context(dev)
     P, d = len(pairs), int(pairs[0][0].shape[1])
     src_off, tgt_off = [0], [0]
     for sd, td, _, _ in pairs:
@@ -58,7 +51,7 @@ def match_many(pairs: Sequence[Tuple[torch.Tensor, torch.Tensor, torch.Tensor, t
                           else xs[0].to(device=dev, dtype=dt)).contiguous()
     sd, td = cat([p[0] for p in pairs], dtype), cat([p[1] for p in pairs], dtype)
     sk, tk = cat([p[2] for p in pairs], torch.float32), cat([p[3] for p in pairs], torch.float32)
-    d_in = host_to_device(src_off + tgt_off, torch.int32, dev)
+    d_in = _capi.host_to_device(src_off + tgt_off, torch.int32, dev)
     h_src, h_tgt = (C.c_int32 * (P + 1))(*src_off), (C.c_int32 * (P + 1))(*tgt_off)
     ns = src_off[-1]
     corr = torch.empty(ns, 2, dtype=torch.int32, device=dev)
@@ -66,8 +59,7 @@ def match_many(pairs: Sequence[Tuple[torch.Tensor, torch.Tensor, torch.Tensor, t
     corr_pos = torch.empty(ns, 6, dtype=torch.float32, device=dev)
     out_src = torch.empty(ns, 3, dtype=torch.float32, device=dev)
     out_tgt = torch.empty(ns, 3, dtype=torch.float32, device=dev)
-    scratch = torch.empty(int(lib.pdsc_match_packed_scratch_bytes(P, h_src, h_tgt)) + 8, dtype=torch.uint8, device=dev)
-    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    scratch = _capi.scratch(lib.pdsc_match_packed_scratch_bytes(P, h_src, h_tgt), dev)
     with torch.cuda.device(dev):
         _capi.check(lib.pdsc_match_packed(engine, P, d, h_src, h_tgt, C.c_void_p(d_in.data_ptr()),
                                           C.c_void_p(d_in.data_ptr() + 4 * (P + 1)), C.c_void_p(sd.data_ptr()),
@@ -75,7 +67,7 @@ def match_many(pairs: Sequence[Tuple[torch.Tensor, torch.Tensor, torch.Tensor, t
                                           C.c_void_p(tk.data_ptr()), 1 if use_mutual else 0, C.c_void_p(corr.data_ptr()),
                                           C.c_void_p(d_out.data_ptr()), C.c_void_p(corr_pos.data_ptr()),
                                           C.c_void_p(out_src.data_ptr()), C.c_void_p(out_tgt.data_ptr()),
-                                          C.c_void_p((scratch.data_ptr() + 7) // 8 * 8), scratch.numel() - 8, stream))
+                                          C.c_void_p(scratch.data_ptr()), scratch.numel(), stream))
     offsets = [int(x) for x in d_out.cpu()] if use_mutual else src_off      # the only host read: it fixes the output shapes
     m = offsets[-1]
     return {"corr": corr[:m].long(), "corr_pos": corr_pos[:m], "src_keypts": out_src[:m], "tgt_keypts": out_tgt[:m],

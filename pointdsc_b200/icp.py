@@ -18,7 +18,6 @@ from typing import Optional, Sequence
 import torch
 
 from . import _capi
-from .frontend import host_to_device
 
 
 @torch.no_grad()
@@ -44,21 +43,15 @@ def icp_refine_packed(src: torch.Tensor, tgt: torch.Tensor, pred_trans: torch.Te
     if tuple(pred_trans.shape) != (B, 4, 4):
         raise ValueError(f"pred_trans must be [{B},4,4], got {tuple(pred_trans.shape)}")
     dev = src.device
-    lib = _capi.load()
-    engine = _capi.utility_engine(dev.index if dev.index is not None else torch.cuda.current_device())
-    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    lib, engine, stream = _capi.device_context(dev)
     s = src.to(torch.float32).contiguous()
     t = tgt.to(torch.float32).contiguous()
     init = pred_trans.to(device=dev, dtype=torch.float32).contiguous()
-    if d_offsets is None:
-        d_offsets = host_to_device(offsets, torch.int32, dev)
-    elif d_offsets.dtype != torch.int32 or d_offsets.device != dev or d_offsets.numel() != B + 1:
-        raise ValueError("d_offsets must be a device int32 tensor of B + 1 offsets")
-    h_off = (C.c_int32 * (B + 1))(*offsets)
+    h_off, d_offsets = _capi.offsets(offsets, d_offsets, dev)
     out = torch.empty(B, 4, 4, dtype=torch.float32, device=dev)
     stats = torch.empty(2, B, dtype=torch.float64, device=dev) if info else None
     ints = torch.empty(2, B, dtype=torch.int32, device=dev) if info else None
-    scratch = torch.empty(int(lib.pdsc_icp_packed_scratch_bytes(B, h_off)) + 8, dtype=torch.uint8, device=dev)
+    scratch = _capi.scratch(lib.pdsc_icp_packed_scratch_bytes(B, h_off), dev)
 
     def ptr(x, row=None):
         return C.c_void_p(x[row].data_ptr()) if x is not None else None
@@ -67,7 +60,7 @@ def icp_refine_packed(src: torch.Tensor, tgt: torch.Tensor, pred_trans: torch.Te
         _capi.check(lib.pdsc_icp_packed(engine, B, h_off, C.c_void_p(d_offsets.data_ptr()), C.c_void_p(s.data_ptr()),
                                         C.c_void_p(t.data_ptr()), C.c_void_p(init.data_ptr()), float(max_correspondence_distance),
                                         int(max_iteration), C.c_void_p(out.data_ptr()), ptr(stats, 0), ptr(stats, 1), ptr(ints, 0),
-                                        ptr(ints, 1), C.c_void_p((scratch.data_ptr() + 7) // 8 * 8), scratch.numel() - 8, stream))
+                                        ptr(ints, 1), C.c_void_p(scratch.data_ptr()), scratch.numel(), stream))
     if not info:
         return out
     return out, {"fitness": stats[0], "inlier_rmse": stats[1], "iterations": ints[0], "status": ints[1]}

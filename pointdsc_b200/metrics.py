@@ -30,13 +30,11 @@ def eval_stats(pred_trans: torch.Tensor, gt_trans: torch.Tensor, src_keypts: tor
     if pt.shape != (b, 4, 4) or gt.shape != (b, 4, 4) or t.shape != (b, n, 3) or pl.shape != (b, n) or gl.shape != (b, n):
         raise ValueError("expected trans [B,4,4], key points [B,N,3], labels [B,N]")
     out = torch.empty(b, 10, dtype=torch.float32, device=dev)
-    lib = _capi.load()
-    engine = _capi.utility_engine(dev.index if dev.index is not None else torch.cuda.current_device())
+    lib, engine, stream = _capi.device_context(dev)
     with torch.cuda.device(dev):
         _capi.check(lib.pdsc_eval_stats(engine, b, n, C.c_void_p(pt.data_ptr()), C.c_void_p(gt.data_ptr()), C.c_void_p(s.data_ptr()),
                                         C.c_void_p(t.data_ptr()), C.c_void_p(pl.data_ptr()), C.c_void_p(gl.data_ptr()),
-                                        float(re_thre), float(te_thre), C.c_void_p(out.data_ptr()),
-                                        C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+                                        float(re_thre), float(te_thre), C.c_void_p(out.data_ptr()), stream))
     return out
 
 
@@ -59,20 +57,12 @@ def eval_stats_packed(pred_trans: torch.Tensor, gt_trans: torch.Tensor, src_keyp
             or pl.shape != (r,) or gl.shape != (r,):
         raise ValueError(f"expected B + 1 offsets ending at R, trans [B,4,4], key points [R,3], labels [R] (got {b + 1} offsets, "
                          f"R = {r}, trans {tuple(pt.shape)})")
-    if d_offsets is None:
-        from .frontend import host_to_device
-        d_offsets = host_to_device(offsets, torch.int32, dev)
-    if d_offsets.dtype != torch.int32 or d_offsets.device != dev or d_offsets.numel() != b + 1:
-        raise ValueError("d_offsets must be a device int32 tensor of B + 1 entries")
-    d_off = d_offsets.contiguous()
-    h_off = (C.c_int32 * (b + 1))(*offsets)
+    h_off, d_off = _capi.offsets(offsets, d_offsets, dev)
     out = torch.empty(b, 10, dtype=torch.float32, device=dev)
-    lib = _capi.load()
-    engine = _capi.utility_engine(dev.index if dev.index is not None else torch.cuda.current_device())
+    lib, engine, stream = _capi.device_context(dev)
     with torch.cuda.device(dev):
         _capi.check(lib.pdsc_eval_stats_packed(engine, b, h_off, C.c_void_p(d_off.data_ptr()), C.c_void_p(pt.data_ptr()),
                                                C.c_void_p(gt.data_ptr()), C.c_void_p(s.data_ptr()), C.c_void_p(t.data_ptr()),
                                                C.c_void_p(pl.data_ptr()), C.c_void_p(gl.data_ptr()), float(re_thre),
-                                               float(te_thre), C.c_void_p(out.data_ptr()),
-                                               C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+                                               float(te_thre), C.c_void_p(out.data_ptr()), stream))
     return out

@@ -27,7 +27,6 @@ import torch
 import torch.nn as nn
 
 from . import _capi
-from .frontend import host_to_device
 
 DEFAULT_PRECISION = os.environ.get("POINTDSC_PRECISION", "fp16x3")
 
@@ -353,12 +352,7 @@ class PointDSC(nn.Module):
             raise ValueError(f"expected B + 1 >= 2 offsets ending at R = {R}, got {len(offsets)} ending at {offsets[-1:]}")
         lib = self._ensure_engine()
         B = len(offsets) - 1
-        h_off = (C.c_int32 * (B + 1))(*offsets)
-        if d_offsets is None:
-            d_offsets = host_to_device(offsets, torch.int32, dev)
-        if d_offsets.dtype != torch.int32 or d_offsets.device != dev or d_offsets.numel() != B + 1:
-            raise ValueError("d_offsets must be a device int32 tensor of B + 1 entries")
-        d_off = d_offsets.contiguous()
+        h_off, d_off = _capi.offsets(offsets, d_offsets, dev)
         cp, s, t = (x.to(torch.float32).contiguous() for x in (corr_pos, src_keypts, tgt_keypts))
         need = int(lib.pdsc_workspace_bytes_packed(self._engine, B, h_off))
         if need == 0:

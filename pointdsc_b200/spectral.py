@@ -24,14 +24,12 @@ def leading_eigenvector(M: torch.Tensor, num_iterations: int = 10, early_exit: b
     dev = M.device
     m = M.to(torch.float32).contiguous()
     b, n = int(m.shape[0]), int(m.shape[1])
-    lib = _capi.load()
-    engine = _capi.utility_engine(dev.index if dev.index is not None else torch.cuda.current_device())
+    lib, engine, stream = _capi.device_context(dev)
     v = torch.empty(b, n, dtype=torch.float32, device=dev)
     iters = torch.empty(b, dtype=torch.int32, device=dev)
-    scratch = torch.empty(int(lib.pdsc_leading_eigenvector_scratch_bytes(b, n)) + 16, dtype=torch.uint8, device=dev)
-    base = (scratch.data_ptr() + 15) // 16 * 16
+    scratch = _capi.scratch(lib.pdsc_leading_eigenvector_scratch_bytes(b, n), dev, align=16)
     with torch.cuda.device(dev):
         _capi.check(lib.pdsc_leading_eigenvector(engine, b, n, C.c_void_p(m.data_ptr()), int(num_iterations), 1 if early_exit else 0,
-                                                 C.c_void_p(v.data_ptr()), C.c_void_p(iters.data_ptr()), C.c_void_p(base),
-                                                 scratch.numel() - 16, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+                                                 C.c_void_p(v.data_ptr()), C.c_void_p(iters.data_ptr()),
+                                                 C.c_void_p(scratch.data_ptr()), scratch.numel(), stream))
     return v, iters
