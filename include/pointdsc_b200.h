@@ -171,12 +171,14 @@ int pdsc_forward_graph(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr
                        const float* d_tgt_keypts, float* d_final_trans, float* d_final_labels, void* d_workspace,
                        size_t workspace_bytes, void* cuda_stream);
 
-/* Same call with HOST buffers (the end-to-end form): copies the inputs host->device, runs
- * pdsc_forward, copies the two outputs device->host and synchronises the stream before returning.
- * Device staging and workspace are owned by the engine and grown on demand.  The key points are copied
- * on `cuda_stream`; corr_pos (half of the input bytes) is copied on an engine-owned side stream, ordered
- * behind `cuda_stream` by an event, while the spatial-consistency kernel (which reads only the key points)
- * runs, and joined again before the first kernel that reads corr_pos. */
+/* Same call with HOST buffers (the end-to-end form): pdsc_forward_host_submit below followed by pdsc_forward_host_wait on
+ * the slot it took, i.e. the pipelined pair with one call in flight, synchronous on return.  It takes a free slot: with one
+ * _submit call in flight it leaves the pipeline as it found it, with two it fails as a third _submit would.  Device staging
+ * and workspace are owned by the engine and grown on demand.  The inputs are copied on an engine-owned side stream (not
+ * ordered behind `cuda_stream`), key points first: above the size that replays a captured graph the forward starts once
+ * they have arrived, so corr_pos (half of the input bytes) is still crossing while the spatial-consistency kernel (which
+ * reads only the key points) runs, and is waited for before the first kernel that reads it.  A failed call returns once
+ * nothing reads the host inputs any more. */
 int pdsc_forward_host(pdsc_engine* e, int32_t B, int32_t N, const float* h_corr_pos, const float* h_src_keypts,
                       const float* h_tgt_keypts, float* h_final_trans, float* h_final_labels, void* cuda_stream);
 

@@ -76,29 +76,23 @@ struct pdsc_engine {
   std::vector<LayerOffsets> layers;
   size_t off_c0t = 0, off_c0b = 0, off_c2t = 0, off_c2b = 0, off_c4 = 0, off_c4b = 0;
   pdsc::TcWeights tc;  // tensor-core operand images (encoder_tc.cu)
-  // engine-owned buffers for pdsc_forward_host
+  // engine-owned workspace of the host-input forwards (pdsc_forward_host, pdsc_forward_host_submit)
   void* host_ws = nullptr;
   size_t host_ws_bytes = 0;
-  float* host_io = nullptr;
-  size_t host_io_floats = 0;
-  // pdsc_forward_host copies corr_pos on a side stream while the SC kernel (which only reads the key points) runs
-  cudaStream_t copy_stream = nullptr;
-  cudaEvent_t copy_fork = nullptr, corr_ready = nullptr;
-  bool corr_pending = false;             // the next pdsc_forward waits for corr_ready before its first reader of corr_pos
-  // pdsc_forward_host_submit / _wait: two calls in flight.  Each slot owns its device copies of the inputs and outputs and
-  // three events; the forwards themselves stay serialised on the caller's stream (one workspace), while the host->device
-  // copies of call t + 1 (h2d_stream) and the device->host copies of call t - 1 (d2h_stream) run beside the forward of call t.
+  // pdsc_forward_host_submit / _wait: two calls in flight (pdsc_forward_host is one call of the pair).  Each slot owns its
+  // device copies of the inputs and outputs and three events; the forwards themselves stay serialised on the caller's stream
+  // (one workspace), while the host->device copies of call t + 1 (h2d_stream) and the device->host copies of call t - 1
+  // (d2h_stream) run beside the forward of call t.
   struct HostSlot {
     float* io = nullptr;
     size_t io_floats = 0;
-    cudaEvent_t in_ready = nullptr, fwd_done = nullptr;
+    cudaEvent_t keys_ready = nullptr, in_ready = nullptr, fwd_done = nullptr;
     bool busy = false;                   // submitted and not yet waited for
     float *h_trans = nullptr, *h_labels = nullptr;   // where _wait delivers the results ...
     const float *d_trans = nullptr, *d_labels = nullptr;   // ... from
     size_t trans_bytes = 0, labels_bytes = 0;
   } slots[2];
   cudaStream_t h2d_stream = nullptr, d2h_stream = nullptr;
-  int next_slot = 0;
   // live profiling (pdsc_profile_*)
   bool profiling = false;
   bool profile_pending = false;
@@ -435,13 +429,10 @@ int pdsc_destroy(pdsc_engine* e) {
   cudaFree(e->d_weights);
   pdsc::tc_free_weights(&e->tc);
   cudaFree(e->host_ws);
-  cudaFree(e->host_io);
-  if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
-  if (e->copy_fork) cudaEventDestroy(e->copy_fork);
-  if (e->corr_ready) cudaEventDestroy(e->corr_ready);
   for (auto& sl : e->slots) {
     if (sl.busy && sl.fwd_done) cudaEventSynchronize(sl.fwd_done);
     cudaFree(sl.io);
+    if (sl.keys_ready) cudaEventDestroy(sl.keys_ready);
     if (sl.in_ready) cudaEventDestroy(sl.in_ready);
     if (sl.fwd_done) cudaEventDestroy(sl.fwd_done);
   }
@@ -565,22 +556,31 @@ int32_t pdsc_launches_per_forward(const pdsc_engine* e, int32_t B, int32_t N) {
   return 2 + enc + 1 + 2 + ((e->cfg.precision == PDSC_FP32_SIMT) ? 3 : 2) + 2 + 3;
 }
 
+// what forward_impl refuses of the engine and the call's shape (a packed call's offsets are checked by its entry point)
+static int check_forward(const pdsc_engine* e, int32_t B, int32_t N, const int32_t* h_offsets) {
+  if (!e->committed) return fail(PDSC_ERR_NOT_COMMITTED, "pdsc_commit_params() has not been called since the last pdsc_set_param()");
+  if (!h_offsets) {
+    if (B <= 0 || N <= 1) return fail(PDSC_ERR_SHAPE, "need B >= 1 and N >= 2 (got B=%d N=%d)", B, N);
+    const int max_n = pdsc::pick_seeds_max_n();
+    if (N > max_n) return fail(PDSC_ERR_UNSUPPORTED, "N=%d exceeds the supported maximum %d", N, max_n);
+  }
+  return PDSC_OK;
+}
+
 // mode 0: testing (PointDSC.py: NMS seeds, per-set early exit, labels = inlier mask, post-refinement)
 // mode 1: non-testing / validation (PointDSC.py:158-165, :176, :190-191): seeds = top-S by confidence, batch-global early
 //         exit, no refinement, final_labels = confidence logits, optional feature-similarity matrix M [B,N,N]
 // h_offsets / d_offsets: a packed call (mode 0, no io), offsets validated by pdsc_forward_packed; N is then ignored
+// corr_ready: if not null, the stream waits for it right behind the SC kernel, which reads only the key points, and before
+//             the first reader of corr_pos (the host-input path copies corr_pos meanwhile)
 static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const int32_t* h_offsets, const int32_t* d_offsets,
                         const float* d_corr_pos, const float* d_src,
                         const float* d_tgt, float* d_final_trans, float* d_final_labels, float* d_M, const pdsc_stage_io* io,
-                        void* d_workspace, size_t workspace_bytes, void* cuda_stream) {
+                        void* d_workspace, size_t workspace_bytes, void* cuda_stream, cudaEvent_t corr_ready = nullptr) {
   using namespace pdsc;
   const int mask_stride = mode == 0 ? 1 : 0;
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (!e->committed) return fail(PDSC_ERR_NOT_COMMITTED, "pdsc_commit_params() has not been called since the last pdsc_set_param()");
-  if (!h_offsets) {
-    if (B <= 0 || N <= 1) return fail(PDSC_ERR_SHAPE, "need B >= 1 and N >= 2 (got B=%d N=%d)", B, N);
-    if (N > pick_seeds_max_n()) return fail(PDSC_ERR_UNSUPPORTED, "N=%d exceeds the supported maximum %d", N, pick_seeds_max_n());
-  }
+  if (int rc = check_forward(e, B, N, h_offsets)) return rc;
   if (!d_src || !d_tgt || !d_final_trans || !d_final_labels) return fail(PDSC_ERR_INVALID_ARGUMENT, "null tensor pointer");
   const bool inject_feat = io && io->in_features;
   if (!inject_feat && !d_corr_pos) return fail(PDSC_ERR_INVALID_ARGUMENT, "corr_pos is null");
@@ -616,10 +616,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
     if (simt) launch_sc_matrix(d_src, d_tgt, w.sc, B, N, e->sigma_spat, st, sets);
     else launch_sc_matrix_tiled(d_src, d_tgt, w.sc, B, N, e->sigma_spat, st, sets);
     mark(1);
-    if (e->corr_pending) {   // host path: corr_pos is still arriving on the side stream
-      PDSC_CUDA(cudaStreamWaitEvent(st, e->corr_ready, 0));
-      e->corr_pending = false;
-    }
+    if (corr_ready) PDSC_CUDA(cudaStreamWaitEvent(st, corr_ready, 0));
     if (io && io->out_sc) {
       if (simt)
         cudaMemcpy2DAsync(io->out_sc, (size_t)N * sizeof(float), w.sc, (size_t)NS * sizeof(float), (size_t)N * sizeof(float),
@@ -1206,67 +1203,10 @@ int pdsc_profile_read(pdsc_engine* e, float* ms_out, int32_t* launches_out) {
 
 int pdsc_forward_host(pdsc_engine* e, int32_t B, int32_t N, const float* h_corr_pos, const float* h_src,
                       const float* h_tgt, float* h_final_trans, float* h_final_labels, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (!h_corr_pos || !h_src || !h_tgt || !h_final_trans || !h_final_labels) return fail(PDSC_ERR_INVALID_ARGUMENT, "null host pointer");
-  if (B <= 0 || N <= 1) return fail(PDSC_ERR_SHAPE, "need B >= 1 and N >= 2 (got B=%d N=%d)", B, N);
-  DeviceGuard g(e->cfg.device);
-  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  const size_t R = (size_t)B * N;
-  const size_t need_ws = pdsc_workspace_bytes(e, B, N);
-  if (need_ws > e->host_ws_bytes) {
-    cudaFree(e->host_ws);
-    e->host_ws = nullptr; e->host_ws_bytes = 0;
-    PDSC_CUDA(cudaMalloc(&e->host_ws, need_ws));
-    e->host_ws_bytes = need_ws;
-  }
-  const size_t in_dim = (size_t)e->cfg.in_dim;
-  const size_t io_floats = R * (in_dim + 3 + 3 + 1) + (size_t)B * 16 + 64;
-  if (io_floats > e->host_io_floats) {
-    cudaFree(e->host_io);
-    e->host_io = nullptr; e->host_io_floats = 0;
-    PDSC_CUDA(cudaMalloc(&e->host_io, io_floats * sizeof(float)));
-    e->host_io_floats = io_floats;
-  }
-  float* d_corr = e->host_io;
-  float* d_src = d_corr + R * in_dim;
-  float* d_tgt = d_src + R * 3;
-  float* d_lab = d_tgt + R * 3;
-  float* d_tr = d_lab + R;
-  if (!e->copy_stream) {
-    PDSC_CUDA(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-    PDSC_CUDA(cudaEventCreateWithFlags(&e->copy_fork, cudaEventDisableTiming));
-    PDSC_CUDA(cudaEventCreateWithFlags(&e->corr_ready, cudaEventDisableTiming));
-  }
-  // key points first (the SC kernel reads only those); corr_pos (half of the input bytes) follows on the side stream,
-  // ordered behind whatever the caller's stream held, and is awaited right behind the SC launch
-  PDSC_CUDA(cudaMemcpyAsync(d_src, h_src, R * 3 * sizeof(float), cudaMemcpyHostToDevice, st));
-  PDSC_CUDA(cudaMemcpyAsync(d_tgt, h_tgt, R * 3 * sizeof(float), cudaMemcpyHostToDevice, st));
-  if (R <= kGraphRows && !e->profiling) {
-    // small call (the evaluation loops' bs = 1): launch-bound, so everything stays on one stream and the forward is one
-    // graph launch over the engine-owned (address-stable) buffers
-    PDSC_CUDA(cudaMemcpyAsync(d_corr, h_corr_pos, R * in_dim * sizeof(float), cudaMemcpyHostToDevice, st));
-    const int rc = pdsc_forward_graph(e, B, N, d_corr, d_src, d_tgt, d_tr, d_lab, e->host_ws, e->host_ws_bytes, cuda_stream);
-    if (rc) return rc;
-    PDSC_CUDA(cudaMemcpyAsync(h_final_trans, d_tr, (size_t)B * 16 * sizeof(float), cudaMemcpyDeviceToHost, st));
-    PDSC_CUDA(cudaMemcpyAsync(h_final_labels, d_lab, R * sizeof(float), cudaMemcpyDeviceToHost, st));
-    PDSC_CUDA(cudaStreamSynchronize(st));
-    return PDSC_OK;
-  }
-  PDSC_CUDA(cudaEventRecord(e->copy_fork, st));
-  PDSC_CUDA(cudaStreamWaitEvent(e->copy_stream, e->copy_fork, 0));
-  PDSC_CUDA(cudaMemcpyAsync(d_corr, h_corr_pos, R * in_dim * sizeof(float), cudaMemcpyHostToDevice, e->copy_stream));
-  PDSC_CUDA(cudaEventRecord(e->corr_ready, e->copy_stream));
-  e->corr_pending = true;
-  const int rc = pdsc_forward(e, B, N, d_corr, d_src, d_tgt, d_tr, d_lab, nullptr, e->host_ws, e->host_ws_bytes, cuda_stream);
-  if (e->corr_pending) {   // the forward failed before its wait: join the side stream so the buffers may be reused
-    cudaStreamWaitEvent(st, e->corr_ready, 0);
-    e->corr_pending = false;
-  }
-  if (rc) return rc;
-  PDSC_CUDA(cudaMemcpyAsync(h_final_trans, d_tr, (size_t)B * 16 * sizeof(float), cudaMemcpyDeviceToHost, st));
-  PDSC_CUDA(cudaMemcpyAsync(h_final_labels, d_lab, R * sizeof(float), cudaMemcpyDeviceToHost, st));
-  PDSC_CUDA(cudaStreamSynchronize(st));
-  return PDSC_OK;
+  int32_t slot = -1;
+  if (int rc = pdsc_forward_host_submit(e, B, N, h_corr_pos, h_src, h_tgt, h_final_trans, h_final_labels, cuda_stream, &slot))
+    return rc;
+  return pdsc_forward_host_wait(e, slot);
 }
 
 int pdsc_forward_host_submit(pdsc_engine* e, int32_t B, int32_t N, const float* h_corr_pos, const float* h_src,
@@ -1274,10 +1214,13 @@ int pdsc_forward_host_submit(pdsc_engine* e, int32_t B, int32_t N, const float* 
                              int32_t* slot_out) {
   if (!e || !slot_out) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine / slot pointer");
   if (!h_corr_pos || !h_src || !h_tgt || !h_final_trans || !h_final_labels) return fail(PDSC_ERR_INVALID_ARGUMENT, "null host pointer");
-  if (B <= 0 || N <= 1) return fail(PDSC_ERR_SHAPE, "need B >= 1 and N >= 2 (got B=%d N=%d)", B, N);
-  pdsc_engine::HostSlot& sl = e->slots[e->next_slot];
-  if (sl.busy)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "both pipeline slots are in flight: pdsc_forward_host_wait(%d) first", e->next_slot);
+  // what the forward would refuse is refused here, before any copy out of the caller's buffers is enqueued
+  if (int rc = check_forward(e, B, N, nullptr)) return rc;
+  // the first free slot: a synchronous pdsc_forward_host between two _submit calls leaves the pipeline's slot free for the
+  // next _submit, and repeated synchronous calls stay on slot 0, whose address-stable buffers replay one cached graph
+  const int slot = !e->slots[0].busy ? 0 : !e->slots[1].busy ? 1 : -1;
+  if (slot < 0) return fail(PDSC_ERR_INVALID_ARGUMENT, "both pipeline slots are in flight: pdsc_forward_host_wait one first");
+  pdsc_engine::HostSlot& sl = e->slots[slot];
   DeviceGuard g(e->cfg.device);
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   const size_t R = (size_t)B * N;
@@ -1302,6 +1245,7 @@ int pdsc_forward_host_submit(pdsc_engine* e, int32_t B, int32_t N, const float* 
     PDSC_CUDA(cudaStreamCreateWithFlags(&e->d2h_stream, cudaStreamNonBlocking));
   }
   if (!sl.in_ready) {
+    PDSC_CUDA(cudaEventCreateWithFlags(&sl.keys_ready, cudaEventDisableTiming));
     PDSC_CUDA(cudaEventCreateWithFlags(&sl.in_ready, cudaEventDisableTiming));
     PDSC_CUDA(cudaEventCreateWithFlags(&sl.fwd_done, cudaEventDisableTiming));
   }
@@ -1310,26 +1254,38 @@ int pdsc_forward_host_submit(pdsc_engine* e, int32_t B, int32_t N, const float* 
   float* d_tgt = d_src + R * 3;
   float* d_lab = d_tgt + R * 3;
   float* d_tr = d_lab + R;
-  // inputs: the slot's previous call has been waited for, so its buffers are free; nothing orders these copies behind the
-  // forward that is running now — that is the overlap
-  PDSC_CUDA(cudaMemcpyAsync(d_src, h_src, R * 3 * sizeof(float), cudaMemcpyHostToDevice, e->h2d_stream));
-  PDSC_CUDA(cudaMemcpyAsync(d_tgt, h_tgt, R * 3 * sizeof(float), cudaMemcpyHostToDevice, e->h2d_stream));
-  PDSC_CUDA(cudaMemcpyAsync(d_corr, h_corr_pos, R * in_dim * sizeof(float), cudaMemcpyHostToDevice, e->h2d_stream));
-  PDSC_CUDA(cudaEventRecord(sl.in_ready, e->h2d_stream));
-  PDSC_CUDA(cudaStreamWaitEvent(st, sl.in_ready, 0));
-  const int rc = (R <= kGraphRows && !e->profiling)
-                     ? pdsc_forward_graph(e, B, N, d_corr, d_src, d_tgt, d_tr, d_lab, e->host_ws, e->host_ws_bytes, cuda_stream)
-                     : pdsc_forward(e, B, N, d_corr, d_src, d_tgt, d_tr, d_lab, nullptr, e->host_ws, e->host_ws_bytes, cuda_stream);
-  if (rc) return rc;
-  PDSC_CUDA(cudaEventRecord(sl.fwd_done, st));
+  // small calls (the evaluation loops' bs = 1) are launch-bound: the forward is one graph launch over the slot's
+  // address-stable buffers, behind all of its inputs.  A larger, eager forward starts once the key points are in (the SC
+  // kernel reads only those) and waits for corr_pos (half of the input bytes) right behind the SC kernel.
+  const bool graph = R <= kGraphRows && !e->profiling;
+  auto enqueue = [&]() -> int {
+    // the slot's previous call has been waited for, so its buffers are free; nothing orders these copies behind the
+    // forward that is running now — that is the overlap
+    PDSC_CUDA(cudaMemcpyAsync(d_src, h_src, R * 3 * sizeof(float), cudaMemcpyHostToDevice, e->h2d_stream));
+    PDSC_CUDA(cudaMemcpyAsync(d_tgt, h_tgt, R * 3 * sizeof(float), cudaMemcpyHostToDevice, e->h2d_stream));
+    PDSC_CUDA(cudaEventRecord(sl.keys_ready, e->h2d_stream));
+    PDSC_CUDA(cudaMemcpyAsync(d_corr, h_corr_pos, R * in_dim * sizeof(float), cudaMemcpyHostToDevice, e->h2d_stream));
+    PDSC_CUDA(cudaEventRecord(sl.in_ready, e->h2d_stream));
+    PDSC_CUDA(cudaStreamWaitEvent(st, graph ? sl.in_ready : sl.keys_ready, 0));
+    const int rc = graph ? pdsc_forward_graph(e, B, N, d_corr, d_src, d_tgt, d_tr, d_lab, e->host_ws, e->host_ws_bytes, cuda_stream)
+                         : forward_impl(e, 0, B, N, nullptr, nullptr, d_corr, d_src, d_tgt, d_tr, d_lab, nullptr, nullptr,
+                                        e->host_ws, e->host_ws_bytes, cuda_stream, sl.in_ready);
+    if (rc) return rc;
+    PDSC_CUDA(cudaEventRecord(sl.fwd_done, st));
+    return PDSC_OK;
+  };
+  if (int rc = enqueue()) {
+    // the slot stays free; every copy already enqueued has finished, so nothing reads the caller's inputs once this returns
+    cudaStreamSynchronize(e->h2d_stream);
+    return rc;
+  }
   // the results leave in _wait (on d2h_stream, beside the NEXT call's forward): a device->host copy into pageable memory blocks
   // its caller until the data has arrived, so issuing it here would hold the host inside _submit for the whole forward
   sl.h_trans = h_final_trans; sl.h_labels = h_final_labels;
   sl.d_trans = d_tr; sl.d_labels = d_lab;
   sl.trans_bytes = (size_t)B * 16 * sizeof(float); sl.labels_bytes = R * sizeof(float);
   sl.busy = true;
-  *slot_out = e->next_slot;
-  e->next_slot ^= 1;
+  *slot_out = slot;
   return PDSC_OK;
 }
 
