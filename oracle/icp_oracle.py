@@ -23,6 +23,9 @@ Every run records the margins that decide whether a float64 computation in anoth
 discrete decisions: the smallest |d^2 - r^2_f| of a nearest neighbour, the smallest gap in d^2 between the nearest and the next
 distinct target position, the smallest distance of |d rmse| from the 1e-6 criterion, and the smallest sigma_2 / sigma_1 of an
 update over two or more correspondences (below rank 2 the rotation is not unique and any two SVDs may pick different ones).
+`late_margins` are the same margins without the first correspondence search, for runs built so that the first search decides
+at an exact edge on purpose.  `decide`, a hook on every search, can override its outcome: that is how a test shows that a
+decision it placed on an edge matters.
 """
 import numpy as np
 from scipy.spatial import cKDTree
@@ -101,29 +104,43 @@ def _status(src: np.ndarray, tgt: np.ndarray, r: float) -> int:
     return 1 if (cells >= MAX_CELLS).any() else 0
 
 
-def icp(src, tgt, init, max_correspondence_distance: float = 0.10, max_iteration: int = 30, search: str = "kdtree") -> dict:
+def icp(src, tgt, init, max_correspondence_distance: float = 0.10, max_iteration: int = 30, search: str = "kdtree",
+        decide=None, record: bool = False) -> dict:
     """Point-to-point ICP of one set.  src, tgt [N,3] float32 (row j of src corresponds to nothing in particular: the target is
     searched), init [4,4] float32.  Returns {'trans' [4,4] float32, 'trans64', 'fitness', 'inlier_rmse', 'iterations', 'status',
-    'margins': {'d2_radius', 'nn_gap', 'rmse_criterion', 'sigma_ratio'}}."""
+    'margins' and 'late_margins': {'d2_radius', 'nn_gap', 'rmse_criterion', 'sigma_ratio'}}.
+
+    decide(search, row, d2, keep) -> (row, keep), when given, sees every correspondence search (0 = the one before the first
+    update): the nearest target row of every source row (-1: none), its d^2 and whether it is kept, and returns the rows and
+    the kept mask to use.  record=True adds 'updates': the (moved source, target) point pairs of every update."""
     src = np.asarray(src, np.float32).astype(np.float64)
     tgt = np.asarray(tgt, np.float32).astype(np.float64)
     T = np.asarray(init, np.float32).astype(np.float64)
     r = float(max_correspondence_distance)
     margins = {"d2_radius": np.inf, "nn_gap": np.inf, "rmse_criterion": np.inf, "sigma_ratio": np.inf}
+    late = dict(margins)
     if _status(src, tgt, r):
         return {"trans": T.astype(np.float32), "trans64": T, "fitness": 0.0, "inlier_rmse": 0.0, "iterations": 0, "status": 1,
-                "margins": margins}
+                "margins": margins, "late_margins": late, "updates": []}
     N = len(src)
     targets = _Targets(tgt, r, search)
     r2f = targets.r2f
 
+    searches = 0
+    updates = []
+
     def correspondences(P):
+        nonlocal searches
         row, d2, gap = targets.nearest(P)
         found = row >= 0
         if found.any():
-            margins["d2_radius"] = min(margins["d2_radius"], float(np.abs(d2[found] - r2f).min()))
-            margins["nn_gap"] = min(margins["nn_gap"], float(gap[found].min()))
+            for m in (margins, late) if searches else (margins,):
+                m["d2_radius"] = min(m["d2_radius"], float(np.abs(d2[found] - r2f).min()))
+                m["nn_gap"] = min(m["nn_gap"], float(gap[found].min()))
         keep = found & (d2 < r2f)
+        if decide is not None:
+            row, keep = decide(searches, row.copy(), d2, keep.copy())
+        searches += 1
         n = int(keep.sum())
         rmse = float(np.sqrt(d2[keep].sum() / n)) if n else 0.0
         return np.nonzero(keep)[0], row[keep], n / N, rmse
@@ -133,20 +150,24 @@ def icp(src, tgt, init, max_correspondence_distance: float = 0.10, max_iteration
     iterations = 0
     for _ in range(max_iteration):
         R, t, ratio = umeyama(P[cs], tgt[ct])
-        margins["sigma_ratio"] = min(margins["sigma_ratio"], ratio)
+        if record:
+            updates.append((P[cs].copy(), tgt[ct].copy()))
+        for m in (margins, late):
+            m["sigma_ratio"] = min(m["sigma_ratio"], ratio)
         U = np.eye(4)
         U[:3, :3], U[:3, 3] = R, t
         T = U @ T
         P = P @ R.T + t
         iterations += 1
         cs, ct, f2, r2 = correspondences(P)
-        margins["rmse_criterion"] = min(margins["rmse_criterion"], abs(abs(rmse - r2) - RELATIVE_RMSE))
+        for m in (margins, late):
+            m["rmse_criterion"] = min(m["rmse_criterion"], abs(abs(rmse - r2) - RELATIVE_RMSE))
         done = abs(fitness - f2) < RELATIVE_FITNESS and abs(rmse - r2) < RELATIVE_RMSE
         fitness, rmse = f2, r2
         if done:
             break
     return {"trans": T.astype(np.float32), "trans64": T, "fitness": fitness, "inlier_rmse": rmse, "iterations": iterations,
-            "status": 0, "margins": margins}
+            "status": 0, "margins": margins, "late_margins": late, "updates": updates}
 
 
 def icp_packed(src, tgt, init, offsets, max_correspondence_distance: float = 0.10, max_iteration: int = 30) -> list:

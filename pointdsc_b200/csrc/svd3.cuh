@@ -16,6 +16,13 @@ namespace pdsc {
 
 // The solver is templated on its scalar: `float` for the forward's per-seed and refinement solves, `double` for the ICP
 // updates (icp.cu).  Each scalar has its own thresholds; the float ones are the literals the float solver has always used.
+//
+// `rank` is the squared ratio sigma_2 / sigma_1 below which u2 is not worth computing and any unit vector orthogonal to u1 will
+// do.  The polar factor of H is determined to |R - R_exact| <= C eps sigma_1 / (sigma_2 + d sigma_3) (C ~ 16, eps the unit
+// roundoff): once sigma_2 / sigma_1 drops under ~8 eps that bound exceeds 2, the distance between any two rotations, and every
+// choice of u2 is as accurate as any other.  Above it Gram-Schmidt's u2 carries the information, so the threshold is (8 eps)^2:
+// 1e-12 ~ (8 * 2^-23)^2 in float, 3.2e-30 ~ (8 * 2^-52)^2 in double.  (The float literal is 10% above (8 eps)^2 = 9.1e-13: at
+// its threshold, sigma_2 / sigma_1 = 1e-6, the bound is 1.9 rather than 2.  It stays as it is, and so does every float solve.)
 template <typename T> struct KabschTol;
 template <> struct KabschTol<float> {
   static constexpr float skip = 1e-9f;     // columns this close to orthogonal (cosine) are left alone
@@ -28,7 +35,7 @@ template <> struct KabschTol<double> {
   static constexpr double skip = 1e-18;
   static constexpr double big = 1e8;
   static constexpr double tiny = 1e-30;
-  static constexpr double rank = 1e-24;
+  static constexpr double rank = 3.2e-30;
   static constexpr double perp = 0.6;
 };
 
