@@ -61,9 +61,14 @@ typedef struct pdsc_config {
   int32_t num_layers;        /* 12 in the released snapshots (ctor default 6)            */
   int32_t num_channels;      /* 128 (only value supported by the kernels)                */
   int32_t num_iterations;    /* power-iteration cap, 10                                  */
-  float ratio;               /* seeds = int(N * ratio), 0.1                              */
-  float inlier_threshold;    /* hypothesis scoring threshold; also selects the refinement
-                                threshold: 0.10 iff == 0.10f else 1.2 (PointDSC.py:415)   */
+  double ratio;              /* seeds: the length of range(N)[:int(N * ratio)], 0.1; any
+                                finite value (a ratio above 1 takes every row, a negative
+                                one drops the last -int(N * ratio)); pdsc_create refuses
+                                a NaN or infinite ratio                                   */
+  double inlier_threshold;   /* hypothesis scoring threshold, compared in float32 as the
+                                reference's tensors are; also selects the refinement
+                                threshold: 0.10 iff == 0.10 exactly, else 1.2
+                                (PointDSC.py:415)                                         */
   float sigma_d;             /* initial value of the `sigma_spat` buffer; a loaded
                                 state dict overrides it, as in the reference              */
   int32_t k;                 /* neighbourhood size of the NSM module, 40                 */
@@ -132,7 +137,7 @@ int pdsc_set_precision(pdsc_engine* e, int32_t precision);
 int pdsc_set_batch_invariant(pdsc_engine* e, int32_t enable);
 
 /* ---- sizes ------------------------------------------------------------------------------------- */
-int32_t pdsc_num_seeds(const pdsc_engine* e, int32_t N);       /* S = int(N * ratio)          */
+int32_t pdsc_num_seeds(const pdsc_engine* e, int32_t N);       /* S = len(range(N)[:int(N * ratio)]) */
 int32_t pdsc_num_neighbours(const pdsc_engine* e, int32_t N);  /* k = min(cfg.k, N - 1)       */
 size_t pdsc_workspace_bytes(const pdsc_engine* e, int32_t B, int32_t N);
 

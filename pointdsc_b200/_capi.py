@@ -31,7 +31,7 @@ PDSC_ERR_SHAPE = 3
 class Config(C.Structure):
     _fields_ = [
         ("in_dim", C.c_int32), ("num_layers", C.c_int32), ("num_channels", C.c_int32),
-        ("num_iterations", C.c_int32), ("ratio", C.c_float), ("inlier_threshold", C.c_float),
+        ("num_iterations", C.c_int32), ("ratio", C.c_double), ("inlier_threshold", C.c_double),
         ("sigma_d", C.c_float), ("k", C.c_int32), ("nms_radius", C.c_float),
         ("precision", C.c_int32), ("device", C.c_int32),
     ]

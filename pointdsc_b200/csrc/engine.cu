@@ -290,9 +290,9 @@ void copy_tap(void* dst, const void* src, size_t bytes, cudaStream_t st) {
   if (dst && bytes) cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st);
 }
 
-float refinement_threshold(float ctor_threshold) {
-  // `if self.inlier_threshold == 0.10` (PointDSC.py:415): Python compares the ctor double with 0.10
-  return (std::fabs((double)ctor_threshold - 0.10) < 1e-7) ? 0.10f : 1.2f;
+float refinement_threshold(double ctor_threshold) {
+  // `if self.inlier_threshold == 0.10` (PointDSC.py:415): Python compares the ctor double with 0.10, exactly
+  return ctor_threshold == 0.10 ? 0.10f : 1.2f;
 }
 
 int encoder_simt(const pdsc_engine* e, const Workspace& w, const CallShape& sh, const float* corr_pos, const pdsc_stage_io* io,
@@ -359,7 +359,7 @@ __global__ void set_table_kernel(const int32_t* __restrict__ offsets, int N_unif
       row0 = offsets ? offsets[b] : b * N_uniform;
       N = offsets ? offsets[b + 1] - row0 : N_uniform;
     }
-    const int S = (int)((double)N * ratio);          // int(num_corr * self.ratio), as pdsc_num_seeds
+    const int S = pdsc::num_seeds(N, ratio);         // as pdsc_num_seeds
     const int k = live ? max(min(k_cfg, N - 1), 0) : 0;
     const int QT = (N + 127) / 128, KT = (N + 63) / 64;
     int sp = 1, TS = KT;
@@ -405,6 +405,7 @@ int pdsc_create(const pdsc_config* cfg, pdsc_engine** out) {
   if (cfg->num_iterations < 1 || cfg->num_iterations > pdsc::kMaxIters)
     return fail(PDSC_ERR_UNSUPPORTED, "num_iterations must be in [1,%d]", pdsc::kMaxIters);
   if (cfg->k < 1 || cfg->k > pdsc::kMaxK) return fail(PDSC_ERR_UNSUPPORTED, "k must be in [1,%d]", pdsc::kMaxK);
+  if (!std::isfinite(cfg->ratio)) return fail(PDSC_ERR_INVALID_ARGUMENT, "ratio must be finite, got %g", cfg->ratio);
   if (cfg->precision < PDSC_FP32_SIMT || cfg->precision > PDSC_FP16X3)
     return fail(PDSC_ERR_INVALID_ARGUMENT, "unknown precision %d", cfg->precision);
   int ndev = 0;
@@ -532,8 +533,8 @@ int pdsc_commit_params(pdsc_engine* e) {
 
 int32_t pdsc_num_seeds(const pdsc_engine* e, int32_t N) {
   if (!e || N < 0) return 0;
-  // int(num_corr * self.ratio) in double precision, as Python evaluates it (PointDSC.py:174)
-  return (int32_t)((double)N * (double)e->cfg.ratio);
+  // the length of argsort(...)[:, 0:int(num_corr * self.ratio)] (PointDSC.py:174, :217)
+  return pdsc::num_seeds(N, e->cfg.ratio);
 }
 int32_t pdsc_num_neighbours(const pdsc_engine* e, int32_t N) {
   if (!e) return 0;
@@ -596,7 +597,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
   const int NS = round_up(N, 64);
   const int S = sh.S, k = sh.k, T = e->cfg.num_iterations;
   const SetDesc* sets = w.sets;
-  set_table_kernel<<<1, 32, 0, st>>>(d_offsets, N, B, (double)e->cfg.ratio, e->cfg.k, e->cfg.precision == PDSC_FP32_SIMT ? 0 : 1,
+  set_table_kernel<<<1, 32, 0, st>>>(d_offsets, N, B, e->cfg.ratio, e->cfg.k, e->cfg.precision == PDSC_FP32_SIMT ? 0 : 1,
                                      sh.attn_split, sh.attn_invariant, device_sm_count(), w.sets, w.tile_set);
   const float* W = e->d_weights;
   const int L = e->cfg.num_layers;
@@ -703,7 +704,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
     // ---- a10 + a11 --------------------------------------------------------------------------------
     launch_seed_hypotheses(d_src, d_tgt, w.knn, w.iterates, w.conv_mask, io ? io->in_seed_trans : nullptr, w.seed_trans,
                            w.counts, w.best_key, io ? io->out_eig : nullptr, io ? io->out_power_iters : nullptr, B, N, S,
-                           k, T, e->cfg.inlier_threshold, mask_stride, st, sets);
+                           k, T, (float)e->cfg.inlier_threshold, mask_stride, st, sets);
     if (io) {
       copy_tap(io->out_seed_trans, w.seed_trans, (size_t)B * S * 16 * sizeof(float), st);
       copy_tap(io->out_inlier_counts, w.counts, (size_t)B * S * sizeof(int32_t), st);
@@ -718,7 +719,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
   // ---- a11 (labels) + a12 ---------------------------------------------------------------------------
   launch_select_refine(d_src, d_tgt, w.seed_trans, w.best_key, d_final_trans, mode == 0 ? d_final_labels : nullptr,
                        io ? io->out_init_trans : nullptr, io ? io->out_best : nullptr,
-                       io ? io->out_refine_solves : nullptr, B, N, S, e->cfg.inlier_threshold,
+                       io ? io->out_refine_solves : nullptr, B, N, S, (float)e->cfg.inlier_threshold,
                        refinement_threshold(e->cfg.inlier_threshold), mode == 0 ? 20 : 0, st, sets);
   if (mode == 1) {
     PDSC_CUDA(cudaMemcpyAsync(d_final_labels, w.conf, R * sizeof(float), cudaMemcpyDeviceToDevice, st));

@@ -11,7 +11,7 @@ namespace pdsc {
 
 struct SetDesc {
   int row0;        // first row of the set in the call's [R] arrays
-  int N, S, k;     // correspondences, seeds S = int(N ratio), neighbours k = min(cfg.k, N - 1)
+  int N, S, k;     // correspondences, seeds S = num_seeds(N, ratio), neighbours k = min(cfg.k, N - 1)
   int qt0, kt0;    // first 128-query tile / 64-key tile of the set in the Q / KV operand images
   int seed0;       // first seed slot of the set ([sum S] arrays)
   int item0;       // first attention work item of the set
@@ -21,6 +21,18 @@ struct SetDesc {
   long long dist0; // first float of the set's seed-row distance block [S][N] (a multiple of 4)
   long long knn0;  // first neighbour slot of the set ([sum S k] arrays; iterates are `iters` times that)
 };
+
+// Seeds of a set of N rows: the length of the slice argsort(...)[:, 0:int(N * ratio)] the reference takes (PointDSC.py:174,
+// :176, :217), the product and the truncation in double as Python evaluates them.  With m = int(N * ratio) that is min(m, N)
+// for m >= 0 and max(N + m, 0) for m < 0: a ratio above 1 takes every row, a negative one drops the last -m.  The product is
+// clamped to [-N, N] before the conversion, so no ratio makes it undefined; a NaN ratio gives 0 (pdsc_create refuses one).
+__host__ __device__ __forceinline__ int num_seeds(int N, double ratio) {
+  const double x = (double)N * ratio;
+  if (!(x > -(double)N)) return 0;                   // m <= -N (or NaN)
+  if (x >= (double)N) return N;                      // m >= N
+  const int m = (int)x;                              // truncation toward zero, as int()
+  return m >= 0 ? m : N + m;
+}
 
 // Key split of the tensor-core attention for ONE set of N rows in a call of the small regime (encoder_tc.cu): sp chunks of TS key
 // tiles, a function of N and the SM count only.  sp == 1 (TS == KT): not split.

@@ -214,7 +214,10 @@ class PointDSC(nn.Module):
         return {n: (float(ms[i]), int(cnt[i])) for i, n in enumerate(_capi.SPANS)}
 
     def num_seeds(self, N: int) -> int:
-        return int(N * self.ratio)
+        """Seeds of a set of N correspondences: the length of the reference's slice argsort(...)[:, 0:int(N * ratio)]
+        (PointDSC.py:174, :217), as pdsc_num_seeds computes it."""
+        m = int(N * self.ratio)
+        return min(m, N) if m >= 0 else max(N + m, 0)
 
     # ------------------------------------------------------------------------------------------
     # the path

@@ -28,9 +28,14 @@ def test_library_builds_and_exports_every_header_symbol():
     assert b"sm_90a" in _capi.load().pdsc_version()
 
 
-def test_struct_layouts_match_the_header():
+def test_config_with_double_ratio_and_stage_io_layouts_match_the_header():
     from pointdsc_b200 import _capi
-    assert ctypes.sizeof(_capi.Config) == 11 * 4
+    # 4 int32, the doubles ratio and inlier_threshold, then 5 four-byte fields and 4 bytes of tail padding
+    assert dict(_capi.Config._fields_)["ratio"] is ctypes.c_double
+    assert dict(_capi.Config._fields_)["inlier_threshold"] is ctypes.c_double
+    assert ctypes.sizeof(_capi.Config) == 56
+    assert _capi.Config.ratio.offset == 16 and _capi.Config.inlier_threshold.offset == 24
+    assert _capi.Config.sigma_d.offset == 32 and _capi.Config.device.offset == 48
     # 5 injection + 14 tap pointers, int32 layer_tap (+4 pad), 3 pointers
     assert ctypes.sizeof(_capi.StageIO) == 19 * 8 + 8 + 24
     assert _capi.StageIO.layer_tap.offset == 19 * 8

@@ -130,10 +130,12 @@ class Conv:
 _convs = {}
 
 
-def layer_convs(dataset, precision, l):
+def layer_convs(dataset, precision, l, sd=None):
+    """Layer l's folded convolutions of the state dict sd (default: the dataset's snapshot; `dataset` names sd in the
+    cache)."""
     key = (dataset, precision, l)
     if key not in _convs:
-        sd = load_snapshot(dataset)
+        sd = load_snapshot(dataset) if sd is None else sd
         pc, nl = f"encoder.blocks.PointCN_layer_{l}", f"encoder.blocks.NonLocal_layer_{l}"
         _convs[key] = {
             "w1": Conv(sd, pc + ".0", pc + ".1", 1.0, precision),
@@ -364,22 +366,25 @@ def check(kernel, precision, got, want, bound, where):
     note(kernel, precision, err, bound)
 
 
-def run_case(dataset, precision, B, N, layers, sets, qrows=None, invariant=False, seed=0):
+def run_case(dataset, precision, B, N, layers, sets, qrows=None, invariant=False, seed=0, model=None, sd=None, args=None):
     """Runs B sets of N correspondences and checks, at every layer in `layers`, PCQ, KV, the attention and MSG on the rows of
-    `sets` (qrows: the query rows within a set the attention is checked at, default all).  Returns (split, [(sp, TS)])."""
+    `sets` (qrows: the query rows within a set the attention is checked at, default all).  Returns (split, [(sp, TS)]).
+    model / sd: the module and the state dict it holds (default: the dataset's 12-layer snapshot model; `dataset` then names
+    sd in the weight cache); args: the call's device inputs (default: synthetic pairs of the dataset's geometry)."""
     from pointdsc_b200.synth import make_pair
-    m = get_model(dataset, precision, invariant)
+    m = get_model(dataset, precision, invariant) if model is None else model
     sms = sm_count()
-    pairs = [make_pair(10000 * seed + 17 * N + b, N, dataset, 0.3 + 0.4 * (b % 3) / 2) for b in range(B)]
-    args = [torch.stack([p[x] for p in pairs]).cuda() for x in ("corr_pos", "src_keypts", "tgt_keypts")]
+    if args is None:
+        pairs = [make_pair(10000 * seed + 17 * N + b, N, dataset, 0.3 + 0.4 * (b % 3) / 2) for b in range(B)]
+        args = [torch.stack([p[x] for p in pairs]).cuda() for x in ("corr_pos", "src_keypts", "tgt_keypts")]
     if precision == "fp32":
         split, per = False, [(1, -(-N // 64))] * B
     else:
         split, per = call_split([N] * B, sms, invariant)
         enc = m.launches_per_forward(B, N) - 12
-        assert enc == 2 + (5 if split else 4) * 12, (enc, split)   # the engine ran the regime restated here
+        assert enc == 2 + (5 if split else 4) * m.num_layers, (enc, split)   # the engine ran the regime restated here
     qrows = np.arange(N) if qrows is None else np.asarray(qrows)
-    sd = load_snapshot(dataset)
+    sd = load_snapshot(dataset) if sd is None else sd
     sc_all = m.run(*args, taps=["sc"])["sc"]
     scs = {b: sc_all[b][torch.from_numpy(qrows).cuda()].cpu().numpy() for b in sets}
     del sc_all
@@ -391,7 +396,7 @@ def run_case(dataset, precision, B, N, layers, sets, qrows=None, invariant=False
         if l > 0 and l - 1 not in prev:
             p = m.run(*args, taps=["layer_features"], layer_tap=l - 1)["layer_features"]
             prev[l - 1] = {b: p[b].cpu().numpy() for b in sets}
-        cv = layer_convs(dataset, precision, l)
+        cv = layer_convs(dataset, precision, l, sd)
         feats = {}
         for b in sets:
             dbg = out["layer_debug"][:, b].cpu().numpy()          # feat1, q, k, v, msg [N,C]

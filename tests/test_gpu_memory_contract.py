@@ -64,7 +64,7 @@ SETDESC_BYTES = 72              # sets.cuh SetDesc: 12 int32 + 3 int64
 TSI = 8                         # sets.cuh kAttnInvariantTiles
 SPLIT_MAX_ITEMS = 320           # encoder_tc.cu kAttnSplitMaxItems
 PARTIAL_BYTES = 65536 + 1024    # encoder_tc.cu kAttnPartialBytes
-RATIO32 = float(np.float32(0.1))   # cfg.ratio is a float; the engine widens it to double
+RATIO = 0.1                     # cfg.ratio
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -165,7 +165,8 @@ def tc_packed_split(Ns, invariant, sms):
 
 
 def num_seeds(N):
-    return int(N * RATIO32)
+    m = int(N * RATIO)                  # sets.cuh num_seeds: the length of range(N)[:m]
+    return min(m, N) if m >= 0 else max(N + m, 0)
 
 
 def mirror_workspace(Ns, precision, invariant, k_cfg, sms, iters=10):
