@@ -5,8 +5,7 @@ import pytest
 import torch
 
 import evaluate
-from test_evaluate_packed_host import _PackedModel, _fake_packed
-from test_mixed_batch_host import _fake_pipeline
+from fakes import _PackedModel, _fake_packed, _fake_pipeline
 
 
 def _fake_icp(monkeypatch, log):

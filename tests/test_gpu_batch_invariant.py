@@ -13,43 +13,13 @@ import pytest
 import torch
 
 from conftest import golden_cases, load_case, registration_ok
+from engine_rules import PARTIAL_BYTES, SPLIT_MAX_ITEMS
+from gpu_models import as_batch, get_model, synth_sets
 
 pytestmark = pytest.mark.gpu
 
 PRECISIONS = list(dict.fromkeys(os.environ.get("PDSC_TEST_PRECISIONS", "fp32,fp16x3").split(",") + ["bf16x3"]))
 TAPS = ["features", "seeds", "best"]
-PARTIAL_BYTES = 65536 + 1024      # one split work item's partial O and (m, l) (encoder_tc.cu)
-
-_models = {}
-
-
-def get_model(precision, invariant=True, dataset="3dmatch", k=40, fresh=False):
-    from conftest import load_snapshot
-    from oracle import pointdsc_oracle as O
-    from pointdsc_b200 import PointDSC
-    key = (precision, invariant, dataset, k)
-    if fresh or key not in _models:
-        cfg = O.default_config(dataset)
-        m = PointDSC(in_dim=6, num_layers=12, num_channels=128, num_iterations=10, ratio=0.1,
-                     inlier_threshold=cfg["inlier_threshold"], sigma_d=cfg["sigma_d"], k=k,
-                     nms_radius=cfg["nms_radius"], precision=precision, batch_invariant=invariant)
-        m.load_state_dict(load_snapshot(dataset), strict=False)
-        m = m.cuda().eval()
-        if fresh:
-            return m
-        _models[key] = m
-    return _models[key]
-
-
-def synth_sets(sizes, seed0=0):
-    from pointdsc_b200.synth import make_pair
-    return [make_pair(seed0 + i, n, "3dmatch", 0.3) for i, n in enumerate(sizes)]
-
-
-def as_batch(pairs):
-    return {"corr_pos": torch.stack([p["corr_pos"] for p in pairs]).cuda(),
-            "src_keypts": torch.stack([p["src_keypts"] for p in pairs]).cuda(),
-            "tgt_keypts": torch.stack([p["tgt_keypts"] for p in pairs]).cuda(), "testing": True}
 
 
 def args(b):
@@ -58,11 +28,11 @@ def args(b):
 
 def invariant_tiles():
     """Key tiles per split of the invariant rule, read back from the workspace of one set of N = 16384 (KT = 256)."""
-    m_def, m_inv = get_model("fp16x3", False), get_model("fp16x3", True)
+    m_def, m_inv = get_model(precision="fp16x3"), get_model(precision="fp16x3", invariant=True)
     lib = m_def._ensure_engine()
     m_inv._ensure_engine()
     diff = int(lib.pdsc_workspace_bytes(m_inv._engine, 1, 16384)) - int(lib.pdsc_workspace_bytes(m_def._engine, 1, 16384))
-    items = diff // PARTIAL_BYTES + 320
+    items = diff // PARTIAL_BYTES + SPLIT_MAX_ITEMS
     assert diff % PARTIAL_BYTES == 0 and items % 128 == 0, diff
     return 256 // (items // 128)
 
@@ -73,14 +43,14 @@ def edge_sizes():
     return sorted({2, 7, 41, 257, 1000, 1003, 2000, 5000, 16384, 64 * tsi, 64 * tsi + 1, 128 * tsi + 1})
 
 
-def assert_same(a, b, what):
+def assert_equal(a, b, what):
     for key in a:
         assert torch.equal(a[key].cpu(), b[key].cpu()), (what, key)
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)
 def test_single_uniform_and_mixed_calls_agree(precision):
-    m = get_model(precision)
+    m = get_model(precision=precision, invariant=True)
     sizes = edge_sizes()
     pairs = synth_sets(sizes, seed0=500)
     uni = synth_sets([1000] * 64, seed0=900)
@@ -92,7 +62,7 @@ def test_single_uniform_and_mixed_calls_agree(precision):
     ub = m.run(*args(as_batch(uni)), taps=TAPS)
     for i in picks:
         row = {k: ub[k][i:i + 1] for k in ["final_trans", "final_labels"] + TAPS}
-        assert_same(uni_singles[i], row, ("uniform", i))
+        assert_equal(uni_singles[i], row, ("uniform", i))
     # one mixed call: the edge sizes interleaved with the uniform sets
     order = []
     for j in range(max(len(pairs), len(uni))):
@@ -106,12 +76,12 @@ def test_single_uniform_and_mixed_calls_agree(precision):
             ref = {"final_trans": singles[j]["final_trans"], "final_labels": singles[j]["final_labels"]}
         else:
             ref = {"final_trans": ub["final_trans"][j:j + 1], "final_labels": ub["final_labels"][j:j + 1]}
-        assert_same(ref, {"final_trans": o["final_trans"], "final_labels": o["final_labels"]}, ("mixed", kind, j))
+        assert_equal(ref, {"final_trans": o["final_trans"], "final_labels": o["final_labels"]}, ("mixed", kind, j))
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)
 def test_permuted_batch(precision):
-    m = get_model(precision)
+    m = get_model(precision=precision, invariant=True)
     pairs = synth_sets([1003] * 16, seed0=300)
     perm = np.random.default_rng(1).permutation(16)
     a = m.run(*args(as_batch(pairs)), taps=TAPS)
@@ -124,41 +94,41 @@ def test_permuted_batch(precision):
     x = m.forward_many([as_batch([p]) for p in mixed])
     y = m.forward_many([as_batch([mixed[i]]) for i in perm])
     for pos, i in enumerate(perm):
-        assert_same({k: x[i][k] for k in ("final_trans", "final_labels")},
+        assert_equal({k: x[i][k] for k in ("final_trans", "final_labels")},
                     {k: y[pos][k] for k in ("final_trans", "final_labels")}, ("mixed permuted", i))
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)
 def test_every_entry_point(precision):
     """Device (eager), graph replay, host (graph and eager), forward_stream, forward_many and forward() on the same sets."""
-    m = get_model(precision)
+    m = get_model(precision=precision, invariant=True)
     pairs = synth_sets([1000] * 40, seed0=700)
     eager = [m.run(*args(as_batch([p])), taps=["best"]) for p in pairs[:3]]
     ref = [{"final_trans": e["final_trans"], "final_labels": e["final_labels"]} for e in eager]
     for _ in range(2):   # capture, then replay
         for r, p in zip(ref, pairs[:3]):
-            assert_same(r, m.run(*args(as_batch([p]))), "graph")
+            assert_equal(r, m.run(*args(as_batch([p]))), "graph")
     for r, p in zip(ref, pairs[:3]):
         b = as_batch([p])
-        assert_same(r, m({k: v for k, v in b.items()}), "forward")
-        assert_same(r, m.run(*(x.cpu() for x in args(b))), "host, graph")
+        assert_equal(r, m({k: v for k, v in b.items()}), "forward")
+        assert_equal(r, m.run(*(x.cpu() for x in args(b))), "host, graph")
     big = as_batch(pairs)                                     # 40 000 rows: the host path's eager branch
     host = m.run(*(x.cpu() for x in args(big)))
     for i, r in enumerate(ref):
-        assert_same(r, {k: v[i:i + 1] for k, v in host.items()}, ("host, eager", i))
+        assert_equal(r, {k: v[i:i + 1] for k, v in host.items()}, ("host, eager", i))
     stream_in = [{k: (v.cpu().pin_memory() if k != "testing" else v) for k, v in as_batch([p]).items()} for p in pairs[:3]]
     for r, o in zip(ref, m.forward_stream(iter(stream_in))):
-        assert_same(r, {"final_trans": o["final_trans"], "final_labels": o["final_labels"]}, "forward_stream")
+        assert_equal(r, {"final_trans": o["final_trans"], "final_labels": o["final_labels"]}, "forward_stream")
     many = m.forward_many([as_batch([p]) for p in pairs[:3]])
     for r, o in zip(ref, many):
-        assert_same(r, {"final_trans": o["final_trans"], "final_labels": o["final_labels"]}, "forward_many")
+        assert_equal(r, {"final_trans": o["final_trans"], "final_labels": o["final_labels"]}, "forward_many")
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)
 def test_run_eval_logits_and_M_at_bs1_equal_batch_of_8(precision):
     """The validation forward: logits and M per set.  Its transform depends on the batch by design (the early exit of the
     power iteration spans the batch, reference PointDSC.py:176), so it is not compared."""
-    m = get_model(precision)
+    m = get_model(precision=precision, invariant=True)
     pairs = synth_sets([1000] * 8, seed0=800)
     batch = m.run_eval(*args(as_batch(pairs)))
     for i in (0, 5, 7):
@@ -175,7 +145,7 @@ def _dump(path, precisions):
     out = {}
     pairs = synth_sets(SM_SIZES, seed0=1200)
     for prec in precisions:
-        m = get_model(prec)
+        m = get_model(precision=prec, invariant=True)
         for n, p in zip(SM_SIZES, pairs):
             r = m.run(*args(as_batch([p])), taps=TAPS)
             for k, v in r.items():
@@ -215,7 +185,7 @@ def test_golden_fixtures_in_invariant_fp16x3():
         groups.setdefault((c["meta"]["dataset"], int(c["meta"].get("k", 40))), []).append(c)
     assert len(groups) >= 2
     for (dataset, k), cases in groups.items():
-        m = get_model("fp16x3", True, dataset, k)
+        m = get_model(dataset, "fp16x3", k=k, invariant=True)
         for c in cases:
             b = {key: torch.from_numpy(np.ascontiguousarray(c[key])).cuda()[None] for key in ("corr_pos", "src_keypts", "tgt_keypts")}
             o = m.run(*args(b))
@@ -231,7 +201,7 @@ def test_golden_fixtures_in_invariant_fp16x3():
 
 
 def test_fp32_flag_changes_nothing():
-    on, off = get_model("fp32", True), get_model("fp32", False)
+    on, off = get_model(precision="fp32", invariant=True), get_model(precision="fp32")
     lib = on._ensure_engine()
     off._ensure_engine()
     for B, N in ((1, 1000), (256, 1000), (1, 16384)):
@@ -240,8 +210,8 @@ def test_fp32_flag_changes_nothing():
     pairs = synth_sets([1000, 5000, 41], seed0=1300)
     for p in pairs:
         b = as_batch([p])
-        assert_same(off.run(*args(b), taps=TAPS), on.run(*args(b), taps=TAPS), "fp32 eager")
-        assert_same(off.run(*args(b)), on.run(*args(b)), "fp32 graph")
+        assert_equal(off.run(*args(b), taps=TAPS), on.run(*args(b), taps=TAPS), "fp32 eager")
+        assert_equal(off.run(*args(b)), on.run(*args(b)), "fp32 graph")
     for x, y in zip(off.forward_many([as_batch([p]) for p in pairs]), on.forward_many([as_batch([p]) for p in pairs])):
         assert torch.equal(x["final_trans"], y["final_trans"]) and torch.equal(x["final_labels"], y["final_labels"])
 
@@ -249,7 +219,7 @@ def test_fp32_flag_changes_nothing():
 def test_launch_count_reports_the_merges():
     """12 layers: the invariant mode merges wherever a set has more than TSI key tiles, whatever the call."""
     tsi = invariant_tiles()
-    inv, dft = get_model("fp16x3", True), get_model("fp16x3", False)
+    inv, dft = get_model(precision="fp16x3", invariant=True), get_model(precision="fp16x3")
     lib = inv._ensure_engine()
     dft._ensure_engine()
 
@@ -263,8 +233,8 @@ def test_launch_count_reports_the_merges():
 
 @pytest.mark.parametrize("precision", ["fp16x3"])
 def test_toggling_the_mode_on_one_module(precision):
-    m = get_model(precision, False, fresh=True)
-    fresh = {False: get_model(precision, False, fresh=True), True: get_model(precision, True, fresh=True)}
+    m = get_model(precision=precision, fresh=True)
+    fresh = {mode: get_model(precision=precision, invariant=mode, fresh=True) for mode in (False, True)}
     p = synth_sets([5000], seed0=1400)[0]
     b = as_batch([p])
     host = [x.cpu() for x in args(b)]
@@ -275,10 +245,10 @@ def test_toggling_the_mode_on_one_module(precision):
         m.set_batch_invariant(mode)
         assert m.batch_invariant is mode
         eager = m.run(*args(b), taps=["features"])
-        assert_same(want[mode][0], eager, ("eager", mode))
-        assert_same(want[mode][1], m.run(*args(b)), ("graph", mode))
-        assert_same(want[mode][1], m.run(*args(b)), ("graph replay", mode))
-        assert_same(want[mode][2], m.run(*host), ("host", mode))
+        assert_equal(want[mode][0], eager, ("eager", mode))
+        assert_equal(want[mode][1], m.run(*args(b)), ("graph", mode))
+        assert_equal(want[mode][1], m.run(*args(b)), ("graph replay", mode))
+        assert_equal(want[mode][2], m.run(*host), ("host", mode))
 
 
 def test_evaluate_groups_equal_single_pairs_in_invariant_mode():

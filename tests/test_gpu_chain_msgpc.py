@@ -9,25 +9,20 @@ The split only moves arithmetic between kernels, so what the taps do must not ch
 - a mixed-size call in the batch-invariant mode gives each set what a call holding it alone gives;
 - results do not depend on what the workspace held (the in-place feat1 update under every poison of the memory contract);
 - feat1(l + 1), from layer_debug at layer l + 1, is PointCN(l + 1) of layer_features at layer l within the float64 bound of
-  test_gpu_encoder.conv_bound.
+  float64_bounds.conv_bound.
 """
 import numpy as np
 import pytest
 import torch
 
-from test_gpu_encoder import check, conv_bound, get_model, layer_convs
-from test_gpu_memory_contract import Call, check_patterns
+from buffer_guards import Call, check_patterns
+from float64_bounds import check, conv_bound, layer_convs
+from gpu_models import get_model, same
 
 pytestmark = pytest.mark.gpu
 
 PRECISIONS = ["fp16x3", "bf16x3", "bf16"]
 TAP_LAYERS = [0, 5, 10, 11]
-
-
-def same(a, b):
-    """Byte equality (NaN-safe)."""
-    a, b = a.contiguous(), b.contiguous()
-    return a.shape == b.shape and a.dtype == b.dtype and torch.equal(a.view(torch.uint8), b.view(torch.uint8))
 
 
 def batch(Ns, seed, dataset="3dmatch"):

@@ -7,7 +7,7 @@ in_dim 8 and a generic loop above, and the seed count S follows the reference's 
 
   (a) Layer counts L in {1, 2, 6, 13, 64}, all four precisions: layer i holds layer i mod 12 of the 3DMatch snapshot, so every
       operand has a trained scale.  PCQ / Q, KV, the attention (+ merge) and MSG / MSGPC are checked against float64 within
-      the bounds of test_gpu_encoder.py, in both attention regimes (bs = 1 at N = 1000 splits the keys, B = 64 at N = 300
+      the bounds of float64_bounds.py, in both attention regimes (bs = 1 at N = 1000 splits the keys, B = 64 at N = 300
       does not); then the end-to-end result against the oracle and the batch against its single-set calls.  Repeating the
       snapshot's layers grows the features from block to block: beyond the first repetition the logits grow until the
       attention's a-posteriori bound is vacuous (its relative logit factor above 1/2: at layer 31 of 64 on an H100, and
@@ -35,18 +35,15 @@ import numpy as np
 import pytest
 import torch
 
-import test_gpu_encoder as E
 from conftest import load_snapshot
+from engine_rules import C_CH, num_seeds
+from float64_bounds import (ALL_PRECISIONS, E_KNN, WORST, check_power, check_sets, check_transforms, run_case,
+                            weighted_kabsch64)
+from gpu_models import get_model, release_all, sm_count
 from oracle import pointdsc_oracle as O
 
-C_CH = 128
 SNAP_LAYERS = 12
 PDSC_ERR_INVALID_ARGUMENT = 1
-
-
-def slice_seeds(N, ratio):
-    """The reference's seed count: the length of argsort(...)[:int(N * ratio)] (PointDSC.py:174, :217)."""
-    return len(range(N)[:int(N * ratio)])
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -71,30 +68,17 @@ def stretched_state(L, in_dim=6, seed=0):
     return sd
 
 
-_models = {}
+_states = {}
 
 
-def get_model(precision="fp32", L=SNAP_LAYERS, in_dim=6, ratio=0.1, inlier_threshold=0.10, invariant=False):
-    """(module, state dict, name of the state dict in test_gpu_encoder's weight cache)."""
-    from pointdsc_b200 import PointDSC
-    key = (precision, L, in_dim, ratio, inlier_threshold, invariant)
-    if key not in _models:
-        cfg = O.default_config("3dmatch")
-        sd = stretched_state(L, in_dim)
-        m = PointDSC(in_dim=in_dim, num_layers=L, num_channels=C_CH, num_iterations=10, ratio=ratio,
-                     inlier_threshold=inlier_threshold, sigma_d=cfg["sigma_d"], k=40, nms_radius=cfg["nms_radius"],
-                     precision=precision, batch_invariant=invariant)
-        res = m.load_state_dict(sd, strict=False)
-        assert res.missing_keys == [] and res.unexpected_keys == ["gamma"]
-        _models[key] = (m.cuda().eval(), sd, f"config-L{L}-in{in_dim}")
-    return _models[key]
-
-
-def release_models():
-    for m, _, _ in _models.values():
-        m._release()
-    _models.clear()
-    torch.cuda.empty_cache()
+def config_model(precision="fp32", L=SNAP_LAYERS, in_dim=6, ratio=0.1, inlier_threshold=0.10, invariant=False):
+    """(module, state dict, name of the state dict in float64_bounds' weight cache)."""
+    name = f"config-L{L}-in{in_dim}"
+    if name not in _states:
+        _states[name] = stretched_state(L, in_dim)
+    m = get_model(precision=precision, invariant=invariant, num_layers=L, in_dim=in_dim, ratio=ratio,
+                  inlier_threshold=inlier_threshold, weights=(name, _states[name]))
+    return m, _states[name], name
 
 
 def oracle_cfg(L=SNAP_LAYERS, ratio=0.1, inlier_threshold=0.10):
@@ -152,8 +136,8 @@ def per_layer_launches(precision, split):
 
 
 def summary(tag):
-    for key in sorted(E.WORST):
-        print(f"{tag}: {key[0]} ({key[1]}) worst error / bound so far {E.WORST[key]:.3g}")
+    for key in sorted(WORST):
+        print(f"{tag}: {key[0]} ({key[1]}) worst error / bound so far {WORST[key]:.3g}")
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -166,15 +150,15 @@ REGIMES = [(1, 1000), (64, 300)]      # bs = 1: the key-split attention; B = 64:
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("precision", E.ALL_PRECISIONS)
+@pytest.mark.parametrize("precision", ALL_PRECISIONS)
 @pytest.mark.parametrize("L", sorted(LAYERS_CHECKED))
 def test_layer_count_against_float64(L, precision):
-    m, sd, name = get_model(precision, L)
-    ref12, _, _ = get_model(precision, SNAP_LAYERS)
-    sms = E.sm_count()
+    m, sd, name = config_model(precision, L)
+    ref12, _, _ = config_model(precision, SNAP_LAYERS)
+    sms = sm_count()
     for B, N in REGIMES:
-        sets = [0] if B == 1 else E.check_sets(B, N)
-        split, per = E.run_case(name, precision, B, N, LAYERS_CHECKED[L], sets, model=m, sd=sd, args=regime_inputs(B, N, L))
+        sets = [0] if B == 1 else check_sets(B, N)
+        split, per = run_case(name, precision, B, N, LAYERS_CHECKED[L], sets, model=m, sd=sd, args=regime_inputs(B, N, L))
         if precision != "fp32" and sms >= 132:
             assert split == (B == 1), (B, N, split)                 # both attention regimes are reached
         # each layer adds its chain launches, the attention and (split) its merge, and nothing else
@@ -196,7 +180,7 @@ def regime_inputs(B, N, L):
 @pytest.mark.parametrize("precision", ["fp32", "fp16x3"])
 @pytest.mark.parametrize("L", [1, 2, 6, 13])
 def test_layer_count_end_to_end(L, precision):
-    m, sd, _ = get_model(precision, L)
+    m, sd, _ = config_model(precision, L)
     cp, s, t, gt = pair_inputs([900 + L, 901 + L], 1000, 6, 0.5)
     out = m.run(cp.cuda(), s.cuda(), t.cuda())
     compared = check_vs_oracle(out, sd, oracle_cfg(L), cp, s, t, gt, f"L={L}")
@@ -219,14 +203,14 @@ IN_DIMS = [1, 3, 6, 8, 9, 12, 64]      # layer0_kernel: registers for in_dim <= 
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("precision", E.ALL_PRECISIONS)
+@pytest.mark.parametrize("precision", ALL_PRECISIONS)
 @pytest.mark.parametrize("in_dim", IN_DIMS)
 def test_input_width_against_float64(in_dim, precision):
     """Layer 0 (float64 within gamma(in_dim + 1) sum |terms|, carried into PCQ's bound) and layer 1 as in (a); end to end
     against the oracle in fp32 and fp16x3."""
-    m, sd, name = get_model(precision, SNAP_LAYERS, in_dim)
+    m, sd, name = config_model(precision, SNAP_LAYERS, in_dim)
     cp, s, t, gt = pair_inputs([700 + in_dim, 701 + in_dim], 1000, in_dim, 0.5)
-    E.run_case(name, precision, 1, 1000, [0, 1], [0], model=m, sd=sd, args=[x[:1].cuda() for x in (cp, s, t)])
+    run_case(name, precision, 1, 1000, [0, 1], [0], model=m, sd=sd, args=[x[:1].cuda() for x in (cp, s, t)])
     if precision in ("fp32", "fp16x3"):
         out = m.run(cp.cuda(), s.cuda(), t.cuda())
         compared = check_vs_oracle(out, sd, oracle_cfg(), cp, s, t, gt, f"in_dim={in_dim}")
@@ -239,7 +223,7 @@ def test_input_width_against_float64(in_dim, precision):
 def test_host_path_at_odd_widths(in_dim):
     """pdsc_forward_host and the submit / wait pair equal the device path bit for bit where R * in_dim is odd, so that the
     slot's src_keypts starts 4-byte aligned only: a graphed size and an eager one (R above the 32,768 graph rows)."""
-    m, _, _ = get_model("fp16x3", SNAP_LAYERS, in_dim)
+    m, _, _ = config_model("fp16x3", SNAP_LAYERS, in_dim)
     for B, N in ((1, 1001), (3, 16383)):
         assert (B * N * in_dim) % 2 == 1
         cp, s, t, _ = pair_inputs(range(60 + B, 60 + 2 * B), N, in_dim, 0.5)
@@ -251,7 +235,7 @@ def test_host_path_at_odd_widths(in_dim):
         for got in [host] + streamed:
             assert torch.equal(got["final_trans"], devo["final_trans"].cpu()), (in_dim, B, N)
             assert torch.equal(got["final_labels"], devo["final_labels"].cpu()), (in_dim, B, N)
-    release_models()
+    release_all()
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -266,7 +250,7 @@ def test_seed_rule_is_the_slice(ratio):
     from pointdsc_b200 import PointDSC
     m = PointDSC(num_layers=1, ratio=ratio)
     for N in list(range(0, 2049)) + [16383, 16384]:
-        assert m.num_seeds(N) == slice_seeds(N, ratio), (N, ratio)
+        assert m.num_seeds(N) == num_seeds(N, ratio), (N, ratio)
     assert PointDSC(num_layers=1, ratio=0.7).num_seeds(10) == 7 == int(10 * 0.7)
     assert int(10 * float(np.float32(0.7))) == 6                  # what a float32 ratio gives
 
@@ -290,7 +274,7 @@ def test_num_seeds_sweep_and_non_finite_ratios():
             got = np.array([lib.pdsc_num_seeds(h, int(n)) for n in Ns])
         finally:
             lib.pdsc_destroy(h)
-        want = np.array([slice_seeds(int(n), ratio) for n in Ns])
+        want = np.array([num_seeds(int(n), ratio) for n in Ns])
         bad = Ns[got != want]
         assert bad.size == 0, (ratio, bad.size, bad[:5].tolist(), got[got != want][:5].tolist())
     for ratio in (math.nan, math.inf, -math.inf):
@@ -317,8 +301,8 @@ RATIO_CASES = [(0.7, 10), (0.7, 1000), (0.35, 20), (1.0, 1000), (1.5, 1000), (-0
 @pytest.mark.gpu
 @pytest.mark.parametrize("ratio,N", RATIO_CASES)
 def test_seed_ratio_forward_vs_oracle(ratio, N):
-    m, sd, _ = get_model("fp32", ratio=ratio)
-    S = slice_seeds(N, ratio)
+    m, sd, _ = config_model("fp32", ratio=ratio)
+    S = num_seeds(N, ratio)
     assert S != int(N * float(np.float32(ratio))) or ratio in (1.0, 1.5, -0.1)   # float32 would change S, or a new range
     cfg = oracle_cfg(ratio=ratio)
     cp, s, t, gt = pair_inputs([300 + N], N, 6, 0.5)
@@ -343,7 +327,7 @@ def test_seed_ratio_forward_vs_oracle(ratio, N):
 def test_ratio_zero_takes_no_seeds():
     """S = 0: no power iteration, the identity is the initial transform, the labels are its inliers and the refinement starts
     from it (the reference itself cannot score zero hypotheses)."""
-    m, _, _ = get_model("fp32", ratio=0.0)
+    m, _, _ = config_model("fp32", ratio=0.0)
     cp, s, t, _ = pair_inputs([808], 1000, 6, 0.5)
     t = t.clone()
     t[0, :500] = s[0, :500] + 0.02 * torch.randn(500, 3, generator=torch.Generator().manual_seed(8))   # inliers of the identity
@@ -362,7 +346,7 @@ def test_ratio_zero_takes_no_seeds():
 @pytest.mark.parametrize("ratio", [1.0, 1.5])
 def test_validation_seeds_are_every_row(ratio):
     """The validation forward's seeds at ratio >= 1: all N rows, in confidence order (ties by index)."""
-    m, _, _ = get_model("fp32", ratio=ratio)
+    m, _, _ = config_model("fp32", ratio=ratio)
     N = 300
     cp, s, t, _ = pair_inputs([41, 42], N, 6, 0.5)
     out = m.run_eval(cp.cuda(), s.cuda(), t.cuda(), want_M=False, taps=["seeds"])
@@ -381,8 +365,8 @@ def test_refinement_switch_is_an_exact_comparison():
     cp, s, t, gt = pair_inputs([606], 1000, 6, 0.5)
     args = [x.cuda() for x in (cp, s, t)]
     taps = ["inlier_counts", "init_trans", "refine_solves"]
-    a = get_model("fp32", inlier_threshold=near)[0].run(*args, taps=taps)
-    b = get_model("fp32", inlier_threshold=0.10)[0].run(*args, taps=taps)
+    a = config_model("fp32", inlier_threshold=near)[0].run(*args, taps=taps)
+    b = config_model("fp32", inlier_threshold=0.10)[0].run(*args, taps=taps)
     assert torch.equal(a["inlier_counts"], b["inlier_counts"]) and torch.equal(a["init_trans"], b["init_trans"])
     init = a["init_trans"][0].cpu()
     refs = {}
@@ -396,19 +380,17 @@ def test_refinement_switch_is_an_exact_comparison():
     (T12, n12), (T10, n10) = refs[1.2], refs[0.10]
     assert n12 != n10 or float((T12 - T10).abs().max()) > 1e-3
     # and the oracle's whole forward at 0.1 + 1e-9 agrees where it registers the pair
-    sd = get_model("fp32", inlier_threshold=near)[1]
+    sd = config_model("fp32", inlier_threshold=near)[1]
     assert check_vs_oracle(a, sd, oracle_cfg(inlier_threshold=near), cp, s, t, gt, "near 0.10") == 1
 
 
 @pytest.mark.gpu
 def test_every_row_a_seed_at_16384():
     """fp16x3, ratio 1, N = 16384: 16,384 seeds (a 1 GiB seed-row distance block).  kNN and the hypotheses of 64 sampled seeds
-    and the power iteration of all of them against float64 (the rules of test_gpu_stages.py and test_gpu_kabsch.py)."""
-    import test_gpu_kabsch as KB
-    import test_gpu_stages as ST
-    release_models()
+    and the power iteration of all of them against float64 (the rules of float64_bounds.py)."""
+    release_all()
     N, k = 16384, 40
-    m, _, _ = get_model("fp16x3", ratio=1.0)
+    m, _, _ = config_model("fp16x3", ratio=1.0)
     cp, s, t, _ = pair_inputs([4242], N, 6, 0.3)
     out = m.run(cp.cuda(), s.cuda(), t.cuda(),
                 taps=["normed", "seeds", "knn_idx", "compat", "eig", "power_iters", "seed_trans"])
@@ -423,16 +405,16 @@ def test_every_row_a_seed_at_16384():
     order = np.argsort(dist, axis=1, kind="stable")
     ref = order[:, 1:k + 1]
     d_got, d_ref = np.take_along_axis(dist, got, 1), np.take_along_axis(dist, ref, 1)
-    assert np.abs(d_got - d_ref).max() <= 2 * ST.E_KNN
+    assert np.abs(d_got - d_ref).max() <= 2 * E_KNN
     full = np.take_along_axis(dist, order[:, :k + 2], 1)
-    sep = (full[:, 1:k + 1] - full[:, 0:k] > 2 * ST.E_KNN) & (full[:, 2:k + 2] - full[:, 1:k + 1] > 2 * ST.E_KNN)
+    sep = (full[:, 1:k + 1] - full[:, 0:k] > 2 * E_KNN) & (full[:, 2:k + 2] - full[:, 1:k + 1] > 2 * E_KNN)
     assert sep.mean() > 0.2 and np.array_equal(got[sep], ref[sep])
     compat = out["compat"][0].cpu().numpy().reshape(N, k, k)
     eig = out["eig"][0].cpu().numpy().reshape(N, k)
-    ratio, band, sure = ST.check_power(compat, eig, int(out["power_iters"][0]), k, 10)
+    ratio, band, sure = check_power(compat, eig, int(out["power_iters"][0]), k, 10)
     src, tgt = s[0].double().numpy(), t[0].double().numpy()
     e = eig[pick].astype(np.float64)
-    kab = KB.weighted_kabsch64(src[got], tgt[got], e / (e.sum(1, keepdims=True) + 1e-6))
-    KB.check_transforms(out["seed_trans"][0].cpu().numpy()[pick], kab, "seed_trans N=16384 S=16384")
+    kab = weighted_kabsch64(src[got], tgt[got], e / (e.sum(1, keepdims=True) + 1e-6))
+    check_transforms(out["seed_trans"][0].cpu().numpy()[pick], kab, "seed_trans N=16384 S=16384")
     print(f"N=S=16384: power iteration worst error / bound {ratio:.3g} (band {band:.3g}), exit compared: {sure}")
-    release_models()
+    release_all()

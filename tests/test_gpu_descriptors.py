@@ -6,26 +6,23 @@ import pytest
 import torch
 
 from conftest import load_snapshot
+from gpu_models import dev
 from oracle import fpfh_oracle as F
 from pointdsc_b200.synth_scene import rigid, scene
 
 pytestmark = pytest.mark.gpu
 
 
-def _dev(x, dtype=torch.float32):
-    return torch.as_tensor(x, dtype=dtype, device="cuda")
-
-
 @pytest.mark.parametrize("n,voxel,offset", [(20000, 0.05, 0.0), (6000, 0.1, 0.0), (5000, 0.3, -40.0), (1, 0.05, 0.0), (300000, 0.025, 3.0)])
 def test_voxel_down_sample_vs_oracle(n, voxel, offset):
     from pointdsc_b200.descriptors import voxel_down_sample
     pts = scene(max(n, 40), seed=n)[:n] + np.float32(offset)
-    got = voxel_down_sample(_dev(pts), voxel).cpu().numpy()
+    got = voxel_down_sample(dev(pts, torch.float32), voxel).cpu().numpy()
     want, keys = F.voxel_down_sample(pts, voxel)
     assert got.shape == want.shape                        # same occupied voxels (the index arithmetic is bit-exact fp64)
     # means: fp64 sum / count on the CPU, 2^-40-voxel fixed point on the device, both rounded to float32 at the end
     assert np.abs(got.astype(np.float64) - want).max() <= 1.0 * np.spacing(np.float32(np.abs(want).max()))
-    again = voxel_down_sample(_dev(pts[::-1].copy()), voxel).cpu().numpy()
+    again = voxel_down_sample(dev(pts[::-1].copy(), torch.float32), voxel).cpu().numpy()
     assert np.array_equal(got, again)                     # the result does not depend on the input order (integer accumulation)
 
 
@@ -35,16 +32,16 @@ def test_voxel_status_is_loud():
     pts = scene(1000, seed=0)
     pts[17, 1] = np.nan
     with pytest.raises(PdscError):
-        voxel_down_sample(_dev(pts), 0.05)
+        voxel_down_sample(dev(pts, torch.float32), 0.05)
     with pytest.raises(PdscError):
-        voxel_down_sample(_dev(scene(1000, seed=0)), 1e-7)          # > 2^21 voxels along an axis
+        voxel_down_sample(dev(scene(1000, seed=0), torch.float32), 1e-7)          # > 2^21 voxels along an axis
     with pytest.raises(PdscError):
         voxel_down_sample(torch.zeros(10, 3), 0.05)                 # CPU tensor: no fallback
 
 
 def _keypoints(n, voxel, seed):
     from pointdsc_b200.descriptors import voxel_down_sample
-    return voxel_down_sample(_dev(scene(n, seed=seed)), voxel)
+    return voxel_down_sample(dev(scene(n, seed=seed), torch.float32), voxel)
 
 
 @pytest.mark.parametrize("n,voxel,max_nn", [(6000, 0.1, 30), (20000, 0.05, 30), (3000, 0.2, 7), (6000, 0.1, 100)])
@@ -70,7 +67,7 @@ def test_normals_vs_oracle(n, voxel, max_nn):
 def test_normals_below_three_neighbours():
     from pointdsc_b200.descriptors import estimate_normals
     pts = np.array([[0, 0, 0], [10, 0, 0], [10.05, 0, 0], [20, 0, 0], [20.05, 0, 0], [20, 0.05, 0.01]], np.float32)
-    got = estimate_normals(_dev(pts), 0.2, 30).cpu().numpy()
+    got = estimate_normals(dev(pts, torch.float32), 0.2, 30).cpu().numpy()
     want = F.estimate_normals(pts, 0.2, 30)
     assert np.array_equal(got[:3], np.tile([0.0, 0.0, 1.0], (3, 1)))
     assert np.allclose(got, want, atol=1e-9)
@@ -97,7 +94,7 @@ def test_fpfh_isolated_points_and_duplicates():
     rng = np.random.default_rng(0)
     pts = np.concatenate([rng.uniform(0, 1, (300, 3)), [[50, 50, 50]], rng.uniform(0, 1, (5, 3)) + 100]).astype(np.float32)
     pts[10] = pts[11]                                            # a duplicate: distance 0, skipped by the weighted sum
-    kp = _dev(pts)
+    kp = dev(pts, torch.float32)
     nrm = estimate_normals(kp, 0.3, 30)
     got = compute_fpfh(kp, nrm, 0.6, 100).cpu().numpy()
     want = F.fpfh(pts, nrm.cpu().numpy(), 0.6, 100)
@@ -110,7 +107,7 @@ def test_neighbourhood_overflow_is_loud():
     from pointdsc_b200.descriptors import estimate_normals
     pts = np.random.default_rng(0).uniform(0, 0.1, (6000, 3)).astype(np.float32)
     with pytest.raises(PdscError):
-        estimate_normals(_dev(pts), 1.0, 30)                      # 6000 points inside every radius > 4096
+        estimate_normals(dev(pts, torch.float32), 1.0, 30)                      # 6000 points inside every radius > 4096
 
 
 def test_descriptor_chain_registers_a_synthetic_pair(tmp_path):
@@ -164,7 +161,7 @@ def test_reference_fixture_of_the_demo_pair(precision):
     model = PointDSC(in_dim=6, num_layers=12, num_channels=128, num_iterations=10, ratio=0.1, inlier_threshold=0.10, sigma_d=0.10,
                      k=40, nms_radius=0.10, precision=precision).cuda().eval()
     model.load_state_dict(load_snapshot("3dmatch"), strict=False)
-    d = [_dev(z[k])[None] for k in ("corr_pos", "src_keypts", "tgt_keypts")]
+    d = [dev(z[k], torch.float32)[None] for k in ("corr_pos", "src_keypts", "tgt_keypts")]
     for batch in (1, 3):                      # bs = 1 (key-split attention) and a small batch (unsplit)
         out = model.run(*[x.repeat(batch, 1, 1) for x in d], taps=["best", "seeds"])
         dT = np.abs(out["final_trans"][batch - 1].cpu().numpy() - z["final_trans"]).max()

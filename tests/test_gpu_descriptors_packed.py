@@ -8,16 +8,13 @@ import numpy as np
 import pytest
 import torch
 
-from test_gpu_memory_contract import FLOAT_WORD, PATTERNS, assert_same, guarded_input, guarded_output, run_guarded, scratch_buffer, tiled
+from buffer_guards import FLOAT_WORD, PATTERNS, assert_same, guarded_input, guarded_output, run_guarded, scratch_buffer, tiled
+from gpu_models import dev
 from pointdsc_b200.synth_scene import rigid, scene
 
 pytestmark = pytest.mark.gpu
 
 VOXEL = 0.08
-
-
-def _dev(x, dtype=torch.float32):
-    return torch.as_tensor(np.ascontiguousarray(x), dtype=dtype, device="cuda")
 
 
 def group_clouds():
@@ -46,7 +43,7 @@ def search_packed(kind, pts, offsets, radius, max_nn, normals=None, normalise=0)
     capi, lib, e = _lib()
     P = len(offsets) - 1
     h = (C.c_int32 * (P + 1))(*offsets)
-    d_off = _dev(offsets, torch.int32)
+    d_off = dev(offsets, torch.int32)
     m = offsets[-1]
     out = torch.empty(m, 3 if kind == "normals" else 33, dtype=torch.float64, device="cuda")
     status = torch.empty(P, dtype=torch.int32, device="cuda")
@@ -63,7 +60,7 @@ def search_packed(kind, pts, offsets, radius, max_nn, normals=None, normalise=0)
 
 def single_chain(cloud, normalise):
     from pointdsc_b200.descriptors import compute_fpfh, estimate_normals, voxel_down_sample
-    kp = voxel_down_sample(_dev(cloud), VOXEL)
+    kp = voxel_down_sample(dev(cloud, torch.float32), VOXEL)
     nrm = estimate_normals(kp, 2 * VOXEL, 30)
     return kp, nrm, compute_fpfh(kp, nrm, 5 * VOXEL, 100, normalise=normalise)
 
@@ -72,7 +69,7 @@ def single_chain(cloud, normalise):
 def test_every_cloud_is_bit_identical_to_the_single_cloud_calls(normalise):
     from pointdsc_b200.descriptors import fpfh_descriptors, fpfh_descriptors_many
     clouds = group_clouds()
-    kp, feat, off, d_off = fpfh_descriptors_many([_dev(c) for c in clouds], VOXEL, normalise=normalise)
+    kp, feat, off, d_off = fpfh_descriptors_many([dev(c, torch.float32) for c in clouds], VOXEL, normalise=normalise)
     assert d_off.dtype == torch.int32 and d_off.cpu().tolist() == off and len(off) == len(clouds) + 1
     assert kp.dtype == torch.float32 and feat.dtype == torch.float64 and tuple(feat.shape) == (off[-1], 33)
     nrm, st = search_packed("normals", kp, off, 2 * VOXEL, 30)
@@ -85,7 +82,7 @@ def test_every_cloud_is_bit_identical_to_the_single_cloud_calls(normalise):
         assert torch.equal(nrm[rows], s_nrm), p
         assert torch.equal(feat[rows], s_feat), p
         if normalise:
-            assert torch.equal(feat[rows], fpfh_descriptors(_dev(c), VOXEL)[1]), p
+            assert torch.equal(feat[rows], fpfh_descriptors(dev(c, torch.float32), VOXEL)[1]), p
         counts.append(off[p + 1] - off[p])
     assert counts[0] == 1 and counts[1] == 1                                   # the 1-point cloud, the one-voxel cloud
     assert counts[2] == counts[3] and torch.equal(feat[off[2]:off[3]], feat[off[3]:off[4]])
@@ -96,9 +93,9 @@ def test_every_cloud_is_bit_identical_to_the_single_cloud_calls(normalise):
 def test_permuting_the_clouds_permutes_the_outputs():
     from pointdsc_b200.descriptors import fpfh_descriptors_many
     clouds = group_clouds()
-    kp, feat, off, _ = fpfh_descriptors_many([_dev(c) for c in clouds], VOXEL)
+    kp, feat, off, _ = fpfh_descriptors_many([dev(c, torch.float32) for c in clouds], VOXEL)
     perm = [5, 2, 0, 4, 1, 3]
-    kp2, feat2, off2, _ = fpfh_descriptors_many([_dev(clouds[q]) for q in perm], VOXEL)
+    kp2, feat2, off2, _ = fpfh_descriptors_many([dev(clouds[q], torch.float32) for q in perm], VOXEL)
     for i, q in enumerate(perm):
         assert torch.equal(kp2[off2[i]:off2[i + 1]], kp[off[q]:off[q + 1]]), (i, q)
         assert torch.equal(feat2[off2[i]:off2[i + 1]], feat[off[q]:off[q + 1]]), (i, q)
@@ -110,22 +107,23 @@ def test_status_lands_on_the_offending_cloud_only():
     bad = scene(1000, seed=4)
     bad[17, 1] = np.nan
     with pytest.raises(PdscError, match="cloud 1:"):
-        fpfh_descriptors_many([_dev(scene(1000, seed=5)), _dev(bad), _dev(scene(900, seed=6))], VOXEL)
+        fpfh_descriptors_many([dev(scene(1000, seed=5), torch.float32), dev(bad, torch.float32),
+                               dev(scene(900, seed=6), torch.float32)], VOXEL)
     # the 4096-candidate overflow on the search of one cloud, next to clean ones
     rng = np.random.default_rng(1)
     sparse = [rng.uniform(0, 100, (n, 3)).astype(np.float32) for n in (300, 70)]
     dense = rng.uniform(0, 0.1, (6000, 3)).astype(np.float32)
     group = [sparse[0], dense, sparse[1]]
     off = np.cumsum([0] + [len(c) for c in group]).tolist()
-    pts = _dev(np.concatenate(group))
+    pts = dev(np.concatenate(group), torch.float32)
     nrm, st = search_packed("normals", pts, off, 1.0, 30)
     assert st == [0, 2, 0]
     _, st2 = search_packed("fpfh", pts, off, 1.0, 30, normals=nrm)
     assert st2 == [0, 2, 0]
     for p in (0, 2):
-        assert torch.equal(nrm[off[p]:off[p + 1]], estimate_normals(_dev(group[p]), 1.0, 30)), p
+        assert torch.equal(nrm[off[p]:off[p + 1]], estimate_normals(dev(group[p], torch.float32), 1.0, 30)), p
     with pytest.raises(PdscError):
-        estimate_normals(_dev(dense), 1.0, 30)
+        estimate_normals(dev(dense, torch.float32), 1.0, 30)
 
 
 def _voxel_packed_guarded(clouds, pat):
@@ -207,9 +205,9 @@ def test_packed_descriptors_register_a_pair_as_the_per_cloud_chain():
     model = PointDSC(in_dim=6, num_layers=12, num_channels=128, num_iterations=10, ratio=0.1, inlier_threshold=0.10, sigma_d=0.10,
                      k=40, nms_radius=0.10).cuda().eval()
     model.load_state_dict(load_snapshot("3dmatch"), strict=False)
-    kp, feat, off, _ = fpfh_descriptors_many([_dev(src), _dev(tgt)], VOXEL)
+    kp, feat, off, _ = fpfh_descriptors_many([dev(src, torch.float32), dev(tgt, torch.float32)], VOXEL)
     packed = (feat[off[0]:off[1]], feat[off[1]:off[2]], kp[off[0]:off[1]], kp[off[1]:off[2]])
-    (skp, sf), (tkp, tf) = fpfh_descriptors(_dev(src), VOXEL), fpfh_descriptors(_dev(tgt), VOXEL)
+    (skp, sf), (tkp, tf) = fpfh_descriptors(dev(src, torch.float32), VOXEL), fpfh_descriptors(dev(tgt, torch.float32), VOXEL)
     res = []
     for pair in (packed, (sf, tf, skp, tkp)):
         m = match_many([pair])
@@ -233,7 +231,7 @@ def test_bad_offsets_are_refused():
     for offsets in ([0], [1, 50, 100], [0, 50, 50, 100], [0, 60, 50, 100]):
         P = len(offsets) - 1
         h = (C.c_int32 * len(offsets))(*offsets)
-        d = _dev(offsets, torch.int32)
+        d = dev(offsets, torch.int32)
         assert lib.pdsc_voxel_down_sample_packed_scratch_bytes(P, h) == 0, offsets
         assert lib.pdsc_fpfh_packed_scratch_bytes(P, h, 30) == 0, offsets
         rcs = (lib.pdsc_voxel_down_sample_packed(e, P, h, p(d), p(pts), VOXEL, p(pts), p(d_out), p(status), p(sc), sc.numel(), None),

@@ -6,10 +6,10 @@ check this file's own float64 helpers and bounds on the CPU.
 
 Several kernels choose a launch path from the shapes, the pointer or the SM count: the matcher's column-chunk count and
 its fp64 shared-memory opt-in, the compaction's passes, the power iteration's rows per CTA R, its bulk-copy path and its
-tile ring, the search's bitonic size P.  Every test recomputes the kernel's choice (`match_plan`, `eig_plan`,
-`search_plan`) and asserts that it reached the path it targets.
+tile ring, the search's bitonic size P.  Every test recomputes the kernel's choice (engine_rules.py: `match_plan`,
+`eig_plan`, `search_plan`) and asserts that it reached the path it targets.
 
-Error model (test_gpu_stages.py's, u = 2^-24 for fp32 and 2^-53 for fp64, gamma(n) = n u / (1 - n u)):
+Error model (float64_bounds.py's, u = 2^-24 for fp32 and 2^-53 for fp64, gamma(n) = n u / (1 - n u)):
   * inputs are exact in float64; every reference below is float64 on the kernel's own fp32 / fp64 inputs;
   * a sum of n terms in any order, fma or not, is within gamma(n) sum |terms| of the exact sum;
   * sqrt, division and a single add / multiply add one rounding (u relative) each; CUDA's acosf adds 2 ulp.
@@ -22,19 +22,17 @@ import numpy as np
 import pytest
 import torch
 
+from buffer_guards import (RE_THRE, TE_THRE, check_network_input, keypoints, match_descriptors, mean_candidates, run_match,
+                           stats_case, surface)
+from engine_rules import CAND_CAP, EIG_COLS, EIG_ROWS, MATCH_MAX_CHUNKS, eig_plan, match_plan, search_plan
+from float64_bounds import U, U64, check_power, gamma, gamma64
+from gpu_models import sm_count
 from oracle import fpfh_oracle as F
 from oracle import frontend_oracle as FO
 from oracle import metrics_oracle as MO
-from test_gpu_stages import check_power, gamma, sm_count
 
-U = 2.0 ** -24
-U64 = 2.0 ** -53
 GOLDEN_FRONT = ["frontend_fcgf32_n300_m0", "frontend_fcgf32_n300_m1", "frontend_fpfh33_n500_m0", "frontend_fpfh33_n500_m1",
                 "frontend_ties_n64_m0"]
-
-
-def gamma64(n):
-    return n * U64 / (1.0 - n * U64)
 
 
 def golden(name):
@@ -58,20 +56,11 @@ def golden(name):
 MATCH_PAIRS = [(1, 1), (1, 5000), (5000, 1), (2, 63), (63, 2), (64, 65), (65, 64), (127, 128), (128, 129), (129, 127),
                (1023, 1025), (1025, 1024), (1024, 1023), (2, 5000), (5000, 64), (5000, 5000), (129, 4091)]
 MATCH_D = [("fp32", d) for d in (1, 15, 16, 17, 32, 48, 64)] + [("fp64", d) for d in (1, 17, 33, 38, 39, 64)]
-MATCH_MAX_CHUNKS = 32
 
 
 def match_err(x, S, D, fp64):
     u, g = (U64, gamma64(D)) if fp64 else (U, gamma(D))
     return 2 * g * S + 2.01 * u * (x + 2 * g * S) + u * 1e-6 + 2 * gamma64(D) * S + 2.01 * U64 * x
-
-
-def match_plan(rows, cols, D, fp64, sms):
-    """(chunks, columns per chunk, dynamic shared memory) of one nearest_columns launch (frontend.cu)."""
-    tt = 32 if fp64 else 64
-    chunks = min(max(-(-4 * sms // -(-rows // 128)), 1), MATCH_MAX_CHUNKS)
-    per = -(-(-(-cols // chunks)) // tt) * tt
-    return -(-cols // per), per, (8 if fp64 else 4) * D * (128 + tt)
 
 
 def nearest64(a, b, fp64, probe=None):
@@ -110,63 +99,6 @@ def nearest64(a, b, fp64, probe=None):
     return want, sure, single, ok, worst
 
 
-def match_descriptors(rng, ns, nt, D, dtype):
-    """Sources near random targets; among the targets and the sources a few exact copies and (D > 1) copies one ulp away in
-    one channel, which no float64 argmin can separate from their original."""
-    unit = lambda f: f / np.linalg.norm(f, axis=1, keepdims=True)      # noqa: E731
-    if D == 1:
-        t, s = rng.uniform(-1, 1, (nt, 1)), rng.uniform(-1, 1, (ns, 1))
-    else:
-        t = unit(rng.standard_normal((nt, D)))
-        s = unit(t[rng.integers(0, nt, ns)] + 0.3 / math.sqrt(D) * rng.standard_normal((ns, D)))
-    t, s = t.astype(dtype), s.astype(dtype)
-    for f in (t, s):
-        n = len(f)
-        if n >= 4:
-            k = max(1, n // 30)
-            f[rng.choice(n, k, replace=False)] = f[rng.integers(0, n, k)]
-            if D > 1:
-                dst, src = rng.choice(n, k, replace=False), rng.integers(0, n, k)
-                f[dst] = f[src]
-                c = rng.integers(0, D, k)
-                f[dst, c] = np.nextafter(f[dst, c], dtype(2))
-    return s, t
-
-
-def run_match(sd, td, sk, tk, mutual):
-    from pointdsc_b200.frontend import match
-    d = lambda x: torch.from_numpy(np.ascontiguousarray(x)).cuda()      # noqa: E731
-    out = match(d(sd), d(td), d(sk), d(tk), use_mutual=mutual)
-    return {"corr": out["corr"].cpu().numpy(), "corr_pos": out["corr_pos"][0].cpu().numpy(),
-            "src": out["src_keypts"][0].cpu().numpy(), "tgt": out["tgt_keypts"][0].cpu().numpy()}
-
-
-def mean_candidates(col, exact):
-    """The fp32 means the kernel may form for one column of corr_pos: an fp64 sum in any order (within gamma64(M) sum |v|),
-    divided by M (one rounding) and rounded to fp32; `exact`: the fp64 sum is exact (dyadic inputs), one candidate."""
-    x = col.astype(np.float64)
-    mean = math.fsum(x) / len(x)
-    if exact:
-        return [np.float32(mean)]
-    d = gamma64(len(x)) * np.abs(x).sum() / len(x) + 4 * U64 * abs(mean)
-    out, hi = [np.float32(mean - d)], np.float32(mean + d)
-    while out[-1] < hi:
-        out.append(np.nextafter(out[-1], np.float32(np.inf)))
-    return out
-
-
-def check_network_input(out, sk, tk, exact):
-    """Exact gathers, and corr_pos = fl32(v - m32) bit for bit for one admissible fp32 mean m32 per column."""
-    corr = out["corr"]
-    assert np.array_equal(out["src"], sk[corr[:, 0]]) and np.array_equal(out["tgt"], tk[corr[:, 1]])
-    if len(corr) == 0:
-        return
-    v = np.concatenate([sk[corr[:, 0]], tk[corr[:, 1]]], 1)
-    for c in range(6):
-        cands = mean_candidates(v[:, c], exact)
-        assert any(np.array_equal(out["corr_pos"][:, c], v[:, c] - m) for m in cands), (c, cands)
-
-
 def check_match(sd, td, sk, tk, outs, exact_mean=False):
     """outs: {mutual: kernel output}.  Returns (rows whose index is determined, rows, worst ratio)."""
     fp64 = sd.dtype == np.float64
@@ -197,10 +129,6 @@ def check_match(sd, td, sk, tk, outs, exact_mean=False):
     for out in outs.values():
         check_network_input(out, sk, tk, exact_mean)
     return int(sure_r.sum()), ns, worst
-
-
-def keypoints(rng, n):
-    return rng.uniform(-3, 3, (n, 3)).astype(np.float32)
 
 
 @pytest.mark.gpu
@@ -306,22 +234,9 @@ def test_match_network_input_across_compaction_passes(grid):
 # gamma(N) w_j of w = M64 v_t; the norm sums N rounded squares of those (3 gamma(N + 1) relative), the square root halves
 # that and adds u, the add of fl(1e-6) and the division add u each, the float64 reference 4 gamma64(N):
 #   |v_t+1 - normalise(w)| <= (1.01 (gamma(N) + 1.5 gamma(N + 1) + 4 u) + 4 gamma64(N)) normalise(w)     per entry.
-# The whole run at the cap goes through test_gpu_stages.check_power with k = N (its Hilbert-metric bound and exit rule).
+# The whole run at the cap goes through float64_bounds.check_power with k = N (its Hilbert-metric bound and exit rule).
 # Measured on an H100 (80GB HBM3, 700 W): worst one-step error / bound = 0.13 (1.5e-4 at N = 24576); whole run / check_power's
 # bound 0.011.
-EIG_ROWS, EIG_COLS = 32, 512
-
-
-def eig_plan(B, N, ptr, sms):
-    """launch_leading_eigenvector's choices: R and its regime, CTAs per set, the bulk-copy path, tiles, rows of the last CTA."""
-    R, regime = EIG_ROWS, "waves"
-    if B * -(-N // EIG_ROWS) < 4 * sms:
-        raw = -(-(B * N) // (2 * sms))
-        R = min(max(raw, 8), EIG_ROWS)
-        regime = "clamp8" if raw < 8 else ("clamp32" if raw > EIG_ROWS else ("mid" if 8 < R < EIG_ROWS else "edge"))
-    nparts = -(-N // R)
-    return {"R": R, "regime": regime, "tma": N % 4 == 0 and ptr % 16 == 0, "ntiles": -(-N // EIG_COLS),
-            "last_rows": N - (nparts - 1) * R}
 
 
 def eig_cases(sms):
@@ -499,7 +414,6 @@ def test_leading_eigenvector_per_set_exit():
 # the final fp32 rounding u.  Counts and the ratios of exact fp32 integers are exact.
 # Measured on an H100 (80GB HBM3, 700 W): worst RE / TE / RMSE error / bound = 0.49 / 0.62 / 0.22.
 STATS_N = [1, 31, 255, 256, 257, 5000, 2 ** 20]
-RE_THRE, TE_THRE = 15.0, 25.0
 
 
 def stats64(pred, gt, src, tgt, pl, gl):
@@ -542,57 +456,6 @@ def stats64(pred, gt, src, tgt, pl, gl):
         exact[:, 8] = np.where(2 * tp + fp + fn > 0, f(2) * f(tp) / (f(2) * f(tp) + f(fp) + f(fn)), 0)
     return {"re": re, "re_tol": re_tol, "te": te, "te_tol": te_tol, "rmse": rmse, "rmse_tol": rmse_tol, "exact": exact,
             "clamp": (c_raw + dc < -1) | (c_raw - dc > 1), "den0": np.stack([tp + fp == 0, tp + fn == 0, 2 * tp + fp + fn == 0], 1)}
-
-
-def rotations(rng, n):
-    q, r = np.linalg.qr(rng.standard_normal((n, 3, 3)))
-    q *= np.sign(np.diagonal(r, axis1=1, axis2=2))[:, None, :]
-    q[np.linalg.det(q) < 0, :, 0] *= -1
-    return q
-
-
-def axis_rotation(axis, ang):
-    a = axis / np.linalg.norm(axis)
-    K = np.array([[0, -a[2], a[1]], [a[2], 0, -a[0]], [-a[1], a[0], 0]])
-    return np.eye(3) + math.sin(ang) * K + (1 - math.cos(ang)) * K @ K
-
-
-def stats_case(rng, B, N):
-    """B sets of N correspondences; from B >= 8 the first sets are the constructed edges: pred == gt (a signed permutation),
-    a 180 degree relative rotation with the clamp active, TE == te_thre exactly, and the label edges (pred all <= 0 with
-    exact +0 and -0, pred all > 0, gt all zero, gt all zero with pred all <= 0, gt all one)."""
-    Rg = rotations(rng, B)
-    gt = np.tile(np.eye(4), (B, 1, 1))
-    gt[:, :3, :3], gt[:, :3, 3] = Rg, rng.uniform(-1, 1, (B, 3))
-    ang = rng.uniform(0, 30, B) * math.pi / 180
-    pred = gt.copy()
-    for b in range(B):
-        pred[b, :3, :3] = Rg[b] @ axis_rotation(rng.standard_normal(3), ang[b])
-    pred[:, :3, 3] += rng.standard_normal((B, 3)) * rng.uniform(0, 0.2, (B, 1))
-    gt, pred = gt.astype(np.float32), pred.astype(np.float32)
-    src = rng.uniform(-2, 2, (B, N, 3)).astype(np.float32)
-    inl = rng.uniform(size=(B, N)) < rng.uniform(0.05, 0.9, (B, 1))
-    tgt = np.einsum("bck,bnk->bnc", gt[:, :3, :3].astype(np.float64), src) + gt[:, None, :3, 3]
-    tgt = np.where(inl[..., None], tgt + 0.01 * rng.standard_normal(tgt.shape), rng.uniform(-2, 2, tgt.shape)).astype(np.float32)
-    gl = inl.astype(np.float32)
-    pl = rng.standard_normal((B, N)).astype(np.float32)
-    pl[:, ::7], pl[:, 3::11] = 0.0, -0.0
-    if B >= 8:
-        perm = np.array([[0, -1, 0], [0, 0, 1], [-1, 0, 0]], np.float32)
-        gt[0, :3, :3] = pred[0, :3, :3] = perm
-        pred[0, :3, 3] = gt[0, :3, 3]
-        # 180 degrees, scaled by 1 + 2^-12 as a nearly orthonormal estimate may be: the trace lies below -1 in any rounding
-        pred[1, :3, :3] = Rg[1] @ axis_rotation(rng.standard_normal(3), math.pi) * (1 + 2.0 ** -12)
-        gt[2, :3, :3] = pred[2, :3, :3] = np.eye(3, dtype=np.float32)
-        gt[2, :3, 3] = 0.0
-        pred[2, :3, 3] = (TE_THRE / 100, 0.0, 0.0)                        # 0.25 m: TE = 25 cm exactly
-        pl[3] = -np.abs(pl[3])
-        pl[4] = np.abs(pl[4]) + 1.0
-        gl[5] = 0.0
-        gl[6], pl[6] = 0.0, -np.abs(pl[6])
-        pl[[3, 6], ::5] = 0.0                                               # +0 and -0 beside negatives: none kept
-        gl[7] = 1.0
-    return pred, gt, src, tgt, pl, gl
 
 
 def check_stats(got, ref):
@@ -646,23 +509,6 @@ def test_eval_stats_against_float64(n):
 # 2.7e-6 (lattice), 2.4e-5 (4096 candidates); worst FPFH error / bound = 0.015.
 C_NORMAL = 8.0
 SEARCH_MAX_NN = [1, 2, 31, 32, 33, 64, 65, 128, 129, 255, 256]
-CAND_CAP = 4096
-
-
-def search_plan(max_nn):
-    """(P, warps per CTA) of launch_hybrid_search."""
-    P = 2
-    while P < max_nn:
-        P <<= 1
-    per_warp = P * 8 + 1024 + CAND_CAP * 8
-    return P, min(8, 200 * 1024 // per_warp)
-
-
-def surface(rng, m):
-    """m points on a smooth, gently curved patch of the unit square (continuous: no ties, no bin-edge features)."""
-    xy = rng.uniform(0, 1, (m, 2))
-    z = 0.1 * np.sin(3 * xy[:, 0]) * np.cos(2 * xy[:, 1]) + 0.002 * rng.standard_normal(m)
-    return np.concatenate([xy, z[:, None]], 1).astype(np.float32)
 
 
 def check_normals(got, pts, radius, max_nn):

@@ -6,25 +6,10 @@ import ctypes as C
 import pytest
 import torch
 
-from conftest import load_snapshot
+from gpu_models import get_model
+from pointdsc_b200.model import DEFAULT_PRECISION
 
 pytestmark = pytest.mark.gpu
-
-_model = None
-
-
-def get_model():
-    global _model
-    if _model is None:
-        from oracle import pointdsc_oracle as O
-        from pointdsc_b200 import PointDSC
-        cfg = O.default_config("3dmatch")
-        m = PointDSC(in_dim=6, num_layers=12, num_channels=128, num_iterations=10, ratio=0.1,
-                     inlier_threshold=cfg["inlier_threshold"], sigma_d=cfg["sigma_d"], k=40, nms_radius=cfg["nms_radius"])
-        m.load_state_dict(load_snapshot("3dmatch"), strict=False)
-        _model = m.cuda().eval()
-    return _model
-
 
 def host_batch(b, n, seed):
     from pointdsc_b200.synth import make_batch
@@ -34,14 +19,14 @@ def host_batch(b, n, seed):
     return d
 
 
-def same(a, b):
+def same_result(a, b):
     return torch.equal(a["final_trans"], b["final_trans"]) and torch.equal(a["final_labels"], b["final_labels"])
 
 
 def test_synchronous_call_beside_a_suspended_stream():
     """model.run with host tensors while a forward_stream generator is suspended with one call in flight: the synchronous
     call (graphed and eager sizes) gives its module result, and the stream then goes on and gives the module results."""
-    m = get_model()
+    m = get_model(precision=DEFAULT_PRECISION)
     batches = [host_batch(b, n, 700 + 10 * i) for i, (b, n) in enumerate([(2, 300), (40, 1000), (1, 1000), (3, 400)])]
     between = [host_batch(1, 500, 800), host_batch(40, 1000, 900)]   # B * N on either side of the graph-replay size
     want = [m(d) for d in batches]
@@ -49,16 +34,16 @@ def test_synchronous_call_beside_a_suspended_stream():
     it = m.forward_stream(iter(batches))
     got = [next(it)]                                   # batch 1 is now in flight
     for d, w in zip(between, want_between):
-        assert same(m.run(d["corr_pos"], d["src_keypts"], d["tgt_keypts"]), w)
+        assert same_result(m.run(d["corr_pos"], d["src_keypts"], d["tgt_keypts"]), w)
     got += list(it)
-    assert len(got) == len(want) and all(same(g, w) for g, w in zip(got, want))
+    assert len(got) == len(want) and all(same_result(g, w) for g, w in zip(got, want))
 
 
 def test_failed_host_call_leaves_both_slots_free():
     """pdsc_forward_host refuses N = 20000 (above the largest supported set); afterwards both pipeline slots take a call,
     and the module's host path still gives its result."""
     from pointdsc_b200 import _capi
-    m = get_model()
+    m = get_model(precision=DEFAULT_PRECISION)
     lib = m._ensure_engine()
     d = host_batch(2, 300, 950)
     ref = m(d)
@@ -83,4 +68,4 @@ def test_failed_host_call_leaves_both_slots_free():
         _capi.check(lib.pdsc_forward_host_wait(m._engine, sl))
     for o in outs:
         assert torch.equal(o[0], ref["final_trans"]) and torch.equal(o[1], ref["final_labels"])
-    assert same(m.run(d["corr_pos"], d["src_keypts"], d["tgt_keypts"]), ref)
+    assert same_result(m.run(d["corr_pos"], d["src_keypts"], d["tgt_keypts"]), ref)

@@ -13,6 +13,7 @@ import pytest
 import torch
 
 from conftest import GOLDEN, load_snapshot
+from gpu_models import ulps
 from oracle import icp_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -55,13 +56,6 @@ def _device(src, tgt, init, offsets=None, **kw):
             info["status"].cpu().numpy())
 
 
-def _ulps(a, b):
-    def ordered(x):
-        i = np.asarray(x, np.float32).view(np.int32).astype(np.int64)
-        return np.where(i < 0, -(i & 0x7FFFFFFF), i)
-    return np.abs(ordered(a) - ordered(b))
-
-
 def _check(dev, b, ref):
     trans, fit, rmse, its, status = dev
     assert O.margin(ref) > MARGIN, ref["margins"]
@@ -69,7 +63,7 @@ def _check(dev, b, ref):
     assert int(its[b]) == ref["iterations"], (int(its[b]), ref["iterations"])
     assert float(fit[b]) == ref["fitness"]
     assert abs(float(rmse[b]) - ref["inlier_rmse"]) <= 1e-12 * ref["inlier_rmse"]
-    assert _ulps(trans[b], ref["trans"]).max() <= 2, (trans[b], ref["trans"])
+    assert ulps(trans[b], ref["trans"]).max() <= 2, (trans[b], ref["trans"])
 
 
 # ---------------------------------------------------------------------------------------------------

@@ -16,10 +16,11 @@ import numpy as np
 import pytest
 import torch
 
+from float64_bounds import C_PRE, C_SVD, EPS64, kabsch_ld
+from gpu_models import ulps
 from oracle import icp_oracle as O
 
 MARGIN = 1e-9
-EPS64 = 2.0 ** -52
 # Parity tolerance (test_gpu_icp._check): T within 2 float32 ulps per entry.  (b) asks a flipped decision to move T by at
 # least FLIP_ULPS ulps, 500 times that.
 FLIP_ULPS = 1000
@@ -30,13 +31,6 @@ CAPS = [1, 30]               # one update (T is the first update, which the firs
 # ---------------------------------------------------------------------------------------------------
 # helpers
 # ---------------------------------------------------------------------------------------------------
-def _ulps(a, b):
-    def ordered(x):
-        i = np.asarray(x, np.float32).view(np.int32).astype(np.int64)
-        return np.where(i < 0, -(i & 0x7FFFFFFF), i)
-    return np.abs(ordered(a) - ordered(b))
-
-
 def _cell(x, lo, h):
     """The device's cell coordinate of x (double arithmetic, as icp.cu computes it)."""
     return np.floor((np.asarray(x, np.float64) - lo) / h)
@@ -247,7 +241,7 @@ def check_edges(sc):
         assert row[j] == t and keep[j] == want_keep, (name, int(row[j]), t, bool(keep[j]))
         other = t + 1 if name.startswith("tie") else None
         flipped = _oracle(src, tgt, init, sc.r, 1, _flip(e, other))
-        moved = _ulps(flipped["trans"], ref["trans"]).max()
+        moved = ulps(flipped["trans"], ref["trans"]).max()
         assert moved > FLIP_ULPS or flipped["fitness"] != ref["fitness"], (name, int(moved))
     for cap in CAPS:
         res = _oracle(src, tgt, init, sc.r, cap)
@@ -463,7 +457,7 @@ def _parity(dev, ref, what, M):
     err_rmse = abs(rmse - ref["inlier_rmse"])
     assert err_rmse <= 1e-12 * ref["inlier_rmse"] + slack_rmse, (what, rmse, ref["inlier_rmse"])
     err = np.abs(trans - ref["trans64"])
-    ok = (_ulps(trans, ref["trans"]) <= 2) | (err <= slack)
+    ok = (ulps(trans, ref["trans"]) <= 2) | (err <= slack)
     assert ok.all(), (what, trans, ref["trans"], slack)
     return max(err_rmse / (1e-12 * ref["inlier_rmse"] + slack_rmse),
                float((err / (slack + 2 * np.spacing(np.abs(ref["trans"])))).max()))
@@ -580,7 +574,6 @@ def near_line_reference(src, tgt, init, r):
     they enter H as N dca dcb^T), the subtractions round relative to m and n, and the products and the fixed-order sum add
     <= 14 eps64 (one term per thread, a 5-level warp tree, 8 warps): E_ij <= C_PRE eps64 sum_k |m_ki| |n_kj|, C_PRE = 32.  E
     lies along the line (the x row), which the near-zero pair s2, s3 does not see: the bound stays far below 1."""
-    from test_gpu_kabsch import C_PRE, C_SVD, kabsch_ld
     ref = O.icp(src, tgt, init, max_correspondence_distance=r, max_iteration=1, record=True)
     a, b = (x.astype(np.longdouble) for x in ref["updates"][0])
     ca, cb = a.mean(0), b.mean(0)

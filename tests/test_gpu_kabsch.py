@@ -22,163 +22,15 @@ import pytest
 import torch
 
 from conftest import load_snapshot
+from float64_bounds import (C_PRE, C_SVD, EPS, EPS64, _gap, assert_rotations, check_transforms, kabsch64, kabsch_ld,
+                            weighted_kabsch64)
+from gpu_models import get_model
 from oracle import pointdsc_oracle as O
 
 pytestmark = pytest.mark.gpu
 
 PRECISIONS = os.environ.get("PDSC_TEST_PRECISIONS", "fp32,fp16x3").split(",")
 HERE = os.path.dirname(os.path.abspath(__file__))
-EPS = 2.0 ** -23
-EPS64 = 2.0 ** -52      # float64 unit roundoff: the bound of the double solver (ICP's updates) uses it in place of eps
-# Solver constant: |R - R64|max <= C_SVD * eps * s1 / (s2 + d s3).  Worst measured on an H100 over the ~1.1e5 matrices of
-# part 1: 5.2 (repeated singular values; random 4.7, ill-conditioned 3.8, reflected 1.8, rank 2 1.8), so 16 leaves 3x.
-C_SVD = 16.0
-# Pre-solver fp32 term (`_h_error`): per-entry bound on |H32 - H64| in units of eps * (its magnitude terms).  Derivation: a
-# weighted centroid is a 4-term fma chain per lane, a 5-level warp tree and a division by a sum with the same error, so it
-# is off by <= 20 eps * max|a|; a centred coordinate then by <= 21 eps * max|a|; each H entry sums k products of such terms
-# (4 fma per lane + the tree: 10 eps relative).  32 covers all three with margin.  Measured on an H100 (part 2's degenerate
-# neighbourhoods): the worst error is 0.002 of the rotation tolerance, 0.018 of the translation one and 0.008 of the centroid
-# one; the bounds are worst cases, the typical rounding errors cancel.
-C_PRE = 32.0
-
-_models = {}
-
-
-def get_model(dataset, precision="fp32", k=40):
-    from pointdsc_b200 import PointDSC
-    key = (dataset, precision, k)
-    if key not in _models:
-        cfg = O.default_config(dataset)
-        m = PointDSC(in_dim=6, num_layers=12, num_channels=128, num_iterations=10, ratio=0.1,
-                     inlier_threshold=cfg["inlier_threshold"], sigma_d=cfg["sigma_d"], k=k,
-                     nms_radius=cfg["nms_radius"], precision=precision)
-        res = m.load_state_dict(load_snapshot(dataset), strict=False)
-        assert res.missing_keys == [] and res.unexpected_keys == ["gamma"]
-        _models[key] = m.cuda().eval()
-    return _models[key]
-
-
-# ---------------------------------------------------------------------------------------------------
-# float64 references
-# ---------------------------------------------------------------------------------------------------
-def kabsch64(H):
-    """R = V diag(1, 1, det(V U^T)) U^T of H [..., 3, 3] (float64, H = U S V^T, H = sum w a b^T so that b ~= R a).
-    Returns R, singular values s [..., 3] (descending), d = det(V U^T), U, V."""
-    U, s, Vt = np.linalg.svd(H)
-    V = np.swapaxes(Vt, -1, -2)
-    d = np.sign(np.linalg.det(V @ np.swapaxes(U, -1, -2)))
-    D = np.broadcast_to(np.eye(3), H.shape).copy()
-    D[..., 2, 2] = d
-    return V @ D @ np.swapaxes(U, -1, -2), s, d, U, V
-
-
-def kabsch_ld(H, sweeps=12):
-    """kabsch64's R, s, d, U, V for float64 H, computed in long double (64-bit significand, 2^-11 of float64's roundoff).
-    LAPACK's float64 SVD is itself off by up to ~50 eps64 s1 / (s2 + d s3) on part 1's families, as much as the solver under
-    test, so the double solver is checked against this: one-sided Jacobi on the columns of H, R = V diag(1, 1, d) U^T in
-    the form v1 u1^T + v2 u2^T + (v1 x v2)(u1 x u2)^T, which needs no u3 (rank-2 H included).  Rows of rank < 2 get the
-    same form with an arbitrary u2 and are not compared (their gap s2 + d s3 is 0)."""
-    H = np.asarray(H, np.float64)
-    m = np.abs(H).max(axis=(1, 2))
-    e = np.where(m > 0, np.floor(np.log2(np.where(m > 0, m, 1.0))), 0.0)
-    G = H.astype(np.longdouble) * np.exp2(-e).astype(np.longdouble)[:, None, None]     # exact power-of-two scaling
-    V = np.broadcast_to(np.eye(3, dtype=np.longdouble), G.shape).copy()
-    one = np.longdouble(1)
-    for _ in range(sweeps):
-        for p, q in ((0, 1), (0, 2), (1, 2)):
-            gp, gq = G[:, :, p].copy(), G[:, :, q].copy()
-            a, b, g = (gp * gp).sum(1), (gq * gq).sum(1), (gp * gq).sum(1)
-            rot = g != 0
-            z = np.where(rot, (b - a) / np.where(rot, 2 * g, one), one)
-            t = np.where(rot, np.sign(z) / (np.abs(z) + np.sqrt(one + z * z)), 0)
-            c = one / np.sqrt(one + t * t)
-            s = c * t
-            G[:, :, p], G[:, :, q] = c[:, None] * gp - s[:, None] * gq, s[:, None] * gp + c[:, None] * gq
-            vp, vq = V[:, :, p].copy(), V[:, :, q].copy()
-            V[:, :, p], V[:, :, q] = c[:, None] * vp - s[:, None] * vq, s[:, None] * vp + c[:, None] * vq
-    n = np.sqrt((G * G).sum(1))                                                         # [P, 3] singular values
-    order = np.argsort(-n, axis=1, kind="stable")
-    n = np.take_along_axis(n, order, 1)
-    G = np.take_along_axis(G, order[:, None, :], 2)
-    V = np.take_along_axis(V, order[:, None, :], 2)
-    safe = lambda x: np.where(x > 0, x, one)  # noqa: E731
-    u1 = G[:, :, 0] / safe(n[:, 0])[:, None]
-    u2 = G[:, :, 1] - u1 * (G[:, :, 1] * u1).sum(1)[:, None]
-    u2 = u2 / safe(np.sqrt((u2 * u2).sum(1)))[:, None]
-    v1, v2 = V[:, :, 0], V[:, :, 1]
-    R = (v1[:, :, None] * u1[:, None, :] + v2[:, :, None] * u2[:, None, :]
-         + np.cross(v1, v2)[:, :, None] * np.cross(u1, u2)[:, None, :])
-    U = np.stack([u1, u2, np.cross(u1, u2)], 2)
-    d = np.where(np.linalg.det(H) < 0, -1.0, 1.0)          # sign(det H) = det(U) det(V) wherever s3 > 0
-    s = (n * np.exp2(e).astype(np.longdouble)[:, None]).astype(np.float64)
-    return R.astype(np.float64), s, d, U.astype(np.float64), V.astype(np.float64)
-
-
-def _gap(s, d):
-    return s[..., 1] + d * s[..., 2]
-
-
-def _h_error(w, a, b, m, n):
-    """Per-entry bound on |H32 - H64| from fp32 centroids, centring and sums.  w [P,k], a/b the points [P,k,3], m/n the
-    centred points [P,k,3] (all float64).  Ma, Mb: the coordinates' magnitude, which the centroid errors scale with."""
-    Ma, Mb = np.abs(a).max(axis=(1, 2)), np.abs(b).max(axis=(1, 2))
-    mi, ni = np.abs(m).max(axis=2), np.abs(n).max(axis=2)
-    return C_PRE * EPS * (Ma * (w * ni).sum(1) + Mb * (w * mi).sum(1) + (w * mi * ni).sum(1)), Ma, Mb
-
-
-def weighted_kabsch64(a, b, w):
-    """oracle.pointdsc_oracle.weighted_kabsch in float64 (the oracle builds its identity in float32): negative weights -> 0,
-    centroids over sum(w) + 1e-6, H = Am^T diag(w) Bm, t = cb - R ca.  a, b [P,k,3], w [P,k].
-    Returns R [P,3,3], t [P,3], ca, cb, H, and the H error bound with its magnitudes."""
-    w = np.where(w < 0, 0.0, w)
-    den = w.sum(1) + 1e-6
-    ca = (a * w[..., None]).sum(1) / den[:, None]
-    cb = (b * w[..., None]).sum(1) / den[:, None]
-    m, n = a - ca[:, None], b - cb[:, None]
-    H = np.einsum("pki,pkj,pk->pij", m, n, w)
-    R, s, d, U, V = kabsch64(H)
-    t = cb - np.einsum("pij,pj->pi", R, ca)
-    EH, Ma, Mb = _h_error(w, a, b, m, n)
-    return dict(R=R, t=t, ca=ca, cb=cb, H=H, s=s, d=d, U=U, V=V, EH=EH, Ma=Ma, Mb=Mb)
-
-
-def assert_rotations(R, what, tol=1e-6):
-    """Finite, orthonormal and det = +1 to `tol`.  1e-6 is ~8 fp32 roundings of a product of unit vectors; the worst measured
-    on an H100 over every part-1 input is 8.6e-7 (|R R^T - I|) and 8.9e-7 (|det R - 1|)."""
-    R = np.asarray(R, np.float64)
-    assert np.isfinite(R).all(), what
-    orth = np.abs(R @ np.swapaxes(R, -1, -2) - np.eye(3)).max(axis=(-1, -2))
-    det = np.abs(np.linalg.det(R) - 1.0)
-    assert orth.max() <= tol and det.max() <= tol, (what, float(orth.max()), float(det.max()))
-
-
-def check_transforms(T, ref, what):
-    """Engine transforms T [P,4,4] against a weighted_kabsch64 result.  Returns the worst ratios (error / tolerance)."""
-    T = np.asarray(T, np.float64)
-    R, t = T[:, :3, :3], T[:, :3, 3]
-    assert_rotations(R, what)
-    s, d, EH, Ma, Mb = ref["s"], ref["d"], ref["EH"], ref["Ma"], ref["Mb"]
-    gap = _gap(s, d)
-    with np.errstate(divide="ignore", invalid="ignore"):
-        # rotation: solver term + pre-solver term over the signed gap; >= 2 is vacuous (entries of two rotations)
-        tol_R = np.where(gap > 0, (C_SVD * EPS * s[:, 0] + 6.0 * EH) / gap, np.inf)
-        # the first singular pair is defined whenever s1 > s2, the gap of singular vectors: R u1 = v1 (rank 1 included)
-        tol_u1 = np.where(s[:, 0] > s[:, 1], (C_SVD * EPS * s[:, 0] + 6.0 * EH) / (s[:, 0] - s[:, 1]), np.inf)
-    err_R = np.abs(R - ref["R"]).max(axis=(1, 2))
-    assert (err_R <= tol_R).all(), (what, np.flatnonzero(err_R > tol_R)[:8], err_R[err_R > tol_R][:8], tol_R[err_R > tol_R][:8])
-    err_u1 = np.abs(np.einsum("pij,pj->pi", R, ref["U"][:, :, 0]) - ref["V"][:, :, 0]).max(1)
-    assert (err_u1 <= tol_u1).all(), (what, err_u1[err_u1 > tol_u1][:8], tol_u1[err_u1 > tol_u1][:8])
-    # t = cb - R ca: its error is the rotation's error at the centroid plus the centroids' own (<= 20 eps Ma, see C_PRE)
-    tol_t = 3.0 * np.minimum(tol_R, 2.0) * Ma + C_PRE * EPS * (Ma + Mb)
-    err_t = np.abs(t - ref["t"]).max(1)
-    assert (err_t <= tol_t).all(), (what, err_t[err_t > tol_t][:8], tol_t[err_t > tol_t][:8])
-    # whatever R is, it maps the weighted centroid onto the target centroid (no division by a gap): the centroids' errors
-    # (<= 20 eps each), R times the source one (3 terms) and the rounding of t = cb - R ca: 96 eps (Ma + Mb)
-    err_c = np.abs(np.einsum("pij,pj->pi", R, ref["ca"]) + t - ref["cb"]).max(1)
-    tol_c = 96.0 * EPS * (Ma + Mb)
-    assert (err_c <= tol_c).all(), (what, err_c[err_c > tol_c][:8], tol_c[err_c > tol_c][:8])
-    ratio = lambda e, tl: float(np.max(np.where(np.isfinite(tl) & (tl < 2), e / tl, 0.0), initial=0.0))  # noqa: E731
-    return dict(R=ratio(err_R, tol_R), u1=ratio(err_u1, tol_u1), t=ratio(err_t, tol_t), c=ratio(err_c, tol_c), tol_R=tol_R)
 
 
 def residual_band(T, src, tgt, thr):
@@ -460,7 +312,7 @@ def seed_geometry_set(seed=0):
 
 @pytest.mark.parametrize("precision", PRECISIONS)
 def test_seed_kabsch_on_degenerate_neighbourhoods(precision):
-    m = get_model("3dmatch", precision, 40)
+    m = get_model("3dmatch", precision)
     src, tgt, knn, fam = seed_geometry_set()
     N, S, k = src.shape[0], knn.shape[0], knn.shape[1]
     rng = np.random.default_rng(1)
@@ -503,7 +355,7 @@ ORACLE_K = (33, 79, 88, 128)    # one per NSM kernel family: one warp (<= 40), 4
 @pytest.mark.parametrize("k", K_SWEEP)
 def test_k_sweep_knn_compat_seed_kabsch(k, precision):
     from pointdsc_b200.synth import make_pair
-    m = get_model("3dmatch", precision, k)
+    m = get_model("3dmatch", precision, k=k)
     n = 300                                                    # S = 30 seeds, k <= n - 1
     p = make_pair(500 + k, n, "3dmatch", 0.6)
     args = [p[x][None].cuda() for x in ("corr_pos", "src_keypts", "tgt_keypts")]
@@ -566,7 +418,7 @@ def test_large_k_set_in_a_mixed_call(precision):
     """k = 128: N = 41 (k = 40, one-warp NSM), N = 90 (k = 89, SIMT with repeated Gram passes) and N = 300 (k = 128) in one
     forward_many call, bit for bit what single calls give."""
     from pointdsc_b200.synth import make_pair
-    m = get_model("3dmatch", precision, 128)
+    m = get_model("3dmatch", precision, k=128)
     pairs = [make_pair(70 + i, n, "3dmatch", 0.5) for i, n in enumerate([41, 300, 90])]
     batch = lambda ps: {"corr_pos": torch.stack([q["corr_pos"] for q in ps]).cuda(),  # noqa: E731
                         "src_keypts": torch.stack([q["src_keypts"] for q in ps]).cuda(),
@@ -639,7 +491,7 @@ def scoring_set(dataset, seed=0):
 
 @pytest.mark.parametrize("dataset", ["3dmatch", "kitti"])
 def test_inlier_counts_and_first_maximum_selection(dataset):
-    m = get_model(dataset, "fp32", 40)
+    m = get_model(dataset, "fp32")
     src, tgt, hyps, thr = scoring_set(dataset)
     out = m.run(*_inputs(src, tgt), taps=["inlier_counts", "best", "init_trans"],
                 inject={"seed_trans": torch.from_numpy(hyps).cuda()[None]})
@@ -659,7 +511,7 @@ def test_inlier_counts_and_first_maximum_selection(dataset):
 
 
 def test_one_seed_and_no_seeds():
-    m = get_model("3dmatch", "fp32", 40)
+    m = get_model("3dmatch", "fp32")
     thr = 0.10
     src, tgt, hyps, _ = scoring_set("3dmatch", seed=3)
     # N = 15: S = 1, the only hypothesis is selected
@@ -784,7 +636,7 @@ def _rot_small(rng, ang):
 @pytest.mark.parametrize("case", ["generic", "planar", "zero_inliers", "chain"])
 @pytest.mark.parametrize("dataset", ["3dmatch", "kitti"])           # tau' = 0.10 and 1.2
 def test_refinement_given_injected_hypothesis(dataset, case):
-    m = get_model(dataset, "fp32", 40)
+    m = get_model(dataset, "fp32")
     src, tgt, T0, need_margin = refinement_case(case, dataset)
     src, tgt, T0 = src.astype(np.float32), tgt.astype(np.float32), T0.astype(np.float32)
     S = m.num_seeds(src.shape[0])

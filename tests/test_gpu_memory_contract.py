@@ -17,7 +17,7 @@ Results must be bit-identical across patterns; every output and tap element must
 SC matrix in the workspace, whose pad columns the contract says are written as 0 (a pad column only feeds discarded query
 rows, so no output shows it).
 
-Workspace regions.  carve() and call_shape() (engine.cu) are restated below (mirror_workspace), including
+Workspace regions.  carve() and call_shape() (engine.cu) are restated in engine_rules.py (mirror_workspace), including
 tc_scratch_bytes_tiles and the key-split rules attn_set_split / attn_set_split_invariant / tc_packed_split (sets.cuh,
 encoder_tc.cu), and every GPU test asserts that the restatement's total equals pdsc_workspace_bytes(_packed), so the map
 cannot drift from the engine.  Float regions get the float patterns.  Control and index regions only get values that keep
@@ -43,377 +43,23 @@ scalars.
 The GPU tests need an H100 (`-m gpu`); the harness self-tests at the end run on the CPU.
 """
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
 import torch
 
-from conftest import load_snapshot
-
-SLACK = 64 * 1024
-SENTINEL = 0x3CC35AA5
-NAN32 = 0x7FC00000
-PATTERNS = ["zero", "ones", "fmax", "fmin"]
-FLOAT_WORD = {"zero": 0x00000000, "ones": 0xFFFFFFFF, "fmax": 0x7F7F7F7F, "fmin": 0xFF7F7F7F}
-INDEX_WORD = {"zero": 0, "ones": 1, "fmax": 1, "fmin": 0}
-MASK_WORD = {"zero": 0, "ones": 0xFFFFFFFF, "fmax": 0, "fmin": 0xFFFFFFFF}
-BEST_QWORD = {"zero": 0, "ones": 0xFFFFFFFF00000000, "fmax": 0, "fmin": 0xFFFFFFFF00000000}
-C_CH = 128                      # num_channels
-SETDESC_BYTES = 72              # sets.cuh SetDesc: 12 int32 + 3 int64
-TSI = 8                         # sets.cuh kAttnInvariantTiles
-SPLIT_MAX_ITEMS = 320           # encoder_tc.cu kAttnSplitMaxItems
-PARTIAL_BYTES = 65536 + 1024    # encoder_tc.cu kAttnPartialBytes
-RATIO = 0.1                     # cfg.ratio
-
-
-# ---------------------------------------------------------------------------------------------------
-# harness
-# ---------------------------------------------------------------------------------------------------
-def tiled(word, n, device, width=4):
-    """n bytes of the little-endian `width`-byte word repeated."""
-    pat = torch.tensor(list(int(word).to_bytes(width, "little")), dtype=torch.uint8)
-    return pat.repeat(n // width + 1)[:n].to(device)
-
-
-def fill_words(buf, word, width=4):
-    """Fill a uint8 tensor (length a multiple of `width`) with a repeated word, without a temporary of its size."""
-    n = buf.numel()
-    assert n % width == 0, (n, width)
-    if n:
-        pat = torch.tensor(list(int(word).to_bytes(width, "little")), dtype=torch.uint8, device=buf.device)
-        buf.view(-1, width).copy_(pat.expand(n // width, width))
-
-
-class Guarded:
-    """`nbytes` at exactly `align` (an address that is a multiple of align but not of 2 align), with at least SLACK bytes of
-    sentinel (or NaN) on either side, all inside one allocation."""
-
-    def __init__(self, nbytes, align, device, slack="sentinel"):
-        self.nbytes, self.align = int(nbytes), int(align)
-        self.raw = torch.empty(2 * SLACK + 2 * self.align + self.nbytes, dtype=torch.uint8, device=device)
-        base = self.raw.data_ptr()
-        addr = -(-(base + SLACK) // self.align) * self.align
-        if addr % (2 * self.align) == 0:
-            addr += self.align
-        self.off = addr - base
-        self.inner = self.raw[self.off:self.off + self.nbytes]
-        word = SENTINEL if slack == "sentinel" else NAN32
-        self.pre_want = tiled(word, self.off, device)
-        self.post_want = tiled(word, self.raw.numel() - self.off - self.nbytes, device)
-        self.raw[:self.off].copy_(self.pre_want)
-        self.raw[self.off + self.nbytes:].copy_(self.post_want)
-
-    @property
-    def ptr(self):
-        return self.raw.data_ptr() + self.off       # (an empty slice reports address 0)
-
-    def typed(self, dtype, shape):
-        return self.inner.view(dtype).view(shape)
-
-    def violations(self):
-        """Offsets, relative to the buffer's first byte, of slack bytes that changed."""
-        pre = torch.nonzero(self.raw[:self.off] != self.pre_want).flatten() - self.off
-        post = torch.nonzero(self.raw[self.off + self.nbytes:] != self.post_want).flatten() + self.nbytes
-        return pre.tolist() + post.tolist()
-
-    def check(self, what):
-        v = self.violations()
-        assert not v, f"{what}: {len(v)} guard bytes changed, first at offsets {v[:8]} from the buffer's first byte"
-
-
-def guarded_input(arr, device):
-    """A float32 / float64 / int32 host array as a device input at 16 B with NaN slack."""
-    arr = np.ascontiguousarray(arr)
-    g = Guarded(arr.nbytes, 16, device, slack="nan")
-    g.inner.copy_(torch.from_numpy(arr.view(np.uint8).reshape(-1)))
-    return g
-
-
-def guarded_output(nbytes, align, device, pattern):
-    g = Guarded(nbytes, align, device)
-    fill_words(g.inner, FLOAT_WORD[pattern]) if nbytes % 4 == 0 else g.inner.copy_(tiled(FLOAT_WORD[pattern], nbytes, device))
-    return g
-
-
-# ---------------------------------------------------------------------------------------------------
-# the workspace, restated (engine.cu call_shape / carve, encoder_tc.cu tc_packed_split / tc_scratch_bytes_tiles, sets.cuh)
-# ---------------------------------------------------------------------------------------------------
-def attn_set_split(N, sms):
-    QT, KT = -(-N // 128), -(-N // 64)
-    if KT < 4:
-        return 1, KT
-    want = -(-sms // QT)
-    ts = max(-(-KT // want), 2)
-    s = -(-KT // ts)
-    return (s, ts) if s >= 2 else (1, KT)
-
-
-def attn_set_split_invariant(N):
-    KT = -(-N // 64)
-    sp = -(-KT // TSI)
-    return sp, -(-KT // sp)
-
-
-def tc_packed_split(Ns, invariant, sms):
-    """(split, items, [(sp, TS)] per set) of a tensor-core call."""
-    per = [attn_set_split_invariant(n) if invariant else attn_set_split(n, sms) for n in Ns]
-    qtiles = sum(-(-n // 128) for n in Ns)
-    items = sum(-(-n // 128) * sp for n, (sp, _) in zip(Ns, per))
-    split = items > qtiles if invariant else (2 * qtiles <= sms and qtiles < items <= SPLIT_MAX_ITEMS)
-    return split, (items if split else qtiles), per
-
-
-def num_seeds(N):
-    m = int(N * RATIO)                  # sets.cuh num_seeds: the length of range(N)[:m]
-    return min(m, N) if m >= 0 else max(N + m, 0)
-
-
-def mirror_workspace(Ns, precision, invariant, k_cfg, sms, iters=10):
-    """[(name, offset, bytes, kind)] and the total of carve(call_shape(Ns)); kind: float / index / mask / best / zero."""
-    R = sum(Ns)
-    B = len(Ns)
-    seeds = sum(num_seeds(n) for n in Ns)
-    dist = sum((num_seeds(n) * n + 3) & ~3 for n in Ns)
-    knn = sum(num_seeds(n) * max(min(k_cfg, n - 1), 0) for n in Ns)
-    sc_row = sum(n * (-(-n // 64) * 64) for n in Ns)
-    sc_tiled = sum(-(-n // 64) * -(-n // 128) * 8192 for n in Ns)
-    qtiles, ktiles = sum(-(-n // 128) for n in Ns), sum(-(-n // 64) for n in Ns)
-    regions, off = [], 0
-
-    def take(name, count, size, kind):
-        nonlocal off
-        off = -(-off // 256) * 256
-        regions.append((name, off, count * size, kind))
-        off += count * size
-
-    take("sc", max(sc_row, sc_tiled), 4, "float")
-    take("feat_a", R * C_CH, 4, "float")
-    take("feat_b", -(-R // 128) * 128 * C_CH, 4, "float")
-    take("msg", R * C_CH, 4, "float")
-    if precision == "fp32":
-        for name in ("q", "k", "v"):
-            take(name, R * C_CH, 4, "float")
-        take("h1", R * 64, 4, "float")
-        take("h2", R * 64, 4, "float")
-    else:
-        split, items, _ = tc_packed_split(Ns, invariant, sms)
-        partial = (items if split else 0) if invariant else SPLIT_MAX_ITEMS
-        take("tc_scratch", (qtiles + ktiles) * 65536 + 1024 + partial * PARTIAL_BYTES, 1, "float")
-    take("normed", R * C_CH, 4, "float")
-    take("conf", R, 4, "float")
-    take("key", R, 4, "float")
-    take("seeds", seeds + 1, 4, "index")
-    take("seedfeat", seeds * C_CH + 1, 4, "float")
-    take("dist", dist + 1, 4, "float")
-    take("knn", knn + 1, 4, "index")
-    take("iterates", knn * iters + 1, 4, "float")
-    take("seed_trans", seeds * 16 + 16, 4, "float")
-    take("counts", seeds + 1, 4, "index")
-    take("conv_mask", B, 4, "mask")
-    take("best_key", B, 8, "best")
-    take("sets", B * SETDESC_BYTES, 1, "zero")
-    take("tile_set", -(-R // 128), 4, "zero")
-    return regions, -(-off // 256) * 256
-
-
-def poison_workspace(ws, regions, pattern):
-    fill_words(ws, FLOAT_WORD[pattern])
-    for name, off, n, kind in regions:
-        seg = ws[off:off + n]
-        if kind == "index":
-            fill_words(seg, INDEX_WORD[pattern])
-        elif kind == "mask":
-            fill_words(seg, MASK_WORD[pattern])
-        elif kind == "best":
-            fill_words(seg, BEST_QWORD[pattern], 8)
-        elif kind == "zero":
-            seg.zero_()
-
-
-# ---------------------------------------------------------------------------------------------------
-# driving the engine
-# ---------------------------------------------------------------------------------------------------
-ALL_TAPS = ["sc", "features", "normed", "confidence", "seeds", "knn_idx", "compat", "eig", "power_iters", "seed_trans",
-            "inlier_counts", "best", "init_trans", "refine_solves", "layer_features", "layer_debug", "timeline"]
-
-
-def sm_count():
-    n = torch.cuda.get_device_properties(0).multi_processor_count
-    env = os.environ.get("PDSC_SM_COUNT", "")
-    return min(n, int(env)) if env.isdigit() and int(env) > 0 else n
-
-
-_models = {}
-
-
-def get_model(precision, invariant=False, k=40, fresh=False):
-    from oracle import pointdsc_oracle as O
-    from pointdsc_b200 import PointDSC
-    key = (precision, invariant, k)
-    if fresh or key not in _models:
-        cfg = O.default_config("3dmatch")
-        m = PointDSC(in_dim=6, num_layers=12, num_channels=128, num_iterations=10, ratio=0.1,
-                     inlier_threshold=cfg["inlier_threshold"], sigma_d=cfg["sigma_d"], k=k,
-                     nms_radius=cfg["nms_radius"], precision=precision, batch_invariant=invariant)
-        res = m.load_state_dict(load_snapshot("3dmatch"), strict=False)
-        assert res.missing_keys == [] and res.unexpected_keys == ["gamma"]
-        m = m.cuda().eval()
-        m._ensure_engine()
-        if fresh:
-            return m
-        _models[key] = m
-    return _models[key]
-
-
-def make_inputs(Ns, seed=0):
-    """Packed corr_pos [R,6], src [R,3], tgt [R,3] float32 (numpy) of sets with N = Ns[b]."""
-    from pointdsc_b200.synth import make_pair
-    pairs = [make_pair(1000 * seed + 37 * n + b, n, "3dmatch", 0.3 + 0.2 * (b % 3)) for b, n in enumerate(Ns)]
-    return [np.concatenate([p[x].numpy() for p in pairs]).astype(np.float32) for x in ("corr_pos", "src_keypts", "tgt_keypts")]
-
-
-def tap_spec(name, B, N, S, k):
-    from pointdsc_b200.model import _TAP_SPECS
-    dtype, shape = _TAP_SPECS[name]
-    return dtype, shape(B, N, S, k, C_CH)
-
-
-def nbytes_of(dtype, shape):
-    return int(np.prod(shape, dtype=np.int64)) * torch.empty((), dtype=dtype).element_size()
-
-
-class Call:
-    """One configuration: its engine, entry point, sets and taps.  run(pattern) runs it on freshly poisoned buffers and
-    returns {output name: device bytes}, having checked every guard."""
-
-    def __init__(self, precision, Ns, entry="forward", invariant=False, k=40, taps=(), layer_tap=0, want_M=False, seed=0):
-        assert entry in ("forward", "packed", "eval", "graph")
-        assert entry == "packed" or len(set(Ns)) == 1
-        self.precision, self.Ns, self.entry, self.taps, self.layer_tap, self.want_M = precision, list(Ns), entry, list(taps), \
-            layer_tap, want_M
-        self.m = get_model(precision, invariant, k)
-        self.lib, self.e = self.m._ensure_engine(), self.m._engine
-        self.dev = torch.device("cuda")
-        self.B, self.R, self.N = len(Ns), sum(Ns), Ns[0]
-        self.S, self.k = int(self.lib.pdsc_num_seeds(self.e, self.N)), int(self.lib.pdsc_num_neighbours(self.e, self.N))
-        self.offsets = np.concatenate([[0], np.cumsum(Ns)]).astype(np.int32)
-        self.h_off = (C.c_int32 * (self.B + 1))(*self.offsets.tolist())
-        if entry == "packed":
-            self.need = int(self.lib.pdsc_workspace_bytes_packed(self.e, self.B, self.h_off))
-        else:
-            self.need = int(self.lib.pdsc_workspace_bytes(self.e, self.B, self.N))
-        self.regions, total = mirror_workspace(Ns, precision, invariant, k, sm_count())
-        assert total == self.need, ("workspace map drifted from the engine", total, self.need)
-        for n in set(Ns):
-            assert int(self.lib.pdsc_num_seeds(self.e, n)) == num_seeds(n)
-        cp, s, t = make_inputs(Ns, seed)
-        self.inputs = {"corr_pos": guarded_input(cp, self.dev), "src": guarded_input(s, self.dev), "tgt": guarded_input(t, self.dev),
-                       "d_offsets": guarded_input(self.offsets, self.dev)}
-        self.ws = Guarded(self.need, 256, self.dev)
-        self.outs = None
-        # the SC matrix (workspace offset 0) is written whole, pad columns as 0: row-major [N, round_up(N, 64)] in fp32,
-        # 64 x 128 tiles of every (key tile, query tile) in the tensor-core modes
-        self.sc_bytes = 4 * (sum(n * (-(-n // 64) * 64) for n in Ns) if precision == "fp32"
-                             else sum(-(-n // 64) * -(-n // 128) * 8192 for n in Ns))
-
-    def _outputs(self, pattern):
-        B, R, N = self.B, self.R, self.N
-        specs = {"final_trans": (torch.float32, (B, 4, 4)), "final_labels": (torch.float32, (R,))}
-        if self.want_M:
-            specs["M"] = (torch.float32, (B, N, N))
-        for name in self.taps:
-            specs[name] = tap_spec(name, B, N, self.S, self.k)
-        outs = {}
-        for name, (dtype, shape) in specs.items():
-            size = torch.empty((), dtype=dtype).element_size()
-            outs[name] = guarded_output(nbytes_of(dtype, shape), size, self.dev, pattern)
-        return outs
-
-    def _poison(self, pattern):
-        poison_workspace(self.ws.inner, self.regions, pattern)
-        if self.outs is None or self.entry != "graph":
-            self.outs = self._outputs(pattern)
-        else:                                     # a replayed graph keeps its output addresses: refill them in place
-            for g in self.outs.values():
-                fill_words(g.inner, FLOAT_WORD[pattern])
-
-    def run(self, pattern):
-        self._poison(pattern)
-        lib, e, o, i = self.lib, self.e, self.outs, self.inputs
-        stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        io_ptr = None
-        if self.taps:
-            io = self._io = _capi().StageIO()
-            for name in self.taps:
-                setattr(io, "out_" + name, o[name].ptr)
-            io.layer_tap = int(self.layer_tap)
-            io_ptr = C.byref(io)
-        P = C.c_void_p
-        args_in = (P(i["corr_pos"].ptr), P(i["src"].ptr), P(i["tgt"].ptr))
-        outs2 = (P(o["final_trans"].ptr), P(o["final_labels"].ptr))
-        if self.entry == "forward":
-            rc = lib.pdsc_forward(e, self.B, self.N, *args_in, *outs2, io_ptr, P(self.ws.ptr), self.need, stream)
-        elif self.entry == "eval":
-            rc = lib.pdsc_forward_eval(e, self.B, self.N, *args_in, *outs2, P(o["M"].ptr) if self.want_M else None, io_ptr,
-                                       P(self.ws.ptr), self.need, stream)
-        elif self.entry == "packed":
-            rc = lib.pdsc_forward_packed(e, self.B, self.h_off, P(i["d_offsets"].ptr), *args_in, *outs2, P(self.ws.ptr), self.need,
-                                         stream)
-        else:
-            rc = lib.pdsc_forward_graph(e, self.B, self.N, *args_in, *outs2, P(self.ws.ptr), self.need, stream)
-        _capi().check(rc)
-        torch.cuda.synchronize()
-        where = (self.precision, self.entry, self.Ns[:8], pattern)
-        self.ws.check(("workspace",) + where)
-        for name, g in list(o.items()) + list(i.items()):
-            g.check((name,) + where)
-        res = {}
-        for name, g in o.items():
-            if name == "timeline":                # documented as never written: it keeps the prefill
-                assert torch.equal(g.inner, tiled(FLOAT_WORD[pattern], g.nbytes, self.dev)), ("timeline written",) + where
-                continue
-            dtype = tap_spec(name, 1, 1, 1, 1)[0] if name in self.taps else torch.float32
-            if dtype == torch.float32 and g.nbytes:
-                assert torch.isfinite(g.inner.view(torch.float32)).all(), (name, "non-finite") + where
-            res[name] = g.inner.clone()
-        res["workspace sc"] = self.ws.inner[:self.sc_bytes].clone()
-        return res
-
-    def regime(self):
-        """(split?, [(sp, TS)]) the engine ran, asserted against pdsc_launches_per_forward for uniform tensor-core calls."""
-        if self.precision == "fp32":
-            return False, [(1, -(-n // 64)) for n in self.Ns]
-        split, _, per = tc_packed_split(self.Ns, self.m.batch_invariant, sm_count())
-        if self.entry != "packed":
-            enc = int(self.lib.pdsc_launches_per_forward(self.e, self.B, self.N)) - 12
-            assert enc == 2 + (5 if split else 4) * 12, (enc, split)
-        return split, per
-
-
-def _capi():
-    from pointdsc_b200 import _capi as capi
-    return capi
-
-
-def assert_same(ref, got, where):
-    assert ref.keys() == got.keys()
-    for name in ref:
-        if not torch.equal(ref[name], got[name]):
-            diff = torch.nonzero(ref[name] != got[name]).flatten()
-            raise AssertionError(f"{where}: {name} differs in {diff.numel()} bytes, first at byte {int(diff[0])}")
-
-
-def check_patterns(call, where):
-    ref = call.run("zero")
-    for p in PATTERNS[1:]:
-        assert_same(ref, call.run(p), where + (p,))
-    return ref
+from buffer_guards import (BEST_QWORD, FLOAT_WORD, INDEX_WORD, MASK_WORD, PATTERNS, SLACK, Call, Guarded, _capi, assert_same,
+                           check_patterns, guarded_input, guarded_output, keypoints, make_inputs, poison_workspace,
+                           run_guarded, scratch_buffer, surface, tiled)
+from engine_rules import eig_plan, match_plan, mirror_workspace, num_seeds, search_plan
+from gpu_models import get_model, sm_count
 
 
 # ---------------------------------------------------------------------------------------------------
 # forward entry points
 # ---------------------------------------------------------------------------------------------------
+ALL_TAPS = ["sc", "features", "normed", "confidence", "seeds", "knn_idx", "compat", "eig", "power_iters", "seed_trans",
+            "inlier_counts", "best", "init_trans", "refine_solves", "layer_features", "layer_debug", "timeline"]
 TAPS_NO_LAYER = [t for t in ALL_TAPS if t not in ("layer_features", "layer_debug")]
 
 # (id, precision, N, B, invariant, expected split or None, layer tap)
@@ -584,18 +230,18 @@ def do_call(m, c, host=False, seed=11):
 def test_call_history_on_one_module():
     """B = 64 x 5000, bs = 1 x 1000 (split, graph replay), N = 2, a packed call, an eval call, then the first shape again on
     one module: each equals the same call on a fresh module, bit for bit; then the uniform calls through the host path."""
-    m = get_model("fp16x3", fresh=True)
+    m = get_model(precision="fp16x3", fresh=True)
     fresh_results = []
     for c in history_calls():
         got = do_call(m, c)
-        f = get_model("fp16x3", fresh=True)
+        f = get_model(precision="fp16x3", fresh=True)
         want = do_call(f, c)
         f._release()
         del f
         fresh_results.append(want)
         for a, b in zip(got, want):
             assert a.numpy().tobytes() == b.numpy().tobytes(), c
-    h = get_model("fp16x3", fresh=True)
+    h = get_model(precision="fp16x3", fresh=True)
     for c, want in zip(history_calls(), fresh_results):
         if c[0] != "run":
             continue
@@ -609,27 +255,11 @@ def test_call_history_on_one_module():
 # ---------------------------------------------------------------------------------------------------
 # front-end entry points
 # ---------------------------------------------------------------------------------------------------
-def scratch_buffer(nbytes, align, pattern):
-    g = Guarded(nbytes, align, torch.device("cuda"))
-    g.inner.copy_(tiled(FLOAT_WORD[pattern], nbytes, g.inner.device))
-    return g
-
-
-def run_guarded(where, outs, scratch, inputs, call):
-    """call(), synchronise, check every guard; returns {name: bytes} of the outputs."""
-    _capi().check(call())
-    torch.cuda.synchronize()
-    for name, g in list(outs.items()) + list(inputs.items()) + [("scratch", scratch)]:
-        g.check((name,) + where)
-    return {n: g.inner.clone() for n, g in outs.items()}
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("fp64", [False, True], ids=["fp32", "fp64"])
 def test_match_poison_and_rows_past_m(fp64):
     """pdsc_match: scratch at exactly 8 B and pdsc_match_scratch_bytes, poisoned; outputs prefilled; rows >= M keep the
     prefill byte for byte (only the first M rows are written); mutual on and off; one chunk, several and the cap."""
-    from test_gpu_front_end import match_plan, keypoints
     lib = _capi().load()
     dev = torch.device("cuda")
     e = _capi().utility_engine(0)
@@ -709,7 +339,6 @@ SIZE_CLASS_MAX_NN = [1, 3, 5, 9, 17, 33, 65, 129, 256]     # P = 2, 4, ..., 256:
 
 @pytest.mark.gpu
 def test_normals_and_fpfh_poison():
-    from test_gpu_front_end import search_plan, surface
     assert sorted({search_plan(n)[0] for n in SIZE_CLASS_MAX_NN}) == [2 ** i for i in range(1, 9)]
     lib = _capi().load()
     dev = torch.device("cuda")
@@ -747,7 +376,6 @@ def test_normals_and_fpfh_poison():
 def test_leading_eigenvector_poison():
     """Scratch at exactly 16 B and pdsc_leading_eigenvector_scratch_bytes, poisoned (done is reset by eig_init_kernel);
     iterations_run prefilled; early exit on and off; the bulk-copy path (N % 4 == 0) and the plain one."""
-    from test_gpu_front_end import eig_plan
     lib = _capi().load()
     dev = torch.device("cuda")
     e = _capi().utility_engine(0)
@@ -879,17 +507,3 @@ def test_each_pattern_reaches_every_word():
     w = torch.tensor([FLOAT_WORD["fmax"], FLOAT_WORD["fmin"] - 2 ** 32, FLOAT_WORD["ones"] - 2 ** 32], dtype=torch.int64)
     f = w.to(torch.int32).view(torch.float32)
     assert float(f[0]) > 3e38 and float(f[1]) < -3e38 and torch.isnan(f[2])
-
-
-def test_split_rules_match_the_encoder_tests():
-    """The restated split rules agree with test_gpu_encoder's on the shapes both use."""
-    import test_gpu_encoder as T
-    for n in (2, 65, 257, 513, 1000, 3000, 5000, 16384):
-        for sms in (132, 114, 66):
-            assert attn_set_split(n, sms) == T.attn_set_split(n, sms)
-        assert attn_set_split_invariant(n) == T.attn_set_split_invariant(n)
-    for Ns in ([1000], [5000], [1003] * 17, [513, 9, 1003, 64]):
-        for inv in (False, True):
-            split, _, per = tc_packed_split(Ns, inv, 132)
-            t_split, t_per = T.call_split(Ns, 132, inv)
-            assert split == t_split and (not split or per == t_per)

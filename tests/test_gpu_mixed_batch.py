@@ -10,47 +10,16 @@ import pytest
 import torch
 
 from conftest import golden_cases, load_case, registration_ok
+from gpu_models import as_batch, get_model, sm_count, synth_sets
 
 pytestmark = pytest.mark.gpu
 
 PRECISIONS = os.environ.get("PDSC_TEST_PRECISIONS", "fp32,fp16x3").split(",")
 
-_models = {}
-
-
-def get_model(dataset, precision, k=40):
-    from conftest import load_snapshot
-    from oracle import pointdsc_oracle as O
-    from pointdsc_b200 import PointDSC
-    key = (dataset, precision, k)
-    if key not in _models:
-        cfg = O.default_config(dataset)
-        m = PointDSC(in_dim=6, num_layers=12, num_channels=128, num_iterations=10, ratio=0.1,
-                     inlier_threshold=cfg["inlier_threshold"], sigma_d=cfg["sigma_d"], k=k,
-                     nms_radius=cfg["nms_radius"], precision=precision)
-        m.load_state_dict(load_snapshot(dataset), strict=False)
-        _models[key] = m.cuda().eval()
-    return _models[key]
-
-
-def synth_sets(sizes, preset="3dmatch", seed0=0):
-    from pointdsc_b200.synth import make_pair
-    return [make_pair(seed0 + i, n, preset, 0.3) for i, n in enumerate(sizes)]
-
-
-def as_batch(pairs):
-    return {"corr_pos": torch.stack([p["corr_pos"] for p in pairs]).cuda(),
-            "src_keypts": torch.stack([p["src_keypts"] for p in pairs]).cuda(),
-            "tgt_keypts": torch.stack([p["tgt_keypts"] for p in pairs]).cuda(), "testing": True}
-
 
 def single(m, pair):
     b = as_batch([pair])
     return m.run(b["corr_pos"], b["src_keypts"], b["tgt_keypts"])
-
-
-def sm_count():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def q_tiles(n):
@@ -137,7 +106,7 @@ def _check_against_fixture(c, T, labels, again_T):
 
 
 def _run_fixtures(cases, precision):
-    m = get_model(cases[0]["meta"]["dataset"], precision, int(cases[0]["meta"].get("k", 40)))
+    m = get_model(cases[0]["meta"]["dataset"], precision, k=int(cases[0]["meta"].get("k", 40)))
     batches = [{"corr_pos": torch.from_numpy(np.ascontiguousarray(c["corr_pos"])).cuda()[None],
                 "src_keypts": torch.from_numpy(np.ascontiguousarray(c["src_keypts"])).cuda()[None],
                 "tgt_keypts": torch.from_numpy(np.ascontiguousarray(c["tgt_keypts"])).cuda()[None], "testing": True} for c in cases]

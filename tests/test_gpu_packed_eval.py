@@ -12,16 +12,14 @@ import numpy as np
 import pytest
 import torch
 
-from test_gpu_front_end import check_network_input, keypoints, match_descriptors, match_plan, run_match, stats_case
-from test_gpu_memory_contract import (FLOAT_WORD, PATTERNS, assert_same, guarded_input, guarded_output, run_guarded,
-                                      scratch_buffer, tiled)
-from test_gpu_mixed_batch import as_batch, get_model, synth_sets
-from test_gpu_stages import sm_count
+from buffer_guards import (FLOAT_WORD, PATTERNS, assert_same, check_network_input, guarded_input, guarded_output, keypoints,
+                           match_descriptors, run_guarded, run_match, scratch_buffer, stats_case, tiled)
+from engine_rules import MATCH_MAX_CHUNKS, match_plan
+from gpu_models import as_batch, get_model, sm_count, synth_sets
 
 pytestmark = pytest.mark.gpu
 
 MATCH_CASES = [("fp32", 32), ("fp64", 33)]      # FCGF, FPFH
-MATCH_MAX_CHUNKS = 32
 # (Ns, Nt) per pair: one row / one column, sizes off the 128-row and 64 / 32-column tiles, Ns > Nt and Nt > Ns
 GROUP = [(1, 1), (130, 70), (70, 130), (1, 300), (300, 1), (1000, 999), (257, 2000), (63, 65)]
 

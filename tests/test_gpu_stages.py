@@ -15,7 +15,6 @@ Error model (u = 2^-24, the fp32 unit roundoff; gamma(n) = n u / (1 - n u)):
 Each tolerance is derived beside its assertion from these rules, and the worst measured error / tolerance ratio on an
 H100 is recorded next to its constant.
 """
-import math
 import os
 
 import numpy as np
@@ -23,50 +22,19 @@ import pytest
 import torch
 
 from conftest import load_snapshot
+from float64_bounds import E_KNN, U, check_power, gamma
+from gpu_models import dev, get_model, sm_count
 from oracle import pointdsc_oracle as O
 
 pytestmark = pytest.mark.gpu
 
 PRECISIONS = os.environ.get("PDSC_TEST_PRECISIONS", "fp32,fp16x3").split(",")
-U = 2.0 ** -24
-
-
-def gamma(n):
-    return n * U / (1.0 - n * U)
-
-
-def sm_count():
-    """The SM count the engine sizes its launches for (PDSC_SM_COUNT lowers it, see device_state.cu)."""
-    n = torch.cuda.get_device_properties(0).multi_processor_count
-    env = os.environ.get("PDSC_SM_COUNT", "")
-    return min(n, int(env)) if env.isdigit() and int(env) > 0 else n
-
-
-_models = {}
-
-
-def get_model(dataset, precision="fp32", k=40, iters=10):
-    from pointdsc_b200 import PointDSC
-    key = (dataset, precision, k, iters)
-    if key not in _models:
-        cfg = O.default_config(dataset)
-        m = PointDSC(in_dim=6, num_layers=12, num_channels=128, num_iterations=iters, ratio=0.1,
-                     inlier_threshold=cfg["inlier_threshold"], sigma_d=cfg["sigma_d"], k=k,
-                     nms_radius=cfg["nms_radius"], precision=precision)
-        res = m.load_state_dict(load_snapshot(dataset), strict=False)
-        assert res.missing_keys == [] and res.unexpected_keys == ["gamma"]
-        _models[key] = m.cuda().eval()
-    return _models[key]
 
 
 def release(m):
     """Drop a model's cached workspaces after a call whose workspace (it holds the SC matrix) runs to gigabytes."""
     m._workspaces.clear()
     torch.cuda.empty_cache()
-
-
-def dev(x):
-    return torch.from_numpy(np.ascontiguousarray(x)).cuda()
 
 
 def run_injected(m, feat, src, tgt, taps, **inject):
@@ -362,15 +330,7 @@ def test_nms_seeds_both_kernels(family, dataset, n, precision):
 # ---------------------------------------------------------------------------------------------------
 # 4. kNN on injected features and seeds
 # ---------------------------------------------------------------------------------------------------
-# A distance 2 - 2 f_s . f_j of unit rows: the fp32 dot of 128 terms is within gamma(128) sum |f_s| |f_j| <= gamma(128)
-# (Cauchy-Schwarz), doubled, plus u 4 for 2 - 2x: E_KNN = 2 gamma(128) + 4 u = 1.55e-5.  The tensor-core mode's fp16
-# hi/lo split drops lo*lo and the lo parts' own rounding: <= 3 2^-22 + 2^-25 (|f_s|_1 + |f_j|_1) = 1.4e-6, and its fp32
-# accumulation over the 24 k-steps adds <= 48 u: below E_KNN.  Two ranks can swap only if their float64 distances are
-# within 2 E_KNN.  Measured on an H100 (80GB HBM3): worst |d64(got) - d64(ref)| / (2 E_KNN) = 0.025 (fp32, N = 16384,
-# k = 128); 91-95 % of the ranks are separated.  Identical rows came out with bitwise identical distances in both modes.
-E_KNN = 2 * gamma(128) + 4 * U
-
-
+# Two ranks may swap only where their float64 distances lie within 2 E_KNN (float64_bounds.py derives E_KNN).
 def knn_features(rng, N):
     """Clustered unit-scale rows (N / 20 centres) with 2 % exact duplicates of other rows."""
     centres = rng.standard_normal((N // 20 + 1, 128))
@@ -424,7 +384,7 @@ def check_knn(got, normed, seeds, k):
 @pytest.mark.parametrize("k", [40, 128])
 @pytest.mark.parametrize("n", [1001, 1290, 2003, 5000, 16384])
 def test_knn_against_float64(n, k, precision):
-    m = get_model("3dmatch", precision, k)
+    m = get_model("3dmatch", precision, k=k)
     S = m.num_seeds(n)
     sms = sm_count()
     seed_ctas = -(-S // 128)
@@ -466,65 +426,9 @@ def test_knn_against_float64(n, k, precision):
 # ---------------------------------------------------------------------------------------------------
 # 5. the power iteration on the tapped compatibility
 # ---------------------------------------------------------------------------------------------------
-# M and the iterates are non-negative, so one fp32 step is the exact step followed by a per-entry relative perturbation:
-# (M v)_i within gamma(k + 2) (k fmas and the two butterfly adds) and the division by the norm u; the norm's own rounding
-# scales every entry alike.  Non-negative matrices do not expand Hilbert's projective metric, and the normalisation does not
-# change it, so after t steps d_H(v32, v64) <= D_t = 2.01 t gamma(k + 3), linear in t.  Both vectors have the norm
-# nrm / (nrm + 1e-6), the fp32 one within ((k + 1) / 2 + 4) u and one more D_t: per entry
-#   |v32 - v64| <= (2 (e^D_t - 1) + ((k + 1) / 2 + 4) u) v64 + 1e-30.
-# Measured on an H100 (80GB HBM3) over the sweep and the caps: worst error / bound = 0.032 (cap 1, k = 40).
-#
-# The exit iteration.  That worst case is wider than allclose's own rtol of 1e-5, so it cannot decide whether fp32 and
-# float64 take the same exit.  The per-step roundings are independent: their sum grows like the square root of their number,
-# so the band is B_t = C_BAND sqrt(t (k + 3)) u v64, C_BAND = 4, and the test asserts that the engine's eig stays inside
-# that band at its exit iteration (measured on an H100: worst error / band 0.12).  An entry's allclose margin |v_t - v_t-1| - (1e-8 + 1e-5 v_t-1)
-# is then known to within B_t + B_t-1 + 3 u (|v_t - v_t-1| + 1e-8 + 1e-5 v_t-1) (the fp32 comparison's own roundings).
-# An iteration's all-seeds decision is sure when every margin is below minus that or one margin is above it; where every
-# decision up to the float64 exit is sure, power_iters must equal the float64 exit (220 of the sweep's 320 sets on an H100).
-C_BAND = 4.0
+# float64_bounds.check_power: eig within its worst-case bound and statistical band, power_iters equal to the float64 exit
+# wherever that exit is sure.
 POWER_K = [1, 2, 3, 31, 32, 33, 39, 40, 41, 47, 48, 49, 79, 80, 81, 88, 89, 96, 127, 128]
-
-
-def power64(M, iters):
-    """The reference iteration in float64 on M [S,k,k]: every iterate [iters,S,k], the exit (first iteration at which
-    allclose holds for all seeds, else the cap) and the margins [iters,S,k] (<= 0: the entry passes)."""
-    v = np.ones(M.shape[:2])
-    its, margins, exit_t = [], [], iters
-    for t in range(1, iters + 1):
-        w = np.einsum("sij,sj->si", M, v)
-        w = w / (np.linalg.norm(w, axis=1, keepdims=True) + 1e-6)
-        margin = np.abs(w - v) - (1e-8 + 1e-5 * np.abs(v))
-        its.append(w)
-        margins.append(margin)
-        if exit_t == iters and (margin <= 0).all():
-            exit_t = t
-        v = w
-    return np.stack(its), exit_t, np.stack(margins)
-
-
-def check_power(compat, eig, power_iters, k, iters):
-    """One set: eig against the float64 iterate at the engine's exit, power_iters against the float64 exit where sure.
-    Returns (eig error / bound, eig error / band, exit compared)."""
-    M = compat.astype(np.float64)
-    its, exit64, margins = power64(M, iters)
-    t = int(power_iters)
-    assert 1 <= t <= iters
-    v64 = its[t - 1]
-    D = 2.01 * t * gamma(k + 3)
-    tol = (2 * math.expm1(D) + ((k + 1) / 2 + 4) * U) * v64 + 1e-30
-    err = np.abs(eig.astype(np.float64) - v64)
-    assert (err <= tol).all(), (t, float(err.max()), np.argwhere(err > tol)[:4])
-    band = lambda tt: C_BAND * math.sqrt(tt * (k + 3)) * U * its[tt - 1]             # noqa: E731
-    assert (err <= band(t) + 1e-30).all(), ("the statistical band", t, float((err / (band(t) + 1e-30)).max()))
-    sure = True
-    for tt in range(1, exit64 + 1):
-        prev = its[tt - 2] if tt > 1 else np.ones_like(v64)
-        w = band(tt) + (band(tt - 1) if tt > 1 else 0.0) + 3 * U * (np.abs(its[tt - 1] - prev) + 1e-8 + 1e-5 * prev)
-        mg = margins[tt - 1]
-        sure &= bool((mg < -w).all() or (mg > w).any())
-    if sure:
-        assert t == exit64, (t, exit64)
-    return float((err / tol).max()), float((err / (band(t) + 1e-30)).max()), sure
 
 
 def power_batch(N, B):
@@ -534,7 +438,7 @@ def power_batch(N, B):
 
 
 def run_power_case(precision, k, iters, B=8, N=400):
-    m = get_model("3dmatch", precision, k, iters)
+    m = get_model("3dmatch", precision, k=k, iters=iters)
     out = m.run(*power_batch(N, B), taps=["compat", "eig", "power_iters"])
     S = m.num_seeds(N)
     compat = out["compat"].cpu().numpy().reshape(B, S, k, k)

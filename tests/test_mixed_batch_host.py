@@ -5,6 +5,7 @@ import pytest
 import torch
 
 import evaluate
+from fakes import _fake_pipeline
 from pointdsc_b200 import PointDSC
 
 
@@ -33,20 +34,6 @@ def test_forward_many_rejects_bad_batches_before_the_engine():
     assert m.forward_many([]) == []
 
 
-class _Event:
-    clock = 0.0
-
-    def __init__(self, enable_timing=False):
-        self.t = None
-
-    def record(self):
-        _Event.clock += 1.0
-        self.t = _Event.clock
-
-    def elapsed_time(self, other):
-        return (other.t - self.t) * 1000.0           # ms: one second per recorded interval step
-
-
 class _Model:
     def __init__(self):
         self.calls = []
@@ -58,23 +45,6 @@ class _Model:
     def forward_many(self, batches):
         self.calls.append([b["src_keypts"].shape[1] for b in batches])
         return [{"final_trans": torch.eye(4)[None], "final_labels": torch.ones(1, b["src_keypts"].shape[1])} for b in batches]
-
-
-def _fake_pipeline(monkeypatch):
-    import pointdsc_b200.frontend as fe
-    import pointdsc_b200.metrics as me
-
-    def match(src_desc, tgt_desc, src_xyz, tgt_xyz, use_mutual=False):
-        n = int(src_desc)
-        return {"src_keypts": torch.zeros(1, n, 3), "tgt_keypts": torch.zeros(1, n, 3), "corr_pos": torch.zeros(1, n, 6)}
-
-    def eval_stats(trans, gt, src, tgt, labels, gt_labels, re_thre, te_thre):
-        return torch.full((1, 10), float(src.shape[1]))
-
-    monkeypatch.setattr(fe, "match", match)
-    monkeypatch.setattr(me, "eval_stats", eval_stats)
-    monkeypatch.setattr(evaluate, "gt_labels", lambda data, gt, thr: torch.ones(1, data["src_keypts"].shape[1]))
-    monkeypatch.setattr(torch.cuda, "Event", _Event)
 
 
 def test_evaluate_groups_pairs_and_splits_the_model_time(monkeypatch):
