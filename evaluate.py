@@ -15,12 +15,14 @@ What it replaces, line by line (reference file:line):
   evaluation/test_3DMatch.py:38-54            .cuda() + model(data)                                 -> model(data) on device tensors
   evaluation/test_3DMatch.py:83-101           TransformationLoss / ClassificationLoss per pair      -> eval_stats (one launch, no sync)
   evaluation/test_3DMatch.py:139-172          scene-level and pair-level summary                    -> summarise
+  evaluation/test_3DMatch.py:59-77            --solver RANSAC: open3d correspondence RANSAC      -> pointdsc_b200.ransac (row f6)
   evaluation/test_3DMatch.py:79-80            --use_icp: icp_refine (open3d registration_icp, r 0.10) -> pointdsc_b200.icp (row f5)
-The statistics of ALL pairs stay on the device and are read once at the end.  With --use_icp the network's transform is refined by
+The statistics of ALL pairs stay on the device and are read once at the end.  With --solver RANSAC the rows the network labelled
+as inliers go through correspondence RANSAC on the device (3-point samples, 5,000 iterations, max correspondence distance = the
+snapshot's inlier_threshold), whose transform and inliers replace the network's; with --use_icp the transform is then refined by
 point-to-point ICP over the pair's correspondence key points (max correspondence distance 0.10 for every snapshot, as the reference
-passes it) after the forward and before the statistics, inside the model time; the labels stay the network's.  RANSAC
-post-processing (open3d) and the FCGF network are out of scope (DESIGN.md section 8); the FCGF descriptors of the reference's data
-set are plain *.npz files and work."""
+passes it).  Both run after the forward and before the statistics, inside the model time, in the drivers' order.  The FCGF
+network is out of scope (DESIGN.md section 8); the FCGF descriptors of the reference's data set are plain *.npz files and work."""
 import argparse
 import json
 import os
@@ -148,7 +150,7 @@ def dataset_pairs(root, scenes, descriptor, device):
 
 
 @torch.no_grad()
-def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1, use_icp=False):
+def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1, use_icp=False, solver="SVD"):
     """The loop of evaluation/test_3DMatch.py:21-103 over an iterable of (scene index, (src xyz, src desc), (tgt xyz, tgt desc),
     gt_trans): returns a [pairs, 13] float64 array, columns = COLUMNS.
     batch_size 1: per pair `match`, labels, `model(data)` and `eval_stats`; the only read from the device inside the loop is the
@@ -160,28 +162,41 @@ def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1, u
     its share of the group's matching.  A model without `forward_packed` that offers `forward_many` (a wrapper or stand-in
     with the mixed-size interface only) is grouped pair by pair instead: `match`, labels, one `forward_many` per group and
     `eval_stats` per pair.
-    use_icp: the forward's transform is refined on the device before the statistics and inside the model-time events
-    (evaluation/test_3DMatch.py:79-80): `icp_refine` per pair, one `icp_refine_packed` per packed group."""
+    solver "RANSAC": the forward's labels and transform are replaced by correspondence RANSAC's over the rows the network kept
+    (evaluation/test_3DMatch.py:59-77, max correspondence distance cfg["inlier_threshold"]), on the device, before ICP and the
+    statistics and inside the model-time events: `ransac_refine` per pair, one `ransac_packed` per packed group.
+    use_icp: the transform is then refined on the device, also inside the model-time events (evaluation/test_3DMatch.py:79-80):
+    `icp_refine` per pair, one `icp_refine_packed` per packed group."""
     from pointdsc_b200.frontend import match, match_many
     from pointdsc_b200.metrics import eval_stats, eval_stats_packed
     rows, scene_ids, data_s, events = [], [], [], []
     packed = batch_size > 1 and hasattr(model, "forward_packed")
     group = []          # pairs waiting for the group: packed ((src xyz, src desc), (tgt xyz, tgt desc), gt), else (data, gt_t, labels)
+    if solver not in ("SVD", "RANSAC"):
+        raise ValueError(f"solver must be SVD or RANSAC, got {solver!r}")
     if use_icp:
         from pointdsc_b200 import icp
+    if solver == "RANSAC":
+        from pointdsc_b200 import ransac
 
-    def refine(data, trans):
-        return icp.icp_refine(data["src_keypts"], data["tgt_keypts"], trans) if use_icp else trans
+    def refine(data, res):
+        """(trans, labels) of a pair after the drivers' post-steps: RANSAC, then ICP."""
+        trans, labels = res["final_trans"], res["final_labels"]
+        if solver == "RANSAC":
+            trans, labels = ransac.ransac_refine(data["src_keypts"], data["tgt_keypts"], labels, cfg["inlier_threshold"])
+        if use_icp:
+            trans = icp.icp_refine(data["src_keypts"], data["tgt_keypts"], trans)
+        return trans, labels
 
     def run_pair_group():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         results = model.forward_many([g[0] for g in group])
-        trans = [refine(data, res["final_trans"]) for (data, _, _), res in zip(group, results)]
+        refined = [refine(data, res) for (data, _, _), res in zip(group, results)]
         e1.record()
-        for (data, gt_t, labels), res, tr in zip(group, results, trans):
-            rows.append(eval_stats(tr, gt_t[None], data["src_keypts"], data["tgt_keypts"], res["final_labels"],
-                                   labels, re_thre=cfg["re_thre"], te_thre=cfg["te_thre"]))
+        for (data, gt_t, labels), (tr, pred) in zip(group, refined):
+            rows.append(eval_stats(tr, gt_t[None], data["src_keypts"], data["tgt_keypts"], pred, labels, re_thre=cfg["re_thre"],
+                                   te_thre=cfg["te_thre"]))
             events.append((e0, e1, len(group)))
         group.clear()
 
@@ -198,11 +213,14 @@ def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1, u
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         res = model.forward_packed(m["corr_pos"], m["src_keypts"], m["tgt_keypts"], off, d_offsets=m["d_offsets"])
-        trans = res["final_trans"]
+        trans, pred = res["final_trans"], res["final_labels"]
+        if solver == "RANSAC":
+            trans, pred = ransac.ransac_packed(m["src_keypts"], m["tgt_keypts"], pred, off, d_offsets=m["d_offsets"],
+                                               max_correspondence_distance=cfg["inlier_threshold"])
         if use_icp:
             trans = icp.icp_refine_packed(m["src_keypts"], m["tgt_keypts"], trans, off, d_offsets=m["d_offsets"])
         e1.record()
-        rows.append(eval_stats_packed(trans, gts, m["src_keypts"], m["tgt_keypts"], res["final_labels"], labels, off,
+        rows.append(eval_stats_packed(trans, gts, m["src_keypts"], m["tgt_keypts"], pred, labels, off,
                                       d_offsets=m["d_offsets"], re_thre=cfg["re_thre"], te_thre=cfg["te_thre"]))
         events.extend([(e0, e1, len(group))] * len(group))
         group.clear()
@@ -233,10 +251,10 @@ def evaluate(model, pairs, cfg, use_mutual=False, device="cuda", batch_size=1, u
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         res = model(data)
-        trans = refine(data, res["final_trans"])
+        trans, pred = refine(data, res)
         e1.record()
-        rows.append(eval_stats(trans, gt_t[None], data["src_keypts"], data["tgt_keypts"], res["final_labels"], labels,
-                               re_thre=cfg["re_thre"], te_thre=cfg["te_thre"]))
+        rows.append(eval_stats(trans, gt_t[None], data["src_keypts"], data["tgt_keypts"], pred, labels, re_thre=cfg["re_thre"],
+                               te_thre=cfg["te_thre"]))
         events.append((e0, e1, 1))
         t_data = time.perf_counter()
     if group:
@@ -300,6 +318,9 @@ def parse_args(argv=None):
                     help="every pair's result independent of --batch_size and of the GPU's SM count (PointDSC batch_invariant)")
     ap.add_argument("--use_icp", action="store_true",
                     help="refine every transform by point-to-point ICP on the device (max correspondence distance 0.10)")
+    ap.add_argument("--solver", default="SVD", choices=["SVD", "RANSAC"],
+                    help="RANSAC: replace the network's transform and labels by correspondence RANSAC over the rows it kept "
+                         "(on the device, 5,000 iterations, max correspondence distance = the snapshot's inlier_threshold)")
     return ap.parse_args(argv)
 
 
@@ -318,7 +339,7 @@ def main(argv=None):
     if args.batch_size < 1:
         sys.exit("--batch_size must be >= 1")
     stats = evaluate(model, pairs, cfg, use_mutual=args.use_mutual or cfg["use_mutual"], batch_size=args.batch_size,
-                     use_icp=args.use_icp)
+                     use_icp=args.use_icp, solver=args.solver)
     summary = summarise(stats, names)
     if args.save_npy:
         np.save(args.save_npy, stats)

@@ -328,6 +328,30 @@ int pdsc_icp_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const i
                     double* d_fitness, double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
                     void* cuda_stream);
 
+/* f6: correspondence RANSAC over the pairs the network kept, replacing the drivers' --solver RANSAC block
+ * (evaluation/test_3DMatch.py:59-77): open3d 0.9's registration_ransac_based_on_correspondence with ransac_n = 3 and
+ * max_iteration = max_validation, over the rows with pred_labels > 0.  open3d is not part of the reference tree: this follows its
+ * published algorithm (oracle/ransac_oracle.py; PARITY UNPINNED), with draws of its own.  B sets as for pdsc_icp_packed (every set
+ * at least one row, else PDSC_ERR_SHAPE and pdsc_ransac_packed_scratch_bytes() returns 0; B <= 65535, else PDSC_ERR_UNSUPPORTED);
+ * d_src / d_tgt [R,3] the key points, d_labels [R] the forward's final_labels.  The candidates of set b are its rows with label > 0
+ * in ascending order, M_b of them.  Iteration i < max_iteration draws candidates (z >> 33) % M_b, z = SplitMix64(seed + (3 i + j + 1)
+ * * 0x9E3779B97F4A7C15) for j = 0, 1, 2, solves the unscaled Umeyama over them in double and counts the candidates with
+ * |R p + t - q|^2 < max_corr_dist * max_corr_dist (in double): good, rmse = sqrt(sum d^2 / good).  The winner is the hypothesis
+ * with the most inliers, then the smallest rmse, then the earliest iteration, among those with good > 0.  Outputs: d_trans
+ * [B,4,4] float32, the winner's 3-point solve; d_out_labels [R] (must not overlap the inputs) 1 on exactly its inliers, 0
+ * elsewhere; optional (may be NULL) d_fitness [B] (good / M_b), d_rmse [B], d_best [B] (the winning iteration, -1 when none),
+ * d_status [B] (0; 1: M_b < 3; 2: no hypothesis with an inlier; both return the identity and all-zero labels), d_hyp_good /
+ * d_hyp_rmse [B, max_iteration] (every hypothesis's key; 0 for a set with status 1).  PDSC_ERR_INVALID_ARGUMENT for null
+ * required pointers, max_corr_dist <= 0 or not finite and max_iteration < 1.  A set's outputs depend on its own rows, labels,
+ * max_corr_dist, max_iteration and seed only: bit for bit the same in any call, in any order, on any SM count.  Scratch:
+ * pdsc_ransac_packed_scratch_bytes() bytes, 16-byte aligned (0 for bad offsets or max_iteration < 1).  No host synchronisation,
+ * no allocation, capturable in a CUDA graph. */
+size_t pdsc_ransac_packed_scratch_bytes(int32_t B, const int32_t* h_offsets, int32_t max_iteration);
+int pdsc_ransac_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
+                       const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration, uint64_t seed,
+                       float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse, int32_t* d_best, int32_t* d_status,
+                       int32_t* d_hyp_good, double* d_hyp_rmse, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+
 /* Vertex positions of a PLY file (ascii or binary_little_endian; x, y, z float or double) into host memory as [n,3] float32.
  * Call with points = NULL to learn *n_vertices, then with a buffer of `capacity` >= n vertices. */
 int pdsc_read_ply(const char* path, float* points, int64_t capacity, int64_t* n_vertices);

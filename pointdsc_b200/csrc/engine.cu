@@ -1017,6 +1017,39 @@ int pdsc_icp_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const i
   return PDSC_OK;
 }
 
+size_t pdsc_ransac_packed_scratch_bytes(int32_t B, const int32_t* h_offsets, int32_t max_iteration) {
+  if (check_offsets("pdsc_ransac_packed_scratch_bytes", "", B, h_offsets, 1)) return 0;
+  if (max_iteration < 1) {
+    fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_ransac_packed_scratch_bytes: max_iteration must be >= 1 (got %d)", max_iteration);
+    return 0;
+  }
+  return pdsc::ransac_scratch_bytes(h_offsets[B], B, max_iteration);
+}
+
+int pdsc_ransac_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
+                       const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration, uint64_t seed,
+                       float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse, int32_t* d_best, int32_t* d_status,
+                       int32_t* d_hyp_good, double* d_hyp_rmse, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_offsets("pdsc_ransac_packed", "", B, h_offsets, 1)) return rc;
+  if (B > 65535) return fail(PDSC_ERR_UNSUPPORTED, "pdsc_ransac_packed: at most 65535 sets per call (got %d)", B);
+  if (!d_offsets || !d_src || !d_tgt || !d_labels || !d_trans || !d_out_labels)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_ransac_packed: null tensor pointer");
+  if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_ransac_packed: max_corr_dist must be positive and finite (got %g)", max_corr_dist);
+  if (max_iteration < 1)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_ransac_packed: max_iteration must be >= 1 (got %d)", max_iteration);
+  if (int rc = check_scratch("pdsc_ransac_packed", "scratch", d_scratch, scratch_bytes,
+                             pdsc::ransac_scratch_bytes(h_offsets[B], B, max_iteration), 16))
+    return rc;
+  DeviceGuard g(e->cfg.device);
+  pdsc::launch_ransac(B, d_offsets, h_offsets[B], d_src, d_tgt, d_labels, max_corr_dist, max_iteration, (unsigned long long)seed,
+                      d_trans, d_out_labels, d_fitness, d_rmse, d_best, d_status, d_hyp_good, d_hyp_rmse, d_scratch,
+                      static_cast<cudaStream_t>(cuda_stream));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
+
 // Host-side PLY vertex reader (ascii / binary_little_endian; x, y, z as float or double; other vertex properties skipped).
 int pdsc_read_ply(const char* path, float* points, int64_t capacity, int64_t* n_vertices) {
   if (!path || !n_vertices) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_read_ply: null argument");
