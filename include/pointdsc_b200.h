@@ -351,6 +351,15 @@ int pdsc_ransac_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, cons
                        const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration, uint64_t seed,
                        float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse, int32_t* d_best, int32_t* d_status,
                        int32_t* d_hyp_good, double* d_hyp_rmse, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+/* pdsc_ransac_packed with one more optional output, d_hyp_trans [B, max_iteration, 12] double (may be NULL): every hypothesis's
+ * [R | t], row-major, the transform its key was scored with; [I | 0] for a set with status 1 and for a sample with a non-finite
+ * coordinate.  A test output: the finish kernel solves every hypothesis once more to write it.  Same arguments, checks, scratch
+ * and results otherwise. */
+int pdsc_ransac_packed_hypotheses(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
+                                  const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration,
+                                  uint64_t seed, float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse,
+                                  int32_t* d_best, int32_t* d_status, int32_t* d_hyp_good, double* d_hyp_rmse, double* d_hyp_trans,
+                                  void* d_scratch, size_t scratch_bytes, void* cuda_stream);
 
 /* Vertex positions of a PLY file (ascii or binary_little_endian; x, y, z float or double) into host memory as [n,3] float32.
  * Call with points = NULL to learn *n_vertices, then with a buffer of `capacity` >= n vertices. */

@@ -1026,28 +1026,48 @@ size_t pdsc_ransac_packed_scratch_bytes(int32_t B, const int32_t* h_offsets, int
   return pdsc::ransac_scratch_bytes(h_offsets[B], B, max_iteration);
 }
 
+// pdsc_ransac_packed and pdsc_ransac_packed_hypotheses: one set of checks and one launch, under the caller's name
+static int ransac_packed(const char* fn, pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                         const float* d_src, const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration,
+                         uint64_t seed, float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse, int32_t* d_best,
+                         int32_t* d_status, int32_t* d_hyp_good, double* d_hyp_rmse, double* d_hyp_trans, void* d_scratch,
+                         size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_offsets(fn, "", B, h_offsets, 1)) return rc;
+  if (B > 65535) return fail(PDSC_ERR_UNSUPPORTED, "%s: at most 65535 sets per call (got %d)", fn, B);
+  if (!d_offsets || !d_src || !d_tgt || !d_labels || !d_trans || !d_out_labels)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_corr_dist must be positive and finite (got %g)", fn, max_corr_dist);
+  if (max_iteration < 1)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_iteration must be >= 1 (got %d)", fn, max_iteration);
+  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::ransac_scratch_bytes(h_offsets[B], B, max_iteration), 16))
+    return rc;
+  DeviceGuard g(e->cfg.device);
+  pdsc::launch_ransac(B, d_offsets, h_offsets[B], d_src, d_tgt, d_labels, max_corr_dist, max_iteration, (unsigned long long)seed,
+                      d_trans, d_out_labels, d_fitness, d_rmse, d_best, d_status, d_hyp_good, d_hyp_rmse, d_hyp_trans, d_scratch,
+                      static_cast<cudaStream_t>(cuda_stream));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
+
 int pdsc_ransac_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
                        const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration, uint64_t seed,
                        float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse, int32_t* d_best, int32_t* d_status,
                        int32_t* d_hyp_good, double* d_hyp_rmse, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_offsets("pdsc_ransac_packed", "", B, h_offsets, 1)) return rc;
-  if (B > 65535) return fail(PDSC_ERR_UNSUPPORTED, "pdsc_ransac_packed: at most 65535 sets per call (got %d)", B);
-  if (!d_offsets || !d_src || !d_tgt || !d_labels || !d_trans || !d_out_labels)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_ransac_packed: null tensor pointer");
-  if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_ransac_packed: max_corr_dist must be positive and finite (got %g)", max_corr_dist);
-  if (max_iteration < 1)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_ransac_packed: max_iteration must be >= 1 (got %d)", max_iteration);
-  if (int rc = check_scratch("pdsc_ransac_packed", "scratch", d_scratch, scratch_bytes,
-                             pdsc::ransac_scratch_bytes(h_offsets[B], B, max_iteration), 16))
-    return rc;
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_ransac(B, d_offsets, h_offsets[B], d_src, d_tgt, d_labels, max_corr_dist, max_iteration, (unsigned long long)seed,
-                      d_trans, d_out_labels, d_fitness, d_rmse, d_best, d_status, d_hyp_good, d_hyp_rmse, d_scratch,
-                      static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
+  return ransac_packed("pdsc_ransac_packed", e, B, h_offsets, d_offsets, d_src, d_tgt, d_labels, max_corr_dist, max_iteration, seed,
+                       d_trans, d_out_labels, d_fitness, d_rmse, d_best, d_status, d_hyp_good, d_hyp_rmse, nullptr, d_scratch,
+                       scratch_bytes, cuda_stream);
+}
+
+int pdsc_ransac_packed_hypotheses(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
+                                  const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration,
+                                  uint64_t seed, float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse,
+                                  int32_t* d_best, int32_t* d_status, int32_t* d_hyp_good, double* d_hyp_rmse, double* d_hyp_trans,
+                                  void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  return ransac_packed("pdsc_ransac_packed_hypotheses", e, B, h_offsets, d_offsets, d_src, d_tgt, d_labels, max_corr_dist,
+                       max_iteration, seed, d_trans, d_out_labels, d_fitness, d_rmse, d_best, d_status, d_hyp_good, d_hyp_rmse,
+                       d_hyp_trans, d_scratch, scratch_bytes, cuda_stream);
 }
 
 // Host-side PLY vertex reader (ascii / binary_little_endian; x, y, z as float or double; other vertex properties skipped).

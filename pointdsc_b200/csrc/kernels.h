@@ -133,12 +133,14 @@ void launch_icp(int B, const int32_t* d_off, long long R, const float* src, cons
 
 // ---- correspondence RANSAC over the pairs the network kept (ransac.cu) ----------------------------------------
 // B sets packed back to back (device offsets [B + 1], R = offsets[B] rows), labels [R] (> 0: a candidate), trans [B,4,4],
-// out_labels [R]; fitness, rmse, best, status [B] and hyp_good, hyp_rmse [B, max_iteration] may be null.  B <= 65535.
+// out_labels [R]; fitness, rmse, best, status [B], hyp_good, hyp_rmse [B, max_iteration] and hyp_trans [B, max_iteration, 12]
+// may be null.  B <= 65535.
 // Scratch: ransac_scratch_bytes(R, B, max_iteration) bytes, 16-byte aligned.
 size_t ransac_scratch_bytes(long long R, int B, int max_iteration);
 void launch_ransac(int B, const int32_t* d_off, long long R, const float* src, const float* tgt, const float* labels, double r,
                    int max_iteration, unsigned long long seed, float* trans, float* out_labels, double* fitness, double* rmse,
-                   int32_t* best, int32_t* status, int32_t* hyp_good, double* hyp_rmse, void* scratch, cudaStream_t st);
+                   int32_t* best, int32_t* status, int32_t* hyp_good, double* hyp_rmse, double* hyp_trans, void* scratch,
+                   cudaStream_t st);
 
 // ---- per-device launch configuration (device_state.cu) ----------------------------------------------------
 // opt `kernel` in to `bytes` of dynamic shared memory on the CURRENT device (no-op if already granted there)

@@ -24,7 +24,8 @@
 // hypotheses of one set).  Chosen from calls at batch size 1 (N = 1,000 / 5,000 / 12,000) and in groups of 8 and 64 sets on an
 // H100 SXM at 700 W (DESIGN.md §4): 32 and 256 were slower than 64 and 128 at most sizes, and 128 was as fast as 64 or faster
 // at every size, within the spread between runs.  CTAs of a set with M < 3 exit at once.  (3) finish: one CTA per set selects the winner, re-solves it with the same (non-inlined) device function,
-// so its T is bit-identical to the one scored, and writes the outputs.
+// so its T is bit-identical to the one scored, and writes the outputs.  When asked for every hypothesis's transform (hyp_trans,
+// a test output) it re-solves each iteration with that same function, so each [R | t] is the one its key was scored with.
 //
 // Cost.  max_iteration * M distance tests per set, about 27 fp64 operations each, plus one 3x3 Jacobi solve per hypothesis.
 #include <math.h>
@@ -137,6 +138,14 @@ __device__ __forceinline__ double ransac_d2(const double* R, const double* t, co
   return __fma_rn(ex, ex, __fma_rn(ey, ey, __dmul_rn(ez, ez)));
 }
 
+// [R | t] row-major, the layout of the winner's T below
+__device__ __forceinline__ void store_rigid(double* out, const Rigid& h) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    out[4 * r] = h.R[3 * r]; out[4 * r + 1] = h.R[3 * r + 1]; out[4 * r + 2] = h.R[3 * r + 2]; out[4 * r + 3] = h.t[r];
+  }
+}
+
 // key a ranks before key b: more inliers, then smaller rmse, then earlier iteration
 __device__ __forceinline__ bool key_before(int ga, double ra, int ia, int gb, double rb, int ib) {
   return ga > gb || (ga == gb && (ra < rb || (ra == rb && ia < ib)));
@@ -225,7 +234,8 @@ __global__ void __launch_bounds__(kRansacThreads) ransac_finish_kernel(const flo
                                                                        float* __restrict__ trans, float* __restrict__ out_labels,
                                                                        double* __restrict__ fitness_out, double* __restrict__ rmse_out,
                                                                        int32_t* __restrict__ best_out, int32_t* __restrict__ status_out,
-                                                                       int32_t* __restrict__ hyp_good, double* __restrict__ hyp_rmse) {
+                                                                       int32_t* __restrict__ hyp_good, double* __restrict__ hyp_rmse,
+                                                                       double* __restrict__ hyp_trans) {
   __shared__ int wg[kRansacWarps], wi[kRansacWarps];
   __shared__ double wr[kRansacWarps];
   __shared__ double T[12];
@@ -245,12 +255,15 @@ __global__ void __launch_bounds__(kRansacThreads) ransac_finish_kernel(const flo
       const double r = s.rmse[k0 + i];
       if (hyp_good) hyp_good[k0 + i] = g;
       if (hyp_rmse) hyp_rmse[k0 + i] = r;
+      if (hyp_trans) store_rigid(hyp_trans + 12 * (k0 + i), ransac_solve(cand, seed, i, M));
       if (g > 0 && (bi < 0 || key_before(g, r, i, bg, br, bi))) { bg = g; br = r; bi = i; }
     }
   } else {
     for (int i = tid; i < max_iteration; i += kRansacThreads) {
       if (hyp_good) hyp_good[k0 + i] = 0;
       if (hyp_rmse) hyp_rmse[k0 + i] = 0.0;
+      if (hyp_trans)
+        for (int k = 0; k < 12; ++k) hyp_trans[12 * (k0 + i) + k] = (k % 5 == 0) ? 1.0 : 0.0;
     }
   }
 #pragma unroll
@@ -266,10 +279,7 @@ __global__ void __launch_bounds__(kRansacThreads) ransac_finish_kernel(const flo
       if (wi[w] >= 0 && (bi < 0 || key_before(wg[w], wr[w], wi[w], bg, br, bi))) { bg = wg[w]; br = wr[w]; bi = wi[w]; }
     win = bi;
     if (bi >= 0) {
-      const Rigid h = ransac_solve(cand, seed, bi, M);
-      for (int r = 0; r < 3; ++r) {
-        T[4 * r] = h.R[3 * r]; T[4 * r + 1] = h.R[3 * r + 1]; T[4 * r + 2] = h.R[3 * r + 2]; T[4 * r + 3] = h.t[r];
-      }
+      store_rigid(T, ransac_solve(cand, seed, bi, M));
     } else {
       for (int k = 0; k < 12; ++k) T[k] = (k % 5 == 0) ? 1.0 : 0.0;
     }
@@ -296,7 +306,8 @@ __global__ void __launch_bounds__(kRansacThreads) ransac_finish_kernel(const flo
 
 void launch_ransac(int B, const int32_t* d_off, long long R, const float* src, const float* tgt, const float* labels, double r,
                    int max_iteration, unsigned long long seed, float* trans, float* out_labels, double* fitness, double* rmse,
-                   int32_t* best, int32_t* status, int32_t* hyp_good, double* hyp_rmse, void* scratch, cudaStream_t st) {
+                   int32_t* best, int32_t* status, int32_t* hyp_good, double* hyp_rmse, double* hyp_trans, void* scratch,
+                   cudaStream_t st) {
   const double r2 = r * r;
   const Offsets off{d_off, 0};
   const RansacScratch s = ransac_carve(scratch, R, B, max_iteration);
@@ -304,7 +315,7 @@ void launch_ransac(int B, const int32_t* d_off, long long R, const float* src, c
   const dim3 grid((unsigned)((max_iteration + kRansacChunk - 1) / kRansacChunk), (unsigned)B);
   ransac_score_kernel<<<grid, kRansacChunk, 0, st>>>(off, r2, max_iteration, seed, s);
   ransac_finish_kernel<<<B, kRansacThreads, 0, st>>>(labels, off, r2, max_iteration, seed, s, trans, out_labels, fitness, rmse, best,
-                                                     status, hyp_good, hyp_rmse);
+                                                     status, hyp_good, hyp_rmse, hyp_trans);
 }
 
 }  // namespace pdsc

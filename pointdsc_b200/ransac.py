@@ -3,7 +3,8 @@
 Replaces the block of evaluation/test_3DMatch.py:59-77 (and test_KITTI.py:59-77), which copies the correspondences the network
 labelled as inliers to the host, runs open3d 0.9's `registration_ransac_based_on_correspondence` (ransac_n 3, 5,000 iterations,
 max correspondence distance = the snapshot's inlier threshold) and replaces pred_trans by its transform and pred_labels by its
-inliers.  Here every set of a group runs on the H100 in one call (pdsc_ransac_packed) and nothing is read back.
+inliers.  Here every set of a group runs on the H100 in one call (pdsc_ransac_packed_hypotheses, which is pdsc_ransac_packed
+with the per-hypothesis transforms as one more optional output) and nothing is read back.
 
     from pointdsc_b200.ransac import ransac_refine      # evaluation/test_3DMatch.py:59-77, test_KITTI.py:59-77
     pred_trans, pred_labels = ransac_refine(src_keypts, tgt_keypts, pred_labels, config.inlier_threshold)
@@ -34,8 +35,9 @@ def ransac_packed(src: torch.Tensor, tgt: torch.Tensor, labels: torch.Tensor, of
     Returns (trans [B,4,4] float32, labels [R] float32: 1 on the winner's inliers).  With info=True a third item
     {'fitness' [B] float64, 'inlier_rmse' [B] float64, 'best_iteration' [B] int32 (-1: none), 'status' [B] int32 (1: fewer than 3
     candidates, 2: no hypothesis with an inlier; both give the identity and all-zero labels)}; with hypotheses=True it also holds
-    'hyp_good' [B, max_iteration] int32 and 'hyp_rmse' [B, max_iteration] float64, every hypothesis's key.  Nothing is read
-    back from the device."""
+    'hyp_good' [B, max_iteration] int32 and 'hyp_rmse' [B, max_iteration] float64, every hypothesis's key, and 'hyp_trans'
+    [B, max_iteration, 12] float64, the [R | t] (row-major) each key was scored with (a test output: it solves every hypothesis
+    once more).  Nothing is read back from the device."""
     if src.device.type != "cuda":
         raise _capi.PdscError("pointdsc_b200.ransac runs on an H100 only: pass CUDA tensors (there is no CPU fallback)")
     offsets = [int(o) for o in offsets]
@@ -61,6 +63,7 @@ def ransac_packed(src: torch.Tensor, tgt: torch.Tensor, labels: torch.Tensor, of
     ints = torch.empty(2, B, dtype=torch.int32, device=dev) if want else None
     hyp_good = torch.empty(B, max(int(max_iteration), 0), dtype=torch.int32, device=dev) if hypotheses else None
     hyp_rmse = torch.empty(B, max(int(max_iteration), 0), dtype=torch.float64, device=dev) if hypotheses else None
+    hyp_trans = torch.empty(B, max(int(max_iteration), 0), 12, dtype=torch.float64, device=dev) if hypotheses else None
     need = lib.pdsc_ransac_packed_scratch_bytes(B, h_off, int(max_iteration)) if max_iteration >= 1 else 0
     scratch = _capi.scratch(need, dev, 16)
 
@@ -70,16 +73,16 @@ def ransac_packed(src: torch.Tensor, tgt: torch.Tensor, labels: torch.Tensor, of
         return C.c_void_p((x[row] if row is not None else x).data_ptr())
 
     with torch.cuda.device(dev):
-        _capi.check(lib.pdsc_ransac_packed(engine, B, h_off, C.c_void_p(d_offsets.data_ptr()), C.c_void_p(s.data_ptr()),
-                                           C.c_void_p(t.data_ptr()), C.c_void_p(lab.data_ptr()), float(max_correspondence_distance),
-                                           int(max_iteration), C.c_uint64(int(seed) % (1 << 64)), C.c_void_p(trans.data_ptr()),
-                                           C.c_void_p(out_labels.data_ptr()), ptr(stats, 0), ptr(stats, 1), ptr(ints, 0), ptr(ints, 1),
-                                           ptr(hyp_good), ptr(hyp_rmse), C.c_void_p(scratch.data_ptr()), scratch.numel(), stream))
+        _capi.check(lib.pdsc_ransac_packed_hypotheses(
+            engine, B, h_off, C.c_void_p(d_offsets.data_ptr()), C.c_void_p(s.data_ptr()), C.c_void_p(t.data_ptr()),
+            C.c_void_p(lab.data_ptr()), float(max_correspondence_distance), int(max_iteration), C.c_uint64(int(seed) % (1 << 64)),
+            C.c_void_p(trans.data_ptr()), C.c_void_p(out_labels.data_ptr()), ptr(stats, 0), ptr(stats, 1), ptr(ints, 0),
+            ptr(ints, 1), ptr(hyp_good), ptr(hyp_rmse), ptr(hyp_trans), C.c_void_p(scratch.data_ptr()), scratch.numel(), stream))
     if not want:
         return trans, out_labels
     extra = {"fitness": stats[0], "inlier_rmse": stats[1], "best_iteration": ints[0], "status": ints[1]}
     if hypotheses:
-        extra.update(hyp_good=hyp_good, hyp_rmse=hyp_rmse)
+        extra.update(hyp_good=hyp_good, hyp_rmse=hyp_rmse, hyp_trans=hyp_trans)
     return trans, out_labels, extra
 
 
