@@ -113,44 +113,21 @@ void tc_free_weights(TcWeights* w) {
   w->arena_bytes = 0;
 }
 
-static inline int q_tiles(int N) { return (N + 127) / 128; }
-
-// key split of the attention (small calls): at most this many work items, each with a 64 KB partial O and 1 KB of (m, l)
-constexpr int kAttnSplitMaxItems = 320;
-constexpr size_t kAttnPartialBytes = 65536 + 1024;
-
-// work items whose partial results the scratch holds: a fixed kAttnSplitMaxItems in the default mode (its split is capped
-// there), every work item of a split call in the batch-invariant mode
-static size_t partial_items(int invariant, int attn_split, int attn_items) {
-  return invariant ? (attn_split ? (size_t)attn_items : 0) : (size_t)kAttnSplitMaxItems;
-}
-
-size_t tc_scratch_bytes_tiles(long long qtiles, long long ktiles, int invariant, int attn_split, int attn_items) {
-  return ((size_t)qtiles + (size_t)ktiles) * 65536 + 1024 + partial_items(invariant, attn_split, attn_items) * kAttnPartialBytes;
-}
-
-// Key split policy.  When a call's (set, query tile) items cover at most half of the SMs (the evaluation loops' bs = 1:
-// 8 items at N = 1000, 40 at N = 5000), the call is in the split regime: each set's items are split along the keys into sp
-// chunks of TS tiles, sp and TS a function of the set's N ONLY (attn_set_split, sets.cuh).  Calls of the small regime therefore
-// agree bit for bit whatever their batch size, and so do calls of the large regime (no split); across the two regimes the
-// softmax sums are associated differently (fp32 rounding, far inside the parity bar).  A call whose split would exceed
-// kAttnSplitMaxItems work items, or in which no set would split, is not split.
-// Batch-invariant mode: every set is split by attn_set_split_invariant (its N alone) in every call; the call runs the merge
-// whenever one of its sets has sp > 1.  No regime, no item cap: the partial buffers are sized by the call's items.
-int tc_packed_split(const int* Ns, int B, int invariant, int* items) {
-  const int num_sms = invariant ? 0 : device_sm_count();
-  long long qtiles = 0, split_items = 0;
-  for (int b = 0; b < B; ++b) {
-    int sp, ts;
-    if (invariant) attn_set_split_invariant(Ns[b], &sp, &ts);
-    else attn_set_split(Ns[b], num_sms, &sp, &ts);
-    qtiles += q_tiles(Ns[b]);
-    split_items += (long long)q_tiles(Ns[b]) * sp;
+TcScratch tc_scratch(void* base, const CallShape& plan) {
+  const size_t items = attn_partial_items(plan);
+  const size_t kv = (size_t)plan.qtiles * 65536;   // a 128-row Q tile and a 64-row K + V tile: 64 KB of hi | lo panels each
+  const size_t o = kv + (size_t)plan.ktiles * 65536;
+  const size_t ml = o + items * 128 * kC * sizeof(float);
+  TcScratch s{};
+  s.bytes = 1024 + ml + items * 128 * 2 * sizeof(float);   // 1024: room to align the start
+  if (base) {
+    uint8_t* p = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(base) + 1023) & ~uintptr_t(1023));
+    s.qimg = p;
+    s.kvimg = p + kv;
+    s.part_o = reinterpret_cast<float*>(p + o);
+    s.part_ml = reinterpret_cast<float*>(p + ml);
   }
-  const bool split = invariant ? split_items > qtiles
-                               : 2 * qtiles <= num_sms && split_items > qtiles && split_items <= kAttnSplitMaxItems;
-  *items = (int)(split ? split_items : qtiles);
-  return split ? 1 : 0;
+  return s;
 }
 
 int tc_launches(int num_layers, int attn_split) {   // layer0 + pad clear + 4 per layer (+ the merge of a key-split attention)
@@ -242,27 +219,25 @@ static cudaError_t tc_configure_fmt() {
 
 template <int FMT>
 static int tc_encoder_forward_fmt(const TcWeights& w, const TcForwardArgs& a, cudaStream_t st) {
-  const long long rows = a.rows;
+  const CallShape& plan = a.plan;
+  const long long rows = (long long)plan.R;
   if (rows >= (1LL << 31)) return (int)cudaErrorInvalidValue;  // kernels index rows with 32-bit arithmetic
-  uint8_t* qimg = static_cast<uint8_t*>(a.scratch);
-  qimg = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(qimg) + 1023) & ~uintptr_t(1023));
-  uint8_t* kvimg = qimg + (size_t)a.qtiles * 65536;
-  float* part_o = reinterpret_cast<float*>(kvimg + (size_t)a.ktiles * 65536);
-  float* part_ml = part_o + partial_items(a.attn_invariant, a.attn_split, a.attn_items) * 128 * kC;
+  const TcScratch s = tc_scratch(a.scratch, plan);
+  uint8_t *qimg = s.qimg, *kvimg = s.kvimg;
   const long long tiles = (rows + 127) / 128;
-  const int num_sms = device_sm_count();
+  const int num_sms = plan.num_sms;
   if (num_sms <= 0) return (int)cudaErrorInvalidDevice;
   const int grid = (int)(tiles < num_sms ? tiles : num_sms);
   const uint8_t* arena = static_cast<const uint8_t*>(w.arena) + (size_t)FMT * w.num_layers * kLayerBytes;
 
   launch_layer0(a.corr_pos, a.l0w, a.l0b, a.feat, rows, a.in_dim, st);
-  tc_clear_pads_kernel<<<a.nsets, 256, 0, st>>>(kvimg, a.sets);
+  tc_clear_pads_kernel<<<plan.B, 256, 0, st>>>(kvimg, a.sets);
   for (int l = 0; l < a.num_layers; ++l) {
     const uint8_t* base = arena + (size_t)l * kLayerBytes;
     const bool last = l + 1 == a.num_layers;
     ChainArgs c{};
     c.rows = rows; c.split = a.split;
-    c.sets = a.sets; c.tile_set = a.tile_set; c.nsets = a.nsets;
+    c.sets = a.sets; c.tile_set = a.tile_set; c.nsets = plan.B;
     c.qimg = qimg; c.kvimg = kvimg; c.bias = reinterpret_cast<const float*>(base + kBias);
     if (l == 0) {   // PointCN + Q
       c.in = a.feat; c.out_f32 = a.feat1; c.wimg = base + kW1; c.wbytes = 131072;
@@ -275,17 +250,17 @@ static int tc_encoder_forward_fmt(const TcWeights& w, const TcForwardArgs& a, cu
     c.in = a.feat1; c.out_f32 = nullptr; c.wimg = base + kWk; c.wbytes = 131072;
     launch_chain<kKV, FMT>(grid, c, st);
     // attention
-    const AttnArgs at{a.split, qimg, kvimg, a.sc, a.msg, a.attn_items, part_o, part_ml, a.sets, a.nsets};
+    const AttnArgs at{a.split, qimg, kvimg, a.sc, a.msg, plan.attn_items, s.part_o, s.part_ml, a.sets, plan.B};
     if (a.attn_events) cudaEventRecord(a.attn_events[2 * l], st);
     tc_attention_persistent_kernel<FMT><<<at.items < num_sms ? at.items : num_sms, kAttnThreads, kAttnPSmem, st>>>(at);
-    if (a.attn_split)   // some sets are split: their merge runs per query tile
-      tc_attention_merge_kernel<<<(unsigned)(a.qtiles * 4), 256, 0, st>>>(part_o, part_ml, a.msg, a.sets, a.nsets);
+    if (plan.attn_split)   // some sets are split: their merge runs per query tile
+      tc_attention_merge_kernel<<<(unsigned)(plan.qtiles * 4), 256, 0, st>>>(s.part_o, s.part_ml, a.msg, a.sets, plan.B);
     if (a.attn_events) cudaEventRecord(a.attn_events[2 * l + 1], st);
     if (a.debug_out && a.debug_layer == l) {
       const size_t plane = (size_t)rows * kC;
       tc_unblock_f32_kernel<<<(unsigned)((plane / 4 + 255) / 256), 256, 0, st>>>(a.feat1, a.debug_out, rows);
       tc_decode_kernel<FMT><<<(unsigned)((plane + 255) / 256), 256, 0, st>>>(qimg, kvimg, a.debug_out + plane, a.debug_out + 2 * plane,
-                                                                             a.debug_out + 3 * plane, rows, a.sets, a.nsets, a.split);
+                                                                             a.debug_out + 3 * plane, rows, a.sets, plan.B, a.split);
       cudaMemcpyAsync(a.debug_out + 4 * plane, a.msg, plane * sizeof(float), cudaMemcpyDeviceToDevice, st);
     }
     // fc_message + residual; then, but for the last layer (the head reads its feat), the next layer's PointCN, which

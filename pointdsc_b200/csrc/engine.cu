@@ -115,6 +115,7 @@ struct pdsc_engine {
 
 namespace {
 
+using pdsc::CallShape;
 using pdsc::kC;
 
 struct Carver {
@@ -142,42 +143,10 @@ struct Workspace {
   size_t bytes;
 };
 
-// What a call needs to size its launches and its workspace: B sets of Ns[b] rows.  N, S and k are the largest of its sets
-// (launch sizes), k_min the smallest k of its sets with seeds, and the totals sum over the sets.
-struct CallShape {
-  int B = 0, N = 0, S = 0, k = 0, k_min = 0;
-  size_t R = 0;
-  size_t sc_rowmajor = 0, sc_tiled = 0;   // floats of the row-major (fp32) and tiled (tensor-core) SC layouts
-  size_t seeds = 0, dist = 0, knn = 0;    // seed slots, seed-row distance floats, neighbour slots
-  long long qtiles = 0, ktiles = 0;
-  int attn_items = 0, attn_split = 0;     // tensor-core calls (tc_packed_split)
-  int attn_invariant = 0;                 // the engine's key-split policy (pdsc_set_batch_invariant)
-};
-
 // h_offsets: the validated offsets of a packed call, or nullptr for a uniform call of B sets of N rows
 CallShape call_shape(const pdsc_engine* e, int B, int N_uniform, const int32_t* h_offsets) {
-  CallShape s;
-  s.B = B;
-  s.k_min = e->cfg.k;
-  std::vector<int> Ns(B);
-  for (int b = 0; b < B; ++b) {
-    const int N = h_offsets ? h_offsets[b + 1] - h_offsets[b] : N_uniform;
-    const int S = pdsc_num_seeds(e, N), k = pdsc_num_neighbours(e, N);
-    Ns[b] = N;
-    s.R += (size_t)N;
-    s.N = std::max(s.N, N); s.S = std::max(s.S, S); s.k = std::max(s.k, k);
-    if (S > 0) s.k_min = std::min(s.k_min, k);
-    s.sc_rowmajor += (size_t)N * pdsc::round_up(N, 64);
-    s.sc_tiled += (size_t)((N + 63) / 64) * ((N + 127) / 128) * 8192;
-    s.seeds += S;
-    s.dist += ((size_t)S * N + 3) & ~size_t(3);       // every set's block starts 16-byte aligned (vector loads)
-    s.knn += (size_t)S * k;
-    s.qtiles += (N + 127) / 128;
-    s.ktiles += (N + 63) / 64;
-  }
-  s.attn_invariant = e->batch_invariant ? 1 : 0;
-  if (e->cfg.precision != PDSC_FP32_SIMT) s.attn_split = pdsc::tc_packed_split(Ns.data(), B, s.attn_invariant, &s.attn_items);
-  return s;
+  return pdsc::plan_call(B, N_uniform, h_offsets, e->cfg.ratio, e->cfg.k, e->cfg.precision != PDSC_FP32_SIMT,
+                         e->batch_invariant ? 1 : 0, pdsc::device_sm_count());
 }
 
 Workspace carve(const pdsc_engine* e, void* ptr, const CallShape& sh) {
@@ -198,7 +167,7 @@ Workspace carve(const pdsc_engine* e, void* ptr, const CallShape& sh) {
     w.h2 = c.take<float>(R * 64);
     w.tc_scratch = nullptr;
   } else {
-    w.tc_scratch = c.take<char>(pdsc::tc_scratch_bytes_tiles(sh.qtiles, sh.ktiles, sh.attn_invariant, sh.attn_split, sh.attn_items));
+    w.tc_scratch = c.take<char>(pdsc::tc_scratch(nullptr, sh).bytes);
   }
   w.normed = c.take<float>(R * kC);
   w.conf = c.take<float>(R);
@@ -359,15 +328,10 @@ __global__ void set_table_kernel(const int32_t* __restrict__ offsets, int N_unif
       row0 = offsets ? offsets[b] : b * N_uniform;
       N = offsets ? offsets[b + 1] - row0 : N_uniform;
     }
-    const int S = pdsc::num_seeds(N, ratio);         // as pdsc_num_seeds
-    const int k = live ? max(min(k_cfg, N - 1), 0) : 0;
-    const int QT = (N + 127) / 128, KT = (N + 63) / 64;
-    int sp = 1, TS = KT;
-    if (split && invariant) pdsc::attn_set_split_invariant(N, &sp, &TS);
-    else if (split) pdsc::attn_set_split(N, num_sms, &sp, &TS);
-    const long long size[7] = {QT, KT, S, (long long)QT * sp,
-                               tiled ? (long long)KT * QT * 8192 : (long long)N * pdsc::round_up(N, 64),
-                               ((long long)S * N + 3) & ~3ll, (long long)S * k};
+    const pdsc::SetSizes z = pdsc::set_sizes(N, ratio, k_cfg);   // the plan's rule (plan_call); N = 0 past the last set
+    int sp = 1, TS = z.KT;
+    if (split) pdsc::attn_key_split(N, invariant, num_sms, &sp, &TS);
+    const long long size[7] = {z.QT, z.KT, z.S, (long long)z.QT * sp, tiled ? z.sc_tiled : z.sc_rowmajor, z.dist, z.knn};
     long long first[7];
 #pragma unroll
     for (int i = 0; i < 7; ++i) {
@@ -377,7 +341,7 @@ __global__ void set_table_kernel(const int32_t* __restrict__ offsets, int N_unif
     }
     if (live) {
       pdsc::SetDesc d;
-      d.row0 = row0; d.N = N; d.S = S; d.k = k;
+      d.row0 = row0; d.N = N; d.S = z.S; d.k = z.k;
       d.qt0 = (int)first[0]; d.kt0 = (int)first[1]; d.seed0 = (int)first[2]; d.item0 = (int)first[3];
       d.sp = sp; d.TS = TS; d.pad0 = d.pad1 = 0;
       d.sc0 = first[4]; d.dist0 = first[5]; d.knn0 = first[6];
@@ -538,8 +502,7 @@ int32_t pdsc_num_seeds(const pdsc_engine* e, int32_t N) {
 }
 int32_t pdsc_num_neighbours(const pdsc_engine* e, int32_t N) {
   if (!e) return 0;
-  const int k = e->cfg.k < N - 1 ? e->cfg.k : N - 1;  // k = min(self.k, num_corr - 1)  (PointDSC.py:250)
-  return k < 0 ? 0 : k;
+  return pdsc::set_sizes(N, e->cfg.ratio, e->cfg.k).k;
 }
 
 size_t pdsc_workspace_bytes(const pdsc_engine* e, int32_t B, int32_t N) {
@@ -586,7 +549,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
   const bool inject_feat = io && io->in_features;
   if (!inject_feat && !d_corr_pos) return fail(PDSC_ERR_INVALID_ARGUMENT, "corr_pos is null");
   if (io && io->in_confidence && !inject_feat) return fail(PDSC_ERR_INVALID_ARGUMENT, "in_confidence requires in_features");
-  DeviceGuard g(e->cfg.device);   // tc_packed_split reads the SM count of the engine's device
+  DeviceGuard g(e->cfg.device);   // the plan reads the SM count of the engine's device
   const CallShape sh = call_shape(e, B, N, h_offsets);
   if (int rc = check_scratch("pdsc_forward", "workspace", d_workspace, workspace_bytes, carve(e, nullptr, sh).bytes, 256))
     return rc;
@@ -594,11 +557,10 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
   const Workspace w = carve(e, d_workspace, sh);
   N = sh.N;                        // a packed call: the largest set, which sizes the launches
   const size_t R = sh.R;
-  const int NS = round_up(N, 64);
   const int S = sh.S, k = sh.k, T = e->cfg.num_iterations;
   const SetDesc* sets = w.sets;
   set_table_kernel<<<1, 32, 0, st>>>(d_offsets, N, B, e->cfg.ratio, e->cfg.k, e->cfg.precision == PDSC_FP32_SIMT ? 0 : 1,
-                                     sh.attn_split, sh.attn_invariant, device_sm_count(), w.sets, w.tile_set);
+                                     sh.attn_split, sh.attn_invariant, sh.num_sms, w.sets, w.tile_set);
   const float* W = e->d_weights;
   const int L = e->cfg.num_layers;
   cudaEvent_t* attn_ev = nullptr;
@@ -620,8 +582,8 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
     if (corr_ready) PDSC_CUDA(cudaStreamWaitEvent(st, corr_ready, 0));
     if (io && io->out_sc) {
       if (simt)
-        cudaMemcpy2DAsync(io->out_sc, (size_t)N * sizeof(float), w.sc, (size_t)NS * sizeof(float), (size_t)N * sizeof(float),
-                          R, cudaMemcpyDeviceToDevice, st);
+        cudaMemcpy2DAsync(io->out_sc, (size_t)N * sizeof(float), w.sc, (size_t)set_sizes(N, e->cfg.ratio, e->cfg.k).NS * sizeof(float),
+                          (size_t)N * sizeof(float), R, cudaMemcpyDeviceToDevice, st);
       else
         launch_sc_untile(w.sc, io->out_sc, B, N, st);
     }
@@ -629,8 +591,8 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
       const int rc = encoder_simt(e, w, sh, d_corr_pos, io, attn_ev, st);
       if (rc) return rc;
     } else {
-      TcForwardArgs a{};
-      a.nsets = B; a.in_dim = e->cfg.in_dim; a.num_layers = e->cfg.num_layers;
+      TcForwardArgs a{sh};
+      a.in_dim = e->cfg.in_dim; a.num_layers = e->cfg.num_layers;
       a.split = (e->cfg.precision == PDSC_BF16X3 || e->cfg.precision == PDSC_FP16X3) ? 1 : 0;
       a.fmt = (e->cfg.precision == PDSC_FP16X3) ? 0 : 1;
       a.corr_pos = d_corr_pos; a.l0w = W + e->off_l0w; a.l0b = W + e->off_l0b;
@@ -640,8 +602,7 @@ static int forward_impl(pdsc_engine* e, int mode, int32_t B, int32_t N, const in
       a.debug_layer = io ? io->layer_tap : -1;
       a.debug_out = io ? io->out_layer_debug : nullptr;
       a.attn_events = attn_ev;
-      a.sets = sets; a.tile_set = w.tile_set; a.rows = (long long)R; a.qtiles = sh.qtiles; a.ktiles = sh.ktiles;
-      a.attn_items = sh.attn_items; a.attn_split = sh.attn_split; a.attn_invariant = sh.attn_invariant;
+      a.sets = sets; a.tile_set = w.tile_set;
       const int rc = tc_encoder_forward(e->tc, a, st);
       if (rc) return fail(PDSC_ERR_CUDA, "tensor-core encoder launch failed: %s", cudaGetErrorString((cudaError_t)rc));
     }

@@ -1,13 +1,13 @@
-"""The engine's launch rules, restated once for the tests: the attention's key split (sets.cuh, encoder_tc.cu
-tc_packed_split), the seed count, the workspace layout (engine.cu call_shape / carve, encoder_tc.cu tc_scratch_bytes_tiles)
-and the front end's launch plans (frontend.cu, eig_power.cu, fpfh.cu).  The tests assert that the engine reaches what these
-predict, and the memory contract that the restated workspace adds up to pdsc_workspace_bytes(_packed), so the restatement
-cannot drift from the engine unnoticed."""
+"""The engine's launch rules, restated once for the tests: the attention's key split (sets.cuh attn_set_split*,
+attn_call_splits), the seed count and a set's sizes (sets.cuh num_seeds, set_sizes), the workspace layout (sets.cuh
+plan_call, engine.cu carve, encoder_tc.cu tc_scratch) and the front end's launch plans (frontend.cu, eig_power.cu, fpfh.cu).
+The tests assert that the engine reaches what these predict, and the memory contract that the restated workspace adds up
+to pdsc_workspace_bytes(_packed), so the restatement cannot drift from the engine unnoticed."""
 C_CH = 128                      # num_channels
 RATIO = 0.1                     # cfg.ratio
 TSI = 8                         # sets.cuh kAttnInvariantTiles
-SPLIT_MAX_ITEMS = 320           # encoder_tc.cu kAttnSplitMaxItems
-PARTIAL_BYTES = 65536 + 1024    # encoder_tc.cu kAttnPartialBytes: one split work item's partial O and (m, l)
+SPLIT_MAX_ITEMS = 320           # sets.cuh kAttnSplitMaxItems
+PARTIAL_BYTES = 65536 + 1024    # encoder_tc.cu tc_scratch: one split work item's partial O and (m, l)
 SETDESC_BYTES = 72              # sets.cuh SetDesc: 12 int32 + 3 int64
 
 
@@ -30,14 +30,24 @@ def attn_set_split_invariant(N):
     return sp, -(-KT // sp)
 
 
+def call_splits(qtiles, items, sms, invariant):
+    """Whether a call of `qtiles` query tiles, `items` work items when its sets are split, runs split."""
+    return items > qtiles if invariant else (2 * qtiles <= sms and qtiles < items <= SPLIT_MAX_ITEMS)
+
+
 def call_split(Ns, sms, invariant):
     """(split?, work items, [(sp, TS)] per set) of a tensor-core call; unsplit, every set is one item per query tile over
     all its key tiles."""
     per = [attn_set_split_invariant(n) if invariant else attn_set_split(n, sms) for n in Ns]
     qtiles = sum(-(-n // 128) for n in Ns)
     items = sum(-(-n // 128) * sp for n, (sp, _) in zip(Ns, per))
-    split = items > qtiles if invariant else (2 * qtiles <= sms and qtiles < items <= SPLIT_MAX_ITEMS)
+    split = call_splits(qtiles, items, sms, invariant)
     return split, (items if split else qtiles), (per if split else [(1, -(-n // 64)) for n in Ns])
+
+
+def partial_items(split, items, invariant):
+    """Work items whose partial O and (m, l) the tensor-core scratch holds."""
+    return (items if split else 0) if invariant else SPLIT_MAX_ITEMS
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -48,16 +58,23 @@ def num_seeds(N, ratio=RATIO):
     return len(range(N)[:int(N * ratio)])
 
 
+def set_sizes(N, k_cfg, ratio=RATIO):
+    """One set's terms of the workspace: seeds, neighbours, query / key tiles, the row length of the row-major SC, the floats
+    of its SC block (row-major and tiled), of its seed-row distance block, and its neighbour slots."""
+    S, k = num_seeds(N, ratio), max(min(k_cfg, N - 1), 0)
+    QT, KT = -(-N // 128), -(-N // 64)
+    return {"S": S, "k": k, "QT": QT, "KT": KT, "NS": KT * 64, "sc_rowmajor": N * KT * 64, "sc_tiled": KT * QT * 8192,
+            "dist": (S * N + 3) & ~3, "knn": S * k}
+
+
 def mirror_workspace(Ns, precision, invariant, k_cfg, sms, iters=10):
     """[(name, offset, bytes, kind)] and the total of carve(call_shape(Ns)); kind: float / index / mask / best / zero."""
     R = sum(Ns)
     B = len(Ns)
-    seeds = sum(num_seeds(n) for n in Ns)
-    dist = sum((num_seeds(n) * n + 3) & ~3 for n in Ns)
-    knn = sum(num_seeds(n) * max(min(k_cfg, n - 1), 0) for n in Ns)
-    sc_row = sum(n * (-(-n // 64) * 64) for n in Ns)
-    sc_tiled = sum(-(-n // 64) * -(-n // 128) * 8192 for n in Ns)
-    qtiles, ktiles = sum(-(-n // 128) for n in Ns), sum(-(-n // 64) for n in Ns)
+    sizes = [set_sizes(n, k_cfg) for n in Ns]
+    seeds, dist, knn = (sum(z[key] for z in sizes) for key in ("S", "dist", "knn"))
+    sc_row, sc_tiled = (sum(z[key] for z in sizes) for key in ("sc_rowmajor", "sc_tiled"))
+    qtiles, ktiles = (sum(z[key] for z in sizes) for key in ("QT", "KT"))
     regions, off = [], 0
 
     def take(name, count, size, kind):
@@ -77,8 +94,7 @@ def mirror_workspace(Ns, precision, invariant, k_cfg, sms, iters=10):
         take("h2", R * 64, 4, "float")
     else:
         split, items, _ = call_split(Ns, sms, invariant)
-        partial = (items if split else 0) if invariant else SPLIT_MAX_ITEMS
-        take("tc_scratch", (qtiles + ktiles) * 65536 + 1024 + partial * PARTIAL_BYTES, 1, "float")
+        take("tc_scratch", (qtiles + ktiles) * 65536 + 1024 + partial_items(split, items, invariant) * PARTIAL_BYTES, 1, "float")
     take("normed", R * C_CH, 4, "float")
     take("conf", R, 4, "float")
     take("key", R, 4, "float")

@@ -17,9 +17,9 @@ Results must be bit-identical across patterns; every output and tap element must
 SC matrix in the workspace, whose pad columns the contract says are written as 0 (a pad column only feeds discarded query
 rows, so no output shows it).
 
-Workspace regions.  carve() and call_shape() (engine.cu) are restated in engine_rules.py (mirror_workspace), including
-tc_scratch_bytes_tiles and the key-split rules attn_set_split / attn_set_split_invariant / tc_packed_split (sets.cuh,
-encoder_tc.cu), and every GPU test asserts that the restatement's total equals pdsc_workspace_bytes(_packed), so the map
+Workspace regions.  carve() (engine.cu) and plan_call() (sets.cuh) are restated in engine_rules.py (mirror_workspace),
+including tc_scratch (encoder_tc.cu) and the key-split rules attn_set_split / attn_set_split_invariant / attn_call_splits
+(sets.cuh), and every GPU test asserts that the restatement's total equals pdsc_workspace_bytes(_packed), so the map
 cannot drift from the engine.  Float regions get the float patterns.  Control and index regions only get values that keep
 every read in bounds, whatever a kernel does with them: seeds / knn / counts 0 or 1 (N >= 2), conv_mask 0 or all ones,
 best_key 0 or 0xFFFFFFFF00000000, and zeros for the descriptor table and tile_set (a zero descriptor is N = 0, which every
