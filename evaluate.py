@@ -17,11 +17,15 @@ What it replaces, line by line (reference file:line):
   evaluation/test_3DMatch.py:139-172          scene-level and pair-level summary                    -> summarise
   evaluation/test_3DMatch.py:59-77            --solver RANSAC: open3d correspondence RANSAC      -> pointdsc_b200.ransac (row f6)
   evaluation/test_3DMatch.py:79-80            --use_icp: icp_refine (open3d registration_icp, r 0.10) -> pointdsc_b200.icp (row f5)
+  baseline_scripts/baseline_3DMatch.py:19-53  --method SM: the spectral-matching baseline in place of the network
+                                                                                         -> pointdsc_b200.spectral
 The statistics of ALL pairs stay on the device and are read once at the end.  With --solver RANSAC the rows the network labelled
 as inliers go through correspondence RANSAC on the device (3-point samples, 5,000 iterations, max correspondence distance = the
 snapshot's inlier_threshold), whose transform and inliers replace the network's; with --use_icp the transform is then refined by
 point-to-point ICP over the pair's correspondence key points (max correspondence distance 0.10 for every snapshot, as the reference
-passes it).  Both run after the forward and before the statistics, inside the model time, in the drivers' order.  The FCGF
+passes it).  Both run after the forward and before the statistics, inside the model time, in the drivers' order.  With
+--method SM the spectral-matching baseline (inlier threshold = the snapshot's) takes the forward's place, inside the model time;
+no network is loaded, and the baseline script has neither RANSAC nor ICP, so --method SM refuses both.  The FCGF
 network is out of scope (DESIGN.md section 8); the FCGF descriptors of the reference's data set are plain *.npz files and work."""
 import argparse
 import json
@@ -147,6 +151,25 @@ def dataset_pairs(root, scenes, descriptor, device):
     for si, scene in enumerate(scenes):
         for src_id, tgt_id, gt in list_pairs(root, scene):
             yield si, load_fragment(root, scene, src_id, descriptor, device), load_fragment(root, scene, tgt_id, descriptor, device), gt
+
+
+class SpectralMatching:
+    """The spectral-matching baseline with the two calls `evaluate` makes of a model: `model(data)` per pair and
+    `forward_packed` per group (baseline_scripts/baseline_3DMatch.py:19-53, `SM(corr, src_keypts, tgt_keypts, args)`)."""
+
+    def __init__(self, inlier_threshold):
+        self.inlier_threshold = float(inlier_threshold)
+
+    def __call__(self, data):
+        from pointdsc_b200.spectral import spectral_matching
+        trans, labels = spectral_matching(data["corr_pos"], data["src_keypts"], data["tgt_keypts"], self.inlier_threshold)
+        return {"final_trans": trans, "final_labels": labels}
+
+    def forward_packed(self, corr_pos, src_keypts, tgt_keypts, offsets, d_offsets=None):
+        from pointdsc_b200.spectral import spectral_matching_packed
+        trans, labels = spectral_matching_packed(corr_pos, src_keypts, tgt_keypts, offsets, d_offsets=d_offsets,
+                                                 inlier_threshold=self.inlier_threshold)
+        return {"final_trans": trans, "final_labels": labels}
 
 
 @torch.no_grad()
@@ -321,6 +344,9 @@ def parse_args(argv=None):
     ap.add_argument("--solver", default="SVD", choices=["SVD", "RANSAC"],
                     help="RANSAC: replace the network's transform and labels by correspondence RANSAC over the rows it kept "
                          "(on the device, 5,000 iterations, max correspondence distance = the snapshot's inlier_threshold)")
+    ap.add_argument("--method", default="PointDSC", choices=["PointDSC", "SM"],
+                    help="SM: the spectral-matching baseline (baseline_scripts/baseline_3DMatch.py) in place of the network, "
+                         "with the snapshot's inlier_threshold; no RANSAC, no ICP")
     return ap.parse_args(argv)
 
 
@@ -328,7 +354,12 @@ def main(argv=None):
     args = parse_args(argv)
     cfg = load_config(args.chosen_snapshot)
     descriptor = args.descriptor or cfg["descriptor"]
-    model = build_model(args.chosen_snapshot, cfg, "cuda", args.precision, args.batch_invariant)
+    if args.method == "SM":
+        if args.solver != "SVD" or args.use_icp:
+            sys.exit("--method SM runs the spectral-matching baseline alone: it takes neither --solver RANSAC nor --use_icp")
+        model = SpectralMatching(cfg["inlier_threshold"])
+    else:
+        model = build_model(args.chosen_snapshot, cfg, "cuda", args.precision, args.batch_invariant)
     if args.synthetic > 0:
         pairs, names = synthetic_pairs(args.synthetic, "cuda", 1.6 * cfg["downsample"]), ["synthetic-a", "synthetic-b"]
     else:

@@ -361,6 +361,24 @@ int pdsc_ransac_packed_hypotheses(pdsc_engine* e, int32_t B, const int32_t* h_of
                                   int32_t* d_best, int32_t* d_status, int32_t* d_hyp_good, double* d_hyp_rmse, double* d_hyp_trans,
                                   void* d_scratch, size_t scratch_bytes, void* cuda_stream);
 
+/* The classical spectral-matching baseline SM (baseline_scripts/baseline_3DMatch.py:19-53) for B sets in one call.  Set b owns
+ * rows [offsets[b], offsets[b+1]) of d_corr_pos [R,6] (the centred corr_pos of the evaluation loop) and of d_src_keypts /
+ * d_tgt_keypts [R,3]; offsets as for pdsc_icp_packed, every set between 1 and 16,384 rows (else PDSC_ERR_SHAPE, and
+ * pdsc_spectral_matching_packed_scratch_bytes() returns 0); B <= 65535, else PDSC_ERR_UNSUPPORTED.  Per set of N rows:
+ * M_ij = max(0, 4.5 - (||c_j[0:3] - c_i[0:3]|| - ||c_j[3:6] - c_i[3:6]||)^2 / (2 sigma^2)), sigma = inlier_threshold / 3,
+ * M_ii = 0 (never stored); v = 1, then exactly ten v <- M v / (||M v|| + 1e-6); labels = 1 on the S = int(N * 0.1) largest
+ * entries of v (ties: the lowest row first), 0 elsewhere; T = rigid_transform_3d(src, tgt, v * labels) (models/common.py:7-45),
+ * the identity when every weight is 0 (S = 0 included).  Outputs: d_trans [B,4,4] float32, d_labels [R] float32, optional
+ * d_eigenvector [R] float32 (v).  PDSC_ERR_INVALID_ARGUMENT for null required pointers and an inlier_threshold <= 0 or not
+ * finite.  A set's outputs depend on its own rows and inlier_threshold only: bit for bit the same in any call, in any order, on any
+ * SM count.  Scratch: pdsc_spectral_matching_packed_scratch_bytes() bytes, 16-byte aligned.  No host synchronisation, no
+ * allocation, capturable in a CUDA graph. */
+size_t pdsc_spectral_matching_packed_scratch_bytes(int32_t B, const int32_t* h_offsets);
+int pdsc_spectral_matching_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                                  const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts, double inlier_threshold,
+                                  float* d_trans, float* d_labels, float* d_eigenvector, void* d_scratch, size_t scratch_bytes,
+                                  void* cuda_stream);
+
 /* Vertex positions of a PLY file (ascii or binary_little_endian; x, y, z float or double) into host memory as [n,3] float32.
  * Call with points = NULL to learn *n_vertices, then with a buffer of `capacity` >= n vertices. */
 int pdsc_read_ply(const char* path, float* points, int64_t capacity, int64_t* n_vertices);

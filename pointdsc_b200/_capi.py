@@ -120,6 +120,9 @@ SYMBOLS = {
                                                 C.c_double, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                                 C.c_void_p]),
+    "pdsc_spectral_matching_packed_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_void_p]),
+    "pdsc_spectral_matching_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "pdsc_read_ply": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
     "pdsc_launches_per_forward": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32]),
     "pdsc_profile_enable": (C.c_int, [C.c_void_p, C.c_int32]),

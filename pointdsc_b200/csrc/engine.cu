@@ -1031,6 +1031,31 @@ int pdsc_ransac_packed_hypotheses(pdsc_engine* e, int32_t B, const int32_t* h_of
                        d_hyp_trans, d_scratch, scratch_bytes, cuda_stream);
 }
 
+size_t pdsc_spectral_matching_packed_scratch_bytes(int32_t B, const int32_t* h_offsets) {
+  if (check_offsets("pdsc_spectral_matching_packed_scratch_bytes", "", B, h_offsets, 1, pdsc::spectral_matching_max_n())) return 0;
+  return pdsc::sm_scratch_bytes(h_offsets[B], B);
+}
+
+int pdsc_spectral_matching_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                                  const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts, double inlier_threshold,
+                                  float* d_trans, float* d_labels, float* d_eigenvector, void* d_scratch, size_t scratch_bytes,
+                                  void* cuda_stream) {
+  const char* fn = "pdsc_spectral_matching_packed";
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_offsets(fn, "", B, h_offsets, 1, pdsc::spectral_matching_max_n())) return rc;
+  if (B > 65535) return fail(PDSC_ERR_UNSUPPORTED, "%s: at most 65535 sets per call (got %d)", fn, B);
+  if (!d_offsets || !d_corr_pos || !d_src_keypts || !d_tgt_keypts || !d_trans || !d_labels)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  if (!(inlier_threshold > 0.0) || !std::isfinite(inlier_threshold))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: inlier_threshold must be positive and finite (got %g)", fn, inlier_threshold);
+  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::sm_scratch_bytes(h_offsets[B], B), 16)) return rc;
+  DeviceGuard g(e->cfg.device);
+  pdsc::launch_spectral_matching(B, h_offsets, d_offsets, d_corr_pos, d_src_keypts, d_tgt_keypts, inlier_threshold, d_trans, d_labels,
+                                 d_eigenvector, d_scratch, static_cast<cudaStream_t>(cuda_stream));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
+
 // Host-side PLY vertex reader (ascii / binary_little_endian; x, y, z as float or double; other vertex properties skipped).
 int pdsc_read_ply(const char* path, float* points, int64_t capacity, int64_t* n_vertices) {
   if (!path || !n_vertices) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_read_ply: null argument");

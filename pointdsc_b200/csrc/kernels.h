@@ -142,6 +142,15 @@ void launch_ransac(int B, const int32_t* d_off, long long R, const float* src, c
                    int32_t* best, int32_t* status, int32_t* hyp_good, double* hyp_rmse, double* hyp_trans, void* scratch,
                    cudaStream_t st);
 
+// ---- the spectral-matching baseline (spectral_matching.cu) ---------------------------------------------------
+// B sets packed back to back (host and device offsets [B + 1], R = offsets[B] rows, every set 1 .. spectral_matching_max_n() rows),
+// corr [R,6], src / tgt [R,3]; trans [B,4,4], labels [R]; eig_out [R] may be null.  B <= 65535.
+// Scratch: sm_scratch_bytes(R, B) bytes, 16-byte aligned.
+int spectral_matching_max_n();
+size_t sm_scratch_bytes(long long R, int B);
+void launch_spectral_matching(int B, const int32_t* h_off, const int32_t* d_off, const float* corr, const float* src, const float* tgt,
+                              double inlier_threshold, float* trans, float* labels, float* eig_out, void* scratch, cudaStream_t st);
+
 // ---- per-device launch configuration (device_state.cu) ----------------------------------------------------
 // opt `kernel` in to `bytes` of dynamic shared memory on the CURRENT device (no-op if already granted there)
 cudaError_t ensure_dynamic_smem(const void* kernel, int bytes);

@@ -15,6 +15,7 @@
 #include "kernels.h"
 #include "sets.cuh"
 #include "svd3.cuh"
+#include "weighted_kabsch.cuh"
 
 namespace pdsc {
 
@@ -183,26 +184,6 @@ void launch_seed_hypotheses(const float* src, const float* tgt, const int32_t* k
 // -------------------------------------------------------------------------------------------------
 // one CTA per set: pick the best hypothesis, write the labels, run the reweighted-Kabsch refinement
 // -------------------------------------------------------------------------------------------------
-constexpr int kRefThreads = 512;
-
-template <int NV>
-__device__ __forceinline__ void block_sum(double (&vals)[NV], double* red /* [16][NV] */, double* out /* [NV] */) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) vals[i] = warp_sum(vals[i]);
-  if (lane == 0) {
-#pragma unroll
-    for (int i = 0; i < NV; ++i) red[warp * NV + i] = vals[i];
-  }
-  __syncthreads();
-  if (threadIdx.x < NV) {
-    double acc = 0.0;
-    for (int w = 0; w < kRefThreads / 32; ++w) acc += red[w * NV + threadIdx.x];
-    out[threadIdx.x] = acc;
-  }
-  __syncthreads();
-}
-
 __global__ void __launch_bounds__(kRefThreads) select_refine_kernel(
     const float* __restrict__ src, const float* __restrict__ tgt, const float* __restrict__ seed_trans,
     const unsigned long long* __restrict__ best_key, float* __restrict__ final_trans, float* __restrict__ final_labels,
@@ -238,23 +219,15 @@ __global__ void __launch_bounds__(kRefThreads) select_refine_kernel(
   long long prev = 0;
   int solves = 0;
   for (int it = 0; it < max_refine; ++it) {
-    // pass 1: inliers of the current transform, weights 1/(1+(d/tau)^2), weighted centroids
-    double acc1[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) acc1[i] = 0.0;
-    for (int j = tid; j < N; j += kRefThreads) {
-      const float ax = ps[(size_t)j * 3], ay = ps[(size_t)j * 3 + 1], az = ps[(size_t)j * 3 + 2];
-      const float bx = pt[(size_t)j * 3], by = pt[(size_t)j * 3 + 1], bz = pt[(size_t)j * 3 + 2];
+    // the inliers of the current transform, weighted 1/(1+(d/tau)^2)
+    auto weight = [&](int, float ax, float ay, float az, float bx, float by, float bz, float& w) {
       const float d = residual(T, ax, ay, az, bx, by, bz);
-      if (d < rthr) {
-        const float q = d / rthr;
-        const float w = 1.0f / (1.0f + q * q);
-        acc1[0] += 1.0; acc1[1] += (double)w;
-        acc1[2] += (double)(ax * w); acc1[3] += (double)(ay * w); acc1[4] += (double)(az * w);
-        acc1[5] += (double)(bx * w); acc1[6] += (double)(by * w); acc1[7] += (double)(bz * w);
-      }
-    }
-    block_sum<8>(acc1, red, tot);
+      if (!(d < rthr)) return false;
+      const float q = d / rthr;
+      w = 1.0f / (1.0f + q * q);
+      return true;
+    };
+    kabsch_centroid_sums(ps, pt, N, weight, red, tot);
     const long long cnt = (long long)(tot[0] + 0.5);
     if (cnt == prev) break;  // inlier count unchanged (PointDSC.py:426); uniform across the CTA
     prev = cnt;
@@ -262,35 +235,7 @@ __global__ void __launch_bounds__(kRefThreads) select_refine_kernel(
     const float cax = (float)tot[2] / den, cay = (float)tot[3] / den, caz = (float)tot[4] / den;
     const float cbx = (float)tot[5] / den, cby = (float)tot[6] / den, cbz = (float)tot[7] / den;
     __syncthreads();  // everyone has read tot[] before pass 2 overwrites it
-
-    // pass 2: H = Am^T diag(w) Bm over the inliers
-    double acc2[9];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) acc2[i] = 0.0;
-    for (int j = tid; j < N; j += kRefThreads) {
-      const float ax = ps[(size_t)j * 3], ay = ps[(size_t)j * 3 + 1], az = ps[(size_t)j * 3 + 2];
-      const float bx = pt[(size_t)j * 3], by = pt[(size_t)j * 3 + 1], bz = pt[(size_t)j * 3 + 2];
-      const float d = residual(T, ax, ay, az, bx, by, bz);
-      if (d < rthr) {
-        const float q = d / rthr;
-        const float w = 1.0f / (1.0f + q * q);
-        const float mx = ax - cax, my = ay - cay, mz = az - caz;
-        const float nx = (bx - cbx) * w, ny = (by - cby) * w, nz = (bz - cbz) * w;
-        acc2[0] += (double)(mx * nx); acc2[1] += (double)(mx * ny); acc2[2] += (double)(mx * nz);
-        acc2[3] += (double)(my * nx); acc2[4] += (double)(my * ny); acc2[5] += (double)(my * nz);
-        acc2[6] += (double)(mz * nx); acc2[7] += (double)(mz * ny); acc2[8] += (double)(mz * nz);
-      }
-    }
-    block_sum<9>(acc2, red, tot);
-    if (tid == 0) {
-      float H[9], R[9];
-#pragma unroll
-      for (int i = 0; i < 9; ++i) H[i] = (float)tot[i];
-      kabsch_rotation(H, R);
-      T[0] = R[0]; T[1] = R[1]; T[2] = R[2];  T[3] = cbx - (R[0] * cax + R[1] * cay + R[2] * caz);
-      T[4] = R[3]; T[5] = R[4]; T[6] = R[5];  T[7] = cby - (R[3] * cax + R[4] * cay + R[5] * caz);
-      T[8] = R[6]; T[9] = R[7]; T[10] = R[8]; T[11] = cbz - (R[6] * cax + R[7] * cay + R[8] * caz);
-    }
+    kabsch_solve(ps, pt, N, weight, cax, cay, caz, cbx, cby, cbz, red, tot, T);
     ++solves;
     __syncthreads();
   }

@@ -51,5 +51,7 @@ from pointdsc_b200.icp import icp_refine, icp_refine_packed
 ic = icp_refine(h["src_keypts"].cuda(), h["tgt_keypts"].cuda(), out["final_trans"])
 ip, ii = icp_refine_packed(pk["src_keypts"], pk["tgt_keypts"], torch.eye(4).expand(3, 4, 4).cuda(), off, d_offsets=pk["d_offsets"],
                            info=True)                    # pdsc_icp_packed, sets of three sizes
+from pointdsc_b200.spectral import spectral_matching_packed
+smt, sml = spectral_matching_packed(pk["corr_pos"], pk["src_keypts"], pk["tgt_keypts"], off, d_offsets=pk["d_offsets"])  # sets of three sizes
 torch.cuda.synchronize()
 print("sanitize_smoke ok", float(st.sum()), int(it.sum()), r["corr"].shape, tuple(feat.shape))
