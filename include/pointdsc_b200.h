@@ -378,6 +378,13 @@ int pdsc_spectral_matching_packed(pdsc_engine* e, int32_t B, const int32_t* h_of
                                   const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts, double inlier_threshold,
                                   float* d_trans, float* d_labels, float* d_eigenvector, void* d_scratch, size_t scratch_bytes,
                                   void* cuda_stream);
+/* pdsc_spectral_matching_packed with one more optional output, d_iterates [10,R] float32 (may be NULL): row t - 1 holds every
+ * set's iterate v_t of the ten power iterations, so that each step can be checked on its own (row 9 is d_eigenvector).  A test
+ * output: the normalisation of iteration t writes it as it writes v_t.  Same arguments, checks, scratch and results otherwise. */
+int pdsc_spectral_matching_packed_iterates(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                                           const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts,
+                                           double inlier_threshold, float* d_trans, float* d_labels, float* d_eigenvector,
+                                           float* d_iterates, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
 
 /* Vertex positions of a PLY file (ascii or binary_little_endian; x, y, z float or double) into host memory as [n,3] float32.
  * Call with points = NULL to learn *n_vertices, then with a buffer of `capacity` >= n vertices. */

@@ -1036,11 +1036,11 @@ size_t pdsc_spectral_matching_packed_scratch_bytes(int32_t B, const int32_t* h_o
   return pdsc::sm_scratch_bytes(h_offsets[B], B);
 }
 
-int pdsc_spectral_matching_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
-                                  const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts, double inlier_threshold,
-                                  float* d_trans, float* d_labels, float* d_eigenvector, void* d_scratch, size_t scratch_bytes,
-                                  void* cuda_stream) {
-  const char* fn = "pdsc_spectral_matching_packed";
+// pdsc_spectral_matching_packed and pdsc_spectral_matching_packed_iterates: one set of checks and one launch, under the caller's name
+static int spectral_matching_packed(const char* fn, pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                                    const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts,
+                                    double inlier_threshold, float* d_trans, float* d_labels, float* d_eigenvector, float* d_iterates,
+                                    void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
   if (int rc = check_offsets(fn, "", B, h_offsets, 1, pdsc::spectral_matching_max_n())) return rc;
   if (B > 65535) return fail(PDSC_ERR_UNSUPPORTED, "%s: at most 65535 sets per call (got %d)", fn, B);
@@ -1051,9 +1051,26 @@ int pdsc_spectral_matching_packed(pdsc_engine* e, int32_t B, const int32_t* h_of
   if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::sm_scratch_bytes(h_offsets[B], B), 16)) return rc;
   DeviceGuard g(e->cfg.device);
   pdsc::launch_spectral_matching(B, h_offsets, d_offsets, d_corr_pos, d_src_keypts, d_tgt_keypts, inlier_threshold, d_trans, d_labels,
-                                 d_eigenvector, d_scratch, static_cast<cudaStream_t>(cuda_stream));
+                                 d_eigenvector, d_iterates, d_scratch, static_cast<cudaStream_t>(cuda_stream));
   PDSC_CUDA(cudaGetLastError());
   return PDSC_OK;
+}
+
+int pdsc_spectral_matching_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                                  const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts, double inlier_threshold,
+                                  float* d_trans, float* d_labels, float* d_eigenvector, void* d_scratch, size_t scratch_bytes,
+                                  void* cuda_stream) {
+  return spectral_matching_packed("pdsc_spectral_matching_packed", e, B, h_offsets, d_offsets, d_corr_pos, d_src_keypts, d_tgt_keypts,
+                                  inlier_threshold, d_trans, d_labels, d_eigenvector, nullptr, d_scratch, scratch_bytes, cuda_stream);
+}
+
+int pdsc_spectral_matching_packed_iterates(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                                           const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts,
+                                           double inlier_threshold, float* d_trans, float* d_labels, float* d_eigenvector,
+                                           float* d_iterates, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  return spectral_matching_packed("pdsc_spectral_matching_packed_iterates", e, B, h_offsets, d_offsets, d_corr_pos, d_src_keypts,
+                                  d_tgt_keypts, inlier_threshold, d_trans, d_labels, d_eigenvector, d_iterates, d_scratch, scratch_bytes,
+                                  cuda_stream);
 }
 
 // Host-side PLY vertex reader (ascii / binary_little_endian; x, y, z as float or double; other vertex properties skipped).

@@ -23,7 +23,8 @@
 //                 ascending order with one fma each, and a row's 32 lane sums are combined by the xor-shuffle tree of warp_sum.
 //                 Writes u = M v.  The first iteration reads no v (v = 1).
 //   norm kernel   one CTA per set: sum u^2 in a fixed order (thread-strided, warp tree, warps in ascending order), then
-//                 v = u / (sqrt(sum) + 1e-6) in place.  The first launch also writes the set table the sort reads.
+//                 v = u / (sqrt(sum) + 1e-6) in place.  The first launch also writes the set table the sort reads; with an
+//                 iterates output (pdsc_spectral_matching_packed_iterates, a test output) iteration t also writes v_t there.
 //   top-S sort    launch_top_seeds (seeds.cu), one CTA per set.
 //   Kabsch        one CTA per set: marks the S selected rows, writes labels and the eigenvector, runs weighted_kabsch.cuh.
 // 22 launches whatever B; no host synchronisation, no allocation, capturable in a CUDA graph.  Every sum's order depends on the
@@ -124,7 +125,8 @@ __global__ void __launch_bounds__(kSmThreads) sm_power_kernel(const float* __res
   }
 }
 
-__global__ void __launch_bounds__(kSmThreads) sm_norm_kernel(float* __restrict__ u, Offsets off, SetDesc* __restrict__ sets) {
+__global__ void __launch_bounds__(kSmThreads) sm_norm_kernel(float* __restrict__ u, Offsets off, SetDesc* __restrict__ sets,
+                                                              float* __restrict__ iterate) {
   __shared__ float part[kSmWarps];
   __shared__ float den_s;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -150,7 +152,11 @@ __global__ void __launch_bounds__(kSmThreads) sm_norm_kernel(float* __restrict__
   }
   __syncthreads();
   const float den = den_s;
-  for (int j = tid; j < N; j += kSmThreads) ub[j] = __fdiv_rn(ub[j], den);
+  for (int j = tid; j < N; j += kSmThreads) {
+    const float x = __fdiv_rn(ub[j], den);
+    ub[j] = x;
+    if (iterate) iterate[(size_t)row0 + j] = x;
+  }
 }
 
 __global__ void __launch_bounds__(kRefThreads) sm_kabsch_kernel(const float* __restrict__ src, const float* __restrict__ tgt,
@@ -197,7 +203,8 @@ size_t sm_scratch_bytes(long long R, int B) {
 }
 
 void launch_spectral_matching(int B, const int32_t* h_off, const int32_t* d_off, const float* corr, const float* src, const float* tgt,
-                              double inlier_threshold, float* trans, float* labels, float* eig_out, void* scratch, cudaStream_t st) {
+                              double inlier_threshold, float* trans, float* labels, float* eig_out, float* iterates, void* scratch,
+                              cudaStream_t st) {
   const long long R = h_off[B];
   int Nmax = 0;
   for (int b = 0; b < B; ++b) Nmax = max(Nmax, h_off[b + 1] - h_off[b]);
@@ -220,7 +227,7 @@ void launch_spectral_matching(int B, const int32_t* h_off, const int32_t* d_off,
     if (RW == 4) sm_power_kernel<4><<<grid, kSmThreads, 0, st>>>(corr, off, vin, uo, coef);
     else if (RW == 2) sm_power_kernel<2><<<grid, kSmThreads, 0, st>>>(corr, off, vin, uo, coef);
     else sm_power_kernel<1><<<grid, kSmThreads, 0, st>>>(corr, off, vin, uo, coef);
-    sm_norm_kernel<<<B, kSmThreads, 0, st>>>(uo, off, t == 0 ? s.sets : nullptr);
+    sm_norm_kernel<<<B, kSmThreads, 0, st>>>(uo, off, t == 0 ? s.sets : nullptr, iterates ? iterates + (size_t)t * R : nullptr);
     vin = uo;
   }
   launch_top_seeds(vin, s.seeds, B, Nmax, num_seeds(Nmax, kSmTopRatio), st, s.sets);

@@ -46,12 +46,15 @@ def leading_eigenvector(M: torch.Tensor, num_iterations: int = 10, early_exit: b
 
 @torch.no_grad()
 def spectral_matching_packed(corr_pos: torch.Tensor, src: torch.Tensor, tgt: torch.Tensor, offsets: Sequence[int],
-                             d_offsets: Optional[torch.Tensor] = None, inlier_threshold: float = 0.10, eigenvector: bool = False):
+                             d_offsets: Optional[torch.Tensor] = None, inlier_threshold: float = 0.10, eigenvector: bool = False,
+                             iterates: bool = False):
     """The spectral-matching baseline of B sets in one call.  corr_pos [R,6], src / tgt [R,3]: set b's rows are
     offsets[b]:offsets[b+1] (the layout `match_many` and `ransac_packed` use), 1 to MAX_ROWS rows each; offsets the host list
     of B + 1 ints, d_offsets the same values as a device int32 tensor (copied from `offsets` when None).  Returns (trans
     [B,4,4] float32, labels [R] float32: 1 on the int(N_b * 0.1) largest eigenvector entries of each set, lowest row first on
-    ties), and the eigenvector [R] float32 as a third item with eigenvector=True.  Nothing is read back from the device."""
+    ties), and the eigenvector [R] float32 as a third item with eigenvector=True.  iterates=True appends every power iterate
+    [10,R] float32, row t - 1 the iterate v_t (pdsc_spectral_matching_packed_iterates, a test output).  Nothing is read back
+    from the device."""
     if corr_pos.device.type != "cuda":
         raise _capi.PdscError("pointdsc_b200.spectral runs on an H100 only: pass CUDA tensors (there is no CPU fallback)")
     offsets = [int(o) for o in offsets]
@@ -71,13 +74,17 @@ def spectral_matching_packed(corr_pos: torch.Tensor, src: torch.Tensor, tgt: tor
     trans = torch.empty(B, 4, 4, dtype=torch.float32, device=dev)
     labels = torch.empty(R, dtype=torch.float32, device=dev)
     eig = torch.empty(R, dtype=torch.float32, device=dev) if eigenvector else None
+    its = torch.empty(10, R, dtype=torch.float32, device=dev) if iterates else None
     scratch = _capi.scratch(lib.pdsc_spectral_matching_packed_scratch_bytes(B, h_off), dev, 16)
+    P = lambda x: C.c_void_p(x.data_ptr()) if x is not None else None                                      # noqa: E731
+    args = [engine, B, h_off, P(d_offsets), P(c), P(s), P(t), float(inlier_threshold), P(trans), P(labels), P(eig)]
+    tail = [P(scratch), scratch.numel(), stream]
     with torch.cuda.device(dev):
-        _capi.check(lib.pdsc_spectral_matching_packed(
-            engine, B, h_off, C.c_void_p(d_offsets.data_ptr()), C.c_void_p(c.data_ptr()), C.c_void_p(s.data_ptr()),
-            C.c_void_p(t.data_ptr()), float(inlier_threshold), C.c_void_p(trans.data_ptr()), C.c_void_p(labels.data_ptr()),
-            C.c_void_p(eig.data_ptr()) if eig is not None else None, C.c_void_p(scratch.data_ptr()), scratch.numel(), stream))
-    return (trans, labels, eig) if eigenvector else (trans, labels)
+        if iterates:
+            _capi.check(lib.pdsc_spectral_matching_packed_iterates(*args, P(its), *tail))
+        else:
+            _capi.check(lib.pdsc_spectral_matching_packed(*args, *tail))
+    return (trans, labels) + ((eig,) if eigenvector else ()) + ((its,) if iterates else ())
 
 
 @torch.no_grad()

@@ -1,6 +1,7 @@
 """The engine's launch rules, restated once for the tests: the attention's key split (sets.cuh attn_set_split*,
 attn_call_splits), the seed count and a set's sizes (sets.cuh num_seeds, set_sizes), the workspace layout (sets.cuh
-plan_call, engine.cu carve, encoder_tc.cu tc_scratch) and the front end's launch plans (frontend.cu, eig_power.cu, fpfh.cu).
+plan_call, engine.cu carve, encoder_tc.cu tc_scratch), the front end's launch plans (frontend.cu, eig_power.cu, fpfh.cu) and the
+spectral-matching baseline's rows per warp (spectral_matching.cu).
 The tests assert that the engine reaches what these predict, and the memory contract that the restated workspace adds up
 to pdsc_workspace_bytes(_packed), so the restatement cannot drift from the engine unnoticed."""
 C_CH = 128                      # num_channels
@@ -147,3 +148,18 @@ def search_plan(max_nn):
         P <<= 1
     per_warp = P * 8 + 1024 + CAND_CAP * 8
     return P, min(8, 200 * 1024 // per_warp)
+
+
+# ---------------------------------------------------------------------------------------------------
+# the spectral-matching baseline
+# ---------------------------------------------------------------------------------------------------
+SM_WARPS, SM_TILE = 8, 512      # spectral_matching.cu kSmWarps, kSmTile: warps per power CTA, columns staged per pass
+
+
+def sm_rows_per_warp(Ns, sms):
+    """RW of launch_spectral_matching: the most rows per warp (4, then 2) whose CTAs over the call's sets still number at
+    least two per SM, else 1."""
+    for rw in (4, 2):
+        if sum(-(-n // (SM_WARPS * rw)) for n in Ns) >= 2 * sms:
+            return rw
+    return 1

@@ -7,6 +7,7 @@ reference is float64 on the engine's own fp32 inputs or taps, and every bound is
     which checks every kernel of a forward's encoder layers; test_gpu_encoder.py sets out their error model.
   * Kabsch (svd3.cuh): weighted_kabsch64 and check_transforms; test_gpu_kabsch.py sets out the solver's bound.
   * The seed-row kNN (E_KNN) and the power iteration (check_power) of test_gpu_stages.py.
+  * The spectral-matching baseline's compatibility entries (entry_width); test_gpu_spectral_matching.py sets out their bound.
 """
 import math
 
@@ -560,3 +561,22 @@ def check_power(compat, eig, power_iters, k, iters):
     if sure:
         assert t == exit64, (t, exit64)
     return float((err / tol).max()), float((err / (band(t) + 1e-30)).max()), sure
+
+
+# ---------------------------------------------------------------------------------------------------
+# the spectral-matching baseline
+# ---------------------------------------------------------------------------------------------------
+def entry_width(corr, thr):
+    """W [N,N] float64 (on corr's device) of test_gpu_spectral_matching.py's header: the bound of |M' - M| per entry."""
+    c = corr.to(torch.float64)
+    ds = torch.cdist(c[:, :3], c[:, :3], compute_mode="donot_use_mm_for_euclid_dist")
+    dt = torch.cdist(c[:, 3:], c[:, 3:], compute_mode="donot_use_mm_for_euclid_dist")
+    m = (ds - dt).abs()
+    em = gamma(5) * (ds + dt) * (1 + 1e-12)
+    del ds, dt
+    cf = 4.5 / thr ** 2
+    e = (2 * m * em + em * em) * cf * (1 + gamma(3)) + gamma(3) * cf * m * m + 4.5 * U
+    mu = 4.5 - m * m * cf
+    W = (mu + e).clamp_min(0.0) - (mu - e).clamp_min(0.0)
+    W.fill_diagonal_(0.0)
+    return W

@@ -18,9 +18,11 @@ own fp32 rows.  Write m = ds - dt for a pair (ds, dt the exact source / target l
     gamma(ceil(N / 256) + 13) relative on the square, half that on the root, plus the root's, the + 1e-6's and the division's
     roundings) moves v_t' by at most e_n = gamma(ceil(N / 256) + 16) relative, and |f| <= 1:
         delta_t <= min(2, a_t / (|x_t| - a_t + 1e-6) + e_n)     (2 when |x_t| <= a_t: two vectors of norm <= 1).
-  v is checked entrywise against delta_10 (a norm bound covers every entry).  pdsc_leading_eigenvector on the materialised fp32
-  M has the same one-step model with its own orders: ceil(N / 32) fmas per lane and the tree again, and a norm summed over
-  ceil(N / 8) per-CTA partials of at most 32 squares each: e_n = gamma(ceil(N / 8) + 40).
+  v is checked entrywise against delta_10 (a norm bound covers every entry); that end-to-end bound is loose, and
+  test_gpu_spectral_steps.py checks every iterate on its own against a per-entry bound of one step.
+  pdsc_leading_eigenvector on the materialised fp32 M has the same one-step model with its own orders: ceil(N / 32) fmas per
+  lane and the tree again, and a norm summed over ceil(N / 8) per-CTA partials of at most 32 squares each:
+  e_n = gamma(ceil(N / 8) + 40).
 Labels.  Always: the top S = int(N * 0.1) of the device's own v, descending, lowest row first on ties, exactly.  Against float64:
   a row whose float64 entry is above the (S+1)-th largest by more than 2 delta_10 is selected, one below the S-th by more than
   2 delta_10 is not; where the selection gap v_(S) - v_(S+1) exceeds 2 delta_10 the labels equal the oracle's.
@@ -37,7 +39,7 @@ import numpy as np
 import pytest
 import torch
 
-from float64_bounds import EPS, U, _h_error, assert_rotations, check_transforms, gamma, weighted_kabsch64
+from float64_bounds import EPS, _h_error, assert_rotations, check_transforms, entry_width, gamma, weighted_kabsch64
 from oracle import sm_oracle as O
 from ransac_samples import C_VALUE
 
@@ -66,22 +68,6 @@ def run(sets, thr, d_offsets=False):
     T, lab, v = spectral_matching_packed(cat(0), cat(1), cat(2), off, d_offsets=d_off, inlier_threshold=thr, eigenvector=True)
     torch.cuda.synchronize()
     return T.cpu().numpy(), lab.cpu().numpy(), v.cpu().numpy(), off
-
-
-def entry_width(corr, thr):
-    """W [N,N] float64 (device) of the header: the bound of |M' - M| per entry."""
-    c = corr.to(torch.float64)
-    ds = torch.cdist(c[:, :3], c[:, :3], compute_mode="donot_use_mm_for_euclid_dist")
-    dt = torch.cdist(c[:, 3:], c[:, 3:], compute_mode="donot_use_mm_for_euclid_dist")
-    m = (ds - dt).abs()
-    em = gamma(5) * (ds + dt) * (1 + 1e-12)
-    del ds, dt
-    cf = 4.5 / thr ** 2
-    e = (2 * m * em + em * em) * cf * (1 + gamma(3)) + gamma(3) * cf * m * m + 4.5 * U
-    mu = 4.5 - m * m * cf
-    W = (mu + e).clamp_min(0.0) - (mu - e).clamp_min(0.0)
-    W.fill_diagonal_(0.0)
-    return W
 
 
 def power_bound(M, W, iterates, e_n):
@@ -276,10 +262,13 @@ def _abi(sets):
     need = int(lib.pdsc_spectral_matching_packed_scratch_bytes(len(sets), h_off))
     P = lambda x: None if x is None else C.c_void_p(x if isinstance(x, int) else x.data_ptr())           # noqa: E731
 
-    def call(trans, labels, eig, scratch, nbytes, stream=None, h=h_off, B=len(sets), thr=0.10):
+    def call(trans, labels, eig, scratch, nbytes, stream=None, h=h_off, B=len(sets), thr=0.10, its=False):
+        """pdsc_spectral_matching_packed, or pdsc_spectral_matching_packed_iterates when `its` (the iterates buffer) is given."""
         st = (stream or torch.cuda.current_stream()).cuda_stream
-        return lib.pdsc_spectral_matching_packed(eng, B, h, P(d_off), P(corr), P(src), P(tgt), thr, P(trans), P(labels), P(eig),
-                                                 P(scratch), nbytes, C.c_void_p(st))
+        args = (eng, B, h, P(d_off), P(corr), P(src), P(tgt), thr, P(trans), P(labels), P(eig))
+        if its is not False:
+            return lib.pdsc_spectral_matching_packed_iterates(*args, P(its), P(scratch), nbytes, C.c_void_p(st))
+        return lib.pdsc_spectral_matching_packed(*args, P(scratch), nbytes, C.c_void_p(st))
     torch.cuda.synchronize()
     return call, need, off
 
@@ -289,12 +278,17 @@ def _abi_group():
 
 
 def test_memory_contract():
-    """Every output is written within its bounds and the same whatever the output and scratch buffers held."""
+    """Every output is written within its bounds and the same whatever the output and scratch buffers held, with and without
+    the iterates output (pdsc_spectral_matching_packed_iterates); the other outputs do not depend on it."""
     from buffer_guards import PATTERNS, guarded_output, scratch_buffer
+    from pointdsc_b200.spectral import spectral_matching_packed
     sets = _abi_group()
     T, lab, v, _ = run(sets, 0.10)
     call, need, off = _abi(sets)
     B, R = len(sets), off[-1]
+    cat = lambda i: torch.from_numpy(np.ascontiguousarray(np.concatenate([x[i] for x in sets]))).cuda()   # noqa: E731
+    its = spectral_matching_packed(cat(0), cat(1), cat(2), off, iterates=True)[2].cpu().numpy()
+    assert np.array_equal(its[-1], v)
     want = {"trans": T, "labels": lab, "eig": v}
     for pattern in PATTERNS:
         outs = {"trans": guarded_output(64 * B, 16, torch.device("cuda"), pattern),
@@ -313,6 +307,18 @@ def test_memory_contract():
         torch.cuda.synchronize()
         lab_only.check(("labels without eig", pattern))
         assert np.array_equal(lab_only.inner.cpu().numpy(), lab.view(np.uint8))
+        # with the iterates output: all ten rows written, and the same bytes in every other output
+        outs["its"] = guarded_output(4 * 10 * R, 4, torch.device("cuda"), pattern)
+        for name in ("trans", "labels", "eig"):
+            outs[name] = guarded_output(outs[name].nbytes, outs[name].align, torch.device("cuda"), pattern)
+        want["its"] = its
+        assert call(outs["trans"].ptr, outs["labels"].ptr, outs["eig"].ptr, scratch.ptr, need, its=outs["its"].ptr) == 0
+        torch.cuda.synchronize()
+        scratch.check(("scratch with iterates", pattern))
+        for name, g in outs.items():
+            g.check((name, "with iterates", pattern))
+            assert np.array_equal(g.inner.cpu().numpy(), np.ascontiguousarray(want[name]).view(np.uint8).reshape(-1)), \
+                (name, "with iterates", pattern)
 
 
 def test_graph_replay_and_errors():
@@ -323,16 +329,17 @@ def test_graph_replay_and_errors():
     scratch = _capi.scratch(need, torch.device("cuda"), 16)
 
     def outs():
-        return (torch.empty(B, 4, 4, device="cuda"), torch.empty(R, device="cuda"), torch.empty(R, device="cuda"))
+        return (torch.empty(B, 4, 4, device="cuda"), torch.empty(R, device="cuda"), torch.empty(R, device="cuda"),
+                torch.empty(10, R, device="cuda"))
     eager = outs()
-    assert call(*eager, scratch, need) == 0
+    assert call(*eager[:3], scratch, need, its=eager[3]) == 0
     graphed = outs()
     g = torch.cuda.CUDAGraph()
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(s):
         with torch.cuda.graph(g, stream=s):
-            assert call(*graphed, scratch, need, stream=s) == 0
+            assert call(*graphed[:3], scratch, need, stream=s, its=graphed[3]) == 0
     torch.cuda.current_stream().wait_stream(s)
     for x in graphed:
         x.fill_(7.0)
@@ -340,12 +347,15 @@ def test_graph_replay_and_errors():
     torch.cuda.synchronize()
     for a, b in zip(eager, graphed):
         assert torch.equal(a, b)
+    assert torch.equal(eager[3][-1], eager[2])
     lib = _capi.load()
     fn = "pdsc_spectral_matching_packed"
     # short scratch, null outputs, a bad threshold
+    eager = eager[:3]
     assert call(*eager, scratch, need - 1) != 0 and fn in lib.pdsc_last_error().decode()
     assert call(None, eager[1], None, scratch, need) != 0 and fn in lib.pdsc_last_error().decode()
     assert call(*eager, scratch, need, thr=0.0) != 0 and fn in lib.pdsc_last_error().decode()
+    assert call(*eager, scratch, need, thr=0.0, its=None) != 0 and fn + "_iterates" in lib.pdsc_last_error().decode()
     # bad offsets: not starting at 0, an empty set, a set above 16,384 rows
     for bad in ([1, 5, 700], [0, 5, 5], [0, 16385]):
         h = (C.c_int32 * len(bad))(*bad)
