@@ -327,6 +327,38 @@ int pdsc_icp_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const i
                     const float* d_tgt, const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans,
                     double* d_fitness, double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
                     void* cuda_stream);
+/* f7: the same ICP between two different clouds, for the multiway registration's local_refinement (multiway/test_multi_ate.py):
+ * pair b's source is rows [src_offsets[b], src_offsets[b+1]) of d_src [Rs,3] and its target rows [tgt_offsets[b],
+ * tgt_offsets[b+1]) of d_tgt [Rt,3] (two fragments, Ns and Nt rows); both offset arrays have B + 1 entries, start at 0 and give
+ * every pair at least one row on each side (else PDSC_ERR_SHAPE, and the scratch-size function returns 0).  Semantics, outputs,
+ * errors and guarantees as pdsc_icp_packed, with fitness = kept / Ns; pdsc_icp_packed is this call with tgt_offsets =
+ * src_offsets, bit for bit.  The host offsets are validated and size the scratch; the device ones are what the kernel reads and
+ * may describe fewer rows: any offsets with at least one row per pair on each side and a last entry no larger than the host
+ * one's (they need not start at 0), such as the d_out_offsets of a pdsc_voxel_down_sample_packed call over clouds the host
+ * offsets describe, so that a down-sampling and an ICP chain on the stream with nothing read back.  Scratch:
+ * pdsc_icp_clouds_packed_scratch_bytes() bytes, 8-byte aligned. */
+size_t pdsc_icp_clouds_packed_scratch_bytes(int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets);
+int pdsc_icp_clouds_packed(pdsc_engine* e, int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                           const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const float* d_src, const float* d_tgt,
+                           const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans, double* d_fitness,
+                           double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
+                           void* cuda_stream);
+/* f7: open3d 0.9's get_information_matrix_from_point_clouds(src, tgt, max_corr_dist, T) for B pairs in one call (recalled, not
+ * checkable here; tests/multiway_oracle.py restates it; PARITY UNPINNED).  Pairs and offsets (device ones included) as
+ * pdsc_icp_clouds_packed.  The source is
+ * moved by d_trans [B,4,4] float32 in fp64; each source row's nearest target row is kept iff d^2 < float32(max_corr_dist^2), ties to
+ * the lowest row; every kept correspondence with target point (x, y, z) adds G G^T for the rows (0, z, -y, 1, 0, 0),
+ * (-z, 0, x, 0, 1, 0) and (y, -x, 0, 0, 0, 1) of G, so d_info[b][5][5] is the number kept.  Outputs: d_info [B,6,6] float64;
+ * optional (may be NULL) d_status [B] (1: a non-finite coordinate, or the target spans 2^21 or more cells of side max_corr_dist
+ * along an axis; such a pair gets the zero matrix).  PDSC_ERR_INVALID_ARGUMENT for null required pointers and max_corr_dist <= 0
+ * or not finite.  Sums run in a fixed order: a pair's matrix is bit for bit the same in any call, in any order, on any SM count.
+ * Scratch: pdsc_information_matrix_packed_scratch_bytes() bytes, 8-byte aligned.  No host synchronisation, no allocation,
+ * capturable in a CUDA graph. */
+size_t pdsc_information_matrix_packed_scratch_bytes(int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets);
+int pdsc_information_matrix_packed(pdsc_engine* e, int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                                   const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const float* d_src, const float* d_tgt,
+                                   const float* d_trans, double max_corr_dist, double* d_info, int32_t* d_status, void* d_scratch,
+                                   size_t scratch_bytes, void* cuda_stream);
 
 /* f6: correspondence RANSAC over the pairs the network kept, replacing the drivers' --solver RANSAC block
  * (evaluation/test_3DMatch.py:59-77): open3d 0.9's registration_ransac_based_on_correspondence with ransac_n = 3 and

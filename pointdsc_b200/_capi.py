@@ -112,6 +112,14 @@ SYMBOLS = {
     "pdsc_icp_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double,
                                   C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                   C.c_void_p]),
+    "pdsc_icp_clouds_packed_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_void_p, C.c_void_p]),
+    "pdsc_icp_clouds_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_double, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "pdsc_information_matrix_packed_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_void_p, C.c_void_p]),
+    "pdsc_information_matrix_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                 C.c_void_p]),
     "pdsc_ransac_packed_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_void_p, C.c_int32]),
     "pdsc_ransac_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double,
                                      C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

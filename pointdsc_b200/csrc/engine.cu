@@ -956,24 +956,80 @@ int pdsc_compute_fpfh_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets
 }
 
 size_t pdsc_icp_packed_scratch_bytes(int32_t B, const int32_t* h_offsets) {
-  return check_offsets("pdsc_icp_packed_scratch_bytes", "", B, h_offsets, 1) ? 0 : pdsc::icp_scratch_bytes(h_offsets[B]);
+  return pdsc_icp_clouds_packed_scratch_bytes(B, h_offsets, h_offsets);
+}
+
+size_t pdsc_icp_clouds_packed_scratch_bytes(int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets) {
+  const char* who = "pdsc_icp_clouds_packed_scratch_bytes";
+  if (check_offsets(who, "source ", B, h_src_offsets, 1) || check_offsets(who, "target ", B, h_tgt_offsets, 1)) return 0;
+  return pdsc::icp_scratch_bytes(h_src_offsets[B], h_tgt_offsets[B]);
+}
+
+// pdsc_icp_packed and pdsc_icp_clouds_packed: one set of checks and one launch, under the caller's name
+static int icp_clouds(const char* fn, pdsc_engine* e, int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                      const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const float* d_src, const float* d_tgt,
+                      const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans, double* d_fitness,
+                      double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
+                      void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  const bool one = h_src_offsets == h_tgt_offsets;     // pdsc_icp_packed: one offsets array for both sides
+  if (int rc = check_offsets(fn, one ? "" : "source ", B, h_src_offsets, 1)) return rc;
+  if (!one)
+    if (int rc = check_offsets(fn, "target ", B, h_tgt_offsets, 1)) return rc;
+  if (!d_src_offsets || !d_tgt_offsets || !d_src || !d_tgt || !d_init || !d_trans)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_corr_dist must be positive and finite (got %g)", fn, max_corr_dist);
+  if (max_iteration < 1) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_iteration must be >= 1 (got %d)", fn, max_iteration);
+  const long long Rs = h_src_offsets[B], Rt = h_tgt_offsets[B];
+  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::icp_scratch_bytes(Rs, Rt), 8)) return rc;
+  DeviceGuard g(e->cfg.device);
+  pdsc::launch_icp(B, d_src_offsets, d_tgt_offsets, Rs, Rt, d_src, d_tgt, d_init, max_corr_dist, max_iteration, d_trans, d_fitness,
+                   d_rmse, d_iterations, d_status, d_scratch, static_cast<cudaStream_t>(cuda_stream));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
 }
 
 int pdsc_icp_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
                     const float* d_tgt, const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans,
                     double* d_fitness, double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
                     void* cuda_stream) {
+  return icp_clouds("pdsc_icp_packed", e, B, h_offsets, h_offsets, d_offsets, d_offsets, d_src, d_tgt, d_init, max_corr_dist,
+                    max_iteration, d_trans, d_fitness, d_rmse, d_iterations, d_status, d_scratch, scratch_bytes, cuda_stream);
+}
+
+int pdsc_icp_clouds_packed(pdsc_engine* e, int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                           const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const float* d_src, const float* d_tgt,
+                           const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans, double* d_fitness,
+                           double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
+                           void* cuda_stream) {
+  return icp_clouds("pdsc_icp_clouds_packed", e, B, h_src_offsets, h_tgt_offsets, d_src_offsets, d_tgt_offsets, d_src, d_tgt,
+                    d_init, max_corr_dist, max_iteration, d_trans, d_fitness, d_rmse, d_iterations, d_status, d_scratch,
+                    scratch_bytes, cuda_stream);
+}
+
+size_t pdsc_information_matrix_packed_scratch_bytes(int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets) {
+  const char* who = "pdsc_information_matrix_packed_scratch_bytes";
+  if (check_offsets(who, "source ", B, h_src_offsets, 1) || check_offsets(who, "target ", B, h_tgt_offsets, 1)) return 0;
+  return pdsc::information_scratch_bytes(h_tgt_offsets[B]);
+}
+
+int pdsc_information_matrix_packed(pdsc_engine* e, int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                                   const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const float* d_src, const float* d_tgt,
+                                   const float* d_trans, double max_corr_dist, double* d_info, int32_t* d_status, void* d_scratch,
+                                   size_t scratch_bytes, void* cuda_stream) {
+  const char* fn = "pdsc_information_matrix_packed";
   if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_offsets("pdsc_icp_packed", "", B, h_offsets, 1)) return rc;
-  if (!d_offsets || !d_src || !d_tgt || !d_init || !d_trans) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_icp_packed: null tensor pointer");
+  if (int rc = check_offsets(fn, "source ", B, h_src_offsets, 1)) return rc;
+  if (int rc = check_offsets(fn, "target ", B, h_tgt_offsets, 1)) return rc;
+  if (!d_src_offsets || !d_tgt_offsets || !d_src || !d_tgt || !d_trans || !d_info)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
   if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_icp_packed: max_corr_dist must be positive and finite (got %g)", max_corr_dist);
-  if (max_iteration < 1) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_icp_packed: max_iteration must be >= 1 (got %d)", max_iteration);
-  if (int rc = check_scratch("pdsc_icp_packed", "scratch", d_scratch, scratch_bytes, pdsc::icp_scratch_bytes(h_offsets[B]), 8))
-    return rc;
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_corr_dist must be positive and finite (got %g)", fn, max_corr_dist);
+  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::information_scratch_bytes(h_tgt_offsets[B]), 8)) return rc;
   DeviceGuard g(e->cfg.device);
-  pdsc::launch_icp(B, d_offsets, h_offsets[B], d_src, d_tgt, d_init, max_corr_dist, max_iteration, d_trans, d_fitness, d_rmse,
-                   d_iterations, d_status, d_scratch, static_cast<cudaStream_t>(cuda_stream));
+  pdsc::launch_information(B, d_src_offsets, d_tgt_offsets, h_tgt_offsets[B], d_src, d_tgt, d_trans, max_corr_dist, d_info, d_status,
+                           d_scratch, static_cast<cudaStream_t>(cuda_stream));
   PDSC_CUDA(cudaGetLastError());
   return PDSC_OK;
 }

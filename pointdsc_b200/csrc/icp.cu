@@ -7,16 +7,24 @@
 // Umeyama update U over C without scaling (svd3.cuh's Jacobi Kabsch in double), sets T <- U T and P <- U P, recomputes C and
 // stops once |d fitness| < 1e-6 and |d rmse| < 1e-6, or after max_iteration updates.
 //
-// Sets.  B sets packed back to back, set b owning rows [off[b], off[b+1]) of src / tgt; one CTA per set runs everything below
-// from its own rows and its own scratch only, with reductions in a fixed order, so a set's result is bit for bit the same
-// whatever else its call holds, in whatever order, on any SM count.  No host synchronisation, capturable in a CUDA graph.
+// Sets.  B pairs packed back to back, pair b owning source rows [src_off[b], src_off[b+1]) of src and target rows
+// [tgt_off[b], tgt_off[b+1]) of tgt (Ns and Nt rows; the correspondence key points of the drivers' --use_icp are the case
+// tgt_off = src_off, two fragments of the multiway registration the general one); fitness = |C| / Ns.  One CTA per pair runs
+// everything below from its own rows and its own scratch only, with reductions in a fixed order, so a pair's result is bit for
+// bit the same whatever else its call holds, in whatever order, on any SM count.  No host synchronisation, capturable in a CUDA
+// graph.
 //
-// Grid.  The target never moves, so each set indexes it once: cells of side h = max(r, sqrt(float32(r^2))) (no kept neighbour is
-// further than one cell away on any axis), keyed as in fpfh.cu (21 bits per axis relative to the set's own minimum, 63 bits),
-// in the set's own open-addressing region of 2^ceil(log2(2 N)) <= 4 N slots starting at slot 4 off[b].  The rows of each cell
-// are counted, scanned and listed; their order inside a cell comes from atomics and does not matter, because the search takes
-// the minimum of (d^2, row).  A set with a non-finite coordinate, or whose target spans 2^21 cells or more along an axis, gets
-// status 1 and returns init after 0 iterations (fitness = rmse = 0).
+// Grid.  The target never moves, so each pair indexes it once: cells of side h = max(r, sqrt(float32(r^2))) (no kept neighbour is
+// further than one cell away on any axis), keyed as in fpfh.cu (21 bits per axis relative to the target's own minimum, 63 bits),
+// in the pair's own open-addressing region of 2^ceil(log2(2 Nt)) <= 4 Nt slots starting at slot 4 tgt_off[b].  The rows of each
+// cell are counted, scanned and listed; their order inside a cell comes from atomics and does not matter, because the search
+// takes the minimum of (d^2, row).  A pair with a non-finite coordinate, or whose target spans 2^21 cells or more along an axis,
+// gets status 1 and returns init after 0 iterations (fitness = rmse = 0).  The moved source lives in scratch rows of the source.
+//
+// Information matrix (open3d 0.9's GetInformationMatrixFromPointClouds, recalled): the same grid and search, the source moved once
+// by T in fp64; every kept correspondence adds G G^T for the three rows (0, z, -y, 1, 0, 0), (-z, 0, x, 0, 1, 0),
+// (y, -x, 0, 0, 0, 1) of G, (x, y, z) its target point.  The CTA sums the ten moments of the kept target points (count, first
+// and second moments) in the fixed order of icp_block_sum and assembles the 6x6 from them; status 1 gives the zero matrix.
 //
 // Search.  The 27 cells around each moved source point.  The cost is the number of target rows in those cells: for key points a
 // few voxels apart that is a handful, but a set whose rows all fall into one cell makes every iteration N^2 (correct, slow).
@@ -46,25 +54,37 @@ __device__ __forceinline__ unsigned long long cell_mix(unsigned long long x) {
   return x;
 }
 
+// the cell index of the targets: Rt = the call's target rows
+struct GridScratch {
+  unsigned long long* keys;  // [4Rt]  cell keys, pair b's region from slot 4 tgt_off[b]
+  int* start;                // [4Rt]  first list entry of the cell
+  int* count;                // [4Rt]  rows of the cell
+  int* list;                 // [Rt]   pair-local target rows grouped by cell
+  int* slot;                 // [Rt]   region slot of every target row
+};
+constexpr size_t kGridBytesPerRow = 72;
+
+GridScratch grid_carve(unsigned char*& p, long long Rt) {
+  GridScratch s;
+  s.keys = reinterpret_cast<unsigned long long*>(p); p += (size_t)Rt * 32;
+  s.start = reinterpret_cast<int*>(p);              p += (size_t)Rt * 16;
+  s.count = reinterpret_cast<int*>(p);              p += (size_t)Rt * 16;
+  s.list = reinterpret_cast<int*>(p);               p += (size_t)Rt * 4;
+  s.slot = reinterpret_cast<int*>(p);               p += (size_t)Rt * 4;
+  return s;
+}
+
 struct IcpScratch {
-  double* P;                 // [R][3] the moved source points
-  unsigned long long* keys;  // [4R]   cell keys, set b's region from slot 4 off[b]
-  int* start;                // [4R]   first list entry of the cell
-  int* count;                // [4R]   rows of the cell
-  int* list;                 // [R]    set-local target rows grouped by cell
-  int* slot;                 // [R]    region slot of every target row
-  int* nn;                   // [R]    kept nearest target row (set-local) of every source row, or -1
+  double* P;                 // [Rs][3] the moved source points
+  GridScratch g;
+  int* nn;                   // [Rs]    kept nearest target row (pair-local) of every source row, or -1
 };
 
-IcpScratch icp_carve(void* scratch, long long R) {
+IcpScratch icp_carve(void* scratch, long long Rs, long long Rt) {
   unsigned char* p = static_cast<unsigned char*>(scratch);
   IcpScratch s;
-  s.P = reinterpret_cast<double*>(p);               p += (size_t)R * 24;
-  s.keys = reinterpret_cast<unsigned long long*>(p); p += (size_t)R * 32;
-  s.start = reinterpret_cast<int*>(p);              p += (size_t)R * 16;
-  s.count = reinterpret_cast<int*>(p);              p += (size_t)R * 16;
-  s.list = reinterpret_cast<int*>(p);               p += (size_t)R * 4;
-  s.slot = reinterpret_cast<int*>(p);               p += (size_t)R * 4;
+  s.P = reinterpret_cast<double*>(p);               p += (size_t)Rs * 24;
+  s.g = grid_carve(p, Rt);
   s.nn = reinterpret_cast<int*>(p);
   return s;
 }
@@ -104,7 +124,8 @@ __device__ __forceinline__ float icp_block_min(float v, float* red) {
 }
 
 struct Grid {
-  const unsigned long long* keys;   // the set's region
+  const float* pt;                  // the pair's target rows
+  const unsigned long long* keys;   // the pair's region
   const int* start;
   const int* count;
   const int* list;
@@ -123,9 +144,10 @@ __device__ __forceinline__ int find_cell(const Grid& g, unsigned long long key) 
 }
 
 // nearest target row (set-local) of p by (d^2, row), searched in the 27 cells around p; row -1 when none
-__device__ __forceinline__ int nearest_target(const Grid& g, const float* __restrict__ pt, double px, double py, double pz, double& best) {
+__device__ __forceinline__ int nearest_target(const Grid& g, double px, double py, double pz, double& best) {
   best = INFINITY;
   int row = -1;
+  const float* pt = g.pt;
   const double fc[3] = {floor((px - g.lo[0]) / g.h), floor((py - g.lo[1]) / g.h), floor((pz - g.lo[2]) / g.h)};
   for (int dx = -1; dx <= 1; ++dx) {
     const double cx = fc[0] + dx;
@@ -153,61 +175,50 @@ __device__ __forceinline__ int nearest_target(const Grid& g, const float* __rest
   }
   return row;
 }
-}  // namespace
 
-size_t icp_scratch_bytes(long long R) { return (size_t)R * 100; }
-
-__global__ void __launch_bounds__(kIcpThreads) icp_kernel(const float* __restrict__ src, const float* __restrict__ tgt,
-                                                          const float* __restrict__ init, Offsets off, double r, double r2f,
-                                                          int max_iteration, IcpScratch s, float* __restrict__ trans,
-                                                          double* __restrict__ fitness_out, double* __restrict__ rmse_out,
-                                                          int32_t* __restrict__ iterations_out, int32_t* __restrict__ status_out) {
-  __shared__ double red[kIcpWarps * 9];
-  __shared__ double tot[9];
-  __shared__ double T[16], U[12];
-  __shared__ float fred[kIcpWarps];
-  __shared__ int bad;
-  __shared__ int part[kIcpThreads];
-  const int b = blockIdx.x, tid = threadIdx.x;
-  const int row0 = off.at(b), N = off.at(b + 1) - row0;
-  const float* ps = src + (size_t)row0 * 3;
-  const float* pt = tgt + (size_t)row0 * 3;
-  double* P = s.P + (size_t)row0 * 3;
-  int* nn = s.nn + row0;
-  if (tid < 16) T[tid] = (double)init[(size_t)b * 16 + tid];
-  if (tid == 0) bad = 0;
-  __syncthreads();
-
-  // ---- the set's minimum and finiteness ----
+// The cell index of a pair's Nt target rows pt, in its region of g starting at slot 4 t0 and at row t0 (every thread calls it).
+// bad (shared, 0 on entry) becomes 1 when a target or one of the Ns source rows ps is not finite, or the targets span 2^21 cells
+// or more along an axis; the index is then not built and the caller returns its status-1 result.
+// g is shared: thread 0 fills it, and every thread reads it after the call.
+__device__ void build_grid(const float* __restrict__ pt, int Nt, const float* __restrict__ ps, int Ns, double h, const GridScratch& gs,
+                           long long t0, float* fred, int* part, int& bad, Grid& g) {
+  const int tid = threadIdx.x;
   float lo[3] = {INFINITY, INFINITY, INFINITY};
   bool finite = true;
-  for (int j = tid; j < N; j += kIcpThreads) {
+  for (int j = tid; j < Nt; j += kIcpThreads) {
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const float t = pt[3 * (size_t)j + c];
-      finite = finite && isfinite(t) && isfinite(ps[3 * (size_t)j + c]);
+      finite = finite && isfinite(t);
       lo[c] = fminf(lo[c], t);
     }
   }
-  if (!finite) bad = 1;                    // benign race: every writer stores 1
-  Grid g;
-  g.h = fmax(r, sqrt(r2f));
+  for (int j = tid; j < Ns; j += kIcpThreads)
 #pragma unroll
-  for (int c = 0; c < 3; ++c) g.lo[c] = (double)icp_block_min(lo[c], fred);
+    for (int c = 0; c < 3; ++c) finite = finite && isfinite(ps[3 * (size_t)j + c]);
+  if (!finite) bad = 1;                    // benign race: every writer stores 1
+  double gl[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) gl[c] = (double)icp_block_min(lo[c], fred);
 
-  // ---- the set's cell index: region init, insertion (with the extent check), scan, lists ----
-  const long long slots = icp_table_slots(N), base = 4ll * row0;
-  unsigned long long* keys = s.keys + base;
-  int* start = s.start + base;
-  int* count = s.count + base;
-  int* list = s.list + row0;
-  int* slot = s.slot + row0;
+  // ---- region init, insertion (with the extent check), scan, lists ----
+  const long long slots = icp_table_slots(Nt), base = 4ll * t0;
+  unsigned long long* keys = gs.keys + base;
+  int* start = gs.start + base;
+  int* count = gs.count + base;
+  int* list = gs.list + t0;
+  int* slot = gs.slot + t0;
+  if (tid == 0) {
+    g.pt = pt; g.keys = keys; g.start = start; g.count = count; g.list = list;
+    g.mask = (unsigned long long)slots - 1;
+    g.h = h;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) g.lo[c] = gl[c];
+  }
   for (long long q = tid; q < slots; q += kIcpThreads) { keys[q] = kEmptyCell; count[q] = 0; }
   __syncthreads();
-  g.keys = keys; g.start = start; g.count = count; g.list = list;
-  g.mask = (unsigned long long)slots - 1;
   if (!bad) {
-    for (int j = tid; j < N; j += kIcpThreads) {
+    for (int j = tid; j < Nt; j += kIcpThreads) {
       double cc[3];
       bool out = false;
 #pragma unroll
@@ -229,16 +240,7 @@ __global__ void __launch_bounds__(kIcpThreads) icp_kernel(const float* __restric
     }
   }
   __syncthreads();
-  if (bad) {
-    if (tid < 16) trans[(size_t)b * 16 + tid] = init[(size_t)b * 16 + tid];
-    if (tid == 0) {
-      if (fitness_out) fitness_out[b] = 0.0;
-      if (rmse_out) rmse_out[b] = 0.0;
-      if (iterations_out) iterations_out[b] = 0;
-      if (status_out) status_out[b] = 1;
-    }
-    return;
-  }
+  if (bad) return;
   {  // exclusive scan of the counts into the starts; the counts become fill cursors
     const long long per = (slots + kIcpThreads - 1) / kIcpThreads;
     const long long q0 = min(slots, (long long)tid * per), q1 = min(slots, q0 + per);
@@ -255,11 +257,51 @@ __global__ void __launch_bounds__(kIcpThreads) icp_kernel(const float* __restric
     for (long long q = q0; q < q1; ++q) { start[q] = run; run += count[q]; count[q] = 0; }
   }
   __syncthreads();
-  for (int j = tid; j < N; j += kIcpThreads) {
+  for (int j = tid; j < Nt; j += kIcpThreads) {
     const int q = slot[j];
     list[start[q] + atomicAdd(&count[q], 1)] = j;
   }
   __syncthreads();
+}
+}  // namespace
+
+size_t icp_scratch_bytes(long long Rs, long long Rt) { return (size_t)Rs * 28 + (size_t)Rt * kGridBytesPerRow; }
+size_t information_scratch_bytes(long long Rt) { return (size_t)Rt * kGridBytesPerRow; }
+
+__global__ void __launch_bounds__(kIcpThreads) icp_kernel(const float* __restrict__ src, const float* __restrict__ tgt,
+                                                          const float* __restrict__ init, Offsets soff, Offsets toff, double r,
+                                                          double r2f, int max_iteration, IcpScratch s, float* __restrict__ trans,
+                                                          double* __restrict__ fitness_out, double* __restrict__ rmse_out,
+                                                          int32_t* __restrict__ iterations_out, int32_t* __restrict__ status_out) {
+  __shared__ double red[kIcpWarps * 9];
+  __shared__ double tot[9];
+  __shared__ double T[16], U[12];
+  __shared__ float fred[kIcpWarps];
+  __shared__ int bad;
+  __shared__ int part[kIcpThreads];
+  __shared__ Grid g;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int s0 = soff.at(b), N = soff.at(b + 1) - s0;
+  const int t0 = toff.at(b), Nt = toff.at(b + 1) - t0;
+  const float* ps = src + (size_t)s0 * 3;
+  const float* pt = tgt + (size_t)t0 * 3;
+  double* P = s.P + (size_t)s0 * 3;
+  int* nn = s.nn + s0;
+  if (tid < 16) T[tid] = (double)init[(size_t)b * 16 + tid];
+  if (tid == 0) bad = 0;
+  __syncthreads();
+
+  build_grid(pt, Nt, ps, N, fmax(r, sqrt(r2f)), s.g, t0, fred, part, bad, g);
+  if (bad) {
+    if (tid < 16) trans[(size_t)b * 16 + tid] = init[(size_t)b * 16 + tid];
+    if (tid == 0) {
+      if (fitness_out) fitness_out[b] = 0.0;
+      if (rmse_out) rmse_out[b] = 0.0;
+      if (iterations_out) iterations_out[b] = 0;
+      if (status_out) status_out[b] = 1;
+    }
+    return;
+  }
 
   // ---- correspondences of the moved cloud (after applying U when `move`): count, sum d^2, sums of P and of its targets ----
   auto correspond = [&](bool move, double (&acc)[8]) {
@@ -280,13 +322,13 @@ __global__ void __launch_bounds__(kIcpThreads) icp_kernel(const float* __restric
       }
       P[3 * (size_t)j] = x; P[3 * (size_t)j + 1] = y; P[3 * (size_t)j + 2] = z;
       double d2;
-      int k = nearest_target(g, pt, x, y, z, d2);
+      int k = nearest_target(g, x, y, z, d2);
       if (k >= 0 && !(d2 < r2f)) k = -1;
       nn[j] = k;
       if (k >= 0) {
         acc[0] += 1.0; acc[1] += d2;
         acc[2] += x; acc[3] += y; acc[4] += z;
-        acc[5] += (double)pt[3 * (size_t)k]; acc[6] += (double)pt[3 * (size_t)k + 1]; acc[7] += (double)pt[3 * (size_t)k + 2];
+        acc[5] += (double)g.pt[3 * (size_t)k]; acc[6] += (double)g.pt[3 * (size_t)k + 1]; acc[7] += (double)g.pt[3 * (size_t)k + 2];
       }
     }
     icp_block_sum<8>(acc, red, tot);
@@ -307,8 +349,8 @@ __global__ void __launch_bounds__(kIcpThreads) icp_kernel(const float* __restric
         const int k = nn[j];
         if (k < 0) continue;
         const double mx = P[3 * (size_t)j] - ax, my = P[3 * (size_t)j + 1] - ay, mz = P[3 * (size_t)j + 2] - az;
-        const double nx = (double)pt[3 * (size_t)k] - bx, ny = (double)pt[3 * (size_t)k + 1] - by,
-                     nz = (double)pt[3 * (size_t)k + 2] - bz;
+        const double nx = (double)g.pt[3 * (size_t)k] - bx, ny = (double)g.pt[3 * (size_t)k + 1] - by,
+                     nz = (double)g.pt[3 * (size_t)k + 2] - bz;
         h[0] += mx * nx; h[1] += mx * ny; h[2] += mx * nz;
         h[3] += my * nx; h[4] += my * ny; h[5] += my * nz;
         h[6] += mz * nx; h[7] += mz * ny; h[8] += mz * nz;
@@ -349,12 +391,81 @@ __global__ void __launch_bounds__(kIcpThreads) icp_kernel(const float* __restric
   }
 }
 
-void launch_icp(int B, const int32_t* d_off, long long R, const float* src, const float* tgt, const float* init, double r,
-                int max_iteration, float* trans, double* fitness, double* rmse, int32_t* iterations, int32_t* status, void* scratch,
-                cudaStream_t st) {
+// One CTA per pair: the information matrix of the source moved by trans against the target (see the header of this file).
+__global__ void __launch_bounds__(kIcpThreads) information_kernel(const float* __restrict__ src, const float* __restrict__ tgt,
+                                                                  const float* __restrict__ trans, Offsets soff, Offsets toff,
+                                                                  double r, double r2f, GridScratch gs, double* __restrict__ info,
+                                                                  int32_t* __restrict__ status_out) {
+  __shared__ double red[kIcpWarps * 10];
+  __shared__ double tot[10];
+  __shared__ double T[12];
+  __shared__ float fred[kIcpWarps];
+  __shared__ int bad;
+  __shared__ int part[kIcpThreads];
+  __shared__ Grid g;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int s0 = soff.at(b), Ns = soff.at(b + 1) - s0;
+  const int t0 = toff.at(b), Nt = toff.at(b + 1) - t0;
+  const float* ps = src + (size_t)s0 * 3;
+  const float* pt = tgt + (size_t)t0 * 3;
+  if (tid < 12) T[tid] = (double)trans[(size_t)b * 16 + tid];
+  if (tid == 0) bad = 0;
+  __syncthreads();
+
+  build_grid(pt, Nt, ps, Ns, fmax(r, sqrt(r2f)), gs, t0, fred, part, bad, g);
+  double* out = info + (size_t)b * 36;
+  if (bad) {
+    for (int i = tid; i < 36; i += kIcpThreads) out[i] = 0.0;
+    if (tid == 0 && status_out) status_out[b] = 1;
+    return;
+  }
+  // moments of the kept target points: count, x, y, z, xx, yy, zz, xy, xz, yz
+  double m[10];
+#pragma unroll
+  for (int i = 0; i < 10; ++i) m[i] = 0.0;
+  for (int j = tid; j < Ns; j += kIcpThreads) {
+    const double ax = ps[3 * (size_t)j], ay = ps[3 * (size_t)j + 1], az = ps[3 * (size_t)j + 2];
+    const double x = T[0] * ax + T[1] * ay + T[2] * az + T[3];
+    const double y = T[4] * ax + T[5] * ay + T[6] * az + T[7];
+    const double z = T[8] * ax + T[9] * ay + T[10] * az + T[11];
+    double d2;
+    const int k = nearest_target(g, x, y, z, d2);
+    if (k < 0 || !(d2 < r2f)) continue;
+    const double qx = pt[3 * (size_t)k], qy = pt[3 * (size_t)k + 1], qz = pt[3 * (size_t)k + 2];
+    m[0] += 1.0; m[1] += qx; m[2] += qy; m[3] += qz;
+    m[4] += qx * qx; m[5] += qy * qy; m[6] += qz * qz;
+    m[7] += qx * qy; m[8] += qx * qz; m[9] += qy * qz;
+  }
+  icp_block_sum<10>(m, red, tot);
+  if (tid == 0) {
+    // sum over C of G G^T: [[S^T S, S^T], [S, n I]] with S = [q]_x summed, i.e. the blocks below
+    const double n = m[0], sx = m[1], sy = m[2], sz = m[3];
+    const double v[36] = {m[5] + m[6], -m[7],        -m[8],        0.0, -sz, sy,
+                          -m[7],       m[4] + m[6],  -m[9],        sz,  0.0, -sx,
+                          -m[8],       -m[9],        m[4] + m[5],  -sy, sx,  0.0,
+                          0.0,         sz,           -sy,          n,   0.0, 0.0,
+                          -sz,         0.0,          sx,           0.0, n,   0.0,
+                          sy,          -sx,          0.0,          0.0, 0.0, n};
+#pragma unroll
+    for (int i = 0; i < 36; ++i) out[i] = v[i];
+    if (status_out) status_out[b] = 0;
+  }
+}
+
+void launch_icp(int B, const int32_t* d_src_off, const int32_t* d_tgt_off, long long Rs, long long Rt, const float* src,
+                const float* tgt, const float* init, double r, int max_iteration, float* trans, double* fitness, double* rmse,
+                int32_t* iterations, int32_t* status, void* scratch, cudaStream_t st) {
   const double r2f = (double)(float)(r * r);
-  icp_kernel<<<B, kIcpThreads, 0, st>>>(src, tgt, init, Offsets{d_off, 0}, r, r2f, max_iteration, icp_carve(scratch, R), trans,
-                                        fitness, rmse, iterations, status);
+  icp_kernel<<<B, kIcpThreads, 0, st>>>(src, tgt, init, Offsets{d_src_off, 0}, Offsets{d_tgt_off, 0}, r, r2f, max_iteration,
+                                        icp_carve(scratch, Rs, Rt), trans, fitness, rmse, iterations, status);
+}
+
+void launch_information(int B, const int32_t* d_src_off, const int32_t* d_tgt_off, long long Rt, const float* src, const float* tgt,
+                        const float* trans, double r, double* info, int32_t* status, void* scratch, cudaStream_t st) {
+  const double r2f = (double)(float)(r * r);
+  unsigned char* p = static_cast<unsigned char*>(scratch);
+  information_kernel<<<B, kIcpThreads, 0, st>>>(src, tgt, trans, Offsets{d_src_off, 0}, Offsets{d_tgt_off, 0}, r, r2f,
+                                                grid_carve(p, Rt), info, status);
 }
 
 }  // namespace pdsc

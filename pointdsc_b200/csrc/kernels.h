@@ -123,13 +123,19 @@ int launch_compute_fpfh(int P, const int32_t* h_off, const int32_t* d_off, const
                         int max_nn, int normalise, double* out, int32_t* status, void* scratch,
                         cudaStream_t st);      // returns cudaError_t
 
-// ---- point-to-point ICP over the correspondence key points (icp.cu) ---------------------------------------------
-// B sets packed back to back (device offsets [B + 1], R = offsets[B] rows), init / trans [B,4,4]; fitness, rmse, iterations and
-// status may be null.  Scratch: icp_scratch_bytes(R) bytes, 8-byte aligned.
-size_t icp_scratch_bytes(long long R);
-void launch_icp(int B, const int32_t* d_off, long long R, const float* src, const float* tgt, const float* init, double r,
-                int max_iteration, float* trans, double* fitness, double* rmse, int32_t* iterations, int32_t* status, void* scratch,
-                cudaStream_t st);
+// ---- point-to-point ICP and information matrices between two clouds (icp.cu) ------------------------------------
+// B pairs: pair b's source is rows [src_off[b], src_off[b+1]) of src, its target rows [tgt_off[b], tgt_off[b+1]) of tgt (device
+// offsets [B + 1]; Rs, Rt = the last entries), init / trans [B,4,4]; fitness, rmse, iterations and status may be null.  The
+// correspondence key points are the case src_off = tgt_off.  Scratch: icp_scratch_bytes(Rs, Rt) bytes, 8-byte aligned.
+size_t icp_scratch_bytes(long long Rs, long long Rt);
+void launch_icp(int B, const int32_t* d_src_off, const int32_t* d_tgt_off, long long Rs, long long Rt, const float* src,
+                const float* tgt, const float* init, double r, int max_iteration, float* trans, double* fitness, double* rmse,
+                int32_t* iterations, int32_t* status, void* scratch, cudaStream_t st);
+// The same pairs, trans [B,4,4] -> info [B,6,6] double; status may be null.  Scratch: information_scratch_bytes(Rt) bytes,
+// 8-byte aligned.
+size_t information_scratch_bytes(long long Rt);
+void launch_information(int B, const int32_t* d_src_off, const int32_t* d_tgt_off, long long Rt, const float* src, const float* tgt,
+                        const float* trans, double r, double* info, int32_t* status, void* scratch, cudaStream_t st);
 
 // ---- correspondence RANSAC over the pairs the network kept (ransac.cu) ----------------------------------------
 // B sets packed back to back (device offsets [B + 1], R = offsets[B] rows), labels [R] (> 0: a candidate), trans [B,4,4],

@@ -48,3 +48,25 @@ def rigid(seed: int = 0, max_angle_deg: float = 40.0, max_shift: float = 0.8):
     R = np.eye(3) + np.sin(a) * K + (1 - np.cos(a)) * K @ K
     t = rng.uniform(-max_shift, max_shift, 3)
     return R, t
+
+
+def fragment_sequence(K: int, seed: int = 0, n_points: int = 20000, layout_seed: int = 11, radius: float = 1.6):
+    """K overlapping views of one room for the multiway registration: [(points [n_points,3] float32 in the fragment's own frame,
+    pose [4,4] float64 that maps the fragment into the room)].  View k is a fresh sampling of the room cropped to a ball of
+    `radius` around a camera that moves along three quarters of a circle, turning with it (so consecutive views overlap most and
+    the first and last least)."""
+    if K < 2:
+        raise ValueError("a fragment sequence needs at least two views")
+    rng = np.random.default_rng(seed)
+    out = []
+    for k in range(K):
+        world = scene(12 * n_points, seed=1000 * seed + k, layout_seed=layout_seed).astype(np.float64)
+        a = 1.5 * np.pi * k / (K - 1)
+        c = np.array([1.5 + 0.5 * np.cos(a), 1.5 + 0.5 * np.sin(a), 1.2])
+        pick = np.nonzero(np.linalg.norm(world - c, axis=1) < radius)[0]
+        pick = rng.choice(pick, n_points, replace=len(pick) < n_points)
+        R = np.array([[np.cos(a), -np.sin(a), 0.0], [np.sin(a), np.cos(a), 0.0], [0.0, 0.0, 1.0]])
+        pose = np.eye(4)
+        pose[:3, :3], pose[:3, 3] = R, c
+        out.append((((world[pick] - c) @ R).astype(np.float32), pose))
+    return out

@@ -51,6 +51,12 @@ from pointdsc_b200.icp import icp_refine, icp_refine_packed
 ic = icp_refine(h["src_keypts"].cuda(), h["tgt_keypts"].cuda(), out["final_trans"])
 ip, ii = icp_refine_packed(pk["src_keypts"], pk["tgt_keypts"], torch.eye(4).expand(3, 4, 4).cuda(), off, d_offsets=pk["d_offsets"],
                            info=True)                    # pdsc_icp_packed, sets of three sizes
+from pointdsc_b200 import multiway as MW
+clouds = [torch.from_numpy(scene(nn, seed=nn)).cuda() for nn in (3000, 1, 900)]
+mt, mi = MW.multi_scale_icp_packed(clouds, [(0, 1), (0, 2), (2, 0)], torch.eye(4).expand(3, 4, 4).cuda())   # down-sampled offsets
+mc = MW.icp_clouds_packed(torch.cat(clouds), torch.cat(clouds[::-1]), torch.eye(4).expand(2, 4, 4).cuda(), [0, 3000, 3001],
+                          [0, 900, 901])          # pdsc_icp_clouds_packed, Ns != Nt, a 1-row side
+mm = MW.information_matrix_packed(torch.cat(clouds), torch.cat(clouds[::-1]), mc, [0, 3000, 3001], [0, 900, 901])
 from pointdsc_b200.spectral import spectral_matching_packed
 smt, sml = spectral_matching_packed(pk["corr_pos"], pk["src_keypts"], pk["tgt_keypts"], off, d_offsets=pk["d_offsets"])  # sets of three sizes
 torch.cuda.synchronize()
