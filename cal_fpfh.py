@@ -49,8 +49,8 @@ def find_inputs(paths):
     return out
 
 
-def output_path(src, root, out_dir=None):
-    stem = os.path.splitext(src)[0] + "_fpfh.npz"
+def output_path(src, root, out_dir=None, suffix="_fpfh.npz"):
+    stem = os.path.splitext(src)[0] + suffix
     return stem if out_dir is None else os.path.join(out_dir, os.path.relpath(stem, root))
 
 
@@ -108,8 +108,9 @@ def _read_group(items):
     return [read_cloud(f) for f, _ in items]
 
 
-def run(paths, voxel_size=0.05, out_dir=None, max_points=4_000_000, describe=describe_on_device, log=print):
-    """Write `<stem>_fpfh.npz` for every input under `paths`; returns the files written, in input order."""
+def run(paths, voxel_size=0.05, out_dir=None, max_points=4_000_000, describe=describe_on_device, log=print, suffix="_fpfh.npz"):
+    """Write `<stem><suffix>` (by default `<stem>_fpfh.npz`) for every input under `paths`, with `describe(clouds, voxel_size)`
+    giving each group's (xyz, feature) pairs; returns the files written, in input order."""
     inputs = find_inputs(paths)
     groups = make_groups([cloud_size(f) for f, _ in inputs], max_points)
     written = []
@@ -125,7 +126,7 @@ def run(paths, voxel_size=0.05, out_dir=None, max_points=4_000_000, describe=des
             results = describe([clouds[k] for k in keep], voxel_size) if keep else []
             for k, (xyz, feat) in zip(keep, results):
                 src, root = inputs[idx[k]]
-                dst = output_path(src, root, out_dir)
+                dst = output_path(src, root, out_dir, suffix)
                 os.makedirs(os.path.dirname(os.path.abspath(dst)), exist_ok=True)
                 np.savez_compressed(dst, points=clouds[k].astype(np.float32), xyz=xyz.astype(np.float32),
                                     feature=feat.astype(np.float32))

@@ -6,8 +6,12 @@ read on the device and without open3d (reference demo_registration.py:37-44, :78
 
 Defaults: the reference's own demo clouds (copied unmodified into the git-ignored oracle/_ref/demo_data by
 `__graft_entry__.build()` when POINTDSC_REFERENCE names a checkout of the reference).  Prints the estimated transformation and, instead of the reference's
-open3d windows, how much of the source cloud lies on the target before and after it.  The FCGF descriptor network is out of scope
-(DESIGN.md section 8): `--descriptor fcgf` is refused."""
+open3d windows, how much of the source cloud lies on the target before and after it.
+
+`--descriptor fcgf --fcgf_weights PATH` describes both clouds with the FCGF network on the device (pointdsc_b200.fcgf, the
+reference's extract_fcgf_features, demo_registration.py:11-34) instead of FPFH: the 3DMatch snapshot pairs with the reference's
+ResUNetBN2C-feat32-3dmatch-v0.05.pth (conv1 kernel 7, voxel 0.05), the KITTI snapshot with ResUNetBN2C-feat32-kitti-v0.3.pth
+(kernel 5, voxel 0.30); the voxel is the snapshot's downsample.  The weights are not shipped."""
 import argparse
 import json
 import os
@@ -47,7 +51,8 @@ def coverage(src, tgt, radius, trans=None, chunk=4096):
 
 
 @torch.no_grad()
-def register(pcd1, pcd2, snapshot="PointDSC_3DMatch_release", device="cuda", verbose=True, return_data=False):
+def register(pcd1, pcd2, snapshot="PointDSC_3DMatch_release", device="cuda", verbose=True, return_data=False, descriptor="fpfh",
+             fcgf_weights=None):
     from pointdsc_b200 import PointDSC
     from pointdsc_b200.descriptors import fpfh_descriptors, read_ply
     from pointdsc_b200.frontend import match
@@ -60,7 +65,12 @@ def register(pcd1, pcd2, snapshot="PointDSC_3DMatch_release", device="cuda", ver
     t0 = time.perf_counter()
     clouds = [torch.from_numpy(read_ply(p)).to(device) for p in (pcd1, pcd2)]
     t1 = time.perf_counter()
-    (src_pts, src_feat), (tgt_pts, tgt_feat) = (fpfh_descriptors(c, cfg["downsample"]) for c in clouds)
+    if descriptor == "fcgf":                                                        # demo_registration.py:11-34
+        from pointdsc_b200.fcgf import fcgf_descriptors_many, model_from_checkpoint
+        kp, feat, off, _ = fcgf_descriptors_many(model_from_checkpoint(fcgf_weights), clouds, cfg["downsample"])
+        (src_pts, src_feat), (tgt_pts, tgt_feat) = ((kp[off[p]:off[p + 1]], feat[off[p]:off[p + 1]]) for p in range(2))
+    else:
+        (src_pts, src_feat), (tgt_pts, tgt_feat) = (fpfh_descriptors(c, cfg["downsample"]) for c in clouds)
     data = match(src_feat, tgt_feat, src_pts, tgt_pts, use_mutual=False)          # demo_registration.py:101-108
     data["testing"] = True
     res = model(data)                                                               # demo_registration.py:117
@@ -90,13 +100,17 @@ def main():
     ap.add_argument("--pcd1", default=os.path.join(REF, "demo_data", "cloud_bin_0.ply"))
     ap.add_argument("--pcd2", default=os.path.join(REF, "demo_data", "cloud_bin_1.ply"))
     ap.add_argument("--descriptor", default="fpfh", choices=["fcgf", "fpfh"])
+    ap.add_argument("--fcgf_weights", default=None, help="the FCGF checkpoint --descriptor fcgf reads")
     ap.add_argument("--use_gpu", default="True")
     a = ap.parse_args()
-    if a.descriptor != "fpfh":
-        sys.exit("the FCGF descriptor network (MinkowskiEngine) is out of scope: use --descriptor fpfh")
+    if a.descriptor == "fcgf" and not (a.fcgf_weights and os.path.exists(a.fcgf_weights)):
+        kitti = a.chosen_snapshot == "PointDSC_KITTI_release"
+        sys.exit(f"--descriptor fcgf needs --fcgf_weights PATH ({a.fcgf_weights} not found).  The reference downloads them from "
+                 "http://node2.chrischoy.org/data/projects/DGR/ResUNetBN2C-feat32-"
+                 + ("kitti-v0.3.pth (conv1 kernel 5, voxel 0.30)" if kitti else "3dmatch-v0.05.pth (conv1 kernel 7, voxel 0.05)"))
     if str(a.use_gpu).lower() in ("false", "0", "no") or not torch.cuda.is_available():
         sys.exit("pointdsc_b200 runs on an H100 only (there is no CPU fallback)")
-    register(a.pcd1, a.pcd2, a.chosen_snapshot)
+    register(a.pcd1, a.pcd2, a.chosen_snapshot, descriptor=a.descriptor, fcgf_weights=a.fcgf_weights)
 
 
 if __name__ == "__main__":

@@ -307,6 +307,40 @@ int pdsc_estimate_normals_packed(pdsc_engine* e, int32_t P, const int32_t* h_off
 int pdsc_compute_fpfh_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
                              const double* d_normals, double radius, int32_t max_nn, int32_t normalise, double* d_fpfh,
                              int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+/* f8: FCGF descriptors, replacing misc/cal_fcgf.py:11-85 extract_features (rgb = normal = None) with the ResUNetBN2C network of
+ * misc/fcgf.py:621-867 (CHANNELS 32/64/128/256, TR_CHANNELS 64/64/64/128, BN, normalize_feature) in MinkowskiEngine 0.5.
+ * MinkowskiEngine is not part of the reference tree: the conventions are restated in oracle/fcgf_oracle.py (PARITY UNPINNED).
+ * Weights live in a handle of their own, like the engine's: pdsc_fcgf_create(conv1_kernel_size (7: the 3DMatch weights at voxel
+ * 0.05; 5: the KITTI weights at voxel 0.30), &h); pdsc_fcgf_set_param(h, name, data, numel) with the checkpoint's state_dict keys
+ * and element counts (convolution kernels `<name>.kernel` in MinkowskiEngine's [K^3, Cin, Cout] / [Cin, Cout] layout, norms
+ * `<name>.bn.{weight,bias,running_mean,running_var}`, `final.bias`; num_batches_tracked is not passed): PDSC_ERR_UNKNOWN_PARAM for
+ * another name, PDSC_ERR_SHAPE for another count; pdsc_fcgf_commit(h) folds every BN (eps 1e-5) in float64 and uploads to the
+ * current device (PDSC_ERR_UNKNOWN_PARAM names a missing entry); pdsc_fcgf_destroy(h) frees it.
+ * pdsc_fcgf_packed: P clouds, cloud p owning rows [offsets[p], offsets[p+1]) of d_points [n,3] float32 (offsets as for
+ * pdsc_voxel_down_sample_packed, n = offsets[P] <= 2^26; h_offsets sizes the launches and the scratch, d_offsets is what the kernels
+ * read).  Per cloud: voxel coordinates floor((double)x / voxel_size), one row per occupied voxel in order of its first point, the
+ * key point = that first point; the 32-channel unit descriptor of every row.  Outputs: d_out_offsets [P+1] (written on the
+ * stream), d_keypts [n,3] and d_desc [n,32] float32 (rows [out_offsets[p], out_offsets[p+1]) are cloud p's; rows at or beyond
+ * out_offsets[P] are not written), d_status [P]: bit 1 = a non-finite coordinate or one outside [-2^20, 2^20) voxels (the point
+ * is left out).  A cloud's rows are bit for bit the same in any call, in any order, on any SM count.  Scratch:
+ * pdsc_fcgf_packed_scratch_bytes() bytes (about 11 KB per input point with conv1_kernel_size 7), 256-byte aligned.  No host
+ * synchronisation, no allocation, capturable in a CUDA graph.
+ * pdsc_fcgf_scratch_layout (a test aid): the byte offsets inside that scratch, after a call, of 37 regions, in this order: every
+ * level's row offsets [P+1] int32 (levels 0..3, tensor strides 1, 2, 4, 8); every level's voxel coordinates [n,3] int32; the conv1
+ * neighbour table [n,K^3]; the same-stride 3^3 tables of levels 0..3, the strided tables of levels 1..3 (a row of level l gathers
+ * level l-1) and the transposed tables of levels 0..2 (a row of level l gathers level l+1), each [n,27] int32 (-1: no neighbour);
+ * then the 18 feature buffers [n,w] float32 (x, t, cat, d, dt of levels 0, 1, 2, then x, t, s8 of level 3) that DESIGN.md's f8
+ * table assigns to each convolution.  Returns the count (0 for bad arguments); writes at most `capacity` offsets. */
+typedef struct pdsc_fcgf pdsc_fcgf;
+int pdsc_fcgf_create(int32_t conv1_kernel_size, pdsc_fcgf** h);
+int pdsc_fcgf_set_param(pdsc_fcgf* h, const char* name, const float* h_data, int64_t numel);
+int pdsc_fcgf_commit(pdsc_fcgf* h);
+int pdsc_fcgf_destroy(pdsc_fcgf* h);
+size_t pdsc_fcgf_packed_scratch_bytes(const pdsc_fcgf* h, int32_t P, const int32_t* h_offsets);
+int pdsc_fcgf_packed(pdsc_engine* e, const pdsc_fcgf* h, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets,
+                     const float* d_points, double voxel_size, float* d_keypts, float* d_desc, int32_t* d_out_offsets,
+                     int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+int32_t pdsc_fcgf_scratch_layout(const pdsc_fcgf* h, int32_t P, const int32_t* h_offsets, int64_t* offsets, int32_t capacity);
 /* f5: point-to-point ICP over the correspondence key points, replacing icp_refine (evaluation/benchmark_utils.py:40-55): open3d 0.9's
  * registration_icp(src, tgt, max_corr_dist, init, TransformationEstimationPointToPoint(False), ICPConvergenceCriteria()) with the
  * criteria fixed at their defaults (relative fitness 1e-6, relative rmse 1e-6).  open3d is not part of the reference tree: this

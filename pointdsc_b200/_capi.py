@@ -134,6 +134,14 @@ SYMBOLS = {
     "pdsc_spectral_matching_packed_iterates": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                          C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                          C.c_void_p, C.c_size_t, C.c_void_p]),
+    "pdsc_fcgf_create": (C.c_int, [C.c_int32, C.POINTER(C.c_void_p)]),
+    "pdsc_fcgf_destroy": (C.c_int, [C.c_void_p]),
+    "pdsc_fcgf_set_param": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64]),
+    "pdsc_fcgf_commit": (C.c_int, [C.c_void_p]),
+    "pdsc_fcgf_packed_scratch_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_void_p]),
+    "pdsc_fcgf_packed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "pdsc_fcgf_scratch_layout": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32]),
     "pdsc_read_ply": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
     "pdsc_launches_per_forward": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32]),
     "pdsc_profile_enable": (C.c_int, [C.c_void_p, C.c_int32]),

@@ -955,6 +955,74 @@ int pdsc_compute_fpfh_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets
                      d_status, d_scratch, scratch_bytes, cuda_stream);
 }
 
+int pdsc_fcgf_create(int32_t conv1_kernel_size, pdsc_fcgf** out) {
+  if (!out) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_fcgf_create: null handle pointer");
+  *out = nullptr;
+  if (conv1_kernel_size != 5 && conv1_kernel_size != 7)
+    return fail(PDSC_ERR_UNSUPPORTED, "pdsc_fcgf_create: conv1_kernel_size must be 5 or 7 (got %d)", conv1_kernel_size);
+  *out = pdsc::fcgf_new(conv1_kernel_size);
+  return PDSC_OK;
+}
+
+int pdsc_fcgf_destroy(pdsc_fcgf* h) {
+  pdsc::fcgf_free(h);
+  return PDSC_OK;
+}
+
+int pdsc_fcgf_set_param(pdsc_fcgf* h, const char* name, const float* h_data, int64_t numel) {
+  if (!h || !name || (!h_data && numel > 0) || numel < 0) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_fcgf_set_param: bad argument");
+  size_t expected = 0;
+  const int rc = pdsc::fcgf_set_param(h, name, h_data, numel, &expected);
+  if (rc == 1) return fail(PDSC_ERR_UNKNOWN_PARAM, "pdsc_fcgf_set_param: unknown parameter '%s'", name);
+  if (rc == 2)
+    return fail(PDSC_ERR_SHAPE, "pdsc_fcgf_set_param: '%s' has %lld elements, expected %zu", name, (long long)numel, expected);
+  return PDSC_OK;
+}
+
+int pdsc_fcgf_commit(pdsc_fcgf* h) {
+  if (!h) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_fcgf_commit: null handle");
+  std::string missing;
+  const int rc = pdsc::fcgf_commit(h, &missing);
+  if (rc < 0) return fail(PDSC_ERR_UNKNOWN_PARAM, "pdsc_fcgf_commit: state-dict entry missing: %s", missing.c_str());
+  if (rc > 0) return fail(PDSC_ERR_CUDA, "pdsc_fcgf_commit: upload failed: %s", cudaGetErrorString((cudaError_t)rc));
+  return PDSC_OK;
+}
+
+// the points of a call bound every level's rows and every int32 table index: at most 2^26 in all
+static constexpr int32_t kFcgfMaxPoints = 1 << 26;
+
+size_t pdsc_fcgf_packed_scratch_bytes(const pdsc_fcgf* h, int32_t P, const int32_t* h_offsets) {
+  if (!h || check_offsets("pdsc_fcgf_packed_scratch_bytes", "", P, h_offsets, 1) || h_offsets[P] > kFcgfMaxPoints) return 0;
+  return pdsc::fcgf_scratch_bytes(P, h_offsets, pdsc::fcgf_kernel_size(h));
+}
+
+int32_t pdsc_fcgf_scratch_layout(const pdsc_fcgf* h, int32_t P, const int32_t* h_offsets, int64_t* offsets, int32_t capacity) {
+  if (!h || check_offsets("pdsc_fcgf_scratch_layout", "", P, h_offsets, 1) || h_offsets[P] > kFcgfMaxPoints) return 0;
+  return pdsc::fcgf_scratch_layout(P, h_offsets, pdsc::fcgf_kernel_size(h), offsets, offsets ? capacity : 0);
+}
+
+int pdsc_fcgf_packed(pdsc_engine* e, const pdsc_fcgf* h, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets,
+                     const float* d_points, double voxel_size, float* d_keypts, float* d_desc, int32_t* d_out_offsets,
+                     int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  const char* fn = "pdsc_fcgf_packed";
+  if (!e || !h) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null engine or weight handle", fn);
+  if (!pdsc::fcgf_committed(h)) return fail(PDSC_ERR_NOT_COMMITTED, "%s: pdsc_fcgf_commit() has not been called since the last "
+                                            "pdsc_fcgf_set_param()", fn);
+  if (int rc = check_offsets(fn, "", P, h_offsets, 1)) return rc;
+  if (h_offsets[P] > kFcgfMaxPoints) return fail(PDSC_ERR_SHAPE, "%s: need at most 2^26 points (got %d)", fn, h_offsets[P]);
+  if (!(voxel_size > 0.0) || !std::isfinite(voxel_size))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: voxel_size must be positive and finite (got %g)", fn, voxel_size);
+  if (!d_offsets || !d_points || !d_keypts || !d_desc || !d_out_offsets || !d_status)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  const int k1 = pdsc::fcgf_kernel_size(h);
+  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::fcgf_scratch_bytes(P, h_offsets, k1), 256)) return rc;
+  DeviceGuard g(e->cfg.device);
+  const int rc = pdsc::launch_fcgf(h, P, h_offsets, d_offsets, d_points, voxel_size, d_keypts, d_desc, d_out_offsets, d_status,
+                                   d_scratch, static_cast<cudaStream_t>(cuda_stream));
+  if (rc) return fail(PDSC_ERR_CUDA, "%s: launch failed: %s", fn, cudaGetErrorString((cudaError_t)rc));
+  return PDSC_OK;
+}
+
 size_t pdsc_icp_packed_scratch_bytes(int32_t B, const int32_t* h_offsets) {
   return pdsc_icp_clouds_packed_scratch_bytes(B, h_offsets, h_offsets);
 }

@@ -43,20 +43,15 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "sets.cuh"
+#include "voxel_hash.cuh"
 #include "warp_select.cuh"
 
 namespace pdsc {
 
 namespace {
-constexpr unsigned long long kEmpty = ~0ull;
+constexpr unsigned long long kEmpty = kEmptyKey;
 constexpr int kCandCap = 4096;          // in-radius candidates one warp can hold
 constexpr double kFix = 1099511627776.0;   // 2^40: fixed-point scale of the offset inside a voxel, in voxel units
-
-__host__ __device__ inline unsigned long long table_slots(long long n) {
-  unsigned long long c = 1024;
-  while (c < 2ull * (unsigned long long)n) c <<= 1;
-  return c;
-}
 
 // first 256-row rank tile of cloud p: a function of the offsets alone (as frontend.cu's tile0); a cloud of n rows owns
 // ceil(n / 256) tiles or one more, which is idle
@@ -72,12 +67,6 @@ struct VoxScratch {
   int* counts;                 // [S]
   uint32_t* cslot;             // [n]   slot of ckeys[i] inside its cloud's region
 };
-
-unsigned long long total_slots(int P, const int32_t* h_off) {
-  unsigned long long s = 0;
-  for (int p = 0; p < P; ++p) s += table_slots((long long)h_off[p + 1] - h_off[p]);
-  return s;
-}
 
 VoxScratch vox_carve(void* scratch, int P, long long n, unsigned long long slots) {
   unsigned char* p = static_cast<unsigned char*>(scratch);
@@ -99,31 +88,6 @@ size_t voxel_scratch_bytes(int P, const int32_t* h_off) {
 }
 
 // ---- voxel down-sampling ---------------------------------------------------------------------------------------
-// exclusive prefix sums of v(0 .. n-1) by ONE CTA of 1024 threads: out_first[0] = 0 (unless null), out_ends[q] = v(0) + .. + v(q)
-template <typename T, typename F>
-__device__ void cta_offsets(int n, F v, T* out_first, T* out_ends) {
-  __shared__ T part[1024];
-  const int per = (n + 1023) / 1024;
-  const int q0 = min(n, (int)threadIdx.x * per), q1 = min(n, q0 + per);
-  T s = 0;
-  for (int q = q0; q < q1; ++q) s += v(q);
-  part[threadIdx.x] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    T run = 0;
-    for (int t = 0; t < 1024; ++t) { const T x = part[t]; part[t] = run; run += x; }
-    if (out_first) out_first[0] = 0;
-  }
-  __syncthreads();
-  T run = part[threadIdx.x];
-  for (int q = q0; q < q1; ++q) { run += v(q); out_ends[q] = run; }
-}
-
-// every cloud's hash-table region: table_slots(n_p) slots (a power of two, at least 1024) from slot0[p]
-__global__ void __launch_bounds__(1024) vox_plan_kernel(int P, Offsets off, unsigned long long* slot0) {
-  cta_offsets<unsigned long long>(P, [&](int q) { return table_slots((long long)off.at(q + 1) - off.at(q)); }, slot0, slot0 + 1);
-}
-
 __global__ void vox_init_kernel(int P, uint32_t* minkey, int* counter, unsigned long long* keys, unsigned long long* sums, int* counts,
                                 unsigned long long slots, int32_t* status) {
   const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -158,11 +122,6 @@ __device__ __forceinline__ float key32_to_float(uint32_t k) {      // inverse of
   return __uint_as_float(u);
 }
 
-__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
-  x ^= x >> 33; x *= 0xff51afd7ed558ccdull; x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull; x ^= x >> 33;
-  return x;
-}
-
 __global__ void vox_insert_kernel(const float* __restrict__ pts, long long n, int P, Offsets off, double voxel,
                                   const uint32_t* __restrict__ minkey, const unsigned long long* __restrict__ slot0,
                                   unsigned long long* keys, unsigned long long* sums, int* counts, int32_t* status) {
@@ -187,15 +146,9 @@ __global__ void vox_insert_kernel(const float* __restrict__ pts, long long n, in
     atomicOr(&status[p], 1);                           // more than 2^21 voxels along an axis, or a non-finite coordinate
     return;
   }
-  const unsigned long long key = ((unsigned long long)ix[0] << 42) | ((unsigned long long)ix[1] << 21) | (unsigned long long)ix[2];
-  const unsigned long long base = slot0[p], mask = slot0[p + 1] - base - 1;
-  unsigned long long s = mix64(key) & mask;
-  while (true) {
-    const unsigned long long prev = atomicCAS(&keys[base + s], kEmpty, key);
-    if (prev == kEmpty || prev == key) break;
-    s = (s + 1) & mask;
-  }
-  s += base;
+  const unsigned long long key = pack_key21(ix[0], ix[1], ix[2]);
+  const unsigned long long base = slot0[p];
+  const unsigned long long s = hash_insert(keys, base, slot0[p + 1] - base - 1, key);
   atomicAdd(&sums[3 * s], q[0]); atomicAdd(&sums[3 * s + 1], q[1]); atomicAdd(&sums[3 * s + 2], q[2]);
   atomicAdd(&counts[s], 1);
 }
@@ -271,7 +224,7 @@ void launch_voxel_down_sample(int P, const int32_t* h_off, const int32_t* d_off,
   const VoxScratch s = vox_carve(scratch, P, n, slots);
   long long most = 0;
   for (int p = 0; p < P; ++p) most = std::max<long long>(most, (long long)h_off[p + 1] - h_off[p]);
-  vox_plan_kernel<<<1, 1024, 0, st>>>(P, off, s.slot0);
+  hash_plan_kernel<<<1, 1024, 0, st>>>(P, off, s.slot0);
   const unsigned long long init = std::max<unsigned long long>(slots, 3ull * P);
   vox_init_kernel<<<(unsigned)((init + 255) / 256), 256, 0, st>>>(P, s.minkey, s.counter, s.keys, s.sums, s.counts, slots, status);
   const int sms = device_sm_count();

@@ -5,7 +5,11 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <string>
+
 #include "sets.cuh"
+
+struct pdsc_fcgf;
 
 namespace pdsc {
 
@@ -147,6 +151,19 @@ void launch_ransac(int B, const int32_t* d_off, long long R, const float* src, c
                    int max_iteration, unsigned long long seed, float* trans, float* out_labels, double* fitness, double* rmse,
                    int32_t* best, int32_t* status, int32_t* hyp_good, double* hyp_rmse, double* hyp_trans, void* scratch,
                    cudaStream_t st);
+
+// ---- f8: FCGF descriptors (fcgf.cu) -----------------------------------------------------------------------------
+// The weight handle of the C ABI (folded, packed and uploaded by fcgf_commit) and the one launch chain of a packed call.
+pdsc_fcgf* fcgf_new(int k1);
+void fcgf_free(pdsc_fcgf* h);
+int fcgf_set_param(pdsc_fcgf* h, const char* name, const float* data, int64_t numel, size_t* expected);   // 1 unknown, 2 size
+int fcgf_commit(pdsc_fcgf* h, std::string* missing);      // -1: *missing names an absent parameter; > 0: a cudaError_t
+bool fcgf_committed(const pdsc_fcgf* h);
+int fcgf_kernel_size(const pdsc_fcgf* h);
+size_t fcgf_scratch_bytes(int P, const int32_t* h_off, int k1);
+int fcgf_scratch_layout(int P, const int32_t* h_off, int k1, int64_t* offsets, int capacity);
+int launch_fcgf(const pdsc_fcgf* h, int P, const int32_t* h_off, const int32_t* d_off, const float* pts, double voxel,
+                float* keypts, float* desc, int32_t* out_off, int32_t* status, void* scratch, cudaStream_t st);   // cudaError_t
 
 // ---- the spectral-matching baseline (spectral_matching.cu) ---------------------------------------------------
 // B sets packed back to back (host and device offsets [B + 1], R = offsets[B] rows, every set 1 .. spectral_matching_max_n() rows),
