@@ -467,6 +467,46 @@ int pdsc_leading_eigenvector(pdsc_engine* e, int32_t B, int32_t N, const float* 
                              float* d_eigenvector, int32_t* d_iterations_run, void* d_scratch, size_t scratch_bytes,
                              void* cuda_stream);
 
+/* f9: the fragments of the multiway experiment (multiway/make_fragments.py): open3d 0.9's ScalableTSDFVolume(RGB8) integration and
+ * the vertices (with colours) of extract_triangle_mesh, for F fragments in one call per stage.  Conventions restated in
+ * numpy under oracle/ (PARITY UNPINNED).  Fragment f owns frames h/d_frame_offsets[f] .. [f+1] (1 .. 256 frames) of
+ * d_depth [NF,H,W] uint16 (metres = raw / depth_scale, 0 at or beyond depth_trunc), d_color [NF,H,W,3] uint8 and d_poses [NF,2,16]
+ * float64 (row-major extrinsic, world to camera, then its inverse, the camera pose); intrinsic is the host {fx, fy, cx, cy}.
+ * A volume unit is 16^3 voxels of side voxel_length.  The three stages share one table (pdsc_tsdf_table_bytes(F, max_units), 8-byte
+ * aligned, max_units units per fragment at most), which the touch initialises and every later stage of the same volume reads:
+ * 1. pdsc_tsdf_touch_packed: d_unit_counts [F] int32 (the units each fragment's frames touch) and d_status [F] int32 (bit 1: more
+ *    than max_units units, the volume is incomplete; bit 2: a point beyond 2^20 units from the origin, skipped).
+ * 2. pdsc_tsdf_integrate_packed with h/d_unit_offsets [F+1] from those counts: d_unit_keys [U,3] int32 (unit coordinates, each
+ *    fragment's sorted ascending), d_tsdf and d_weight [U,16,16,16] float32 and d_voxel_color [U,16,16,16,3] float32 (0 .. 255), bit
+ *    for bit the float32 restatement.  Unit offsets above the touch's counts leave the extra rows at the end of their fragment
+ *    with coordinates INT32_MIN and weight 0; nothing is written outside the table, the scratch and the outputs.  At most 65535
+ *    frames per call.  Scratch: pdsc_tsdf_integrate_scratch_bytes() bytes, 8-byte aligned.
+ * 3. pdsc_extract_vertices_count_packed: d_vertex_ends [U] int64 (inclusive ends of every unit's vertices) and d_vertex_offsets
+ *    [F+1] int64; then pdsc_extract_vertices_packed: d_vertices and d_vertex_colors [V,3] float64 (colours in 0 .. 1), ordered by
+ *    (fragment, unit, x, y, z, edge axis).
+ * Everything runs on the caller's stream with no host synchronisation and no allocation; a fragment's outputs are bit for bit the
+ * same in any group, in any order, at any SM count. */
+size_t pdsc_tsdf_table_bytes(int32_t F, int32_t max_units);
+int pdsc_tsdf_touch_packed(pdsc_engine* e, int32_t F, const int32_t* h_frame_offsets, const int32_t* d_frame_offsets, int32_t height,
+                           int32_t width, const double* intrinsic, const uint16_t* d_depth, const double* d_poses, double depth_scale,
+                           double depth_trunc, double voxel_length, double sdf_trunc, int32_t max_units, int32_t* d_unit_counts,
+                           int32_t* d_status, void* d_table, size_t table_bytes, void* cuda_stream);
+size_t pdsc_tsdf_integrate_scratch_bytes(int32_t F, const int32_t* h_unit_offsets);
+int pdsc_tsdf_integrate_packed(pdsc_engine* e, int32_t F, const int32_t* h_frame_offsets, const int32_t* d_frame_offsets,
+                               const int32_t* h_unit_offsets, const int32_t* d_unit_offsets, int32_t height, int32_t width,
+                               const double* intrinsic, const uint16_t* d_depth, const uint8_t* d_color, const double* d_poses,
+                               double depth_scale, double depth_trunc, double voxel_length, double sdf_trunc, int32_t max_units,
+                               void* d_table, size_t table_bytes, int32_t* d_unit_keys, float* d_tsdf, float* d_weight,
+                               float* d_voxel_color, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+int pdsc_extract_vertices_count_packed(pdsc_engine* e, int32_t F, const int32_t* h_unit_offsets, const int32_t* d_unit_offsets,
+                                       int32_t max_units, void* d_table, size_t table_bytes, const int32_t* d_unit_keys,
+                                       const float* d_tsdf, const float* d_weight, int64_t* d_vertex_ends, int64_t* d_vertex_offsets,
+                                       void* cuda_stream);
+int pdsc_extract_vertices_packed(pdsc_engine* e, int32_t F, const int32_t* h_unit_offsets, const int32_t* d_unit_offsets,
+                                 int32_t max_units, void* d_table, size_t table_bytes, const int32_t* d_unit_keys, const float* d_tsdf,
+                                 const float* d_weight, const float* d_voxel_color, double voxel_length, const int64_t* d_vertex_ends,
+                                 double* d_vertices, double* d_vertex_colors, void* cuda_stream);
+
 /* ---- live profiling with CUDA events on the caller's stream ------------------------------------------
  * When enabled, pdsc_forward() records an event pair around each stage below (and around EVERY launch of
  * the dominant kernel, the per-layer attention).  pdsc_profile_read() waits for the last forward's events

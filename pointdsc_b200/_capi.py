@@ -142,6 +142,21 @@ SYMBOLS = {
     "pdsc_fcgf_packed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "pdsc_fcgf_scratch_layout": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32]),
+    "pdsc_tsdf_table_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
+    "pdsc_tsdf_touch_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int32, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "pdsc_tsdf_integrate_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_void_p]),
+    "pdsc_tsdf_integrate_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                             C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_double,
+                                             C.c_double, C.c_double, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "pdsc_extract_vertices_count_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                                     C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                     C.c_void_p]),
+    "pdsc_extract_vertices_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p]),
     "pdsc_read_ply": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
     "pdsc_launches_per_forward": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32]),
     "pdsc_profile_enable": (C.c_int, [C.c_void_p, C.c_int32]),

@@ -1102,6 +1102,129 @@ int pdsc_information_matrix_packed(pdsc_engine* e, int32_t B, const int32_t* h_s
   return PDSC_OK;
 }
 
+namespace {
+constexpr int kTsdfMaxUnits = 1 << 22;
+
+// the frame offsets, image and volume parameters every TSDF stage of a call checks alike
+pdsc_status check_tsdf(const char* fn, int32_t F, const int32_t* h_frame_offsets, int32_t height, int32_t width,
+                       const double* intrinsic, double voxel_length, double sdf_trunc, int32_t max_units) {
+  if (pdsc_status rc = check_offsets(fn, "frame ", F, h_frame_offsets, 1, pdsc::kMaxFragmentFrames)) return rc;
+  if (h_frame_offsets[F] > 65535) return fail(PDSC_ERR_SHAPE, "%s: at most 65535 frames per call (got %d)", fn, h_frame_offsets[F]);
+  if (height < 1 || width < 1 || (long long)height * width > (1 << 26))
+    return fail(PDSC_ERR_SHAPE, "%s: image %d x %d outside 1 .. 2^26 pixels", fn, width, height);
+  if (!intrinsic) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null intrinsic", fn);
+  for (int i = 0; i < 4; ++i)
+    if (!std::isfinite(intrinsic[i]) || (i < 2 && !(intrinsic[i] > 0.0)))
+      return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: intrinsic %d (%g) must be finite, and the focal lengths positive", fn, i, intrinsic[i]);
+  if (!(voxel_length > 0.0) || !std::isfinite(voxel_length) || !(sdf_trunc > 0.0) || !std::isfinite(sdf_trunc))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: voxel_length (%g) and sdf_trunc (%g) must be positive and finite", fn, voxel_length,
+                sdf_trunc);
+  if (max_units < 1 || max_units > kTsdfMaxUnits)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_units %d outside [1, %d]", fn, max_units, kTsdfMaxUnits);
+  return PDSC_OK;
+}
+
+pdsc_status check_units(const char* fn, int32_t F, const int32_t* h_unit_offsets, int32_t max_units, const void* d_table,
+                        size_t table_bytes) {
+  if (max_units < 1 || max_units > kTsdfMaxUnits)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_units %d outside [1, %d]", fn, max_units, kTsdfMaxUnits);
+  if (pdsc_status rc = check_offsets(fn, "unit ", F, h_unit_offsets, 0, max_units)) return rc;
+  return check_scratch(fn, "table", d_table, table_bytes, pdsc::tsdf_table_bytes(F, max_units), 8);
+}
+}  // namespace
+
+size_t pdsc_tsdf_table_bytes(int32_t F, int32_t max_units) {
+  if (F < 1 || max_units < 1 || max_units > kTsdfMaxUnits) return 0;
+  return pdsc::tsdf_table_bytes(F, max_units);
+}
+
+int pdsc_tsdf_touch_packed(pdsc_engine* e, int32_t F, const int32_t* h_frame_offsets, const int32_t* d_frame_offsets, int32_t height,
+                           int32_t width, const double* intrinsic, const uint16_t* d_depth, const double* d_poses, double depth_scale,
+                           double depth_trunc, double voxel_length, double sdf_trunc, int32_t max_units, int32_t* d_unit_counts,
+                           int32_t* d_status, void* d_table, size_t table_bytes, void* cuda_stream) {
+  const char* fn = "pdsc_tsdf_touch_packed";
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_tsdf(fn, F, h_frame_offsets, height, width, intrinsic, voxel_length, sdf_trunc, max_units)) return rc;
+  if (!(depth_scale > 0.0) || !std::isfinite(depth_scale))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: depth_scale must be positive and finite (got %g)", fn, depth_scale);
+  if (!d_frame_offsets || !d_depth || !d_poses || !d_unit_counts || !d_status)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  if (int rc = check_scratch(fn, "table", d_table, table_bytes, pdsc::tsdf_table_bytes(F, max_units), 8)) return rc;
+  DeviceGuard g(e->cfg.device);
+  pdsc::launch_tsdf_touch(F, h_frame_offsets[F], d_frame_offsets, height, width, intrinsic, d_depth, d_poses, depth_scale, depth_trunc,
+                          voxel_length, sdf_trunc, max_units, d_unit_counts, d_status, d_table, static_cast<cudaStream_t>(cuda_stream));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
+
+size_t pdsc_tsdf_integrate_scratch_bytes(int32_t F, const int32_t* h_unit_offsets) {
+  if (check_offsets("pdsc_tsdf_integrate_scratch_bytes", "unit ", F, h_unit_offsets, 0, kTsdfMaxUnits)) return 0;
+  return pdsc::tsdf_integrate_scratch_bytes(F, h_unit_offsets[F]);
+}
+
+int pdsc_tsdf_integrate_packed(pdsc_engine* e, int32_t F, const int32_t* h_frame_offsets, const int32_t* d_frame_offsets,
+                               const int32_t* h_unit_offsets, const int32_t* d_unit_offsets, int32_t height, int32_t width,
+                               const double* intrinsic, const uint16_t* d_depth, const uint8_t* d_color, const double* d_poses,
+                               double depth_scale, double depth_trunc, double voxel_length, double sdf_trunc, int32_t max_units,
+                               void* d_table, size_t table_bytes, int32_t* d_unit_keys, float* d_tsdf, float* d_weight,
+                               float* d_voxel_color, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  const char* fn = "pdsc_tsdf_integrate_packed";
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_tsdf(fn, F, h_frame_offsets, height, width, intrinsic, voxel_length, sdf_trunc, max_units)) return rc;
+  if (int rc = check_units(fn, F, h_unit_offsets, max_units, d_table, table_bytes)) return rc;
+  if (!(depth_scale > 0.0) || !std::isfinite(depth_scale))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: depth_scale must be positive and finite (got %g)", fn, depth_scale);
+  const long long U = h_unit_offsets[F];
+  if (!d_frame_offsets || !d_unit_offsets || !d_depth || !d_color || !d_poses || (U > 0 && (!d_unit_keys || !d_tsdf || !d_weight ||
+                                                                                             !d_voxel_color)))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::tsdf_integrate_scratch_bytes(F, U), 8)) return rc;
+  DeviceGuard g(e->cfg.device);
+  pdsc::launch_tsdf_integrate(F, d_frame_offsets, d_unit_offsets, U, height, width, intrinsic, d_depth, d_color, d_poses, depth_scale,
+                              depth_trunc, voxel_length, sdf_trunc, max_units, d_table, d_unit_keys, d_tsdf, d_weight, d_voxel_color,
+                              d_scratch, static_cast<cudaStream_t>(cuda_stream));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
+
+int pdsc_extract_vertices_count_packed(pdsc_engine* e, int32_t F, const int32_t* h_unit_offsets, const int32_t* d_unit_offsets,
+                                       int32_t max_units, void* d_table, size_t table_bytes, const int32_t* d_unit_keys,
+                                       const float* d_tsdf, const float* d_weight, int64_t* d_vertex_ends, int64_t* d_vertex_offsets,
+                                       void* cuda_stream) {
+  const char* fn = "pdsc_extract_vertices_count_packed";
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_units(fn, F, h_unit_offsets, max_units, d_table, table_bytes)) return rc;
+  const int U = h_unit_offsets[F];
+  if (!d_unit_offsets || !d_vertex_offsets || (U > 0 && (!d_unit_keys || !d_tsdf || !d_weight || !d_vertex_ends)))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  DeviceGuard g(e->cfg.device);
+  pdsc::launch_vertex_count(F, d_unit_offsets, U, max_units, d_table, d_unit_keys, d_tsdf, d_weight,
+                            reinterpret_cast<long long*>(d_vertex_ends), reinterpret_cast<long long*>(d_vertex_offsets),
+                            static_cast<cudaStream_t>(cuda_stream));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
+
+int pdsc_extract_vertices_packed(pdsc_engine* e, int32_t F, const int32_t* h_unit_offsets, const int32_t* d_unit_offsets,
+                                 int32_t max_units, void* d_table, size_t table_bytes, const int32_t* d_unit_keys, const float* d_tsdf,
+                                 const float* d_weight, const float* d_voxel_color, double voxel_length, const int64_t* d_vertex_ends,
+                                 double* d_vertices, double* d_vertex_colors, void* cuda_stream) {
+  const char* fn = "pdsc_extract_vertices_packed";
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_units(fn, F, h_unit_offsets, max_units, d_table, table_bytes)) return rc;
+  if (!(voxel_length > 0.0) || !std::isfinite(voxel_length))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: voxel_length must be positive and finite (got %g)", fn, voxel_length);
+  const int U = h_unit_offsets[F];
+  if (!d_unit_offsets || (U > 0 && (!d_unit_keys || !d_tsdf || !d_weight || !d_voxel_color || !d_vertex_ends)))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  DeviceGuard g(e->cfg.device);
+  pdsc::launch_vertex_write(F, d_unit_offsets, U, max_units, d_table, d_unit_keys, d_tsdf, d_weight, d_voxel_color, voxel_length,
+                            reinterpret_cast<const long long*>(d_vertex_ends), d_vertices, d_vertex_colors,
+                            static_cast<cudaStream_t>(cuda_stream));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
+
 size_t pdsc_ransac_packed_scratch_bytes(int32_t B, const int32_t* h_offsets, int32_t max_iteration) {
   if (check_offsets("pdsc_ransac_packed_scratch_bytes", "", B, h_offsets, 1)) return 0;
   if (max_iteration < 1) {

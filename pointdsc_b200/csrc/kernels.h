@@ -176,6 +176,26 @@ void launch_spectral_matching(int B, const int32_t* h_off, const int32_t* d_off,
                               double inlier_threshold, float* trans, float* labels, float* eig_out, float* iterates, void* scratch,
                               cudaStream_t st);
 
+// ---- f9: TSDF integration and surface vertices of RGB-D fragments (fragments.cu) ---------------------------------------
+// F fragments of 1 .. kMaxFragmentFrames frames each (device frame offsets [F + 1], NF frames): depth [NF,H,W] uint16, colour
+// [NF,H,W,3] uint8, poses [NF,2,16] float64 (extrinsic, camera pose), intrinsic the host fx, fy, cx, cy.  The table
+// (tsdf_table_bytes(F, max_units), 8-byte aligned) is written by the touch and read by every later stage of the same volume.
+constexpr int kMaxFragmentFrames = 256;
+size_t tsdf_table_bytes(int F, int max_units);
+size_t tsdf_integrate_scratch_bytes(int F, long long U);
+void launch_tsdf_touch(int F, int NF, const int32_t* d_frame_off, int H, int W, const double* intrinsic, const uint16_t* depth,
+                       const double* poses, double depth_scale, double depth_trunc, double voxel, double trunc, int max_units,
+                       int32_t* counts, int32_t* status, void* table, cudaStream_t st);
+void launch_tsdf_integrate(int F, const int32_t* d_frame_off, const int32_t* d_unit_off, long long U, int H, int W,
+                           const double* intrinsic, const uint16_t* depth, const uint8_t* color, const double* poses,
+                           double depth_scale, double depth_trunc, double voxel, double trunc, int max_units, void* table,
+                           int32_t* unit_keys, float* tsdf, float* weight, float* color_out, void* scratch, cudaStream_t st);
+void launch_vertex_count(int F, const int32_t* d_unit_off, int U, int max_units, void* table, const int32_t* unit_keys,
+                         const float* tsdf, const float* weight, long long* ends, long long* frag_off, cudaStream_t st);
+void launch_vertex_write(int F, const int32_t* d_unit_off, int U, int max_units, void* table, const int32_t* unit_keys,
+                         const float* tsdf, const float* weight, const float* color, double voxel, const long long* ends,
+                         double* vertices, double* colors, cudaStream_t st);
+
 // ---- per-device launch configuration (device_state.cu) ----------------------------------------------------
 // opt `kernel` in to `bytes` of dynamic shared memory on the CURRENT device (no-op if already granted there)
 cudaError_t ensure_dynamic_smem(const void* kernel, int bytes);

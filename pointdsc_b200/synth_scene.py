@@ -70,3 +70,68 @@ def fragment_sequence(K: int, seed: int = 0, n_points: int = 20000, layout_seed:
         pose[:3, :3], pose[:3, 3] = R, c
         out.append((((world[pick] - c) @ R).astype(np.float32), pose))
     return out
+
+
+def room_shapes(layout_seed: int = 11):
+    """The analytic room `render_rgbd` ray-casts: the six faces of [0, 3]^3, two spheres (centre, radius) and one axis-aligned
+    box (lo, hi), placed by `layout_seed`."""
+    lay = np.random.default_rng(layout_seed)
+    spheres = [(lay.uniform(0.8, 2.2, 3), float(lay.uniform(0.2, 0.4))) for _ in range(2)]
+    c, h = lay.uniform(0.8, 2.2, 3), lay.uniform(0.15, 0.35, 3)
+    return {"room": 3.0, "spheres": spheres, "box": (c - h, c + h)}
+
+
+def render_rgbd(camera_pose: np.ndarray, width: int, height: int, fx: float, fy: float, cx: float, cy: float,
+                layout_seed: int = 11):
+    """Ray-cast the room of `room_shapes` from a pinhole camera (x right, y down, z forward; `camera_pose` maps camera to world):
+    (depth [H,W] uint16 millimetres of the nearest hit along the optical axis, colour [H,W,3] uint8 of a smooth procedural texture
+    of the hit point, so the photometric term has gradients)."""
+    shapes = room_shapes(layout_seed)
+    v, u = np.meshgrid(np.arange(height, dtype=np.float64), np.arange(width, dtype=np.float64), indexing="ij")
+    d_cam = np.stack([(u - cx) / fx, (v - cy) / fy, np.ones_like(u)], -1)          # z = 1: the ray parameter is the depth
+    R, o = np.asarray(camera_pose, np.float64)[:3, :3], np.asarray(camera_pose, np.float64)[:3, 3]
+    d = d_cam @ R.T
+    t = np.full(u.shape, np.inf)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        for a in range(3):                                                           # the room's faces from the inside
+            for wall in (0.0, shapes["room"]):
+                ta = (wall - o[a]) / d[..., a]
+                t = np.where((ta > 0) & (ta < t), ta, t)
+        for c, r in shapes["spheres"]:
+            oc = o - c
+            b = d @ oc
+            a2 = np.einsum("hwk,hwk->hw", d, d)
+            disc = b * b - a2 * (oc @ oc - r * r)
+            ts = (-b - np.sqrt(disc)) / a2
+            t = np.where((disc >= 0) & (ts > 0) & (ts < t), ts, t)
+        lo, hi = shapes["box"]
+        t1, t2 = (lo - o) / d, (hi - o) / d
+        tn, tf = np.minimum(t1, t2).max(-1), np.maximum(t1, t2).min(-1)
+        t = np.where((tn <= tf) & (tn > 0) & (tn < t), tn, t)
+    p = o + t[..., None] * d
+    depth = np.where(np.isfinite(t), np.round(t * 1000.0), 0).clip(0, 65535).astype(np.uint16)
+    tex = np.stack([np.sin(2.1 * p[..., 0] + 1.3 * p[..., 1]), np.sin(1.7 * p[..., 1] + 2.3 * p[..., 2] + 1.0),
+                    np.sin(2.9 * p[..., 2] + 1.1 * p[..., 0] + 2.0)], -1)
+    color = np.where(np.isfinite(t)[..., None], 128 + 100 * tex, 0).astype(np.uint8)
+    return depth, color
+
+
+def camera_path(n: int, seed: int = 0):
+    """n camera poses [n,4,4] float64 inside the room, looking at its centre from a slowly moving point (consecutive frames of an
+    RGB-D sequence)."""
+    rng = np.random.default_rng(seed)
+    a0 = rng.uniform(0, 2 * np.pi)
+    out = []
+    for k in range(n):
+        a = a0 + 0.02 * k
+        eye = np.array([1.5 + 0.6 * np.cos(a), 1.5 + 0.6 * np.sin(a), 1.3 + 0.05 * np.sin(0.3 * k)])
+        fwd = np.array([1.5, 1.5, 1.2]) - eye + np.array([0.4 * np.cos(a + 1.0), 0.4 * np.sin(a + 1.0), 0.0])
+        fwd /= np.linalg.norm(fwd)
+        right = np.cross(fwd, [0.0, 0.0, 1.0])
+        right /= np.linalg.norm(right)
+        down = np.cross(fwd, right)
+        pose = np.eye(4)
+        pose[:3, :3] = np.stack([right, down, fwd], 1)
+        pose[:3, 3] = eye
+        out.append(pose)
+    return np.stack(out)
