@@ -18,6 +18,7 @@
 //               previous iterate and latches a per-set `done` flag — later iterations of a finished set are no-ops, which is
 //               how the data-dependent early exit runs without a host synchronisation.
 // Rows whose address is not 16-byte aligned (N % 4 != 0) cannot be bulk-copied: that case takes plain coalesced loads.
+#include "abi.h"
 #include "common.cuh"
 #include "kernels.h"
 #include "tc_ptx.cuh"
@@ -26,6 +27,10 @@ namespace pdsc {
 using namespace ptx;
 
 constexpr int kEigRows = 32, kEigCols = 512, kEigThreads = 256;       // kEigRows: the maximum; R = rows_per_cta at run time
+// the largest N accepted: the gemv's two tile stages and its copy of v (N rounded up to kEigCols) fit in 227 KB of shared memory
+constexpr int kEigMaxN = 24576;
+static_assert(kEigMaxN % kEigCols == 0 && 2 * kEigRows * kEigCols * 4 + 64 + kEigMaxN * 4 <= 227 * 1024,
+              "eig_gemv_kernel's shared memory at N = kEigMaxN");
 
 __global__ void __launch_bounds__(kEigThreads) eig_gemv_kernel(const float* __restrict__ M, const float* __restrict__ v,
                                                                float* __restrict__ u, float* __restrict__ partial_ss,
@@ -158,9 +163,27 @@ size_t eig_scratch_bytes(int B, int N) {
   return (size_t)B * N * 4 + (size_t)B * nparts * 4 + (size_t)B * 4 + 256;
 }
 
+}  // namespace pdsc
+
+// ---- C ABI ------------------------------------------------------------------------------------------------------
+using namespace pdsc;
+
+extern "C" {
+
+size_t pdsc_leading_eigenvector_scratch_bytes(int32_t B, int32_t N) { return (B > 0 && N > 0) ? eig_scratch_bytes(B, N) : 0; }
+
 // v [B,N] receives the eigenvector, iters_run [B] the iterations executed per set.  scratch: u [B,N] | partial [B,nparts] | done [B]
-int launch_leading_eigenvector(const float* M, float* v, int* iters_run, int B, int N, int iters, int early_exit, void* scratch,
-                               cudaStream_t st) {
+int pdsc_leading_eigenvector(pdsc_engine* e, int32_t B, int32_t N, const float* d_M, int32_t num_iterations, int32_t early_exit,
+                             float* d_eigenvector, int32_t* d_iterations_run, void* d_scratch, size_t scratch_bytes,
+                             void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (B <= 0 || N <= 0) return fail(PDSC_ERR_SHAPE, "need B >= 1 and N >= 1 (got B=%d N=%d)", B, N);
+  if (num_iterations < 1 || num_iterations > 1000) return fail(PDSC_ERR_INVALID_ARGUMENT, "num_iterations %d out of range", num_iterations);
+  if (N > kEigMaxN) return fail(PDSC_ERR_UNSUPPORTED, "N=%d exceeds the supported maximum %d", N, kEigMaxN);
+  if (!d_M || !d_eigenvector || !d_iterations_run) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_leading_eigenvector: null tensor pointer");
+  if (int rc = check_scratch("pdsc_leading_eigenvector", "scratch", d_scratch, scratch_bytes, eig_scratch_bytes(B, N), 16)) return rc;
+  DeviceGuard g(engine_config(e).device);
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   // rows per CTA: 32 when the grid is many waves anyway, else what makes it one wave of two CTAs per SM
   const int sms = device_sm_count();
   int R = kEigRows;
@@ -169,21 +192,23 @@ int launch_leading_eigenvector(const float* M, float* v, int* iters_run, int B, 
     R = R < 8 ? 8 : (R > kEigRows ? kEigRows : R);
   }
   const int nparts = (N + R - 1) / R;
-  float* u = static_cast<float*>(scratch);
+  float* u = static_cast<float*>(d_scratch);
   float* partial = u + (size_t)B * N;
   int* done = reinterpret_cast<int*>(partial + (size_t)B * ((N + 7) / 8));
   const int NP = (N + kEigCols - 1) / kEigCols * kEigCols;
   const int smem = 2 * R * kEigCols * 4 + 64 + NP * 4;
-  if (smem > 227 * 1024) return (int)cudaErrorInvalidValue;
-  const cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(eig_gemv_kernel), smem);
-  if (e != cudaSuccess) return (int)e;
-  const int use_tma = (N % 4 == 0) && (reinterpret_cast<uintptr_t>(M) % 16 == 0);
-  eig_init_kernel<<<(unsigned)(((long long)B * N + 255) / 256), 256, 0, st>>>(v, done, iters_run, B, N);
-  for (int t = 0; t < iters; ++t) {
-    eig_gemv_kernel<<<dim3(nparts, B), kEigThreads, smem, st>>>(M, v, u, partial, done, N, use_tma, R);
-    eig_norm_kernel<<<B, 256, 0, st>>>(u, v, partial, done, iters_run, N, nparts, early_exit);
+  const int use_tma = (N % 4 == 0) && (reinterpret_cast<uintptr_t>(d_M) % 16 == 0);
+  cudaError_t err = ensure_dynamic_smem(reinterpret_cast<const void*>(eig_gemv_kernel), smem);
+  if (err == cudaSuccess) {
+    eig_init_kernel<<<(unsigned)(((long long)B * N + 255) / 256), 256, 0, st>>>(d_eigenvector, done, d_iterations_run, B, N);
+    for (int t = 0; t < num_iterations; ++t) {
+      eig_gemv_kernel<<<dim3(nparts, B), kEigThreads, smem, st>>>(d_M, d_eigenvector, u, partial, done, N, use_tma, R);
+      eig_norm_kernel<<<B, 256, 0, st>>>(u, d_eigenvector, partial, done, d_iterations_run, N, nparts, early_exit);
+    }
+    err = cudaGetLastError();
   }
-  return (int)cudaGetLastError();
+  if (err != cudaSuccess) return fail(PDSC_ERR_CUDA, "power iteration launch failed: %s", cudaGetErrorString(err));
+  return PDSC_OK;
 }
 
-}  // namespace pdsc
+}  // extern "C"

@@ -1,57 +1,31 @@
-// Host side of the engine: parameter store (state-dict keys), BatchNorm folding, workspace carving,
-// stage orchestration for PointDSC.forward in testing mode (reference models/PointDSC.py:128-197),
-// and the C ABI declared in include/pointdsc_b200.h.
+// Host side of the forward engine: parameter store (state-dict keys), BatchNorm folding, workspace carving, stage
+// orchestration for PointDSC.forward in testing mode (reference models/PointDSC.py:128-197), graphs, the host-input pipeline
+// and profiling: the engine's entry points of include/pointdsc_b200.h.  The entry points of the other algorithms live in the
+// files that hold their kernels; what they share (abi.h) is defined here.
 #include <cuda_runtime.h>
 
-#include <algorithm>
-#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
-#include <cstring>
 #include <map>
 #include <string>
 #include <utility>
 #include <vector>
 
 #include "../../include/pointdsc_b200.h"
+#include "abi.h"
 #include "common.cuh"
 #include "encoder_tc.h"
 #include "kernels.h"
 
+using pdsc::check_offsets;
+using pdsc::check_scratch;
+using pdsc::DeviceGuard;
+using pdsc::fail;
+
 namespace {
 
 thread_local std::string g_last_error;
-
-pdsc_status fail(pdsc_status code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_last_error = buf;
-  return code;
-}
-
-#define PDSC_CUDA(expr)                                                                      \
-  do {                                                                                       \
-    cudaError_t err__ = (expr);                                                              \
-    if (err__ != cudaSuccess)                                                                \
-      return fail(PDSC_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(err__), __FILE__, __LINE__); \
-  } while (0)
-
-struct DeviceGuard {
-  int prev = -1;
-  explicit DeviceGuard(int dev) {
-    cudaGetDevice(&prev);
-    if (prev != dev) cudaSetDevice(dev);
-    else prev = -1;
-  }
-  ~DeviceGuard() {
-    if (prev >= 0) cudaSetDevice(prev);
-  }
-};
 
 constexpr size_t kGraphRows = 32768;   // B * N up to which the host path replays a captured graph (launch-bound regime)
 constexpr double kBnEps = 1e-5;  // torch.nn.BatchNorm1d default (reference PointDSC.py:14, :59)
@@ -112,6 +86,45 @@ struct pdsc_engine {
   cudaStream_t capture_stream = nullptr;   // graphs are captured here (the caller's stream may be the legacy default stream,
                                            // which cannot be captured) and launched into the caller's stream
 };
+
+// ---- abi.h ----------------------------------------------------------------------------------------
+namespace pdsc {
+
+pdsc_status fail(pdsc_status code, const char* fmt, ...) {
+  char buf[512];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof(buf), fmt, ap);
+  va_end(ap);
+  g_last_error = buf;
+  return code;
+}
+
+pdsc_status check_offsets(const char* who, const char* what, int32_t n, const int32_t* h_offsets, int min_rows, int max_rows) {
+  if (n < 1) return fail(PDSC_ERR_SHAPE, "%s: need at least one set (got %d)", who, n);
+  if (!h_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null host offsets", who);
+  if (h_offsets[0] != 0) return fail(PDSC_ERR_SHAPE, "%s: %soffsets[0] must be 0 (got %d)", who, what, h_offsets[0]);
+  for (int b = 0; b < n; ++b) {
+    const long long rows = (long long)h_offsets[b + 1] - h_offsets[b];
+    if (rows < min_rows)
+      return fail(PDSC_ERR_SHAPE, "%s: set %d has %lld %srows: offsets must increase by at least %d per set", who, b, rows, what,
+                  min_rows);
+    if (rows > max_rows)
+      return fail(PDSC_ERR_SHAPE, "%s: set %d has %lld %srows, above the supported maximum %d", who, b, rows, what, max_rows);
+  }
+  return PDSC_OK;
+}
+
+pdsc_status check_scratch(const char* who, const char* noun, const void* ptr, size_t bytes, size_t need, size_t align) {
+  if (!ptr || bytes < need || reinterpret_cast<uintptr_t>(ptr) % align)
+    return fail(PDSC_ERR_WORKSPACE, "%s: %s too small or not %zu-byte aligned (%zu bytes given, %zu needed)", who, noun, align,
+                bytes, need);
+  return PDSC_OK;
+}
+
+const pdsc_config& engine_config(const pdsc_engine* e) { return e->cfg; }
+
+}  // namespace pdsc
 
 namespace {
 
@@ -227,32 +240,6 @@ bool fold_conv(const pdsc_engine* e, const std::string& conv, const std::string&
   }
   while (arena->size() % 4) arena->push_back(0.f);
   return true;
-}
-
-// Host offsets [n + 1] of a call of n sets packed back to back: n >= 1, offsets[0] = 0, and every set between min_rows and
-// max_rows rows.  `what` prefixes "offsets" and "rows" in the message ("source " / "target " for a group of pairs, else "").
-pdsc_status check_offsets(const char* who, const char* what, int32_t n, const int32_t* h_offsets, int min_rows,
-                          int max_rows = INT_MAX) {
-  if (n < 1) return fail(PDSC_ERR_SHAPE, "%s: need at least one set (got %d)", who, n);
-  if (!h_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null host offsets", who);
-  if (h_offsets[0] != 0) return fail(PDSC_ERR_SHAPE, "%s: %soffsets[0] must be 0 (got %d)", who, what, h_offsets[0]);
-  for (int b = 0; b < n; ++b) {
-    const long long rows = (long long)h_offsets[b + 1] - h_offsets[b];
-    if (rows < min_rows)
-      return fail(PDSC_ERR_SHAPE, "%s: set %d has %lld %srows: offsets must increase by at least %d per set", who, b, rows, what,
-                  min_rows);
-    if (rows > max_rows)
-      return fail(PDSC_ERR_SHAPE, "%s: set %d has %lld %srows, above the supported maximum %d", who, b, rows, what, max_rows);
-  }
-  return PDSC_OK;
-}
-
-// A caller's workspace or scratch buffer: at least `need` bytes at an `align`-byte boundary.
-pdsc_status check_scratch(const char* who, const char* noun, const void* ptr, size_t bytes, size_t need, size_t align) {
-  if (!ptr || bytes < need || reinterpret_cast<uintptr_t>(ptr) % align)
-    return fail(PDSC_ERR_WORKSPACE, "%s: %s too small or not %zu-byte aligned (%zu bytes given, %zu needed)", who, noun, align,
-                bytes, need);
-  return PDSC_OK;
 }
 
 void copy_tap(void* dst, const void* src, size_t bytes, cudaStream_t st) {
@@ -782,677 +769,6 @@ int pdsc_forward_eval(pdsc_engine* e, int32_t B, int32_t N, const float* d_corr_
                       size_t workspace_bytes, void* cuda_stream) {
   return forward_impl(e, 1, B, N, nullptr, nullptr, d_corr_pos, d_src, d_tgt, d_final_trans, d_confidence, d_M, io, d_workspace,
                       workspace_bytes, cuda_stream);
-}
-
-static int eval_stats_impl(pdsc_engine* e, int32_t B, const int32_t* d_offsets, int32_t N, const float* d_pred_trans,
-                           const float* d_gt_trans, const float* d_src, const float* d_tgt, const float* d_pred_labels,
-                           const float* d_gt_labels, float re_thre, float te_thre, float* d_stats, void* cuda_stream) {
-  if (!d_pred_trans || !d_gt_trans || !d_src || !d_tgt || !d_pred_labels || !d_gt_labels || !d_stats)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_eval_stats: null tensor pointer");
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_eval_stats(d_pred_trans, d_gt_trans, d_src, d_tgt, d_pred_labels, d_gt_labels, d_stats, B, d_offsets, N, re_thre,
-                          te_thre, static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
-}
-
-int pdsc_eval_stats(pdsc_engine* e, int32_t B, int32_t N, const float* d_pred_trans, const float* d_gt_trans,
-                    const float* d_src, const float* d_tgt, const float* d_pred_labels, const float* d_gt_labels,
-                    float re_thre, float te_thre, float* d_stats, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (B <= 0 || N <= 0) return fail(PDSC_ERR_SHAPE, "need B >= 1 and N >= 1 (got B=%d N=%d)", B, N);
-  return eval_stats_impl(e, B, nullptr, N, d_pred_trans, d_gt_trans, d_src, d_tgt, d_pred_labels, d_gt_labels, re_thre, te_thre,
-                         d_stats, cuda_stream);
-}
-
-int pdsc_eval_stats_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
-                           const float* d_pred_trans, const float* d_gt_trans, const float* d_src, const float* d_tgt,
-                           const float* d_pred_labels, const float* d_gt_labels, float re_thre, float te_thre, float* d_stats,
-                           void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_offsets("pdsc_eval_stats_packed", "", B, h_offsets, 1)) return rc;
-  if (!d_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_eval_stats_packed: null device offsets");
-  return eval_stats_impl(e, B, d_offsets, 0, d_pred_trans, d_gt_trans, d_src, d_tgt, d_pred_labels, d_gt_labels, re_thre, te_thre,
-                         d_stats, cuda_stream);
-}
-
-size_t pdsc_leading_eigenvector_scratch_bytes(int32_t B, int32_t N) {
-  return (B > 0 && N > 0) ? pdsc::eig_scratch_bytes(B, N) : 0;
-}
-
-int pdsc_leading_eigenvector(pdsc_engine* e, int32_t B, int32_t N, const float* d_M, int32_t num_iterations, int32_t early_exit,
-                             float* d_eigenvector, int32_t* d_iterations_run, void* d_scratch, size_t scratch_bytes,
-                             void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (B <= 0 || N <= 0) return fail(PDSC_ERR_SHAPE, "need B >= 1 and N >= 1 (got B=%d N=%d)", B, N);
-  if (num_iterations < 1 || num_iterations > 1000) return fail(PDSC_ERR_INVALID_ARGUMENT, "num_iterations %d out of range", num_iterations);
-  if (N > 24576) return fail(PDSC_ERR_UNSUPPORTED, "N=%d exceeds the supported maximum 24576", N);
-  if (!d_M || !d_eigenvector || !d_iterations_run) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_leading_eigenvector: null tensor pointer");
-  if (int rc = check_scratch("pdsc_leading_eigenvector", "scratch", d_scratch, scratch_bytes, pdsc::eig_scratch_bytes(B, N), 16))
-    return rc;
-  DeviceGuard g(e->cfg.device);
-  const int rc = pdsc::launch_leading_eigenvector(d_M, d_eigenvector, d_iterations_run, B, N, num_iterations, early_exit, d_scratch,
-                                                  static_cast<cudaStream_t>(cuda_stream));
-  if (rc) return fail(PDSC_ERR_CUDA, "power iteration launch failed: %s", cudaGetErrorString((cudaError_t)rc));
-  return PDSC_OK;
-}
-
-size_t pdsc_voxel_down_sample_scratch_bytes(int64_t n) {
-  if (n <= 0 || n > (1ll << 30)) return 0;
-  const int32_t off[2] = {0, (int32_t)n};
-  return pdsc::voxel_scratch_bytes(1, off);
-}
-
-size_t pdsc_voxel_down_sample_packed_scratch_bytes(int32_t P, const int32_t* h_offsets) {
-  if (check_offsets("pdsc_voxel_down_sample_packed_scratch_bytes", "", P, h_offsets, 1) || h_offsets[P] > (1 << 30)) return 0;
-  return pdsc::voxel_scratch_bytes(P, h_offsets);
-}
-
-static int voxel_impl(const char* who, pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets,
-                      const float* d_points, double voxel_size, float* d_out_points, int32_t* d_out_first, int32_t* d_out_ends,
-                      int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  if (h_offsets[P] > (1 << 30)) return fail(PDSC_ERR_SHAPE, "%s: need at most 2^30 points (got %d)", who, h_offsets[P]);
-  if (!(voxel_size > 0.0)) return fail(PDSC_ERR_INVALID_ARGUMENT, "voxel_size must be positive (got %g)", voxel_size);
-  if (!d_points || !d_out_points || !d_out_ends || !d_status) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", who);
-  if (int rc = check_scratch(who, "scratch", d_scratch, scratch_bytes, pdsc::voxel_scratch_bytes(P, h_offsets), 8)) return rc;
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_voxel_down_sample(P, h_offsets, d_offsets, d_points, voxel_size, d_out_points, d_out_first, d_out_ends, d_status,
-                                 d_scratch, static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
-}
-
-int pdsc_voxel_down_sample(pdsc_engine* e, int64_t n, const float* d_points, double voxel_size, float* d_out_points,
-                           int32_t* d_count, int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (n <= 0 || n > (1ll << 30)) return fail(PDSC_ERR_SHAPE, "need 1 <= n <= 2^30 points (got %lld)", (long long)n);
-  // the packed call with one cloud: its offsets need no device table, and its end row is the count
-  const int32_t off[2] = {0, (int32_t)n};
-  return voxel_impl("pdsc_voxel_down_sample", e, 1, off, nullptr, d_points, voxel_size, d_out_points, nullptr, d_count, d_status,
-                    d_scratch, scratch_bytes, cuda_stream);
-}
-
-int pdsc_voxel_down_sample_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
-                                  double voxel_size, float* d_out_points, int32_t* d_out_offsets, int32_t* d_status, void* d_scratch,
-                                  size_t scratch_bytes, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_offsets("pdsc_voxel_down_sample_packed", "", P, h_offsets, 1)) return rc;
-  if (!d_offsets || !d_out_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_voxel_down_sample_packed: null offsets");
-  return voxel_impl("pdsc_voxel_down_sample_packed", e, P, h_offsets, d_offsets, d_points, voxel_size, d_out_points, d_out_offsets,
-                    d_out_offsets + 1, d_status, d_scratch, scratch_bytes, cuda_stream);
-}
-
-size_t pdsc_fpfh_scratch_bytes(int32_t m, int32_t max_nn) { return (m > 0 && max_nn > 0) ? pdsc::fpfh_scratch_bytes(m, max_nn) : 0; }
-
-size_t pdsc_fpfh_packed_scratch_bytes(int32_t P, const int32_t* h_offsets, int32_t max_nn) {
-  if (check_offsets("pdsc_fpfh_packed_scratch_bytes", "", P, h_offsets, 1) || max_nn <= 0) return 0;
-  return pdsc::fpfh_scratch_bytes(h_offsets[P], max_nn);
-}
-
-static int check_search_args(const char* who, pdsc_engine* e, int32_t m, double radius, int32_t max_nn, const void* a, const void* b,
-                             const void* c, void* d_scratch, size_t scratch_bytes) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (m <= 0) return fail(PDSC_ERR_SHAPE, "%s: need m >= 1 points (got %d)", who, m);
-  if (!(radius > 0.0)) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: radius must be positive (got %g)", who, radius);
-  if (max_nn < 1 || max_nn > 256) return fail(PDSC_ERR_UNSUPPORTED, "%s: max_nn %d outside [1, 256]", who, max_nn);
-  if (!a || !b || !c) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", who);
-  return check_scratch(who, "scratch", d_scratch, scratch_bytes, pdsc::fpfh_scratch_bytes(m, max_nn), 8);
-}
-
-static int search_impl(const char* who, pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets,
-                       const float* d_points, const double* d_normals, double radius, int32_t max_nn, int32_t normalise, double* d_out,
-                       int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  const int bad = check_search_args(who, e, h_offsets[P], radius, max_nn, d_points, d_out, d_status, d_scratch, scratch_bytes);
-  if (bad) return bad;
-  DeviceGuard g(e->cfg.device);
-  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  PDSC_CUDA(cudaMemsetAsync(d_status, 0, 4 * (size_t)P, st));
-  const int rc = d_normals ? pdsc::launch_compute_fpfh(P, h_offsets, d_offsets, d_points, d_normals, radius, max_nn, normalise, d_out,
-                                                       d_status, d_scratch, st)
-                           : pdsc::launch_estimate_normals(P, h_offsets, d_offsets, d_points, radius, max_nn, d_out, d_status, d_scratch,
-                                                           st);
-  if (rc) return fail(PDSC_ERR_CUDA, "%s: launch failed: %s", who, cudaGetErrorString((cudaError_t)rc));
-  return PDSC_OK;
-}
-
-int pdsc_estimate_normals(pdsc_engine* e, int32_t m, const float* d_points, double radius, int32_t max_nn, double* d_normals,
-                          int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (m <= 0) return fail(PDSC_ERR_SHAPE, "pdsc_estimate_normals: need m >= 1 points (got %d)", m);
-  const int32_t off[2] = {0, m};                      // the packed call with one cloud and no device table
-  return search_impl("pdsc_estimate_normals", e, 1, off, nullptr, d_points, nullptr, radius, max_nn, 0, d_normals, d_status, d_scratch,
-                     scratch_bytes, cuda_stream);
-}
-
-int pdsc_estimate_normals_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
-                                 double radius, int32_t max_nn, double* d_normals, int32_t* d_status, void* d_scratch,
-                                 size_t scratch_bytes, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_offsets("pdsc_estimate_normals_packed", "", P, h_offsets, 1)) return rc;
-  if (!d_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_estimate_normals_packed: null device offsets");
-  return search_impl("pdsc_estimate_normals_packed", e, P, h_offsets, d_offsets, d_points, nullptr, radius, max_nn, 0, d_normals,
-                     d_status, d_scratch, scratch_bytes, cuda_stream);
-}
-
-int pdsc_compute_fpfh(pdsc_engine* e, int32_t m, const float* d_points, const double* d_normals, double radius, int32_t max_nn,
-                      int32_t normalise, double* d_fpfh, int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (m <= 0) return fail(PDSC_ERR_SHAPE, "pdsc_compute_fpfh: need m >= 1 points (got %d)", m);
-  if (!d_normals) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_compute_fpfh: null normals");
-  const int32_t off[2] = {0, m};
-  return search_impl("pdsc_compute_fpfh", e, 1, off, nullptr, d_points, d_normals, radius, max_nn, normalise, d_fpfh, d_status,
-                     d_scratch, scratch_bytes, cuda_stream);
-}
-
-int pdsc_compute_fpfh_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
-                             const double* d_normals, double radius, int32_t max_nn, int32_t normalise, double* d_fpfh,
-                             int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_offsets("pdsc_compute_fpfh_packed", "", P, h_offsets, 1)) return rc;
-  if (!d_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_compute_fpfh_packed: null device offsets");
-  if (!d_normals) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_compute_fpfh_packed: null normals");
-  return search_impl("pdsc_compute_fpfh_packed", e, P, h_offsets, d_offsets, d_points, d_normals, radius, max_nn, normalise, d_fpfh,
-                     d_status, d_scratch, scratch_bytes, cuda_stream);
-}
-
-int pdsc_fcgf_create(int32_t conv1_kernel_size, pdsc_fcgf** out) {
-  if (!out) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_fcgf_create: null handle pointer");
-  *out = nullptr;
-  if (conv1_kernel_size != 5 && conv1_kernel_size != 7)
-    return fail(PDSC_ERR_UNSUPPORTED, "pdsc_fcgf_create: conv1_kernel_size must be 5 or 7 (got %d)", conv1_kernel_size);
-  *out = pdsc::fcgf_new(conv1_kernel_size);
-  return PDSC_OK;
-}
-
-int pdsc_fcgf_destroy(pdsc_fcgf* h) {
-  pdsc::fcgf_free(h);
-  return PDSC_OK;
-}
-
-int pdsc_fcgf_set_param(pdsc_fcgf* h, const char* name, const float* h_data, int64_t numel) {
-  if (!h || !name || (!h_data && numel > 0) || numel < 0) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_fcgf_set_param: bad argument");
-  size_t expected = 0;
-  const int rc = pdsc::fcgf_set_param(h, name, h_data, numel, &expected);
-  if (rc == 1) return fail(PDSC_ERR_UNKNOWN_PARAM, "pdsc_fcgf_set_param: unknown parameter '%s'", name);
-  if (rc == 2)
-    return fail(PDSC_ERR_SHAPE, "pdsc_fcgf_set_param: '%s' has %lld elements, expected %zu", name, (long long)numel, expected);
-  return PDSC_OK;
-}
-
-int pdsc_fcgf_commit(pdsc_fcgf* h) {
-  if (!h) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_fcgf_commit: null handle");
-  std::string missing;
-  const int rc = pdsc::fcgf_commit(h, &missing);
-  if (rc < 0) return fail(PDSC_ERR_UNKNOWN_PARAM, "pdsc_fcgf_commit: state-dict entry missing: %s", missing.c_str());
-  if (rc > 0) return fail(PDSC_ERR_CUDA, "pdsc_fcgf_commit: upload failed: %s", cudaGetErrorString((cudaError_t)rc));
-  return PDSC_OK;
-}
-
-// the points of a call bound every level's rows and every int32 table index: at most 2^26 in all
-static constexpr int32_t kFcgfMaxPoints = 1 << 26;
-
-size_t pdsc_fcgf_packed_scratch_bytes(const pdsc_fcgf* h, int32_t P, const int32_t* h_offsets) {
-  if (!h || check_offsets("pdsc_fcgf_packed_scratch_bytes", "", P, h_offsets, 1) || h_offsets[P] > kFcgfMaxPoints) return 0;
-  return pdsc::fcgf_scratch_bytes(P, h_offsets, pdsc::fcgf_kernel_size(h));
-}
-
-int32_t pdsc_fcgf_scratch_layout(const pdsc_fcgf* h, int32_t P, const int32_t* h_offsets, int64_t* offsets, int32_t capacity) {
-  if (!h || check_offsets("pdsc_fcgf_scratch_layout", "", P, h_offsets, 1) || h_offsets[P] > kFcgfMaxPoints) return 0;
-  return pdsc::fcgf_scratch_layout(P, h_offsets, pdsc::fcgf_kernel_size(h), offsets, offsets ? capacity : 0);
-}
-
-int pdsc_fcgf_packed(pdsc_engine* e, const pdsc_fcgf* h, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets,
-                     const float* d_points, double voxel_size, float* d_keypts, float* d_desc, int32_t* d_out_offsets,
-                     int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  const char* fn = "pdsc_fcgf_packed";
-  if (!e || !h) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null engine or weight handle", fn);
-  if (!pdsc::fcgf_committed(h)) return fail(PDSC_ERR_NOT_COMMITTED, "%s: pdsc_fcgf_commit() has not been called since the last "
-                                            "pdsc_fcgf_set_param()", fn);
-  if (int rc = check_offsets(fn, "", P, h_offsets, 1)) return rc;
-  if (h_offsets[P] > kFcgfMaxPoints) return fail(PDSC_ERR_SHAPE, "%s: need at most 2^26 points (got %d)", fn, h_offsets[P]);
-  if (!(voxel_size > 0.0) || !std::isfinite(voxel_size))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: voxel_size must be positive and finite (got %g)", fn, voxel_size);
-  if (!d_offsets || !d_points || !d_keypts || !d_desc || !d_out_offsets || !d_status)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
-  const int k1 = pdsc::fcgf_kernel_size(h);
-  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::fcgf_scratch_bytes(P, h_offsets, k1), 256)) return rc;
-  DeviceGuard g(e->cfg.device);
-  const int rc = pdsc::launch_fcgf(h, P, h_offsets, d_offsets, d_points, voxel_size, d_keypts, d_desc, d_out_offsets, d_status,
-                                   d_scratch, static_cast<cudaStream_t>(cuda_stream));
-  if (rc) return fail(PDSC_ERR_CUDA, "%s: launch failed: %s", fn, cudaGetErrorString((cudaError_t)rc));
-  return PDSC_OK;
-}
-
-size_t pdsc_icp_packed_scratch_bytes(int32_t B, const int32_t* h_offsets) {
-  return pdsc_icp_clouds_packed_scratch_bytes(B, h_offsets, h_offsets);
-}
-
-size_t pdsc_icp_clouds_packed_scratch_bytes(int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets) {
-  const char* who = "pdsc_icp_clouds_packed_scratch_bytes";
-  if (check_offsets(who, "source ", B, h_src_offsets, 1) || check_offsets(who, "target ", B, h_tgt_offsets, 1)) return 0;
-  return pdsc::icp_scratch_bytes(h_src_offsets[B], h_tgt_offsets[B]);
-}
-
-// pdsc_icp_packed and pdsc_icp_clouds_packed: one set of checks and one launch, under the caller's name
-static int icp_clouds(const char* fn, pdsc_engine* e, int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
-                      const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const float* d_src, const float* d_tgt,
-                      const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans, double* d_fitness,
-                      double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
-                      void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  const bool one = h_src_offsets == h_tgt_offsets;     // pdsc_icp_packed: one offsets array for both sides
-  if (int rc = check_offsets(fn, one ? "" : "source ", B, h_src_offsets, 1)) return rc;
-  if (!one)
-    if (int rc = check_offsets(fn, "target ", B, h_tgt_offsets, 1)) return rc;
-  if (!d_src_offsets || !d_tgt_offsets || !d_src || !d_tgt || !d_init || !d_trans)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
-  if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_corr_dist must be positive and finite (got %g)", fn, max_corr_dist);
-  if (max_iteration < 1) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_iteration must be >= 1 (got %d)", fn, max_iteration);
-  const long long Rs = h_src_offsets[B], Rt = h_tgt_offsets[B];
-  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::icp_scratch_bytes(Rs, Rt), 8)) return rc;
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_icp(B, d_src_offsets, d_tgt_offsets, Rs, Rt, d_src, d_tgt, d_init, max_corr_dist, max_iteration, d_trans, d_fitness,
-                   d_rmse, d_iterations, d_status, d_scratch, static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
-}
-
-int pdsc_icp_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
-                    const float* d_tgt, const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans,
-                    double* d_fitness, double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
-                    void* cuda_stream) {
-  return icp_clouds("pdsc_icp_packed", e, B, h_offsets, h_offsets, d_offsets, d_offsets, d_src, d_tgt, d_init, max_corr_dist,
-                    max_iteration, d_trans, d_fitness, d_rmse, d_iterations, d_status, d_scratch, scratch_bytes, cuda_stream);
-}
-
-int pdsc_icp_clouds_packed(pdsc_engine* e, int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
-                           const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const float* d_src, const float* d_tgt,
-                           const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans, double* d_fitness,
-                           double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
-                           void* cuda_stream) {
-  return icp_clouds("pdsc_icp_clouds_packed", e, B, h_src_offsets, h_tgt_offsets, d_src_offsets, d_tgt_offsets, d_src, d_tgt,
-                    d_init, max_corr_dist, max_iteration, d_trans, d_fitness, d_rmse, d_iterations, d_status, d_scratch,
-                    scratch_bytes, cuda_stream);
-}
-
-size_t pdsc_information_matrix_packed_scratch_bytes(int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets) {
-  const char* who = "pdsc_information_matrix_packed_scratch_bytes";
-  if (check_offsets(who, "source ", B, h_src_offsets, 1) || check_offsets(who, "target ", B, h_tgt_offsets, 1)) return 0;
-  return pdsc::information_scratch_bytes(h_tgt_offsets[B]);
-}
-
-int pdsc_information_matrix_packed(pdsc_engine* e, int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
-                                   const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const float* d_src, const float* d_tgt,
-                                   const float* d_trans, double max_corr_dist, double* d_info, int32_t* d_status, void* d_scratch,
-                                   size_t scratch_bytes, void* cuda_stream) {
-  const char* fn = "pdsc_information_matrix_packed";
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_offsets(fn, "source ", B, h_src_offsets, 1)) return rc;
-  if (int rc = check_offsets(fn, "target ", B, h_tgt_offsets, 1)) return rc;
-  if (!d_src_offsets || !d_tgt_offsets || !d_src || !d_tgt || !d_trans || !d_info)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
-  if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_corr_dist must be positive and finite (got %g)", fn, max_corr_dist);
-  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::information_scratch_bytes(h_tgt_offsets[B]), 8)) return rc;
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_information(B, d_src_offsets, d_tgt_offsets, h_tgt_offsets[B], d_src, d_tgt, d_trans, max_corr_dist, d_info, d_status,
-                           d_scratch, static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
-}
-
-namespace {
-constexpr int kTsdfMaxUnits = 1 << 22;
-
-// the frame offsets, image and volume parameters every TSDF stage of a call checks alike
-pdsc_status check_tsdf(const char* fn, int32_t F, const int32_t* h_frame_offsets, int32_t height, int32_t width,
-                       const double* intrinsic, double voxel_length, double sdf_trunc, int32_t max_units) {
-  if (pdsc_status rc = check_offsets(fn, "frame ", F, h_frame_offsets, 1, pdsc::kMaxFragmentFrames)) return rc;
-  if (h_frame_offsets[F] > 65535) return fail(PDSC_ERR_SHAPE, "%s: at most 65535 frames per call (got %d)", fn, h_frame_offsets[F]);
-  if (height < 1 || width < 1 || (long long)height * width > (1 << 26))
-    return fail(PDSC_ERR_SHAPE, "%s: image %d x %d outside 1 .. 2^26 pixels", fn, width, height);
-  if (!intrinsic) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null intrinsic", fn);
-  for (int i = 0; i < 4; ++i)
-    if (!std::isfinite(intrinsic[i]) || (i < 2 && !(intrinsic[i] > 0.0)))
-      return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: intrinsic %d (%g) must be finite, and the focal lengths positive", fn, i, intrinsic[i]);
-  if (!(voxel_length > 0.0) || !std::isfinite(voxel_length) || !(sdf_trunc > 0.0) || !std::isfinite(sdf_trunc))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: voxel_length (%g) and sdf_trunc (%g) must be positive and finite", fn, voxel_length,
-                sdf_trunc);
-  if (max_units < 1 || max_units > kTsdfMaxUnits)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_units %d outside [1, %d]", fn, max_units, kTsdfMaxUnits);
-  return PDSC_OK;
-}
-
-pdsc_status check_units(const char* fn, int32_t F, const int32_t* h_unit_offsets, int32_t max_units, const void* d_table,
-                        size_t table_bytes) {
-  if (max_units < 1 || max_units > kTsdfMaxUnits)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_units %d outside [1, %d]", fn, max_units, kTsdfMaxUnits);
-  if (pdsc_status rc = check_offsets(fn, "unit ", F, h_unit_offsets, 0, max_units)) return rc;
-  return check_scratch(fn, "table", d_table, table_bytes, pdsc::tsdf_table_bytes(F, max_units), 8);
-}
-}  // namespace
-
-size_t pdsc_tsdf_table_bytes(int32_t F, int32_t max_units) {
-  if (F < 1 || max_units < 1 || max_units > kTsdfMaxUnits) return 0;
-  return pdsc::tsdf_table_bytes(F, max_units);
-}
-
-int pdsc_tsdf_touch_packed(pdsc_engine* e, int32_t F, const int32_t* h_frame_offsets, const int32_t* d_frame_offsets, int32_t height,
-                           int32_t width, const double* intrinsic, const uint16_t* d_depth, const double* d_poses, double depth_scale,
-                           double depth_trunc, double voxel_length, double sdf_trunc, int32_t max_units, int32_t* d_unit_counts,
-                           int32_t* d_status, void* d_table, size_t table_bytes, void* cuda_stream) {
-  const char* fn = "pdsc_tsdf_touch_packed";
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_tsdf(fn, F, h_frame_offsets, height, width, intrinsic, voxel_length, sdf_trunc, max_units)) return rc;
-  if (!(depth_scale > 0.0) || !std::isfinite(depth_scale))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: depth_scale must be positive and finite (got %g)", fn, depth_scale);
-  if (!d_frame_offsets || !d_depth || !d_poses || !d_unit_counts || !d_status)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
-  if (int rc = check_scratch(fn, "table", d_table, table_bytes, pdsc::tsdf_table_bytes(F, max_units), 8)) return rc;
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_tsdf_touch(F, h_frame_offsets[F], d_frame_offsets, height, width, intrinsic, d_depth, d_poses, depth_scale, depth_trunc,
-                          voxel_length, sdf_trunc, max_units, d_unit_counts, d_status, d_table, static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
-}
-
-size_t pdsc_tsdf_integrate_scratch_bytes(int32_t F, const int32_t* h_unit_offsets) {
-  if (check_offsets("pdsc_tsdf_integrate_scratch_bytes", "unit ", F, h_unit_offsets, 0, kTsdfMaxUnits)) return 0;
-  return pdsc::tsdf_integrate_scratch_bytes(F, h_unit_offsets[F]);
-}
-
-int pdsc_tsdf_integrate_packed(pdsc_engine* e, int32_t F, const int32_t* h_frame_offsets, const int32_t* d_frame_offsets,
-                               const int32_t* h_unit_offsets, const int32_t* d_unit_offsets, int32_t height, int32_t width,
-                               const double* intrinsic, const uint16_t* d_depth, const uint8_t* d_color, const double* d_poses,
-                               double depth_scale, double depth_trunc, double voxel_length, double sdf_trunc, int32_t max_units,
-                               void* d_table, size_t table_bytes, int32_t* d_unit_keys, float* d_tsdf, float* d_weight,
-                               float* d_voxel_color, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  const char* fn = "pdsc_tsdf_integrate_packed";
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_tsdf(fn, F, h_frame_offsets, height, width, intrinsic, voxel_length, sdf_trunc, max_units)) return rc;
-  if (int rc = check_units(fn, F, h_unit_offsets, max_units, d_table, table_bytes)) return rc;
-  if (!(depth_scale > 0.0) || !std::isfinite(depth_scale))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: depth_scale must be positive and finite (got %g)", fn, depth_scale);
-  const long long U = h_unit_offsets[F];
-  if (!d_frame_offsets || !d_unit_offsets || !d_depth || !d_color || !d_poses || (U > 0 && (!d_unit_keys || !d_tsdf || !d_weight ||
-                                                                                             !d_voxel_color)))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
-  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::tsdf_integrate_scratch_bytes(F, U), 8)) return rc;
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_tsdf_integrate(F, d_frame_offsets, d_unit_offsets, U, height, width, intrinsic, d_depth, d_color, d_poses, depth_scale,
-                              depth_trunc, voxel_length, sdf_trunc, max_units, d_table, d_unit_keys, d_tsdf, d_weight, d_voxel_color,
-                              d_scratch, static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
-}
-
-int pdsc_extract_vertices_count_packed(pdsc_engine* e, int32_t F, const int32_t* h_unit_offsets, const int32_t* d_unit_offsets,
-                                       int32_t max_units, void* d_table, size_t table_bytes, const int32_t* d_unit_keys,
-                                       const float* d_tsdf, const float* d_weight, int64_t* d_vertex_ends, int64_t* d_vertex_offsets,
-                                       void* cuda_stream) {
-  const char* fn = "pdsc_extract_vertices_count_packed";
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_units(fn, F, h_unit_offsets, max_units, d_table, table_bytes)) return rc;
-  const int U = h_unit_offsets[F];
-  if (!d_unit_offsets || !d_vertex_offsets || (U > 0 && (!d_unit_keys || !d_tsdf || !d_weight || !d_vertex_ends)))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_vertex_count(F, d_unit_offsets, U, max_units, d_table, d_unit_keys, d_tsdf, d_weight,
-                            reinterpret_cast<long long*>(d_vertex_ends), reinterpret_cast<long long*>(d_vertex_offsets),
-                            static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
-}
-
-int pdsc_extract_vertices_packed(pdsc_engine* e, int32_t F, const int32_t* h_unit_offsets, const int32_t* d_unit_offsets,
-                                 int32_t max_units, void* d_table, size_t table_bytes, const int32_t* d_unit_keys, const float* d_tsdf,
-                                 const float* d_weight, const float* d_voxel_color, double voxel_length, const int64_t* d_vertex_ends,
-                                 double* d_vertices, double* d_vertex_colors, void* cuda_stream) {
-  const char* fn = "pdsc_extract_vertices_packed";
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_units(fn, F, h_unit_offsets, max_units, d_table, table_bytes)) return rc;
-  if (!(voxel_length > 0.0) || !std::isfinite(voxel_length))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: voxel_length must be positive and finite (got %g)", fn, voxel_length);
-  const int U = h_unit_offsets[F];
-  if (!d_unit_offsets || (U > 0 && (!d_unit_keys || !d_tsdf || !d_weight || !d_voxel_color || !d_vertex_ends)))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_vertex_write(F, d_unit_offsets, U, max_units, d_table, d_unit_keys, d_tsdf, d_weight, d_voxel_color, voxel_length,
-                            reinterpret_cast<const long long*>(d_vertex_ends), d_vertices, d_vertex_colors,
-                            static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
-}
-
-size_t pdsc_ransac_packed_scratch_bytes(int32_t B, const int32_t* h_offsets, int32_t max_iteration) {
-  if (check_offsets("pdsc_ransac_packed_scratch_bytes", "", B, h_offsets, 1)) return 0;
-  if (max_iteration < 1) {
-    fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_ransac_packed_scratch_bytes: max_iteration must be >= 1 (got %d)", max_iteration);
-    return 0;
-  }
-  return pdsc::ransac_scratch_bytes(h_offsets[B], B, max_iteration);
-}
-
-// pdsc_ransac_packed and pdsc_ransac_packed_hypotheses: one set of checks and one launch, under the caller's name
-static int ransac_packed(const char* fn, pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
-                         const float* d_src, const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration,
-                         uint64_t seed, float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse, int32_t* d_best,
-                         int32_t* d_status, int32_t* d_hyp_good, double* d_hyp_rmse, double* d_hyp_trans, void* d_scratch,
-                         size_t scratch_bytes, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_offsets(fn, "", B, h_offsets, 1)) return rc;
-  if (B > 65535) return fail(PDSC_ERR_UNSUPPORTED, "%s: at most 65535 sets per call (got %d)", fn, B);
-  if (!d_offsets || !d_src || !d_tgt || !d_labels || !d_trans || !d_out_labels)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
-  if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_corr_dist must be positive and finite (got %g)", fn, max_corr_dist);
-  if (max_iteration < 1)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_iteration must be >= 1 (got %d)", fn, max_iteration);
-  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::ransac_scratch_bytes(h_offsets[B], B, max_iteration), 16))
-    return rc;
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_ransac(B, d_offsets, h_offsets[B], d_src, d_tgt, d_labels, max_corr_dist, max_iteration, (unsigned long long)seed,
-                      d_trans, d_out_labels, d_fitness, d_rmse, d_best, d_status, d_hyp_good, d_hyp_rmse, d_hyp_trans, d_scratch,
-                      static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
-}
-
-int pdsc_ransac_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
-                       const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration, uint64_t seed,
-                       float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse, int32_t* d_best, int32_t* d_status,
-                       int32_t* d_hyp_good, double* d_hyp_rmse, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  return ransac_packed("pdsc_ransac_packed", e, B, h_offsets, d_offsets, d_src, d_tgt, d_labels, max_corr_dist, max_iteration, seed,
-                       d_trans, d_out_labels, d_fitness, d_rmse, d_best, d_status, d_hyp_good, d_hyp_rmse, nullptr, d_scratch,
-                       scratch_bytes, cuda_stream);
-}
-
-int pdsc_ransac_packed_hypotheses(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
-                                  const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration,
-                                  uint64_t seed, float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse,
-                                  int32_t* d_best, int32_t* d_status, int32_t* d_hyp_good, double* d_hyp_rmse, double* d_hyp_trans,
-                                  void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  return ransac_packed("pdsc_ransac_packed_hypotheses", e, B, h_offsets, d_offsets, d_src, d_tgt, d_labels, max_corr_dist,
-                       max_iteration, seed, d_trans, d_out_labels, d_fitness, d_rmse, d_best, d_status, d_hyp_good, d_hyp_rmse,
-                       d_hyp_trans, d_scratch, scratch_bytes, cuda_stream);
-}
-
-size_t pdsc_spectral_matching_packed_scratch_bytes(int32_t B, const int32_t* h_offsets) {
-  if (check_offsets("pdsc_spectral_matching_packed_scratch_bytes", "", B, h_offsets, 1, pdsc::spectral_matching_max_n())) return 0;
-  return pdsc::sm_scratch_bytes(h_offsets[B], B);
-}
-
-// pdsc_spectral_matching_packed and pdsc_spectral_matching_packed_iterates: one set of checks and one launch, under the caller's name
-static int spectral_matching_packed(const char* fn, pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
-                                    const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts,
-                                    double inlier_threshold, float* d_trans, float* d_labels, float* d_eigenvector, float* d_iterates,
-                                    void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_offsets(fn, "", B, h_offsets, 1, pdsc::spectral_matching_max_n())) return rc;
-  if (B > 65535) return fail(PDSC_ERR_UNSUPPORTED, "%s: at most 65535 sets per call (got %d)", fn, B);
-  if (!d_offsets || !d_corr_pos || !d_src_keypts || !d_tgt_keypts || !d_trans || !d_labels)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
-  if (!(inlier_threshold > 0.0) || !std::isfinite(inlier_threshold))
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: inlier_threshold must be positive and finite (got %g)", fn, inlier_threshold);
-  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, pdsc::sm_scratch_bytes(h_offsets[B], B), 16)) return rc;
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_spectral_matching(B, h_offsets, d_offsets, d_corr_pos, d_src_keypts, d_tgt_keypts, inlier_threshold, d_trans, d_labels,
-                                 d_eigenvector, d_iterates, d_scratch, static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
-}
-
-int pdsc_spectral_matching_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
-                                  const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts, double inlier_threshold,
-                                  float* d_trans, float* d_labels, float* d_eigenvector, void* d_scratch, size_t scratch_bytes,
-                                  void* cuda_stream) {
-  return spectral_matching_packed("pdsc_spectral_matching_packed", e, B, h_offsets, d_offsets, d_corr_pos, d_src_keypts, d_tgt_keypts,
-                                  inlier_threshold, d_trans, d_labels, d_eigenvector, nullptr, d_scratch, scratch_bytes, cuda_stream);
-}
-
-int pdsc_spectral_matching_packed_iterates(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
-                                           const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts,
-                                           double inlier_threshold, float* d_trans, float* d_labels, float* d_eigenvector,
-                                           float* d_iterates, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  return spectral_matching_packed("pdsc_spectral_matching_packed_iterates", e, B, h_offsets, d_offsets, d_corr_pos, d_src_keypts,
-                                  d_tgt_keypts, inlier_threshold, d_trans, d_labels, d_eigenvector, d_iterates, d_scratch, scratch_bytes,
-                                  cuda_stream);
-}
-
-// Host-side PLY vertex reader (ascii / binary_little_endian; x, y, z as float or double; other vertex properties skipped).
-int pdsc_read_ply(const char* path, float* points, int64_t capacity, int64_t* n_vertices) {
-  if (!path || !n_vertices) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_read_ply: null argument");
-  FILE* f = fopen(path, "rb");
-  if (!f) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_read_ply: cannot open %s", path);
-  struct Closer { FILE* f; ~Closer() { fclose(f); } } closer{f};
-  char line[512];
-  if (!fgets(line, sizeof line, f) || strncmp(line, "ply", 3) != 0) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s is not a PLY file", path);
-  int format = -1;                    // 0 ascii, 1 binary little endian
-  long long n = -1;
-  bool in_vertex = false, vertex_first = true, seen_element = false;
-  struct Prop { int size; bool is_float; int axis; };
-  std::vector<Prop> props;
-  while (true) {
-    if (!fgets(line, sizeof line, f)) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: header ends before end_header", path);
-    char a[64] = {0}, b[64] = {0}, c[64] = {0};
-    const int got = sscanf(line, "%63s %63s %63s", a, b, c);
-    if (got < 1) continue;
-    if (!strcmp(a, "end_header")) break;
-    if (!strcmp(a, "format")) {
-      if (!strcmp(b, "ascii")) format = 0;
-      else if (!strcmp(b, "binary_little_endian")) format = 1;
-      else return fail(PDSC_ERR_UNSUPPORTED, "%s: PLY format %s is not supported", path, b);
-    } else if (!strcmp(a, "element")) {
-      in_vertex = !strcmp(b, "vertex");
-      if (in_vertex) { n = atoll(c); vertex_first = !seen_element; }
-      seen_element = true;
-    } else if (!strcmp(a, "property") && in_vertex) {
-      if (!strcmp(b, "list")) return fail(PDSC_ERR_UNSUPPORTED, "%s: list properties on vertices are not supported", path);
-      Prop p{0, false, -1};
-      if (!strcmp(b, "char") || !strcmp(b, "uchar") || !strcmp(b, "int8") || !strcmp(b, "uint8")) p.size = 1;
-      else if (!strcmp(b, "short") || !strcmp(b, "ushort") || !strcmp(b, "int16") || !strcmp(b, "uint16")) p.size = 2;
-      else if (!strcmp(b, "int") || !strcmp(b, "uint") || !strcmp(b, "int32") || !strcmp(b, "uint32")) p.size = 4;
-      else if (!strcmp(b, "float") || !strcmp(b, "float32")) { p.size = 4; p.is_float = true; }
-      else if (!strcmp(b, "double") || !strcmp(b, "float64")) { p.size = 8; p.is_float = true; }
-      else return fail(PDSC_ERR_UNSUPPORTED, "%s: unknown property type %s", path, b);
-      if (!strcmp(c, "x")) p.axis = 0; else if (!strcmp(c, "y")) p.axis = 1; else if (!strcmp(c, "z")) p.axis = 2;
-      if (p.axis >= 0 && !p.is_float) return fail(PDSC_ERR_UNSUPPORTED, "%s: integer coordinates are not supported", path);
-      props.push_back(p);
-    }
-  }
-  if (format < 0 || n < 0) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: no format / vertex element in the header", path);
-  if (!vertex_first) return fail(PDSC_ERR_UNSUPPORTED, "%s: the vertex element must come first", path);
-  int have = 0;
-  for (const Prop& p : props) if (p.axis >= 0) have |= 1 << p.axis;
-  if (have != 7) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: vertex properties x, y, z not all present", path);
-  *n_vertices = n;
-  if (!points) return PDSC_OK;                        // size query
-  if (capacity < n) return fail(PDSC_ERR_SHAPE, "pdsc_read_ply: buffer holds %lld vertices, the file has %lld", (long long)capacity, n);
-  if (format == 0) {
-    for (long long i = 0; i < n; ++i) {
-      for (const Prop& p : props) {
-        double v;
-        if (fscanf(f, "%lf", &v) != 1) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: truncated at vertex %lld", path, i);
-        if (p.axis >= 0) points[3 * i + p.axis] = (float)v;
-      }
-    }
-  } else {
-    size_t stride = 0;
-    for (const Prop& p : props) stride += (size_t)p.size;
-    std::vector<unsigned char> row(stride * 4096);
-    for (long long i0 = 0; i0 < n; i0 += 4096) {
-      const size_t rows = (size_t)std::min<long long>(4096, n - i0);
-      if (fread(row.data(), stride, rows, f) != rows) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: truncated at vertex %lld", path, i0);
-      for (size_t r = 0; r < rows; ++r) {
-        size_t off = r * stride;
-        for (const Prop& p : props) {
-          if (p.axis >= 0) {
-            if (p.size == 4) { float v; memcpy(&v, &row[off], 4); points[3 * (i0 + (long long)r) + p.axis] = v; }
-            else { double v; memcpy(&v, &row[off], 8); points[3 * (i0 + (long long)r) + p.axis] = (float)v; }
-          }
-          off += (size_t)p.size;
-        }
-      }
-    }
-  }
-  return PDSC_OK;
-}
-
-size_t pdsc_match_scratch_bytes(int32_t Ns, int32_t Nt) {
-  return (Ns > 0 && Nt > 0) ? pdsc::match_scratch_bytes(Ns, Nt) : 0;
-}
-
-size_t pdsc_match_packed_scratch_bytes(int32_t P, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets) {
-  const char* who = "pdsc_match_packed_scratch_bytes";
-  if (check_offsets(who, "source ", P, h_src_offsets, 1) || check_offsets(who, "target ", P, h_tgt_offsets, 1)) return 0;
-  return pdsc::match_scratch_bytes(h_src_offsets[P], h_tgt_offsets[P]);
-}
-
-static int match_impl(pdsc_engine* e, int32_t P, int32_t D, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
-                      const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const void* d_src_desc, const void* d_tgt_desc,
-                      int32_t desc_is_fp64, const float* d_src_keypts, const float* d_tgt_keypts, int32_t use_mutual,
-                      int32_t* d_corr, int32_t* d_out_first, int32_t* d_out_ends, float* d_corr_pos, float* d_out_src,
-                      float* d_out_tgt, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  if (D < 1 || D > pdsc::match_max_dim()) return fail(PDSC_ERR_UNSUPPORTED, "descriptor dimension %d outside [1, %d]", D, pdsc::match_max_dim());
-  if (e->cfg.in_dim != 6) return fail(PDSC_ERR_UNSUPPORTED, "pdsc_match builds the in_dim = 6 input (engine has in_dim = %d)", e->cfg.in_dim);
-  if (!d_src_desc || !d_tgt_desc || !d_src_keypts || !d_tgt_keypts || !d_corr || !d_out_ends || !d_corr_pos || !d_out_src || !d_out_tgt)
-    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_match: null tensor pointer");
-  if (int rc = check_scratch("pdsc_match", "scratch", d_scratch, scratch_bytes,
-                             pdsc::match_scratch_bytes(h_src_offsets[P], h_tgt_offsets[P]), 8))
-    return rc;
-  DeviceGuard g(e->cfg.device);
-  pdsc::launch_match(P, h_src_offsets, h_tgt_offsets, d_src_offsets, d_tgt_offsets, d_src_desc, d_tgt_desc, desc_is_fp64,
-                     d_src_keypts, d_tgt_keypts, D, use_mutual, d_scratch, d_corr, d_out_first, d_out_ends, d_corr_pos, d_out_src,
-                     d_out_tgt, static_cast<cudaStream_t>(cuda_stream));
-  PDSC_CUDA(cudaGetLastError());
-  return PDSC_OK;
-}
-
-int pdsc_match(pdsc_engine* e, int32_t Ns, int32_t Nt, int32_t D, const void* d_src_desc, const void* d_tgt_desc,
-               int32_t desc_is_fp64, const float* d_src_keypts, const float* d_tgt_keypts, int32_t use_mutual,
-               int32_t* d_corr, int32_t* d_count, float* d_corr_pos, float* d_out_src, float* d_out_tgt, void* d_scratch,
-               size_t scratch_bytes, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (Ns <= 0 || Nt <= 0) return fail(PDSC_ERR_SHAPE, "need Ns >= 1 and Nt >= 1 (got %d, %d)", Ns, Nt);
-  // the packed call with one pair: its offsets need no device table, and its end row is the count
-  const int32_t src_off[2] = {0, Ns}, tgt_off[2] = {0, Nt};
-  return match_impl(e, 1, D, src_off, tgt_off, nullptr, nullptr, d_src_desc, d_tgt_desc, desc_is_fp64, d_src_keypts, d_tgt_keypts,
-                    use_mutual, d_corr, nullptr, d_count, d_corr_pos, d_out_src, d_out_tgt, d_scratch, scratch_bytes, cuda_stream);
-}
-
-int pdsc_match_packed(pdsc_engine* e, int32_t P, int32_t D, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
-                      const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const void* d_src_desc, const void* d_tgt_desc,
-                      int32_t desc_is_fp64, const float* d_src_keypts, const float* d_tgt_keypts, int32_t use_mutual,
-                      int32_t* d_corr, int32_t* d_out_offsets, float* d_corr_pos, float* d_out_src, float* d_out_tgt,
-                      void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
-  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
-  if (int rc = check_offsets("pdsc_match_packed", "source ", P, h_src_offsets, 1)) return rc;
-  if (int rc = check_offsets("pdsc_match_packed", "target ", P, h_tgt_offsets, 1)) return rc;
-  if (!d_src_offsets || !d_tgt_offsets || !d_out_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_match_packed: null offsets");
-  return match_impl(e, P, D, h_src_offsets, h_tgt_offsets, d_src_offsets, d_tgt_offsets, d_src_desc, d_tgt_desc, desc_is_fp64,
-                    d_src_keypts, d_tgt_keypts, use_mutual, d_corr, d_out_offsets, d_out_offsets + 1, d_corr_pos, d_out_src,
-                    d_out_tgt, d_scratch, scratch_bytes, cuda_stream);
 }
 
 int pdsc_profile_enable(pdsc_engine* e, int32_t enable) {

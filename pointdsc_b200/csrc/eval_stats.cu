@@ -13,8 +13,8 @@
 // Counts are exact integers (fp32 holds them below 2^24); sums of distances are accumulated in fp64.
 #include <cmath>
 
+#include "abi.h"
 #include "common.cuh"
-#include "kernels.h"
 #include "sets.cuh"
 
 namespace pdsc {
@@ -91,12 +91,45 @@ __global__ void __launch_bounds__(kStatsThreads) eval_stats_kernel(const float* 
   }
 }
 
-void launch_eval_stats(const float* pred_trans, const float* gt_trans, const float* src, const float* tgt,
-                       const float* pred_labels, const float* gt_labels, float* stats, int B, const int32_t* d_offsets, int N,
-                       float re_thre, float te_thre, cudaStream_t st) {
-  if (B <= 0) return;
-  eval_stats_kernel<<<B, kStatsThreads, 0, st>>>(pred_trans, gt_trans, src, tgt, pred_labels, gt_labels, stats,
-                                                 Offsets{d_offsets, d_offsets ? 0 : N}, re_thre, te_thre);
+// set b: rows [offsets[b], offsets[b+1]), or b * N without a table
+static int eval_stats_impl(pdsc_engine* e, int32_t B, const int32_t* d_offsets, int32_t N, const float* d_pred_trans,
+                           const float* d_gt_trans, const float* d_src, const float* d_tgt, const float* d_pred_labels,
+                           const float* d_gt_labels, float re_thre, float te_thre, float* d_stats, void* cuda_stream) {
+  if (!d_pred_trans || !d_gt_trans || !d_src || !d_tgt || !d_pred_labels || !d_gt_labels || !d_stats)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_eval_stats: null tensor pointer");
+  DeviceGuard g(engine_config(e).device);
+  eval_stats_kernel<<<B, kStatsThreads, 0, static_cast<cudaStream_t>(cuda_stream)>>>(
+      d_pred_trans, d_gt_trans, d_src, d_tgt, d_pred_labels, d_gt_labels, d_stats, Offsets{d_offsets, d_offsets ? 0 : N}, re_thre,
+      te_thre);
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
 }
 
 }  // namespace pdsc
+
+// ---- C ABI ------------------------------------------------------------------------------------------------------
+using namespace pdsc;
+
+extern "C" {
+
+int pdsc_eval_stats(pdsc_engine* e, int32_t B, int32_t N, const float* d_pred_trans, const float* d_gt_trans,
+                    const float* d_src, const float* d_tgt, const float* d_pred_labels, const float* d_gt_labels,
+                    float re_thre, float te_thre, float* d_stats, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (B <= 0 || N <= 0) return fail(PDSC_ERR_SHAPE, "need B >= 1 and N >= 1 (got B=%d N=%d)", B, N);
+  return eval_stats_impl(e, B, nullptr, N, d_pred_trans, d_gt_trans, d_src, d_tgt, d_pred_labels, d_gt_labels, re_thre, te_thre,
+                         d_stats, cuda_stream);
+}
+
+int pdsc_eval_stats_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                           const float* d_pred_trans, const float* d_gt_trans, const float* d_src, const float* d_tgt,
+                           const float* d_pred_labels, const float* d_gt_labels, float re_thre, float te_thre, float* d_stats,
+                           void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_offsets("pdsc_eval_stats_packed", "", B, h_offsets, 1)) return rc;
+  if (!d_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_eval_stats_packed: null device offsets");
+  return eval_stats_impl(e, B, d_offsets, 0, d_pred_trans, d_gt_trans, d_src, d_tgt, d_pred_labels, d_gt_labels, re_thre, te_thre,
+                         d_stats, cuda_stream);
+}
+
+}  // extern "C"

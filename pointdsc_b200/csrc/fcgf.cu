@@ -33,6 +33,7 @@
 #include <vector>
 
 #include "../../include/pointdsc_b200.h"
+#include "abi.h"
 #include "common.cuh"
 #include "kernels.h"
 #include "voxel_hash.cuh"
@@ -43,6 +44,8 @@ namespace {
 
 constexpr int kLevels = 4;
 constexpr int kCoordLimit = 1 << 20;     // |voxel coordinate| bound: 21-bit fields with a 2^20 bias
+// the points of a call bound every level's rows and every int32 table index: at most 2^26 in all
+constexpr int32_t kFcgfMaxPoints = 1 << 26;
 constexpr int kScanBlock = 1024;         // items per block of the representative scan
 constexpr double kBnEps = 1e-5;
 
@@ -448,35 +451,51 @@ static std::vector<ParamSpec> fcgf_param_specs(int k1) {
   return v;
 }
 
-pdsc_fcgf* fcgf_new(int k1) {
-  pdsc_fcgf* h = new pdsc_fcgf();
-  h->k1 = k1;
-  return h;
+static size_t fcgf_scratch_bytes(int P, const int32_t* h_off, int k1) { return carve(nullptr, P, h_off, k1).bytes; }
+
+}  // namespace pdsc
+
+// ---- C ABI ------------------------------------------------------------------------------------------------------
+using namespace pdsc;
+
+extern "C" {
+
+int pdsc_fcgf_create(int32_t conv1_kernel_size, pdsc_fcgf** out) {
+  if (!out) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_fcgf_create: null handle pointer");
+  *out = nullptr;
+  if (conv1_kernel_size != 5 && conv1_kernel_size != 7)
+    return fail(PDSC_ERR_UNSUPPORTED, "pdsc_fcgf_create: conv1_kernel_size must be 5 or 7 (got %d)", conv1_kernel_size);
+  *out = new pdsc_fcgf();
+  (*out)->k1 = conv1_kernel_size;
+  return PDSC_OK;
 }
 
-void fcgf_free(pdsc_fcgf* h) {
-  if (!h) return;
+int pdsc_fcgf_destroy(pdsc_fcgf* h) {
+  if (!h) return PDSC_OK;
   if (h->d_arena) cudaFree(h->d_arena);
   delete h;
+  return PDSC_OK;
 }
 
-// 0, or 1 (unknown name) / 2 (wrong size) with *expected set
-int fcgf_set_param(pdsc_fcgf* h, const char* name, const float* data, int64_t numel, size_t* expected) {
+int pdsc_fcgf_set_param(pdsc_fcgf* h, const char* name, const float* h_data, int64_t numel) {
+  if (!h || !name || (!h_data && numel > 0) || numel < 0) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_fcgf_set_param: bad argument");
   for (const ParamSpec& p : fcgf_param_specs(h->k1)) {
     if (p.name != name) continue;
-    *expected = p.numel;
-    if ((size_t)numel != p.numel) return 2;
-    h->params[p.name].assign(data, data + numel);
+    if ((size_t)numel != p.numel)
+      return fail(PDSC_ERR_SHAPE, "pdsc_fcgf_set_param: '%s' has %lld elements, expected %zu", name, (long long)numel, p.numel);
+    h->params[p.name].assign(h_data, h_data + numel);
     h->committed = false;
-    return 0;
+    return PDSC_OK;
   }
-  return 1;
+  return fail(PDSC_ERR_UNKNOWN_PARAM, "pdsc_fcgf_set_param: unknown parameter '%s'", name);
 }
 
-// folds BN in float64 and uploads; returns the first missing parameter's name in *missing, or a CUDA error
-int fcgf_commit(pdsc_fcgf* h, std::string* missing) {
+// folds BN in float64 and uploads
+int pdsc_fcgf_commit(pdsc_fcgf* h) {
+  if (!h) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_fcgf_commit: null handle");
   for (const ParamSpec& p : fcgf_param_specs(h->k1))
-    if (!h->params.count(p.name)) { *missing = p.name; return -1; }
+    if (!h->params.count(p.name))
+      return fail(PDSC_ERR_UNKNOWN_PARAM, "pdsc_fcgf_commit: state-dict entry missing: %s", p.name.c_str());
   std::vector<float> arena;
   auto put = [&](const float* src, size_t n) {
     while (arena.size() % 4) arena.push_back(0.f);
@@ -508,39 +527,54 @@ int fcgf_commit(pdsc_fcgf* h, std::string* missing) {
   if (h->d_arena) { cudaFree(h->d_arena); h->d_arena = nullptr; }
   cudaError_t e = cudaMalloc(&h->d_arena, arena.size() * 4);
   if (e == cudaSuccess) e = cudaMemcpy(h->d_arena, arena.data(), arena.size() * 4, cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) return (int)e;
+  if (e != cudaSuccess) return fail(PDSC_ERR_CUDA, "pdsc_fcgf_commit: upload failed: %s", cudaGetErrorString(e));
   h->committed = true;
-  return 0;
+  return PDSC_OK;
 }
 
-bool fcgf_committed(const pdsc_fcgf* h) { return h->committed; }
-int fcgf_kernel_size(const pdsc_fcgf* h) { return h->k1; }
+size_t pdsc_fcgf_packed_scratch_bytes(const pdsc_fcgf* h, int32_t P, const int32_t* h_offsets) {
+  if (!h || check_offsets("pdsc_fcgf_packed_scratch_bytes", "", P, h_offsets, 1) || h_offsets[P] > kFcgfMaxPoints) return 0;
+  return fcgf_scratch_bytes(P, h_offsets, h->k1);
+}
 
-size_t fcgf_scratch_bytes(int P, const int32_t* h_off, int k1) { return carve(nullptr, P, h_off, k1).bytes; }
-
-int fcgf_scratch_layout(int P, const int32_t* h_off, int k1, int64_t* offsets, int capacity) {
-  const Scratch s = carve(nullptr, P, h_off, k1);
+int32_t pdsc_fcgf_scratch_layout(const pdsc_fcgf* h, int32_t P, const int32_t* h_offsets, int64_t* offsets, int32_t capacity) {
+  if (!h || check_offsets("pdsc_fcgf_scratch_layout", "", P, h_offsets, 1) || h_offsets[P] > kFcgfMaxPoints) return 0;
+  const Scratch s = carve(nullptr, P, h_offsets, h->k1);
   const int n = (int)s.reported.size();
-  for (int i = 0; i < n && i < capacity; ++i) offsets[i] = (int64_t)s.reported[i];
+  for (int i = 0; offsets && i < n && i < capacity; ++i) offsets[i] = (int64_t)s.reported[i];
   return n;
 }
 
-int launch_fcgf(const pdsc_fcgf* h, int P, const int32_t* h_off, const int32_t* d_off, const float* pts, double voxel,
-                float* keypts, float* desc, int32_t* out_off, int32_t* status, void* scratch, cudaStream_t st) {
-  const Scratch s = carve(scratch, P, h_off, h->k1);
-  const long long n = h_off[P];
-  const unsigned long long S = total_slots(P, h_off);
+int pdsc_fcgf_packed(pdsc_engine* e, const pdsc_fcgf* h, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets,
+                     const float* d_points, double voxel_size, float* d_keypts, float* d_desc, int32_t* d_out_offsets,
+                     int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  const char* fn = "pdsc_fcgf_packed";
+  if (!e || !h) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null engine or weight handle", fn);
+  if (!h->committed) return fail(PDSC_ERR_NOT_COMMITTED, "%s: pdsc_fcgf_commit() has not been called since the last "
+                                 "pdsc_fcgf_set_param()", fn);
+  if (int rc = check_offsets(fn, "", P, h_offsets, 1)) return rc;
+  if (h_offsets[P] > kFcgfMaxPoints) return fail(PDSC_ERR_SHAPE, "%s: need at most 2^26 points (got %d)", fn, h_offsets[P]);
+  if (!(voxel_size > 0.0) || !std::isfinite(voxel_size))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: voxel_size must be positive and finite (got %g)", fn, voxel_size);
+  if (!d_offsets || !d_points || !d_keypts || !d_desc || !d_out_offsets || !d_status)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, fcgf_scratch_bytes(P, h_offsets, h->k1), 256)) return rc;
+  DeviceGuard g(engine_config(e).device);
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  const Scratch s = carve(d_scratch, P, h_offsets, h->k1);
+  const long long n = h_offsets[P];
+  const unsigned long long S = total_slots(P, h_offsets);
   const int blocks = (int)((n + kScanBlock - 1) / kScanBlock);
   const unsigned g256 = (unsigned)((n + 255) / 256);
-  hash_plan_kernel<<<1, 1024, 0, st>>>(P, Offsets{d_off, 0}, s.slot0);
+  hash_plan_kernel<<<1, 1024, 0, st>>>(P, Offsets{d_offsets, 0}, s.slot0);
   fq_init_kernel<<<(unsigned)((std::max<unsigned long long>(S, P) + 255) / 256), 256, 0, st>>>(
-      s.keys[0], s.keys[1], s.keys[2], s.keys[3], s.first[0], s.first[1], s.first[2], s.first[3], S, P, status);
+      s.keys[0], s.keys[1], s.keys[2], s.keys[3], s.first[0], s.first[1], s.first[2], s.first[3], S, P, d_status);
   // the level's items' coordinates go to the (not yet used) conv1 table before their rows are numbered
   int32_t* tmp = s.map_c1;
   for (int l = 0; l < kLevels; ++l) {
-    const int32_t* in_off = l == 0 ? d_off : s.lvl_off[l - 1];
-    fq_insert_kernel<<<g256, 256, 0, st>>>(l, n, P, in_off, pts, voxel, l ? s.coords[l - 1] : nullptr, s.slot0, s.keys[l], s.first[l],
-                                           s.islot, tmp, status);
+    const int32_t* in_off = l == 0 ? d_offsets : s.lvl_off[l - 1];
+    fq_insert_kernel<<<g256, 256, 0, st>>>(l, n, P, in_off, d_points, voxel_size, l ? s.coords[l - 1] : nullptr, s.slot0, s.keys[l], s.first[l],
+                                           s.islot, tmp, d_status);
     fq_flag_kernel<<<blocks, kScanBlock, 0, st>>>(n, s.islot, s.first[l], s.flags, s.bbase + 1);
     fq_scan_kernel<<<1, 1024, 0, st>>>(blocks, s.bbase);
     fq_write_kernel<<<g256, 256, 0, st>>>(l, n, s.flags, s.bbase, s.islot, tmp, s.row_of[l], s.coords[l], s.rep0);
@@ -576,10 +610,11 @@ int launch_fcgf(const pdsc_fcgf* h, int P, const int32_t* h_off, const int32_t* 
     if (t.cout == 32) fconv_kernel<32><<<dim3(gx, 1), 256, 0, st>>>(a);
     else fconv_kernel<64><<<dim3(gx, t.cout / 64), 256, 0, st>>>(a);
   }
-  fhead_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(s.feat[F_CAT0], A + h->w_tr, A + h->w_f, A + h->b_f, s.lvl_off[0] + P, n, desc,
-                                                        s.rep0, pts, keypts);
-  cudaMemcpyAsync(out_off, s.lvl_off[0], (size_t)(P + 1) * 4, cudaMemcpyDeviceToDevice, st);
-  return (int)cudaGetLastError();
+  fhead_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(s.feat[F_CAT0], A + h->w_tr, A + h->w_f, A + h->b_f, s.lvl_off[0] + P, n, d_desc,
+                                                        s.rep0, d_points, d_keypts);
+  cudaMemcpyAsync(d_out_offsets, s.lvl_off[0], (size_t)(P + 1) * 4, cudaMemcpyDeviceToDevice, st);
+  if (const cudaError_t err = cudaGetLastError()) return fail(PDSC_ERR_CUDA, "%s: launch failed: %s", fn, cudaGetErrorString(err));
+  return PDSC_OK;
 }
 
-}  // namespace pdsc
+}  // extern "C"

@@ -39,7 +39,12 @@
 #include <math.h>
 
 #include <algorithm>
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+#include <vector>
 
+#include "abi.h"
 #include "common.cuh"
 #include "kernels.h"
 #include "sets.cuh"
@@ -52,6 +57,7 @@ namespace {
 constexpr unsigned long long kEmpty = kEmptyKey;
 constexpr int kCandCap = 4096;          // in-radius candidates one warp can hold
 constexpr double kFix = 1099511627776.0;   // 2^40: fixed-point scale of the offset inside a voxel, in voxel units
+constexpr int kVoxelMaxPoints = 1 << 30;   // the points of a voxel call: rows and the slots of a cloud's region (2 n) fit 32 bits
 
 // first 256-row rank tile of cloud p: a function of the offsets alone (as frontend.cu's tile0); a cloud of n rows owns
 // ceil(n / 256) tiles or one more, which is idle
@@ -215,28 +221,40 @@ __global__ void __launch_bounds__(256) vox_rank_kernel(int P, Offsets off, const
   }
 }
 
-void launch_voxel_down_sample(int P, const int32_t* h_off, const int32_t* d_off, const float* pts, double voxel, float* out_pts,
-                              int32_t* out_first, int32_t* out_ends, int32_t* status, void* scratch, cudaStream_t st) {
+// pdsc_voxel_down_sample and pdsc_voxel_down_sample_packed: cloud p's voxel means end at row out_ends[p], written by the call,
+// as is out_first[0] = 0 unless out_first is null
+static int voxel_impl(const char* who, pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets,
+                      const float* d_points, double voxel_size, float* d_out_points, int32_t* d_out_first, int32_t* d_out_ends,
+                      int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (h_offsets[P] > kVoxelMaxPoints) return fail(PDSC_ERR_SHAPE, "%s: need at most 2^30 points (got %d)", who, h_offsets[P]);
+  if (!(voxel_size > 0.0)) return fail(PDSC_ERR_INVALID_ARGUMENT, "voxel_size must be positive (got %g)", voxel_size);
+  if (!d_points || !d_out_points || !d_out_ends || !d_status) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", who);
+  if (int rc = check_scratch(who, "scratch", d_scratch, scratch_bytes, voxel_scratch_bytes(P, h_offsets), 8)) return rc;
+  DeviceGuard g(engine_config(e).device);
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   // without a device table (one cloud) the kernels read the offsets {0, n} as 0 * n, 1 * n
-  const Offsets off{d_off, d_off ? 0 : h_off[1]};
-  const long long n = h_off[P];
-  const unsigned long long slots = total_slots(P, h_off);
-  const VoxScratch s = vox_carve(scratch, P, n, slots);
+  const Offsets off{d_offsets, d_offsets ? 0 : h_offsets[1]};
+  const long long n = h_offsets[P];
+  const unsigned long long slots = total_slots(P, h_offsets);
+  const VoxScratch s = vox_carve(d_scratch, P, n, slots);
   long long most = 0;
-  for (int p = 0; p < P; ++p) most = std::max<long long>(most, (long long)h_off[p + 1] - h_off[p]);
+  for (int p = 0; p < P; ++p) most = std::max<long long>(most, (long long)h_offsets[p + 1] - h_offsets[p]);
   hash_plan_kernel<<<1, 1024, 0, st>>>(P, off, s.slot0);
   const unsigned long long init = std::max<unsigned long long>(slots, 3ull * P);
-  vox_init_kernel<<<(unsigned)((init + 255) / 256), 256, 0, st>>>(P, s.minkey, s.counter, s.keys, s.sums, s.counts, slots, status);
+  vox_init_kernel<<<(unsigned)((init + 255) / 256), 256, 0, st>>>(P, s.minkey, s.counter, s.keys, s.sums, s.counts, slots, d_status);
   const int sms = device_sm_count();
   long long bx = (most + 255) / 256, by = std::min(P, 65535);
   bx = std::min<long long>(bx, std::max<long long>(1, 8LL * sms / by));
-  vox_bounds_kernel<<<dim3((unsigned)bx, (unsigned)by), 256, 0, st>>>(pts, P, off, s.minkey);
-  vox_insert_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pts, n, P, off, voxel, s.minkey, s.slot0, s.keys, s.sums, s.counts,
-                                                                  status);
+  vox_bounds_kernel<<<dim3((unsigned)bx, (unsigned)by), 256, 0, st>>>(d_points, P, off, s.minkey);
+  vox_insert_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_points, n, P, off, voxel_size, s.minkey, s.slot0, s.keys, s.sums,
+                                                                  s.counts, d_status);
   vox_compact_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, st>>>(s.keys, slots, P, off, s.slot0, s.ckeys, s.cslot, s.counter);
-  vox_offsets_kernel<<<1, 1024, 0, st>>>(P, s.counter, out_first, out_ends);
-  vox_rank_kernel<<<(unsigned)rank_tile0(Offsets{h_off, 0}, P), 256, 0, st>>>(P, off, s.ckeys, s.cslot, s.counter, s.slot0, s.sums,
-                                                                              s.counts, s.minkey, voxel, out_ends, out_pts);
+  vox_offsets_kernel<<<1, 1024, 0, st>>>(P, s.counter, d_out_first, d_out_ends);
+  vox_rank_kernel<<<(unsigned)rank_tile0(Offsets{h_offsets, 0}, P), 256, 0, st>>>(P, off, s.ckeys, s.cslot, s.counter, s.slot0, s.sums,
+                                                                                  s.counts, s.minkey, voxel_size, d_out_ends,
+                                                                                  d_out_points);
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
 }
 
 // ---- hybrid (radius + max_nn) neighbour search --------------------------------------------------------------------
@@ -294,8 +312,8 @@ __global__ void __launch_bounds__(256) hybrid_search_kernel(const float* __restr
   if (lane == 0) nb_cnt[i] = want;
 }
 
-static int launch_hybrid_search(int nclouds, const int32_t* h_off, const int32_t* d_off, const float* pts, double radius, int max_nn,
-                                int32_t* nb_idx, int32_t* nb_cnt, int32_t* status, cudaStream_t st) {
+static cudaError_t launch_hybrid_search(int nclouds, const int32_t* h_off, const int32_t* d_off, const float* pts, double radius,
+                                        int max_nn, int32_t* nb_idx, int32_t* nb_cnt, int32_t* status, cudaStream_t st) {
   const int m = h_off[nclouds];
   const Offsets off{d_off, d_off ? 0 : h_off[1]};     // no device table: one cloud, offsets {0, m}
   int P = 2;
@@ -305,10 +323,10 @@ static int launch_hybrid_search(int nclouds, const int32_t* h_off, const int32_t
   warps = warps > 8 ? 8 : warps;
   const int smem = (int)(per_warp * warps);
   const cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(hybrid_search_kernel), smem);
-  if (e != cudaSuccess) return (int)e;
+  if (e != cudaSuccess) return e;
   hybrid_search_kernel<<<(m + warps - 1) / warps, warps * 32, smem, st>>>(pts, m, nclouds, off, (float)(radius * radius), max_nn, P,
                                                                          warps, nb_idx, nb_cnt, status);
-  return 0;
+  return cudaSuccess;
 }
 
 // ---- normals --------------------------------------------------------------------------------------------------
@@ -491,35 +509,205 @@ __global__ void __launch_bounds__(256) fpfh_kernel(const float* __restrict__ pts
   if (lane == 0) out[33 * (size_t)i + 32] = res[1];
 }
 
-// ---- host side -------------------------------------------------------------------------------------------------
-size_t fpfh_scratch_bytes(int m, int max_nn) {
+// ---- normals and FPFH -------------------------------------------------------------------------------------------
+// scratch: spfh [m][33] double | nb_idx [m][max_nn] | nb_cnt [m]; normals use the neighbour lists only
+static size_t fpfh_scratch_bytes(int m, int max_nn) {
   return (size_t)m * max_nn * 4 + (size_t)m * 4 + 16 + (size_t)m * 33 * 8;
 }
 
-int launch_estimate_normals(int P, const int32_t* h_off, const int32_t* d_off, const float* pts, double radius, int max_nn,
-                            double* normals, int32_t* status, void* scratch, cudaStream_t st) {
-  const int m = h_off[P];
-  unsigned char* p = static_cast<unsigned char*>(scratch);
-  int32_t* nb_idx = reinterpret_cast<int32_t*>(p + (size_t)m * 33 * 8);
-  int32_t* nb_cnt = nb_idx + (size_t)m * max_nn;
-  const int rc = launch_hybrid_search(P, h_off, d_off, pts, radius, max_nn, nb_idx, nb_cnt, status, st);
-  if (rc) return rc;
-  normals_kernel<<<(m + 127) / 128, 128, 0, st>>>(pts, m, max_nn, nb_idx, nb_cnt, normals);
-  return (int)cudaGetLastError();
-}
-
-int launch_compute_fpfh(int P, const int32_t* h_off, const int32_t* d_off, const float* pts, const double* normals, double radius,
-                        int max_nn, int normalise, double* out, int32_t* status, void* scratch, cudaStream_t st) {
-  const int m = h_off[P];
-  unsigned char* p = static_cast<unsigned char*>(scratch);
+// the normals (d_normals null) or the FPFH (d_normals given) of P clouds: one set of checks and one neighbour search, under the
+// caller's name
+static int search_impl(const char* who, pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets,
+                       const float* d_points, const double* d_normals, double radius, int32_t max_nn, int32_t normalise, double* d_out,
+                       int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  const int m = h_offsets[P];
+  if (!(radius > 0.0)) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: radius must be positive (got %g)", who, radius);
+  if (max_nn < 1 || max_nn > 256) return fail(PDSC_ERR_UNSUPPORTED, "%s: max_nn %d outside [1, 256]", who, max_nn);
+  if (!d_points || !d_out || !d_status) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", who);
+  if (int rc = check_scratch(who, "scratch", d_scratch, scratch_bytes, fpfh_scratch_bytes(m, max_nn), 8)) return rc;
+  DeviceGuard g(engine_config(e).device);
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  PDSC_CUDA(cudaMemsetAsync(d_status, 0, 4 * (size_t)P, st));
+  unsigned char* p = static_cast<unsigned char*>(d_scratch);
   double* spfh = reinterpret_cast<double*>(p);
   int32_t* nb_idx = reinterpret_cast<int32_t*>(p + (size_t)m * 33 * 8);
   int32_t* nb_cnt = nb_idx + (size_t)m * max_nn;
-  const int rc = launch_hybrid_search(P, h_off, d_off, pts, radius, max_nn, nb_idx, nb_cnt, status, st);
-  if (rc) return rc;
-  spfh_kernel<<<(m + 7) / 8, 256, 0, st>>>(pts, normals, m, max_nn, nb_idx, nb_cnt, spfh);
-  fpfh_kernel<<<(m + 7) / 8, 256, 0, st>>>(pts, m, max_nn, nb_idx, nb_cnt, spfh, normalise, out);
-  return (int)cudaGetLastError();
+  cudaError_t err = launch_hybrid_search(P, h_offsets, d_offsets, d_points, radius, max_nn, nb_idx, nb_cnt, d_status, st);
+  if (err == cudaSuccess) {
+    if (!d_normals) {
+      normals_kernel<<<(m + 127) / 128, 128, 0, st>>>(d_points, m, max_nn, nb_idx, nb_cnt, d_out);
+    } else {
+      spfh_kernel<<<(m + 7) / 8, 256, 0, st>>>(d_points, d_normals, m, max_nn, nb_idx, nb_cnt, spfh);
+      fpfh_kernel<<<(m + 7) / 8, 256, 0, st>>>(d_points, m, max_nn, nb_idx, nb_cnt, spfh, normalise, d_out);
+    }
+    err = cudaGetLastError();
+  }
+  if (err != cudaSuccess) return fail(PDSC_ERR_CUDA, "%s: launch failed: %s", who, cudaGetErrorString(err));
+  return PDSC_OK;
 }
 
 }  // namespace pdsc
+
+// ---- C ABI ------------------------------------------------------------------------------------------------------
+using namespace pdsc;
+
+extern "C" {
+
+size_t pdsc_voxel_down_sample_scratch_bytes(int64_t n) {
+  if (n <= 0 || n > kVoxelMaxPoints) return 0;
+  const int32_t off[2] = {0, (int32_t)n};
+  return voxel_scratch_bytes(1, off);
+}
+
+size_t pdsc_voxel_down_sample_packed_scratch_bytes(int32_t P, const int32_t* h_offsets) {
+  if (check_offsets("pdsc_voxel_down_sample_packed_scratch_bytes", "", P, h_offsets, 1) || h_offsets[P] > kVoxelMaxPoints) return 0;
+  return voxel_scratch_bytes(P, h_offsets);
+}
+
+int pdsc_voxel_down_sample(pdsc_engine* e, int64_t n, const float* d_points, double voxel_size, float* d_out_points,
+                           int32_t* d_count, int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (n <= 0 || n > kVoxelMaxPoints) return fail(PDSC_ERR_SHAPE, "need 1 <= n <= 2^30 points (got %lld)", (long long)n);
+  // the packed call with one cloud: its offsets need no device table, and its end row is the count
+  const int32_t off[2] = {0, (int32_t)n};
+  return voxel_impl("pdsc_voxel_down_sample", e, 1, off, nullptr, d_points, voxel_size, d_out_points, nullptr, d_count, d_status,
+                    d_scratch, scratch_bytes, cuda_stream);
+}
+
+int pdsc_voxel_down_sample_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
+                                  double voxel_size, float* d_out_points, int32_t* d_out_offsets, int32_t* d_status, void* d_scratch,
+                                  size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_offsets("pdsc_voxel_down_sample_packed", "", P, h_offsets, 1)) return rc;
+  if (!d_offsets || !d_out_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_voxel_down_sample_packed: null offsets");
+  return voxel_impl("pdsc_voxel_down_sample_packed", e, P, h_offsets, d_offsets, d_points, voxel_size, d_out_points, d_out_offsets,
+                    d_out_offsets + 1, d_status, d_scratch, scratch_bytes, cuda_stream);
+}
+
+size_t pdsc_fpfh_scratch_bytes(int32_t m, int32_t max_nn) { return (m > 0 && max_nn > 0) ? fpfh_scratch_bytes(m, max_nn) : 0; }
+
+size_t pdsc_fpfh_packed_scratch_bytes(int32_t P, const int32_t* h_offsets, int32_t max_nn) {
+  if (check_offsets("pdsc_fpfh_packed_scratch_bytes", "", P, h_offsets, 1) || max_nn <= 0) return 0;
+  return fpfh_scratch_bytes(h_offsets[P], max_nn);
+}
+
+int pdsc_estimate_normals(pdsc_engine* e, int32_t m, const float* d_points, double radius, int32_t max_nn, double* d_normals,
+                          int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (m <= 0) return fail(PDSC_ERR_SHAPE, "pdsc_estimate_normals: need m >= 1 points (got %d)", m);
+  const int32_t off[2] = {0, m};                      // the packed call with one cloud and no device table
+  return search_impl("pdsc_estimate_normals", e, 1, off, nullptr, d_points, nullptr, radius, max_nn, 0, d_normals, d_status, d_scratch,
+                     scratch_bytes, cuda_stream);
+}
+
+int pdsc_estimate_normals_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
+                                 double radius, int32_t max_nn, double* d_normals, int32_t* d_status, void* d_scratch,
+                                 size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_offsets("pdsc_estimate_normals_packed", "", P, h_offsets, 1)) return rc;
+  if (!d_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_estimate_normals_packed: null device offsets");
+  return search_impl("pdsc_estimate_normals_packed", e, P, h_offsets, d_offsets, d_points, nullptr, radius, max_nn, 0, d_normals,
+                     d_status, d_scratch, scratch_bytes, cuda_stream);
+}
+
+int pdsc_compute_fpfh(pdsc_engine* e, int32_t m, const float* d_points, const double* d_normals, double radius, int32_t max_nn,
+                      int32_t normalise, double* d_fpfh, int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (m <= 0) return fail(PDSC_ERR_SHAPE, "pdsc_compute_fpfh: need m >= 1 points (got %d)", m);
+  if (!d_normals) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_compute_fpfh: null normals");
+  const int32_t off[2] = {0, m};
+  return search_impl("pdsc_compute_fpfh", e, 1, off, nullptr, d_points, d_normals, radius, max_nn, normalise, d_fpfh, d_status,
+                     d_scratch, scratch_bytes, cuda_stream);
+}
+
+int pdsc_compute_fpfh_packed(pdsc_engine* e, int32_t P, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_points,
+                             const double* d_normals, double radius, int32_t max_nn, int32_t normalise, double* d_fpfh,
+                             int32_t* d_status, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_offsets("pdsc_compute_fpfh_packed", "", P, h_offsets, 1)) return rc;
+  if (!d_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_compute_fpfh_packed: null device offsets");
+  if (!d_normals) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_compute_fpfh_packed: null normals");
+  return search_impl("pdsc_compute_fpfh_packed", e, P, h_offsets, d_offsets, d_points, d_normals, radius, max_nn, normalise, d_fpfh,
+                     d_status, d_scratch, scratch_bytes, cuda_stream);
+}
+
+// Host-side PLY vertex reader (ascii / binary_little_endian; x, y, z as float or double; other vertex properties skipped).
+int pdsc_read_ply(const char* path, float* points, int64_t capacity, int64_t* n_vertices) {
+  if (!path || !n_vertices) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_read_ply: null argument");
+  FILE* f = fopen(path, "rb");
+  if (!f) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_read_ply: cannot open %s", path);
+  struct Closer { FILE* f; ~Closer() { fclose(f); } } closer{f};
+  char line[512];
+  if (!fgets(line, sizeof line, f) || strncmp(line, "ply", 3) != 0) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s is not a PLY file", path);
+  int format = -1;                    // 0 ascii, 1 binary little endian
+  long long n = -1;
+  bool in_vertex = false, vertex_first = true, seen_element = false;
+  struct Prop { int size; bool is_float; int axis; };
+  std::vector<Prop> props;
+  while (true) {
+    if (!fgets(line, sizeof line, f)) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: header ends before end_header", path);
+    char a[64] = {0}, b[64] = {0}, c[64] = {0};
+    const int got = sscanf(line, "%63s %63s %63s", a, b, c);
+    if (got < 1) continue;
+    if (!strcmp(a, "end_header")) break;
+    if (!strcmp(a, "format")) {
+      if (!strcmp(b, "ascii")) format = 0;
+      else if (!strcmp(b, "binary_little_endian")) format = 1;
+      else return fail(PDSC_ERR_UNSUPPORTED, "%s: PLY format %s is not supported", path, b);
+    } else if (!strcmp(a, "element")) {
+      in_vertex = !strcmp(b, "vertex");
+      if (in_vertex) { n = atoll(c); vertex_first = !seen_element; }
+      seen_element = true;
+    } else if (!strcmp(a, "property") && in_vertex) {
+      if (!strcmp(b, "list")) return fail(PDSC_ERR_UNSUPPORTED, "%s: list properties on vertices are not supported", path);
+      Prop p{0, false, -1};
+      if (!strcmp(b, "char") || !strcmp(b, "uchar") || !strcmp(b, "int8") || !strcmp(b, "uint8")) p.size = 1;
+      else if (!strcmp(b, "short") || !strcmp(b, "ushort") || !strcmp(b, "int16") || !strcmp(b, "uint16")) p.size = 2;
+      else if (!strcmp(b, "int") || !strcmp(b, "uint") || !strcmp(b, "int32") || !strcmp(b, "uint32")) p.size = 4;
+      else if (!strcmp(b, "float") || !strcmp(b, "float32")) { p.size = 4; p.is_float = true; }
+      else if (!strcmp(b, "double") || !strcmp(b, "float64")) { p.size = 8; p.is_float = true; }
+      else return fail(PDSC_ERR_UNSUPPORTED, "%s: unknown property type %s", path, b);
+      if (!strcmp(c, "x")) p.axis = 0; else if (!strcmp(c, "y")) p.axis = 1; else if (!strcmp(c, "z")) p.axis = 2;
+      if (p.axis >= 0 && !p.is_float) return fail(PDSC_ERR_UNSUPPORTED, "%s: integer coordinates are not supported", path);
+      props.push_back(p);
+    }
+  }
+  if (format < 0 || n < 0) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: no format / vertex element in the header", path);
+  if (!vertex_first) return fail(PDSC_ERR_UNSUPPORTED, "%s: the vertex element must come first", path);
+  int have = 0;
+  for (const Prop& p : props) if (p.axis >= 0) have |= 1 << p.axis;
+  if (have != 7) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: vertex properties x, y, z not all present", path);
+  *n_vertices = n;
+  if (!points) return PDSC_OK;                        // size query
+  if (capacity < n) return fail(PDSC_ERR_SHAPE, "pdsc_read_ply: buffer holds %lld vertices, the file has %lld", (long long)capacity, n);
+  if (format == 0) {
+    for (long long i = 0; i < n; ++i) {
+      for (const Prop& p : props) {
+        double v;
+        if (fscanf(f, "%lf", &v) != 1) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: truncated at vertex %lld", path, i);
+        if (p.axis >= 0) points[3 * i + p.axis] = (float)v;
+      }
+    }
+  } else {
+    size_t stride = 0;
+    for (const Prop& p : props) stride += (size_t)p.size;
+    std::vector<unsigned char> row(stride * 4096);
+    for (long long i0 = 0; i0 < n; i0 += 4096) {
+      const size_t rows = (size_t)std::min<long long>(4096, n - i0);
+      if (fread(row.data(), stride, rows, f) != rows) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: truncated at vertex %lld", path, i0);
+      for (size_t r = 0; r < rows; ++r) {
+        size_t off = r * stride;
+        for (const Prop& p : props) {
+          if (p.axis >= 0) {
+            if (p.size == 4) { float v; memcpy(&v, &row[off], 4); points[3 * (i0 + (long long)r) + p.axis] = v; }
+            else { double v; memcpy(&v, &row[off], 8); points[3 * (i0 + (long long)r) + p.axis] = (float)v; }
+          }
+          off += (size_t)p.size;
+        }
+      }
+    }
+  }
+  return PDSC_OK;
+}
+
+}  // extern "C"

@@ -26,7 +26,9 @@
 #include <stdint.h>
 
 #include <algorithm>
+#include <cmath>
 
+#include "abi.h"
 #include "common.cuh"
 #include "kernels.h"
 #include "sets.cuh"
@@ -37,7 +39,10 @@ namespace pdsc {
 namespace {
 constexpr int kRes = 16;
 constexpr int kUnitVoxels = kRes * kRes * kRes;
-constexpr int kMaskWords = kMaxFragmentFrames / 32;
+constexpr int kMaxFrames = 256;          // frames of one fragment: the bits of a unit's frame mask
+constexpr int kMaxCallFrames = 65535;    // frames of one call: the touch kernel's grid's y dimension
+constexpr int kMaxUnits = 1 << 22;       // units of one fragment (max_units)
+constexpr int kMaskWords = kMaxFrames / 32;
 constexpr int kKeyBias = 1 << 20;
 constexpr int kStage = kRes + 2;
 constexpr int kStageCells = kStage * kStage * kStage;
@@ -411,32 +416,109 @@ __global__ void __launch_bounds__(256) vertex_write_kernel(int F, Offsets uoff, 
     }
 }
 
-}  // namespace
-
 size_t tsdf_table_bytes(int F, int max_units) {
   return (size_t)F * table_slots(max_units) * (8 + 4 * kMaskWords + 4);
 }
 
 size_t tsdf_integrate_scratch_bytes(int F, long long U) { return (size_t)U * 24 + (size_t)F * 4; }
 
-void launch_tsdf_touch(int F, int NF, const int32_t* d_frame_off, int H, int W, const double* intrinsic, const uint16_t* depth,
-                       const double* poses, double depth_scale, double depth_trunc, double voxel, double trunc, int max_units,
-                       int32_t* counts, int32_t* status, void* table, cudaStream_t st) {
-  const Table t = table_carve(table, F, max_units);
-  const Camera c{H, W, intrinsic[0], intrinsic[1], intrinsic[2], intrinsic[3], depth_scale, depth_trunc, voxel, trunc};
-  const long long n = (long long)F * t.slots;
-  table_init_kernel<<<(unsigned)std::min<long long>((n + 255) / 256, 65536), 256, 0, st>>>(t, n, F, counts, status);
-  const int pts = ((W + 3) / 4) * ((H + 3) / 4);
-  touch_kernel<<<dim3((pts + 127) / 128, NF), 128, 0, st>>>(F, Offsets{d_frame_off, 0}, depth, poses, c, max_units, t, counts, status);
+// the frame offsets, image and volume parameters every TSDF stage of a call checks alike
+pdsc_status check_tsdf(const char* fn, int32_t F, const int32_t* h_frame_offsets, int32_t height, int32_t width,
+                       const double* intrinsic, double voxel_length, double sdf_trunc, int32_t max_units) {
+  if (pdsc_status rc = check_offsets(fn, "frame ", F, h_frame_offsets, 1, kMaxFrames)) return rc;
+  if (h_frame_offsets[F] > kMaxCallFrames)
+    return fail(PDSC_ERR_SHAPE, "%s: at most %d frames per call (got %d)", fn, kMaxCallFrames, h_frame_offsets[F]);
+  if (height < 1 || width < 1 || (long long)height * width > (1 << 26))
+    return fail(PDSC_ERR_SHAPE, "%s: image %d x %d outside 1 .. 2^26 pixels", fn, width, height);
+  if (!intrinsic) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null intrinsic", fn);
+  for (int i = 0; i < 4; ++i)
+    if (!std::isfinite(intrinsic[i]) || (i < 2 && !(intrinsic[i] > 0.0)))
+      return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: intrinsic %d (%g) must be finite, and the focal lengths positive", fn, i, intrinsic[i]);
+  if (!(voxel_length > 0.0) || !std::isfinite(voxel_length) || !(sdf_trunc > 0.0) || !std::isfinite(sdf_trunc))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: voxel_length (%g) and sdf_trunc (%g) must be positive and finite", fn, voxel_length,
+                sdf_trunc);
+  if (max_units < 1 || max_units > kMaxUnits)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_units %d outside [1, %d]", fn, max_units, kMaxUnits);
+  return PDSC_OK;
 }
 
-void launch_tsdf_integrate(int F, const int32_t* d_frame_off, const int32_t* d_unit_off, long long U, int H, int W,
-                           const double* intrinsic, const uint16_t* depth, const uint8_t* color, const double* poses,
-                           double depth_scale, double depth_trunc, double voxel, double trunc, int max_units, void* table,
-                           int32_t* unit_keys, float* tsdf, float* weight, float* color_out, void* scratch, cudaStream_t st) {
-  const Table t = table_carve(table, F, max_units);
-  const Camera c{H, W, intrinsic[0], intrinsic[1], intrinsic[2], intrinsic[3], depth_scale, depth_trunc, voxel, trunc};
-  unsigned char* p = static_cast<unsigned char*>(scratch);
+pdsc_status check_units(const char* fn, int32_t F, const int32_t* h_unit_offsets, int32_t max_units, const void* d_table,
+                        size_t table_bytes) {
+  if (max_units < 1 || max_units > kMaxUnits)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_units %d outside [1, %d]", fn, max_units, kMaxUnits);
+  if (pdsc_status rc = check_offsets(fn, "unit ", F, h_unit_offsets, 0, max_units)) return rc;
+  return check_scratch(fn, "table", d_table, table_bytes, tsdf_table_bytes(F, max_units), 8);
+}
+
+Camera camera(int H, int W, const double* intrinsic, double depth_scale, double depth_trunc, double voxel, double trunc) {
+  return Camera{H, W, intrinsic[0], intrinsic[1], intrinsic[2], intrinsic[3], depth_scale, depth_trunc, voxel, trunc};
+}
+
+}  // namespace
+}  // namespace pdsc
+
+// ---- C ABI ------------------------------------------------------------------------------------------------------
+using namespace pdsc;
+
+extern "C" {
+
+size_t pdsc_tsdf_table_bytes(int32_t F, int32_t max_units) {
+  if (F < 1 || max_units < 1 || max_units > kMaxUnits) return 0;
+  return tsdf_table_bytes(F, max_units);
+}
+
+int pdsc_tsdf_touch_packed(pdsc_engine* e, int32_t F, const int32_t* h_frame_offsets, const int32_t* d_frame_offsets, int32_t height,
+                           int32_t width, const double* intrinsic, const uint16_t* d_depth, const double* d_poses, double depth_scale,
+                           double depth_trunc, double voxel_length, double sdf_trunc, int32_t max_units, int32_t* d_unit_counts,
+                           int32_t* d_status, void* d_table, size_t table_bytes, void* cuda_stream) {
+  const char* fn = "pdsc_tsdf_touch_packed";
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_tsdf(fn, F, h_frame_offsets, height, width, intrinsic, voxel_length, sdf_trunc, max_units)) return rc;
+  if (!(depth_scale > 0.0) || !std::isfinite(depth_scale))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: depth_scale must be positive and finite (got %g)", fn, depth_scale);
+  if (!d_frame_offsets || !d_depth || !d_poses || !d_unit_counts || !d_status)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  if (int rc = check_scratch(fn, "table", d_table, table_bytes, tsdf_table_bytes(F, max_units), 8)) return rc;
+  DeviceGuard g(engine_config(e).device);
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  const Table t = table_carve(d_table, F, max_units);
+  const Camera c = camera(height, width, intrinsic, depth_scale, depth_trunc, voxel_length, sdf_trunc);
+  const long long n = (long long)F * t.slots;
+  table_init_kernel<<<(unsigned)std::min<long long>((n + 255) / 256, 65536), 256, 0, st>>>(t, n, F, d_unit_counts, d_status);
+  const int pts = ((width + 3) / 4) * ((height + 3) / 4);
+  touch_kernel<<<dim3((pts + 127) / 128, h_frame_offsets[F]), 128, 0, st>>>(F, Offsets{d_frame_offsets, 0}, d_depth, d_poses, c,
+                                                                             max_units, t, d_unit_counts, d_status);
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
+
+size_t pdsc_tsdf_integrate_scratch_bytes(int32_t F, const int32_t* h_unit_offsets) {
+  if (check_offsets("pdsc_tsdf_integrate_scratch_bytes", "unit ", F, h_unit_offsets, 0, kMaxUnits)) return 0;
+  return tsdf_integrate_scratch_bytes(F, h_unit_offsets[F]);
+}
+
+int pdsc_tsdf_integrate_packed(pdsc_engine* e, int32_t F, const int32_t* h_frame_offsets, const int32_t* d_frame_offsets,
+                               const int32_t* h_unit_offsets, const int32_t* d_unit_offsets, int32_t height, int32_t width,
+                               const double* intrinsic, const uint16_t* d_depth, const uint8_t* d_color, const double* d_poses,
+                               double depth_scale, double depth_trunc, double voxel_length, double sdf_trunc, int32_t max_units,
+                               void* d_table, size_t table_bytes, int32_t* d_unit_keys, float* d_tsdf, float* d_weight,
+                               float* d_voxel_color, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  const char* fn = "pdsc_tsdf_integrate_packed";
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_tsdf(fn, F, h_frame_offsets, height, width, intrinsic, voxel_length, sdf_trunc, max_units)) return rc;
+  if (int rc = check_units(fn, F, h_unit_offsets, max_units, d_table, table_bytes)) return rc;
+  if (!(depth_scale > 0.0) || !std::isfinite(depth_scale))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: depth_scale must be positive and finite (got %g)", fn, depth_scale);
+  const long long U = h_unit_offsets[F];
+  if (!d_frame_offsets || !d_unit_offsets || !d_depth || !d_color || !d_poses || (U > 0 && (!d_unit_keys || !d_tsdf || !d_weight ||
+                                                                                             !d_voxel_color)))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, tsdf_integrate_scratch_bytes(F, U), 8)) return rc;
+  DeviceGuard g(engine_config(e).device);
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  const Table t = table_carve(d_table, F, max_units);
+  const Camera c = camera(height, width, intrinsic, depth_scale, depth_trunc, voxel_length, sdf_trunc);
+  unsigned char* p = static_cast<unsigned char*>(d_scratch);
   unsigned long long* list_key = reinterpret_cast<unsigned long long*>(p); p += (size_t)U * 8;
   long long* list_slot = reinterpret_cast<long long*>(p);                 p += (size_t)U * 8;
   long long* unit_slot = reinterpret_cast<long long*>(p);                 p += (size_t)U * 8;
@@ -444,28 +526,58 @@ void launch_tsdf_integrate(int F, const int32_t* d_frame_off, const int32_t* d_u
   launch_fill_u32(reinterpret_cast<uint32_t*>(cursor), 0u, F, st);
   launch_fill_u64(list_key, kEmptyKey, 2 * U, st);          // list_key and list_slot: empty key, slot -1
   const long long n = (long long)F * t.slots;
-  const Offsets uoff{d_unit_off, 0};
+  const Offsets uoff{d_unit_offsets, 0};
   unit_list_kernel<<<(unsigned)std::min<long long>((n + 255) / 256, 65536), 256, 0, st>>>(F, uoff, t, cursor, list_key, list_slot);
-  if (U == 0) return;
-  unit_rank_kernel<<<(unsigned)((U + 255) / 256), 256, 0, st>>>(F, uoff, U, t, list_key, list_slot, unit_keys, unit_slot);
-  integrate_kernel<<<(unsigned)U, 256, 0, st>>>(F, Offsets{d_frame_off, 0}, uoff, depth, color, poses, c, t, unit_keys, unit_slot, tsdf,
-                                                weight, color_out);
+  if (U > 0) {
+    unit_rank_kernel<<<(unsigned)((U + 255) / 256), 256, 0, st>>>(F, uoff, U, t, list_key, list_slot, d_unit_keys, unit_slot);
+    integrate_kernel<<<(unsigned)U, 256, 0, st>>>(F, Offsets{d_frame_offsets, 0}, uoff, d_depth, d_color, d_poses, c, t, d_unit_keys,
+                                                  unit_slot, d_tsdf, d_weight, d_voxel_color);
+  }
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
 }
 
-void launch_vertex_count(int F, const int32_t* d_unit_off, int U, int max_units, void* table, const int32_t* unit_keys,
-                         const float* tsdf, const float* weight, long long* ends, long long* frag_off, cudaStream_t st) {
-  const Volume vol{table_carve(table, F, max_units), U, unit_keys, tsdf, weight, nullptr};
-  const Offsets uoff{d_unit_off, 0};
+int pdsc_extract_vertices_count_packed(pdsc_engine* e, int32_t F, const int32_t* h_unit_offsets, const int32_t* d_unit_offsets,
+                                       int32_t max_units, void* d_table, size_t table_bytes, const int32_t* d_unit_keys,
+                                       const float* d_tsdf, const float* d_weight, int64_t* d_vertex_ends, int64_t* d_vertex_offsets,
+                                       void* cuda_stream) {
+  const char* fn = "pdsc_extract_vertices_count_packed";
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_units(fn, F, h_unit_offsets, max_units, d_table, table_bytes)) return rc;
+  const int U = h_unit_offsets[F];
+  if (!d_unit_offsets || !d_vertex_offsets || (U > 0 && (!d_unit_keys || !d_tsdf || !d_weight || !d_vertex_ends)))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  DeviceGuard g(engine_config(e).device);
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  const Volume vol{table_carve(d_table, F, max_units), U, d_unit_keys, d_tsdf, d_weight, nullptr};
+  const Offsets uoff{d_unit_offsets, 0};
+  long long* ends = reinterpret_cast<long long*>(d_vertex_ends);
   if (U > 0) vertex_count_kernel<<<U, 256, 0, st>>>(F, uoff, vol, ends);
-  vertex_scan_kernel<<<1, 1024, 0, st>>>(F, uoff, U, ends, frag_off);
+  vertex_scan_kernel<<<1, 1024, 0, st>>>(F, uoff, U, ends, reinterpret_cast<long long*>(d_vertex_offsets));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
 }
 
-void launch_vertex_write(int F, const int32_t* d_unit_off, int U, int max_units, void* table, const int32_t* unit_keys,
-                         const float* tsdf, const float* weight, const float* color, double voxel, const long long* ends,
-                         double* vertices, double* colors, cudaStream_t st) {
-  if (U == 0) return;
-  const Volume vol{table_carve(table, F, max_units), U, unit_keys, tsdf, weight, color};
-  vertex_write_kernel<<<U, 256, 0, st>>>(F, Offsets{d_unit_off, 0}, vol, voxel, ends, vertices, colors);
+int pdsc_extract_vertices_packed(pdsc_engine* e, int32_t F, const int32_t* h_unit_offsets, const int32_t* d_unit_offsets,
+                                 int32_t max_units, void* d_table, size_t table_bytes, const int32_t* d_unit_keys, const float* d_tsdf,
+                                 const float* d_weight, const float* d_voxel_color, double voxel_length, const int64_t* d_vertex_ends,
+                                 double* d_vertices, double* d_vertex_colors, void* cuda_stream) {
+  const char* fn = "pdsc_extract_vertices_packed";
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_units(fn, F, h_unit_offsets, max_units, d_table, table_bytes)) return rc;
+  if (!(voxel_length > 0.0) || !std::isfinite(voxel_length))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: voxel_length must be positive and finite (got %g)", fn, voxel_length);
+  const int U = h_unit_offsets[F];
+  if (!d_unit_offsets || (U > 0 && (!d_unit_keys || !d_tsdf || !d_weight || !d_voxel_color || !d_vertex_ends)))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  DeviceGuard g(engine_config(e).device);
+  if (U > 0) {
+    const Volume vol{table_carve(d_table, F, max_units), U, d_unit_keys, d_tsdf, d_weight, d_voxel_color};
+    vertex_write_kernel<<<U, 256, 0, static_cast<cudaStream_t>(cuda_stream)>>>(
+        F, Offsets{d_unit_offsets, 0}, vol, voxel_length, reinterpret_cast<const long long*>(d_vertex_ends), d_vertices, d_vertex_colors);
+  }
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
 }
 
-}  // namespace pdsc
+}  // extern "C"

@@ -36,6 +36,7 @@
 // are separated (tests); exact duplicates resolve to the first one, as in numpy.
 #include <cfloat>
 
+#include "abi.h"
 #include "common.cuh"
 #include "kernels.h"
 #include "sets.cuh"
@@ -308,24 +309,78 @@ static void launch_match_t(int P, const int32_t* h_src_off, const int32_t* h_tgt
                                                        out_first, out_ends, corr_pos, out_src, out_tgt);
 }
 
-size_t match_scratch_bytes(int Ns, int Nt) {
+static size_t match_scratch_bytes(int Ns, int Nt) {
   const size_t rows = (size_t)(Ns > Nt ? Ns : Nt);
   return (size_t)(Ns + Nt) * sizeof(int32_t) + rows * kMatchMaxChunks * sizeof(MatchPartial<double>) + 32;
 }
-int match_max_dim() { return kMatchMaxD; }
 
-void launch_match(int P, const int32_t* h_src_off, const int32_t* h_tgt_off, const int32_t* d_src_off, const int32_t* d_tgt_off,
-                  const void* src_desc, const void* tgt_desc, int desc_is_fp64, const float* src_keypts, const float* tgt_keypts,
-                  int D, int mutual, void* scratch, int32_t* corr, int32_t* out_first, int32_t* out_ends, float* corr_pos,
-                  float* out_src, float* out_tgt, cudaStream_t st) {
+// pdsc_match and pdsc_match_packed: P pairs packed back to back (null device tables: one pair).  Pair p's kept rows end at
+// out_ends[p], written by the call, as is out_first[0] = 0 unless out_first is null.
+static int match_impl(pdsc_engine* e, int32_t P, int32_t D, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                      const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const void* d_src_desc, const void* d_tgt_desc,
+                      int32_t desc_is_fp64, const float* d_src_keypts, const float* d_tgt_keypts, int32_t use_mutual,
+                      int32_t* d_corr, int32_t* d_out_first, int32_t* d_out_ends, float* d_corr_pos, float* d_out_src,
+                      float* d_out_tgt, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (D < 1 || D > kMatchMaxD) return fail(PDSC_ERR_UNSUPPORTED, "descriptor dimension %d outside [1, %d]", D, kMatchMaxD);
+  const int in_dim = engine_config(e).in_dim;
+  if (in_dim != 6) return fail(PDSC_ERR_UNSUPPORTED, "pdsc_match builds the in_dim = 6 input (engine has in_dim = %d)", in_dim);
+  if (!d_src_desc || !d_tgt_desc || !d_src_keypts || !d_tgt_keypts || !d_corr || !d_out_ends || !d_corr_pos || !d_out_src || !d_out_tgt)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_match: null tensor pointer");
+  if (int rc = check_scratch("pdsc_match", "scratch", d_scratch, scratch_bytes, match_scratch_bytes(h_src_offsets[P], h_tgt_offsets[P]),
+                             8))
+    return rc;
+  DeviceGuard g(engine_config(e).device);
   // without a device table (one pair) the kernels read the offsets {0, N} as 0 * N, 1 * N
-  const Offsets so{d_src_off, d_src_off ? 0 : h_src_off[1]}, to{d_tgt_off, d_tgt_off ? 0 : h_tgt_off[1]};
-  if (desc_is_fp64)
-    launch_match_t<double>(P, h_src_off, h_tgt_off, so, to, static_cast<const double*>(src_desc), static_cast<const double*>(tgt_desc),
-                           src_keypts, tgt_keypts, D, mutual, scratch, corr, out_first, out_ends, corr_pos, out_src, out_tgt, st);
-  else
-    launch_match_t<float>(P, h_src_off, h_tgt_off, so, to, static_cast<const float*>(src_desc), static_cast<const float*>(tgt_desc),
-                          src_keypts, tgt_keypts, D, mutual, scratch, corr, out_first, out_ends, corr_pos, out_src, out_tgt, st);
+  const Offsets so{d_src_offsets, d_src_offsets ? 0 : h_src_offsets[1]}, to{d_tgt_offsets, d_tgt_offsets ? 0 : h_tgt_offsets[1]};
+  auto run = [&](auto* src_desc, auto* tgt_desc) {
+    launch_match_t(P, h_src_offsets, h_tgt_offsets, so, to, src_desc, tgt_desc, d_src_keypts, d_tgt_keypts, D, use_mutual, d_scratch,
+                   d_corr, d_out_first, d_out_ends, d_corr_pos, d_out_src, d_out_tgt, static_cast<cudaStream_t>(cuda_stream));
+  };
+  if (desc_is_fp64) run(static_cast<const double*>(d_src_desc), static_cast<const double*>(d_tgt_desc));
+  else run(static_cast<const float*>(d_src_desc), static_cast<const float*>(d_tgt_desc));
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
 }
 
 }  // namespace pdsc
+
+// ---- C ABI ------------------------------------------------------------------------------------------------------
+using namespace pdsc;
+
+extern "C" {
+
+size_t pdsc_match_scratch_bytes(int32_t Ns, int32_t Nt) { return (Ns > 0 && Nt > 0) ? match_scratch_bytes(Ns, Nt) : 0; }
+
+size_t pdsc_match_packed_scratch_bytes(int32_t P, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets) {
+  const char* who = "pdsc_match_packed_scratch_bytes";
+  if (check_offsets(who, "source ", P, h_src_offsets, 1) || check_offsets(who, "target ", P, h_tgt_offsets, 1)) return 0;
+  return match_scratch_bytes(h_src_offsets[P], h_tgt_offsets[P]);
+}
+
+int pdsc_match(pdsc_engine* e, int32_t Ns, int32_t Nt, int32_t D, const void* d_src_desc, const void* d_tgt_desc,
+               int32_t desc_is_fp64, const float* d_src_keypts, const float* d_tgt_keypts, int32_t use_mutual,
+               int32_t* d_corr, int32_t* d_count, float* d_corr_pos, float* d_out_src, float* d_out_tgt, void* d_scratch,
+               size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (Ns <= 0 || Nt <= 0) return fail(PDSC_ERR_SHAPE, "need Ns >= 1 and Nt >= 1 (got %d, %d)", Ns, Nt);
+  // the packed call with one pair: its offsets need no device table, and its end row is the count
+  const int32_t src_off[2] = {0, Ns}, tgt_off[2] = {0, Nt};
+  return match_impl(e, 1, D, src_off, tgt_off, nullptr, nullptr, d_src_desc, d_tgt_desc, desc_is_fp64, d_src_keypts, d_tgt_keypts,
+                    use_mutual, d_corr, nullptr, d_count, d_corr_pos, d_out_src, d_out_tgt, d_scratch, scratch_bytes, cuda_stream);
+}
+
+int pdsc_match_packed(pdsc_engine* e, int32_t P, int32_t D, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                      const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const void* d_src_desc, const void* d_tgt_desc,
+                      int32_t desc_is_fp64, const float* d_src_keypts, const float* d_tgt_keypts, int32_t use_mutual,
+                      int32_t* d_corr, int32_t* d_out_offsets, float* d_corr_pos, float* d_out_src, float* d_out_tgt,
+                      void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_offsets("pdsc_match_packed", "source ", P, h_src_offsets, 1)) return rc;
+  if (int rc = check_offsets("pdsc_match_packed", "target ", P, h_tgt_offsets, 1)) return rc;
+  if (!d_src_offsets || !d_tgt_offsets || !d_out_offsets) return fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_match_packed: null offsets");
+  return match_impl(e, P, D, h_src_offsets, h_tgt_offsets, d_src_offsets, d_tgt_offsets, d_src_desc, d_tgt_desc, desc_is_fp64,
+                    d_src_keypts, d_tgt_keypts, use_mutual, d_corr, d_out_offsets, d_out_offsets + 1, d_corr_pos, d_out_src,
+                    d_out_tgt, d_scratch, scratch_bytes, cuda_stream);
+}
+
+}  // extern "C"

@@ -30,6 +30,9 @@
 // few voxels apart that is a handful, but a set whose rows all fall into one cell makes every iteration N^2 (correct, slow).
 #include <math.h>
 
+#include <cmath>
+
+#include "abi.h"
 #include "common.cuh"
 #include "kernels.h"
 #include "sets.cuh"
@@ -265,6 +268,7 @@ __device__ void build_grid(const float* __restrict__ pt, int Nt, const float* __
 }
 }  // namespace
 
+// scratch of B pairs with Rs source and Rt target rows in all, 8-byte aligned
 size_t icp_scratch_bytes(long long Rs, long long Rt) { return (size_t)Rs * 28 + (size_t)Rt * kGridBytesPerRow; }
 size_t information_scratch_bytes(long long Rt) { return (size_t)Rt * kGridBytesPerRow; }
 
@@ -452,20 +456,96 @@ __global__ void __launch_bounds__(kIcpThreads) information_kernel(const float* _
   }
 }
 
-void launch_icp(int B, const int32_t* d_src_off, const int32_t* d_tgt_off, long long Rs, long long Rt, const float* src,
-                const float* tgt, const float* init, double r, int max_iteration, float* trans, double* fitness, double* rmse,
-                int32_t* iterations, int32_t* status, void* scratch, cudaStream_t st) {
-  const double r2f = (double)(float)(r * r);
-  icp_kernel<<<B, kIcpThreads, 0, st>>>(src, tgt, init, Offsets{d_src_off, 0}, Offsets{d_tgt_off, 0}, r, r2f, max_iteration,
-                                        icp_carve(scratch, Rs, Rt), trans, fitness, rmse, iterations, status);
-}
-
-void launch_information(int B, const int32_t* d_src_off, const int32_t* d_tgt_off, long long Rt, const float* src, const float* tgt,
-                        const float* trans, double r, double* info, int32_t* status, void* scratch, cudaStream_t st) {
-  const double r2f = (double)(float)(r * r);
-  unsigned char* p = static_cast<unsigned char*>(scratch);
-  information_kernel<<<B, kIcpThreads, 0, st>>>(src, tgt, trans, Offsets{d_src_off, 0}, Offsets{d_tgt_off, 0}, r, r2f,
-                                                grid_carve(p, Rt), info, status);
+// pdsc_icp_packed and pdsc_icp_clouds_packed: one set of checks and one launch, under the caller's name
+static int icp_clouds(const char* fn, pdsc_engine* e, int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                      const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const float* d_src, const float* d_tgt,
+                      const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans, double* d_fitness,
+                      double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
+                      void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  const bool one = h_src_offsets == h_tgt_offsets;     // pdsc_icp_packed: one offsets array for both sides
+  if (int rc = check_offsets(fn, one ? "" : "source ", B, h_src_offsets, 1)) return rc;
+  if (!one)
+    if (int rc = check_offsets(fn, "target ", B, h_tgt_offsets, 1)) return rc;
+  if (!d_src_offsets || !d_tgt_offsets || !d_src || !d_tgt || !d_init || !d_trans)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_corr_dist must be positive and finite (got %g)", fn, max_corr_dist);
+  if (max_iteration < 1) return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_iteration must be >= 1 (got %d)", fn, max_iteration);
+  const long long Rs = h_src_offsets[B], Rt = h_tgt_offsets[B];
+  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, icp_scratch_bytes(Rs, Rt), 8)) return rc;
+  DeviceGuard g(engine_config(e).device);
+  const double r2f = (double)(float)(max_corr_dist * max_corr_dist);
+  icp_kernel<<<B, kIcpThreads, 0, static_cast<cudaStream_t>(cuda_stream)>>>(
+      d_src, d_tgt, d_init, Offsets{d_src_offsets, 0}, Offsets{d_tgt_offsets, 0}, max_corr_dist, r2f, max_iteration,
+      icp_carve(d_scratch, Rs, Rt), d_trans, d_fitness, d_rmse, d_iterations, d_status);
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
 }
 
 }  // namespace pdsc
+
+// ---- C ABI ------------------------------------------------------------------------------------------------------
+using namespace pdsc;
+
+extern "C" {
+
+size_t pdsc_icp_packed_scratch_bytes(int32_t B, const int32_t* h_offsets) {
+  return pdsc_icp_clouds_packed_scratch_bytes(B, h_offsets, h_offsets);
+}
+
+size_t pdsc_icp_clouds_packed_scratch_bytes(int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets) {
+  const char* who = "pdsc_icp_clouds_packed_scratch_bytes";
+  if (check_offsets(who, "source ", B, h_src_offsets, 1) || check_offsets(who, "target ", B, h_tgt_offsets, 1)) return 0;
+  return icp_scratch_bytes(h_src_offsets[B], h_tgt_offsets[B]);
+}
+
+int pdsc_icp_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
+                    const float* d_tgt, const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans,
+                    double* d_fitness, double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
+                    void* cuda_stream) {
+  return icp_clouds("pdsc_icp_packed", e, B, h_offsets, h_offsets, d_offsets, d_offsets, d_src, d_tgt, d_init, max_corr_dist,
+                    max_iteration, d_trans, d_fitness, d_rmse, d_iterations, d_status, d_scratch, scratch_bytes, cuda_stream);
+}
+
+int pdsc_icp_clouds_packed(pdsc_engine* e, int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                           const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const float* d_src, const float* d_tgt,
+                           const float* d_init, double max_corr_dist, int32_t max_iteration, float* d_trans, double* d_fitness,
+                           double* d_rmse, int32_t* d_iterations, int32_t* d_status, void* d_scratch, size_t scratch_bytes,
+                           void* cuda_stream) {
+  return icp_clouds("pdsc_icp_clouds_packed", e, B, h_src_offsets, h_tgt_offsets, d_src_offsets, d_tgt_offsets, d_src, d_tgt,
+                    d_init, max_corr_dist, max_iteration, d_trans, d_fitness, d_rmse, d_iterations, d_status, d_scratch,
+                    scratch_bytes, cuda_stream);
+}
+
+size_t pdsc_information_matrix_packed_scratch_bytes(int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets) {
+  const char* who = "pdsc_information_matrix_packed_scratch_bytes";
+  if (check_offsets(who, "source ", B, h_src_offsets, 1) || check_offsets(who, "target ", B, h_tgt_offsets, 1)) return 0;
+  return information_scratch_bytes(h_tgt_offsets[B]);
+}
+
+int pdsc_information_matrix_packed(pdsc_engine* e, int32_t B, const int32_t* h_src_offsets, const int32_t* h_tgt_offsets,
+                                   const int32_t* d_src_offsets, const int32_t* d_tgt_offsets, const float* d_src, const float* d_tgt,
+                                   const float* d_trans, double max_corr_dist, double* d_info, int32_t* d_status, void* d_scratch,
+                                   size_t scratch_bytes, void* cuda_stream) {
+  const char* fn = "pdsc_information_matrix_packed";
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_offsets(fn, "source ", B, h_src_offsets, 1)) return rc;
+  if (int rc = check_offsets(fn, "target ", B, h_tgt_offsets, 1)) return rc;
+  if (!d_src_offsets || !d_tgt_offsets || !d_src || !d_tgt || !d_trans || !d_info)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_corr_dist must be positive and finite (got %g)", fn, max_corr_dist);
+  const long long Rt = h_tgt_offsets[B];
+  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, information_scratch_bytes(Rt), 8)) return rc;
+  DeviceGuard g(engine_config(e).device);
+  const double r2f = (double)(float)(max_corr_dist * max_corr_dist);
+  unsigned char* p = static_cast<unsigned char*>(d_scratch);
+  information_kernel<<<B, kIcpThreads, 0, static_cast<cudaStream_t>(cuda_stream)>>>(
+      d_src, d_tgt, d_trans, Offsets{d_src_offsets, 0}, Offsets{d_tgt_offsets, 0}, max_corr_dist, r2f, grid_carve(p, Rt), d_info,
+      d_status);
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
+}
+
+}  // extern "C"

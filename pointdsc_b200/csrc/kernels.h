@@ -5,11 +5,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include <string>
-
 #include "sets.cuh"
-
-struct pdsc_fcgf;
 
 namespace pdsc {
 
@@ -93,108 +89,6 @@ void launch_select_refine(const float* src, const float* tgt, const float* seed_
                           float* init_trans_out, int32_t* best_out, int32_t* refine_solves, int B, int N, int S,
                           float inlier_threshold, float refine_threshold, int max_refine, cudaStream_t st,
                           const SetDesc* sets);
-
-// ---- f3: per-pair evaluation statistics (eval_stats.cu), 10 floats per set -----------------------------------
-void launch_eval_stats(const float* pred_trans, const float* gt_trans, const float* src, const float* tgt,
-                       const float* pred_labels, const float* gt_labels, float* stats, int B, const int32_t* d_offsets, int N,
-                       float re_thre, float te_thre, cudaStream_t st);   // set b: rows [offsets[b], offsets[b+1]), or b * N without a table
-
-// ---- f1: correspondence front end (frontend.cu): nearest neighbour in descriptor space, mutual check, centred input ----
-// P pairs packed back to back (offsets [P + 1], host and device; null device tables: one pair).  Pair p's kept rows end at
-// out_ends[p], written by the call, as is out_first[0] = 0 unless out_first is null.
-size_t match_scratch_bytes(int Ns, int Nt);      // Ns, Nt: the call's total source / target rows
-int match_max_dim();
-void launch_match(int P, const int32_t* h_src_off, const int32_t* h_tgt_off, const int32_t* d_src_off, const int32_t* d_tgt_off,
-                  const void* src_desc, const void* tgt_desc, int desc_is_fp64, const float* src_keypts, const float* tgt_keypts,
-                  int D, int mutual, void* scratch, int32_t* corr, int32_t* out_first, int32_t* out_ends, float* corr_pos,
-                  float* out_src, float* out_tgt, cudaStream_t st);
-
-// ---- f4: N x N power iteration (eig_power.cu) -----------------------------------------------------------------
-size_t eig_scratch_bytes(int B, int N);
-int launch_leading_eigenvector(const float* M, float* v, int* iters_run, int B, int N, int iters, int early_exit, void* scratch,
-                               cudaStream_t st);   // returns cudaError_t
-
-// ---- f2: descriptor front end (fpfh.cu): voxel down-sampling, normals, FPFH -------------------------------------
-// P clouds packed back to back (offsets [P + 1], host and device; null device tables: one cloud), status [P].  Cloud p's voxel
-// means end at row out_ends[p], written by the call, as is out_first[0] = 0 unless out_first is null.
-size_t voxel_scratch_bytes(int P, const int32_t* h_off);
-void launch_voxel_down_sample(int P, const int32_t* h_off, const int32_t* d_off, const float* pts, double voxel, float* out_pts,
-                              int32_t* out_first, int32_t* out_ends, int32_t* status, void* scratch, cudaStream_t st);
-size_t fpfh_scratch_bytes(int m, int max_nn);      // m: the call's total key points
-int launch_estimate_normals(int P, const int32_t* h_off, const int32_t* d_off, const float* pts, double radius, int max_nn,
-                            double* normals, int32_t* status, void* scratch, cudaStream_t st);      // returns cudaError_t
-int launch_compute_fpfh(int P, const int32_t* h_off, const int32_t* d_off, const float* pts, const double* normals, double radius,
-                        int max_nn, int normalise, double* out, int32_t* status, void* scratch,
-                        cudaStream_t st);      // returns cudaError_t
-
-// ---- point-to-point ICP and information matrices between two clouds (icp.cu) ------------------------------------
-// B pairs: pair b's source is rows [src_off[b], src_off[b+1]) of src, its target rows [tgt_off[b], tgt_off[b+1]) of tgt (device
-// offsets [B + 1]; Rs, Rt = the last entries), init / trans [B,4,4]; fitness, rmse, iterations and status may be null.  The
-// correspondence key points are the case src_off = tgt_off.  Scratch: icp_scratch_bytes(Rs, Rt) bytes, 8-byte aligned.
-size_t icp_scratch_bytes(long long Rs, long long Rt);
-void launch_icp(int B, const int32_t* d_src_off, const int32_t* d_tgt_off, long long Rs, long long Rt, const float* src,
-                const float* tgt, const float* init, double r, int max_iteration, float* trans, double* fitness, double* rmse,
-                int32_t* iterations, int32_t* status, void* scratch, cudaStream_t st);
-// The same pairs, trans [B,4,4] -> info [B,6,6] double; status may be null.  Scratch: information_scratch_bytes(Rt) bytes,
-// 8-byte aligned.
-size_t information_scratch_bytes(long long Rt);
-void launch_information(int B, const int32_t* d_src_off, const int32_t* d_tgt_off, long long Rt, const float* src, const float* tgt,
-                        const float* trans, double r, double* info, int32_t* status, void* scratch, cudaStream_t st);
-
-// ---- correspondence RANSAC over the pairs the network kept (ransac.cu) ----------------------------------------
-// B sets packed back to back (device offsets [B + 1], R = offsets[B] rows), labels [R] (> 0: a candidate), trans [B,4,4],
-// out_labels [R]; fitness, rmse, best, status [B], hyp_good, hyp_rmse [B, max_iteration] and hyp_trans [B, max_iteration, 12]
-// may be null.  B <= 65535.
-// Scratch: ransac_scratch_bytes(R, B, max_iteration) bytes, 16-byte aligned.
-size_t ransac_scratch_bytes(long long R, int B, int max_iteration);
-void launch_ransac(int B, const int32_t* d_off, long long R, const float* src, const float* tgt, const float* labels, double r,
-                   int max_iteration, unsigned long long seed, float* trans, float* out_labels, double* fitness, double* rmse,
-                   int32_t* best, int32_t* status, int32_t* hyp_good, double* hyp_rmse, double* hyp_trans, void* scratch,
-                   cudaStream_t st);
-
-// ---- f8: FCGF descriptors (fcgf.cu) -----------------------------------------------------------------------------
-// The weight handle of the C ABI (folded, packed and uploaded by fcgf_commit) and the one launch chain of a packed call.
-pdsc_fcgf* fcgf_new(int k1);
-void fcgf_free(pdsc_fcgf* h);
-int fcgf_set_param(pdsc_fcgf* h, const char* name, const float* data, int64_t numel, size_t* expected);   // 1 unknown, 2 size
-int fcgf_commit(pdsc_fcgf* h, std::string* missing);      // -1: *missing names an absent parameter; > 0: a cudaError_t
-bool fcgf_committed(const pdsc_fcgf* h);
-int fcgf_kernel_size(const pdsc_fcgf* h);
-size_t fcgf_scratch_bytes(int P, const int32_t* h_off, int k1);
-int fcgf_scratch_layout(int P, const int32_t* h_off, int k1, int64_t* offsets, int capacity);
-int launch_fcgf(const pdsc_fcgf* h, int P, const int32_t* h_off, const int32_t* d_off, const float* pts, double voxel,
-                float* keypts, float* desc, int32_t* out_off, int32_t* status, void* scratch, cudaStream_t st);   // cudaError_t
-
-// ---- the spectral-matching baseline (spectral_matching.cu) ---------------------------------------------------
-// B sets packed back to back (host and device offsets [B + 1], R = offsets[B] rows, every set 1 .. spectral_matching_max_n() rows),
-// corr [R,6], src / tgt [R,3]; trans [B,4,4], labels [R]; eig_out [R] and iterates [10,R] (row t - 1: iterate v_t, a test
-// output) may be null.  B <= 65535.
-// Scratch: sm_scratch_bytes(R, B) bytes, 16-byte aligned.
-int spectral_matching_max_n();
-size_t sm_scratch_bytes(long long R, int B);
-void launch_spectral_matching(int B, const int32_t* h_off, const int32_t* d_off, const float* corr, const float* src, const float* tgt,
-                              double inlier_threshold, float* trans, float* labels, float* eig_out, float* iterates, void* scratch,
-                              cudaStream_t st);
-
-// ---- f9: TSDF integration and surface vertices of RGB-D fragments (fragments.cu) ---------------------------------------
-// F fragments of 1 .. kMaxFragmentFrames frames each (device frame offsets [F + 1], NF frames): depth [NF,H,W] uint16, colour
-// [NF,H,W,3] uint8, poses [NF,2,16] float64 (extrinsic, camera pose), intrinsic the host fx, fy, cx, cy.  The table
-// (tsdf_table_bytes(F, max_units), 8-byte aligned) is written by the touch and read by every later stage of the same volume.
-constexpr int kMaxFragmentFrames = 256;
-size_t tsdf_table_bytes(int F, int max_units);
-size_t tsdf_integrate_scratch_bytes(int F, long long U);
-void launch_tsdf_touch(int F, int NF, const int32_t* d_frame_off, int H, int W, const double* intrinsic, const uint16_t* depth,
-                       const double* poses, double depth_scale, double depth_trunc, double voxel, double trunc, int max_units,
-                       int32_t* counts, int32_t* status, void* table, cudaStream_t st);
-void launch_tsdf_integrate(int F, const int32_t* d_frame_off, const int32_t* d_unit_off, long long U, int H, int W,
-                           const double* intrinsic, const uint16_t* depth, const uint8_t* color, const double* poses,
-                           double depth_scale, double depth_trunc, double voxel, double trunc, int max_units, void* table,
-                           int32_t* unit_keys, float* tsdf, float* weight, float* color_out, void* scratch, cudaStream_t st);
-void launch_vertex_count(int F, const int32_t* d_unit_off, int U, int max_units, void* table, const int32_t* unit_keys,
-                         const float* tsdf, const float* weight, long long* ends, long long* frag_off, cudaStream_t st);
-void launch_vertex_write(int F, const int32_t* d_unit_off, int U, int max_units, void* table, const int32_t* unit_keys,
-                         const float* tsdf, const float* weight, const float* color, double voxel, const long long* ends,
-                         double* vertices, double* colors, cudaStream_t st);
 
 // ---- per-device launch configuration (device_state.cu) ----------------------------------------------------
 // opt `kernel` in to `bytes` of dynamic shared memory on the CURRENT device (no-op if already granted there)

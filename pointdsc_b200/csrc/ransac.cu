@@ -30,6 +30,9 @@
 // Cost.  max_iteration * M distance tests per set, about 27 fp64 operations each, plus one 3x3 Jacobi solve per hypothesis.
 #include <math.h>
 
+#include <cmath>
+
+#include "abi.h"
 #include "common.cuh"
 #include "kernels.h"
 #include "sets.cuh"
@@ -45,6 +48,7 @@ constexpr int kRansacChunk = PDSC_RANSAC_CHUNK;   // hypotheses (threads) per sc
 constexpr int kRansacTile = 256;                  // candidates per shared-memory tile of the scoring kernel
 constexpr int kRansacThreads = 256;               // candidates and finish kernels
 constexpr int kRansacWarps = kRansacThreads / 32;
+constexpr int kRansacMaxSets = 65535;             // the scoring kernel's sets are its grid's y dimension
 
 // set b's region: candidates [row0, row0 + M_b) as 6 doubles (source x y z, target x y z); keys [b * max_iteration, ...)
 struct RansacScratch {
@@ -304,18 +308,71 @@ __global__ void __launch_bounds__(kRansacThreads) ransac_finish_kernel(const flo
     out_labels[row0 + rows[k]] = ransac_d2(R, t, cand + 6 * (size_t)k) < r2 ? 1.0f : 0.0f;
 }
 
-void launch_ransac(int B, const int32_t* d_off, long long R, const float* src, const float* tgt, const float* labels, double r,
-                   int max_iteration, unsigned long long seed, float* trans, float* out_labels, double* fitness, double* rmse,
-                   int32_t* best, int32_t* status, int32_t* hyp_good, double* hyp_rmse, double* hyp_trans, void* scratch,
-                   cudaStream_t st) {
-  const double r2 = r * r;
-  const Offsets off{d_off, 0};
-  const RansacScratch s = ransac_carve(scratch, R, B, max_iteration);
-  ransac_candidates_kernel<<<B, kRansacThreads, 0, st>>>(src, tgt, labels, off, s);
+// pdsc_ransac_packed and pdsc_ransac_packed_hypotheses: one set of checks and one launch, under the caller's name
+static int ransac_packed(const char* fn, pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                         const float* d_src, const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration,
+                         uint64_t seed, float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse, int32_t* d_best,
+                         int32_t* d_status, int32_t* d_hyp_good, double* d_hyp_rmse, double* d_hyp_trans, void* d_scratch,
+                         size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_offsets(fn, "", B, h_offsets, 1)) return rc;
+  if (B > kRansacMaxSets) return fail(PDSC_ERR_UNSUPPORTED, "%s: at most %d sets per call (got %d)", fn, kRansacMaxSets, B);
+  if (!d_offsets || !d_src || !d_tgt || !d_labels || !d_trans || !d_out_labels)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  if (!(max_corr_dist > 0.0) || !std::isfinite(max_corr_dist))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_corr_dist must be positive and finite (got %g)", fn, max_corr_dist);
+  if (max_iteration < 1)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: max_iteration must be >= 1 (got %d)", fn, max_iteration);
+  const long long R = h_offsets[B];
+  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, ransac_scratch_bytes(R, B, max_iteration), 16)) return rc;
+  DeviceGuard g(engine_config(e).device);
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  const double r2 = max_corr_dist * max_corr_dist;
+  const Offsets off{d_offsets, 0};
+  const RansacScratch s = ransac_carve(d_scratch, R, B, max_iteration);
+  ransac_candidates_kernel<<<B, kRansacThreads, 0, st>>>(d_src, d_tgt, d_labels, off, s);
   const dim3 grid((unsigned)((max_iteration + kRansacChunk - 1) / kRansacChunk), (unsigned)B);
-  ransac_score_kernel<<<grid, kRansacChunk, 0, st>>>(off, r2, max_iteration, seed, s);
-  ransac_finish_kernel<<<B, kRansacThreads, 0, st>>>(labels, off, r2, max_iteration, seed, s, trans, out_labels, fitness, rmse, best,
-                                                     status, hyp_good, hyp_rmse, hyp_trans);
+  ransac_score_kernel<<<grid, kRansacChunk, 0, st>>>(off, r2, max_iteration, (unsigned long long)seed, s);
+  ransac_finish_kernel<<<B, kRansacThreads, 0, st>>>(d_labels, off, r2, max_iteration, (unsigned long long)seed, s, d_trans,
+                                                     d_out_labels, d_fitness, d_rmse, d_best, d_status, d_hyp_good, d_hyp_rmse,
+                                                     d_hyp_trans);
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
 }
 
 }  // namespace pdsc
+
+// ---- C ABI ------------------------------------------------------------------------------------------------------
+using namespace pdsc;
+
+extern "C" {
+
+size_t pdsc_ransac_packed_scratch_bytes(int32_t B, const int32_t* h_offsets, int32_t max_iteration) {
+  if (check_offsets("pdsc_ransac_packed_scratch_bytes", "", B, h_offsets, 1)) return 0;
+  if (max_iteration < 1) {
+    fail(PDSC_ERR_INVALID_ARGUMENT, "pdsc_ransac_packed_scratch_bytes: max_iteration must be >= 1 (got %d)", max_iteration);
+    return 0;
+  }
+  return ransac_scratch_bytes(h_offsets[B], B, max_iteration);
+}
+
+int pdsc_ransac_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
+                       const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration, uint64_t seed,
+                       float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse, int32_t* d_best, int32_t* d_status,
+                       int32_t* d_hyp_good, double* d_hyp_rmse, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  return ransac_packed("pdsc_ransac_packed", e, B, h_offsets, d_offsets, d_src, d_tgt, d_labels, max_corr_dist, max_iteration, seed,
+                       d_trans, d_out_labels, d_fitness, d_rmse, d_best, d_status, d_hyp_good, d_hyp_rmse, nullptr, d_scratch,
+                       scratch_bytes, cuda_stream);
+}
+
+int pdsc_ransac_packed_hypotheses(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets, const float* d_src,
+                                  const float* d_tgt, const float* d_labels, double max_corr_dist, int32_t max_iteration,
+                                  uint64_t seed, float* d_trans, float* d_out_labels, double* d_fitness, double* d_rmse,
+                                  int32_t* d_best, int32_t* d_status, int32_t* d_hyp_good, double* d_hyp_rmse, double* d_hyp_trans,
+                                  void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  return ransac_packed("pdsc_ransac_packed_hypotheses", e, B, h_offsets, d_offsets, d_src, d_tgt, d_labels, max_corr_dist,
+                       max_iteration, seed, d_trans, d_out_labels, d_fitness, d_rmse, d_best, d_status, d_hyp_good, d_hyp_rmse,
+                       d_hyp_trans, d_scratch, scratch_bytes, cuda_stream);
+}
+
+}  // extern "C"

@@ -34,6 +34,9 @@
 // 24 FP32 instructions plus the two square-root sequences, 10 N^2 entries per set.
 #include <math.h>
 
+#include <cmath>
+
+#include "abi.h"
 #include "common.cuh"
 #include "kernels.h"
 #include "sets.cuh"
@@ -48,6 +51,7 @@ constexpr int kSmTile = 512;               // columns staged per pass (14 KB)
 constexpr int kSmIterations = 10;          // baseline_3DMatch.py:41
 constexpr double kSmTopRatio = 0.1;        // top_ratio, baseline_3DMatch.py:19
 constexpr int kSmMaxN = 16384;             // the a6' sort's limit (seeds.cu)
+constexpr int kSmMaxSets = 65535;          // the power kernel's sets are its grid's y dimension
 
 __host__ __device__ inline size_t align16(size_t x) { return (x + 15) / 16 * 16; }
 
@@ -196,26 +200,36 @@ __global__ void __launch_bounds__(kRefThreads) sm_kabsch_kernel(const float* __r
   if (tid < 16) trans[(size_t)b * 16 + tid] = (tid < 12) ? T[tid] : (tid == 15 ? 1.0f : 0.0f);
 }
 
-int spectral_matching_max_n() { return kSmMaxN; }
-
 size_t sm_scratch_bytes(long long R, int B) {
   return align16((size_t)B * sizeof(SetDesc)) + 2 * align16((size_t)R * 4) + (size_t)R * 4;
 }
 
-void launch_spectral_matching(int B, const int32_t* h_off, const int32_t* d_off, const float* corr, const float* src, const float* tgt,
-                              double inlier_threshold, float* trans, float* labels, float* eig_out, float* iterates, void* scratch,
-                              cudaStream_t st) {
-  const long long R = h_off[B];
+// pdsc_spectral_matching_packed and pdsc_spectral_matching_packed_iterates: one set of checks and one launch, under the caller's name
+static int spectral_matching_packed(const char* fn, pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                                    const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts,
+                                    double inlier_threshold, float* d_trans, float* d_labels, float* d_eigenvector, float* d_iterates,
+                                    void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (!e) return fail(PDSC_ERR_INVALID_ARGUMENT, "null engine");
+  if (int rc = check_offsets(fn, "", B, h_offsets, 1, kSmMaxN)) return rc;
+  if (B > kSmMaxSets) return fail(PDSC_ERR_UNSUPPORTED, "%s: at most %d sets per call (got %d)", fn, kSmMaxSets, B);
+  if (!d_offsets || !d_corr_pos || !d_src_keypts || !d_tgt_keypts || !d_trans || !d_labels)
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: null tensor pointer", fn);
+  if (!(inlier_threshold > 0.0) || !std::isfinite(inlier_threshold))
+    return fail(PDSC_ERR_INVALID_ARGUMENT, "%s: inlier_threshold must be positive and finite (got %g)", fn, inlier_threshold);
+  const long long R = h_offsets[B];
+  if (int rc = check_scratch(fn, "scratch", d_scratch, scratch_bytes, sm_scratch_bytes(R, B), 16)) return rc;
+  DeviceGuard g(engine_config(e).device);
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   int Nmax = 0;
-  for (int b = 0; b < B; ++b) Nmax = max(Nmax, h_off[b + 1] - h_off[b]);
-  const Offsets off{d_off, 0};
-  const SmScratch s = sm_carve(scratch, R, B);
+  for (int b = 0; b < B; ++b) Nmax = max(Nmax, h_offsets[b + 1] - h_offsets[b]);
+  const Offsets off{d_offsets, 0};
+  const SmScratch s = sm_carve(d_scratch, R, B);
   const float coef = (float)(4.5 / (inlier_threshold * inlier_threshold));     // 1 / (2 sigma^2), sigma = tau / 3
   // rows per warp: the most that still gives two CTAs per SM over the call's sets
   const long long want = 2LL * device_sm_count();
   auto ctas = [&](int rows) {
     long long n = 0;
-    for (int b = 0; b < B; ++b) n += (h_off[b + 1] - h_off[b] + rows - 1) / rows;
+    for (int b = 0; b < B; ++b) n += (h_offsets[b + 1] - h_offsets[b] + rows - 1) / rows;
     return n;
   };
   const int RW = ctas(kSmWarps * 4) >= want ? 4 : (ctas(kSmWarps * 2) >= want ? 2 : 1);
@@ -224,14 +238,45 @@ void launch_spectral_matching(int B, const int32_t* h_off, const int32_t* d_off,
   float* bufs[2] = {s.a, s.b};
   for (int t = 0; t < kSmIterations; ++t) {
     float* uo = bufs[t & 1];
-    if (RW == 4) sm_power_kernel<4><<<grid, kSmThreads, 0, st>>>(corr, off, vin, uo, coef);
-    else if (RW == 2) sm_power_kernel<2><<<grid, kSmThreads, 0, st>>>(corr, off, vin, uo, coef);
-    else sm_power_kernel<1><<<grid, kSmThreads, 0, st>>>(corr, off, vin, uo, coef);
-    sm_norm_kernel<<<B, kSmThreads, 0, st>>>(uo, off, t == 0 ? s.sets : nullptr, iterates ? iterates + (size_t)t * R : nullptr);
+    if (RW == 4) sm_power_kernel<4><<<grid, kSmThreads, 0, st>>>(d_corr_pos, off, vin, uo, coef);
+    else if (RW == 2) sm_power_kernel<2><<<grid, kSmThreads, 0, st>>>(d_corr_pos, off, vin, uo, coef);
+    else sm_power_kernel<1><<<grid, kSmThreads, 0, st>>>(d_corr_pos, off, vin, uo, coef);
+    sm_norm_kernel<<<B, kSmThreads, 0, st>>>(uo, off, t == 0 ? s.sets : nullptr, d_iterates ? d_iterates + (size_t)t * R : nullptr);
     vin = uo;
   }
   launch_top_seeds(vin, s.seeds, B, Nmax, num_seeds(Nmax, kSmTopRatio), st, s.sets);
-  sm_kabsch_kernel<<<B, kRefThreads, 0, st>>>(src, tgt, vin, s.seeds, off, trans, labels, eig_out);
+  sm_kabsch_kernel<<<B, kRefThreads, 0, st>>>(d_src_keypts, d_tgt_keypts, vin, s.seeds, off, d_trans, d_labels, d_eigenvector);
+  PDSC_CUDA(cudaGetLastError());
+  return PDSC_OK;
 }
 
 }  // namespace pdsc
+
+// ---- C ABI ------------------------------------------------------------------------------------------------------
+using namespace pdsc;
+
+extern "C" {
+
+size_t pdsc_spectral_matching_packed_scratch_bytes(int32_t B, const int32_t* h_offsets) {
+  if (check_offsets("pdsc_spectral_matching_packed_scratch_bytes", "", B, h_offsets, 1, kSmMaxN)) return 0;
+  return sm_scratch_bytes(h_offsets[B], B);
+}
+
+int pdsc_spectral_matching_packed(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                                  const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts, double inlier_threshold,
+                                  float* d_trans, float* d_labels, float* d_eigenvector, void* d_scratch, size_t scratch_bytes,
+                                  void* cuda_stream) {
+  return spectral_matching_packed("pdsc_spectral_matching_packed", e, B, h_offsets, d_offsets, d_corr_pos, d_src_keypts, d_tgt_keypts,
+                                  inlier_threshold, d_trans, d_labels, d_eigenvector, nullptr, d_scratch, scratch_bytes, cuda_stream);
+}
+
+int pdsc_spectral_matching_packed_iterates(pdsc_engine* e, int32_t B, const int32_t* h_offsets, const int32_t* d_offsets,
+                                           const float* d_corr_pos, const float* d_src_keypts, const float* d_tgt_keypts,
+                                           double inlier_threshold, float* d_trans, float* d_labels, float* d_eigenvector,
+                                           float* d_iterates, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  return spectral_matching_packed("pdsc_spectral_matching_packed_iterates", e, B, h_offsets, d_offsets, d_corr_pos, d_src_keypts,
+                                  d_tgt_keypts, inlier_threshold, d_trans, d_labels, d_eigenvector, d_iterates, d_scratch, scratch_bytes,
+                                  cuda_stream);
+}
+
+}  // extern "C"
